@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- samples/sec of `forward_kld` on the flagship neural-spline stack (BASELINE.json metric).
 
-    python bench.py --gpus 1 --steps 20 --warmup 5          # ours, one B200
+    python bench.py --gpus 1 --steps 20 --warmup 5          # ours, one H100
     torchrun --nproc-per-node N ... bench.py --gpus N ...    # data parallel: batch sharded, one all-reduce
     python bench.py --impl reference ...                     # CPU arm: the unmodified reference on the host cores
     python bench.py --impl reference-eager ...               # the unmodified reference, PyTorch eager on cuda:0
@@ -17,9 +17,12 @@ One "step" = one full `forward_kld` pass over one batch (all 64 layers + base de
 
 Timed region: W warm-up steps, then exactly K steps between barrier+synchronize, CUDA events on the
 launching stream, max over ranks.  Inputs rotate through NBUF distinct device batches whose total size
-exceeds L2 (so no step re-reads its input from L2); the packed weights (85 MB) cycle through L2 as they
+(160 MB) exceeds L2 (so no step re-reads its input from L2); the packed weights cycle through L2 as they
 do in real use.  `e2e` is the same pass through the C-ABI host entry point (`nfb_flow_forward_kld_host`):
 pinned host batch -> H2D -> kernels -> D2H of the scalar loss, every step.
+--dump-outputs DIR writes what the timed paths returned in their last step (DIR/forward_kld.npy: the loss of the
+device path; DIR/forward_kld_host.npy: the loss of the host entry point), float64.  Inputs and weights are seeded,
+so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -74,7 +77,7 @@ def oracle_spec(kind=KIND, layers=LAYERS):
 
 
 class ClockSampler(threading.Thread):
-    """Samples nvidia-smi SM clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """Samples nvidia-smi SM clocks / throttle reasons during the timed region (read-only queries)."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -107,20 +110,20 @@ class ClockSampler(threading.Thread):
 
 # ---------------------------------------------------------------------------------------------------------
 # CPU legs.  `--impl reference` and the GPU line's `cpu_baseline` both time the UNMODIFIED reference package
-# (baseline/_ref/normflows, copied verbatim from /root/reference by __graft_entry__.build()) on the host cores.
+# (oracle/_ref/normflows, installed by __graft_entry__.build() through oracle/reference.py) on the host cores.
 # The batch is data-parallel, so it is sharded over worker processes exactly like the GPU arm shards it over
 # GPUs: every worker builds the same model (same seed) with the reference's own classes and runs
 # `model.forward_kld(x_shard)` under no_grad.  The oracle port (oracle/nf_oracle.py) is the fallback only when
-# baseline/_ref is absent (kind "port").
+# oracle/_ref is absent (kind "port").
 # ---------------------------------------------------------------------------------------------------------
-REF_DIR = os.path.join(ROOT, "baseline", "_ref")
+REF_DIR = os.path.join(ROOT, "oracle", "_ref")
 _W = {}
 
 
 def usable_cpus():
-    """Host cores this process may actually use: min(affinity, cgroup CPU quota).  The GPU boxes of the pool show
-    128 logical CPUs but run the job in a cgroup with a 16-CPU quota (cpu.max = "1600000 100000"); sizing the
-    worker pool by os.cpu_count() oversubscribes the quota 8x and throttles (measured: 3.7 k samples/s either way)."""
+    """Host cores this process may actually use: min(affinity, cgroup CPU quota).  A container can show many more
+    logical CPUs than its cgroup quota (cpu.max) lets it run; sizing the worker pool by os.cpu_count() would then
+    oversubscribe the quota and throttle."""
     n = len(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else (os.cpu_count() or 1)
     try:
         q, p = open("/sys/fs/cgroup/cpu.max").read().split()[:2]
@@ -220,8 +223,8 @@ class CpuReference:
             p.join(timeout=10)
 
     def describe(self, steps, warmup, wall):
-        what = ("unmodified reference package (baseline/_ref/normflows, torch CPU fp32) model.forward_kld under no_grad"
-                if self.use_ref else "oracle/nf_oracle.py (numpy fp32 port; baseline/_ref absent) forward_kld")
+        what = ("unmodified reference package (oracle/_ref/normflows, torch CPU fp32) model.forward_kld under no_grad"
+                if self.use_ref else "oracle/nf_oracle.py (numpy fp32 port; oracle/_ref absent) forward_kld")
         return (f"{what}; {self.workers} worker processes x {self.threads} torch threads, {self.rows} rows each = "
                 f"{self.rows_total} rows per step, {warmup} warm-up + {steps} timed steps ({wall:.1f} s wall incl. start-up)")
 
@@ -249,7 +252,7 @@ def time_cpu_reference(rows_total, steps, warmup, kind=KIND):
 
 def cpu_baseline(kind=KIND):
     """GPU line's `cpu_baseline` (rank 0, N = 1): 1 warm-up + 2 timed passes of the reference over a bounded sample
-    (16 384 rows = 4096 per worker at 16 usable cores; ~4 s per pass there)."""
+    (16 384 rows = 4096 per worker at 16 usable cores)."""
     return time_cpu_reference(16384 if usable_cpus() >= 8 else 4096, steps=2, warmup=1, kind=kind)
 
 
@@ -262,7 +265,7 @@ def run_reference(args):
         return
     steps = max(1, args.steps)
     # full batch when the run is short; otherwise a bounded sample (>= 4096 rows per worker process) so that
-    # warm-up + K steps end within a few minutes on the 16-CPU quota of the GPU boxes (~4 k samples/s)
+    # warm-up + K steps end within a few minutes on a 16-core host
     cores = usable_cpus()
     if cores < 8:
         rows = min(args.batch, 4096)
@@ -323,12 +326,16 @@ def main():
     ap.add_argument("--no-reference-eager", action="store_true")
     ap.add_argument("--no-train-step", action="store_true")
     ap.add_argument("--no-extra-configs", action="store_true", help="skip BASELINE configs C1 / C2' / C3 / C5 (extra keys)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     if args.impl == "reference":
         return run_reference(args)
     if args.impl == "reference-eager":
         return run_reference_eager_cuda(args)
 
+    import numpy as np
     import torch
     import torch.distributed as dist
     import normflows as nf
@@ -351,11 +358,11 @@ def main():
         torch.cuda.synchronize()
         dist.barrier()
     warmup = max(3, args.warmup)
-    steps = max(1, args.steps)
+    steps = args.steps
     B = args.batch
 
     model = build_model().to(dev)
-    nbuf = max(2, (160 << 20) // (B * D * 4) + 1)  # rotating inputs: > 126 MB L2 in total
+    nbuf = max(2, (160 << 20) // (B * D * 4) + 1)  # rotating inputs: 160 MB in total, over three times the 50 MB L2
     g = torch.Generator().manual_seed(1234 + rank)
     xs_host = [(torch.randn(B, D, generator=g) * 1.5).pin_memory() for _ in range(2)]
     xs = [(torch.randn(B, D, generator=g) * 1.5).to(dev) for _ in range(nbuf)]
@@ -375,7 +382,7 @@ def main():
     stack = model._stack()
     launches_per_step = stack.launch_count()
     fused = stack.fused_layers()
-    assert len(fused) == 2 * LAYERS, "flagship stack must run on the fused tcgen05 kernel"
+    assert len(fused) == 2 * LAYERS, "flagship stack must run on the fused tensor-core kernel"
     torch.cuda.synchronize()
     if world > 1:
         dist.barrier()
@@ -398,6 +405,9 @@ def main():
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         elapsed_ms = float(t)
     loss_val = float(loss)
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "forward_kld.npy"), np.array([loss_val], dtype=np.float64))
 
     # ---- e2e through the host-buffer C-ABI entry point (H2D + kernels + D2H each step) ----
     for i in range(3):
@@ -409,6 +419,8 @@ def main():
     for i in range(steps):
         e2e_loss = model.forward_kld_host(xs_host[i % 2], dev)  # synchronous: returns the host float
     e2e_s = time.perf_counter() - t0
+    if args.dump_outputs and rank == 0:
+        np.save(os.path.join(args.dump_outputs, "forward_kld_host.npy"), np.array([float(e2e_loss)], dtype=np.float64))
     if world > 1:
         t = torch.tensor([e2e_s], device=dev)
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -438,30 +450,19 @@ def main():
         e1.record()
         torch.cuda.synchronize()
         k_ms = e0.elapsed_time(e1) / n_l  # includes a 65 K-element fill and a 2 KB memset (~4 us)
-        peaks = {}
-        try:
-            peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        except Exception:
-            pass
-        # the probe times the kernel alone, back to back for ~60 ms: the BURST figure is the honest denominator
-        peak = peaks.get("bf16_tflops", 1650.0)
+        # NVIDIA's data sheet for the H100 SXM: 989 TFLOP/s dense FP16 (700 W card).  A data-sheet rate, not a measured
+        # one: `clocks` shows the SM clock the run actually had.
+        peak = 989.0
         flops = FLOPS_PER_SAMPLE_LAYER[KIND] * B * LAYERS
         achieved = flops / (k_ms * 1e-3) / 1e12
-        traffic = None
-        tfile = os.path.join(ROOT, "profiles", "traffic.json")
-        if os.path.exists(tfile):
-            traffic = json.load(open(tfile)).get("dram_bytes_per_launch")
         roof = {"kernel": "nfb::fused_rqs_kernel, whole stack in one persistent launch: 32 x (LULinearPermute + MADE "
                           "conditioner + RQ spline + log-det), (layer, tile) work units",
                 "bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
-                "traffic": traffic, "kernel_ms": k_ms,
-                "peak_source": "MEASURED_PEAKS.json bf16_tflops (burst; of measured)" if peaks else "fallback 1650 (of fallback)",
+                "kernel_ms": k_ms, "peak_source": "H100 SXM data sheet, dense FP16",
                 "note": "algorithmic = dense fp32-equivalent GEMM flops of the reference (1.327 MFLOP/sample/layer x 32 "
                         "layers, SURVEY 8d).  The kernel runs every product as 3 fp16 tensor-core passes (split "
                         "precision with power-of-two operand scaling, needed for the rtol 1e-4 bar) so frac <= 1/3 by "
-                        "construction, and skips the all-zero blocks of the MADE masks (~31 % of the dense MMA work); "
-                        "ncu (profiles/r02b_fused_stack_ncu_summary.md): tensor pipe 29 % active after the zero-block "
-                        "skipping of round 2b (42 % before it), SM clock 1.81 GHz under this kernel's load"}
+                        "construction, and skips the all-zero [64 x 64] blocks of the MADE masks"}
 
     # ---- training step (extra key; every rank takes part): forward_kld + native backward (tensor-core dgrad /
     # wgrad, analytic spline adjoint) + DDP-style bucketed gradient all-reduce (NCCL when world > 1) + Adam step.
@@ -539,18 +540,18 @@ def main():
         except Exception as e:
             line["extra"] = {"unavailable": repr(e)[:200]}
     if world == 1 and reference_available() and not args.no_reference_eager:
-        # the denominator of north_star's >= 10x target: the unmodified reference, PyTorch eager, same B200
+        # the denominator of north_star's >= 10x target: the unmodified reference, PyTorch eager, same GPU
         try:
             out = subprocess.run([sys.executable, os.path.abspath(__file__), "--impl", "reference-eager",
                                   "--steps", "50", "--batch", str(B)], capture_output=True, text=True, timeout=600)
             ref = json.loads([ln for ln in out.stdout.splitlines() if ln.startswith("{")][-1])
-            line["reference_eager_b200"] = {
+            line["reference_eager"] = {
                 "value": ref["value"], "unit": "samples/s", "ms_per_step": ref["ms_per_step_median"],
-                "loss": ref["loss"], "how": "baseline/_ref/normflows (unmodified) model.forward_kld under no_grad on "
+                "loss": ref["loss"], "how": "oracle/_ref/normflows (unmodified) model.forward_kld under no_grad on "
                 "cuda:0, same model/seed/batch, 10 warm-up + 50 timed passes, CUDA events, median",
                 "speedup_device": value / ref["value"], "speedup_e2e": e2e_value / ref["value"], "target": 10.0}
         except Exception as e:  # reported, never fatal
-            line["reference_eager_b200"] = {"unavailable": repr(e)[:200]}
+            line["reference_eager"] = {"unavailable": repr(e)[:200]}
     if not args.no_cpu_baseline and world == 1:  # reported baseline: rank 0 at N = 1 only
         line["cpu_baseline"], _ = cpu_baseline()
     print(json.dumps(line), flush=True)

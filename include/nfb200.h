@@ -1,4 +1,4 @@
-/* nfb200.h -- C ABI of libnfb200.so: the B200-native coupling-stack hot path of normflows.
+/* nfb200.h -- C ABI of libnfb200.so: the coupling-stack hot path of normflows as native H100 (sm_90a) kernels.
  *
  * The reference (normflows 1.7.3, pure Python/PyTorch) has no FFI; its seam for this path is the
  * `Flow` protocol `forward(z)/inverse(z) -> (z', log_det[B])` (normflows/flows/base.py:13-24) driven
@@ -297,7 +297,7 @@ int nfb_flow_repack(nfb_flow_t* f, void* stream);
 int nfb_flow_num_layers(const nfb_flow_t* f);
 /* how many CUDA kernels the last pass launched (bench.py reports it as gpu_launches) */
 int64_t nfb_flow_last_launch_count(const nfb_flow_t* f);
-/* 1 if layer `index` runs on the fused tcgen05 kernel in the density direction */
+/* 1 if layer `index` runs on the fused tensor-core kernel in the density direction */
 int nfb_flow_layer_is_fused(const nfb_flow_t* f, int32_t index);
 
 /* flows/base.py:13-24: apply ONE layer.  log_det_dev [rows]: overwritten (accumulate=0) or += . */

@@ -6,7 +6,7 @@
 // last-to-first calling `.inverse`) and the sampling pass (core.py:52-54).
 //
 // Execution plan ("groups"):
-//   FUSED  : [LULinearPermute +] neural-spline block on the tcgen05 kernel (nfb_fused_rqs.cu)
+//   FUSED  : [LULinearPermute +] neural-spline block on the wgmma kernel (nfb_fused_rqs.cu)
 //   AFFINE : a maximal run of low-dimensional affine-family layers in one kernel (nfb_affine.cu)
 //   SINGLE : any other layer through the generic fp32 kernels (nfb_kernels.cu)
 #include <algorithm>
@@ -24,17 +24,16 @@
 static thread_local std::string g_err;
 static constexpr float kLog2eHost = 1.4426950408889634f;
 
-// tcgen05.mma adds each K=16 step into the fp32 TMEM accumulator with truncation (round toward zero), so a
-// chain of n MMA steps comes out short by a small one-sided amount: per step half an ulp of the running sum,
-// E[ulp(s)/|s|] = 2^-23 / (2 ln 2) = 8.6e-8 for a log-uniform mantissa, times 2/3 because the partial sums of
-// a random-sign dot product grow like sqrt(k/n):  0.5 * 8.6e-8 * 2/3 = 2.9e-8 per step.  Measured on B200
-// against the fp64 oracle (tools/gpu_debug.py bias, profiles/r01c_acc_bias.log): uncompensated, log_prob of
-// a 4-layer d=64 stack is high by 1.3e-3 (autoregressive) / 0.8e-3 (coupling) with an rms of 1.7e-3 / 0.8e-3
-// -- the bias IS the error budget of the fused path -- and per-GEMM gains fitted from four gain settings put
-// the loss at 2.9e-8 per step for the 24-step LU map, the 12-step first layer and the 48-step hidden layers
-// alike.  The packer therefore scales each GEMM's weights by 1 + kAccStepGain * steps; the bias test in
-// tests/test_gpu_parity.py pins the residual.  (Counting, per row of a masked net, only the steps in which
-// the row has a non-zero weight was tried and is no better: mean +1.0e-4 / rms 8.6e-4 against +2e-5 / 6.9e-4.)  NFB_ACC_COMP_STEP overrides the constant (calibration runs).
+// The tensor core adds each K=16 step into the fp32 accumulator with truncation (round toward zero), so a chain
+// of n MMA steps comes out short by a small one-sided amount: per step half an ulp of the running sum,
+// E[ulp(s)/|s|] = 2^-23 / (2 ln 2) = 8.6e-8 for a log-uniform mantissa, times 2/3 because the partial sums of a
+// random-sign dot product grow like sqrt(k/n): ~2.9e-8 per step.  The packer therefore scales each GEMM's weights by
+// 1 + kAccStepGain * steps.  Measured on H100 (wgmma) against the fp64 oracle (tools/gpu_debug.py bias: 4-layer d=64
+// stacks, 3000 rows, |log_prob| ~ 270): mean signed log_prob error +8.0e-4 (autoregressive) / +4.0e-4 (coupling)
+// uncompensated, +3.5e-4 / +1.2e-4 at 1.5e-8 per step, -8.6e-5 / -1.4e-4 at 2.9e-8, and +1.2e-4 / -7e-6 at 2.4e-8 =
+// kAccStepGain, between the two stacks' zero crossings.  The plain-fp32 kernels' own bias on the same rows is
+// -4.8e-5 / -2.9e-5; test_trained_weights_parity pins the residual.  NFB_ACC_COMP_STEP overrides the constant
+// (calibration runs).
 static float acc_gain(int mma_steps) {
     static const float per_step = [] {
         const char* e = getenv("NFB_ACC_COMP_STEP");
@@ -143,8 +142,7 @@ struct FusedPack {
     std::vector<FusedStep> steps_host;
     DevBuf wstream, steps, uncond;
     std::vector<float> bias_h, bias_f;
-    std::vector<int> in_idx, tr_idx, id_idx, chunk_order;
-    unsigned char blk_sig[7 * 4] = {};     // see FusedLayer::blk_sig
+    std::vector<int> in_idx, tr_idx, id_idx;
     struct Rec { int row0, nrows, kc; size_t off_hi, off_lo; };
     struct Gemm { DevBuf src_row, src_col, row_scale, recs_dev; const float* W; const float* M; int src_cols, n_pad, k_pad;
                   int max_rows = 0; std::vector<Rec> recs; };
@@ -158,7 +156,7 @@ struct FusedPack {
     bool images_dirty = true;              // per-layer device images (layer_dev, layer_fwd_dev, pair_dev) need a refresh
     int ar_passes_fwd = 0;
     bool fold_ok = false;                  // decided per repack (scale plan permitting)
-    DevBuf pair_steps_fold_dev, in_idx_dev, fold_lu, fold_G, fold_delta, fold_recs;
+    DevBuf in_idx_dev, fold_lu, fold_G, fold_delta, fold_recs;
     std::vector<float> fold_delta_host;    // W0 b_lu in sorted hidden order
     int pw_fold = 0;
     FusedLayer host_layer{}, host_pair{};  // packed descriptors (host copies)
@@ -209,7 +207,7 @@ struct nfb_flow {
     int D = 0;
     bool finalized = false;
     bool use_tc = true;
-    int sm_count = 148;
+    int sm_count = 132;
     std::vector<std::unique_ptr<Layer>> layers;
     std::vector<Group> groups;
     const float* base_loc = nullptr;
@@ -226,7 +224,7 @@ struct nfb_flow {
     std::vector<std::pair<int, int>> fwd_units;
     int fwd_trailing_lu = -1, fwd_n = 0;
     DevBuf fwd_layers;
-    DevBuf zA, zB, logq, hA, hB, hT, params, E, scratch_sum, loss, err, ar_tmp, pair_tmp, host_x, zfinal, prof, norms;
+    DevBuf zA, zB, logq, hA, hB, hT, params, E, scratch_sum, loss, err, ar_tmp, pair_tmp, host_x, zfinal, norms;
     long long launches = 0;
     // host-buffer entry points: chunked H2D on a copy stream, gated tile by tile inside the whole-stack kernel
     cudaStream_t copy_stream = nullptr;
@@ -269,7 +267,7 @@ int copy_net(const nfb_resnet_desc_t& d, NetDesc& n) {
 int pack_net_generic(const NetDesc& n, NetPack& p, cudaStream_t st) {
     p.wb.clear();
     size_t slot = 0;  // the masked-weight buffers are kept across repacks (a cudaFree + cudaMalloc pair per matrix and
-                      // optimizer step was most of the packer's host time: ADVICE r1, profiles/r02b_repack.md)
+                      // optimizer step was most of the packer's host time)
     auto eff = [&](const float* w, const float* m, size_t cnt, const float** out) -> int {
         if (!m) { *out = w; return NFB_OK; }
         if (slot == p.owned.size()) p.owned.emplace_back();
@@ -314,11 +312,6 @@ int run_net_generic(nfb_flow* f, const NetDesc& n, const NetPack& p, const float
 // ------------------------------------------------------------------------------------------
 // fused pack
 // ------------------------------------------------------------------------------------------
-uint16_t make_ctl(int col, int first, int wait, int signal) {
-    return (uint16_t)((col & 511) | ((first & 1) << 9) | ((wait & 7) << 10) | ((signal & 7) << 13));
-}
-int chunk_col_host(int i) { return i * 256; }
-
 int build_fused(nfb_flow* f, Layer& L, cudaStream_t st) {
     FusedPack& F = L.fused;
     F.ok = false; F.pair_ok = false;
@@ -329,31 +322,16 @@ int build_fused(nfb_flow* f, Layer& L, cudaStream_t st) {
     if (L.K != 8 || L.D > 64 || n.H % 64 != 0 || n.H > 256 || n.in > 64 || T > 64 || T < 1) return NFB_OK;
     if (n.out != T * 23) return NFB_OK;
     const int H = n.H, n_hidden = 1 + 2 * n.nb;
-    // final layer: F features (x24 columns) per MMA chunk.  One record = one [N x 64] bf16 tile <= 32 KB,
-    // so N = 24 F <= 240; large N keeps the per-record issue bubble (~330 cycles) hidden behind
-    // 120-cycle MMAs (measured: tools/ring_bench.cu).
-    int fpc = 2;
-    {   // even features-per-chunk <= 10 that wastes the fewest padded feature slots (ties: larger N)
-        int best = 1 << 30;
-        for (int c = 2; c <= 10; c += 2) {
-            const int slots = (T + c - 1) / c * c;
-            if (slots <= best && !(slots == best && c < fpc)) { best = slots; fpc = c; }
-            if (c >= T + (T & 1)) break;
-        }
-        // T = 64: 10 -> 70 slots beats 8 -> 64 because 120-cycle MMAs hide the per-record bubble
-        if (T > 40 && fpc < 10) fpc = 10;
-        if (const char* e = getenv("NFB_FPC")) {   // (measurement override: features per final-layer chunk, even, 2..10)
-            const int v = atoi(e);
-            if (v >= 2 && v <= 10 && v % 2 == 0) fpc = v;
-        }
-    }
-    const int n_chunks = (T + fpc - 1) / fpc;
+    // final layer: fpc features (x24 columns: 23 parameters + 1 pad) per record; a record of N = 48 rows keeps the
+    // accumulator of the final layer at 24 registers and its staging tile small (nfb_fused_rqs.cu)
+    const int fpc = kFusedFeaturesPerChunk;
+    const int n_chunks = ((T + fpc - 1) / fpc + 1) & ~1;   // even: a record carries one chunk per consumer warpgroup
     const int kcs_h = H / 64;
     const int crow = fpc * 24;  // rows (MMA N) per final-layer chunk
-    if (n_hidden > 7 || (n_chunks + 1) * fpc > 82 || n_chunks > 16) return NFB_OK;  // tables inside FusedLayer
+    if (n_hidden > 7) return NFB_OK;  // tables inside FusedLayer
 
     // ---- MADE masks: sort hidden units by degree so that every masked matrix is block-triangular, and
-    //      find the all-zero [rows x 64-column] blocks to drop (nets/made.py:57-76 degree rules) ----
+    //      find the all-zero [64 x 64] blocks to drop (nets/made.py:57-76 degree rules) ----
     const bool masked = n.m0 != nullptr;
     std::vector<int> perm(H);
     for (int i = 0; i < H; ++i) perm[i] = i;
@@ -367,21 +345,13 @@ int build_fused(nfb_flow* f, Layer& L, cudaStream_t st) {
         NFB_TRY(download(n.mf, (size_t)n.out * H, m_fin));
     }
     F.hperm = perm;
-    // first row (multiple of 16, in sorted order) of a hidden GEMM that has a non-zero in K-chunk kc
-    auto hidden_row0 = [&](int kc) -> int {
-        if (!masked || m_hid.empty()) return 0;
-        for (int i = 0; i < H; ++i)
+    // does output slice j (rows [64 j, 64 j + 64) in sorted order) of a hidden GEMM have a non-zero in K-chunk kc?
+    auto hidden_needs = [&](int j, int kc) -> bool {
+        if (!masked || m_hid.empty()) return true;
+        for (int i = 64 * j; i < 64 * j + 64; ++i)
             for (int k = kc * 64; k < kc * 64 + 64; ++k)
-                if (m_hid[(size_t)perm[i] * H + perm[k]] != 0.f) return i & ~15;
-        return H;  // no row uses this K-chunk at all
-    };
-    // the same per K=16 slab s of K-chunk kc (-1: no row reaches the slab)
-    auto hidden_row0_slab = [&](int kc, int s) -> int {
-        if (!masked || m_hid.empty()) return 0;
-        for (int i = 0; i < H; ++i)
-            for (int k = kc * 64 + 16 * s; k < kc * 64 + 16 * s + 16; ++k)
-                if (m_hid[(size_t)perm[i] * H + perm[k]] != 0.f) return i & ~15;
-        return -1;
+                if (m_hid[(size_t)perm[i] * H + perm[k]] != 0.f) return true;
+        return false;
     };
     // does chunk c of the final layer have a non-zero in K-chunk kc?
     auto final_needs = [&](int c, int kc) -> bool {
@@ -393,31 +363,6 @@ int build_fused(nfb_flow* f, Layer& L, cudaStream_t st) {
                 if (m_fin[(size_t)(t * 23 + q) * H + perm[k]] != 0.f) return true;
         }
         return false;
-    };
-
-    // first row (multiple of 16) of final-layer chunk c that has a non-zero in K-chunk kc: the features of a chunk are in
-    // ascending order and a feature sees the hidden units of smaller degree only, so the rows that need a LATE K-chunk are
-    // the chunk's last ones -- the MMA runs on rows [r0, nrows) only, like the shrinking N of the hidden layers
-    auto final_row0_slab = [&](int c, int kc, int s, int nrows) -> int {   // (relative to the chunk; -1: no row)
-        if (!masked) return 0;
-        for (int i = 0; i < nrows; ++i) {
-            const int t = fpc * c + i / 24, q = i % 24;
-            if (t >= T || q >= 23) continue;
-            for (int k = kc * 64 + 16 * s; k < kc * 64 + 16 * s + 16; ++k)
-                if (m_fin[(size_t)(t * 23 + q) * H + perm[k]] != 0.f) return i & ~15;
-        }
-        return -1;
-    };
-    auto final_row0 = [&](int c, int kc, int nrows) -> int {
-        static const bool no_shrink = getenv("NFB_NO_FINAL_SHRINK") != nullptr;   // (A/B measurements)
-        if (!masked || kc == 0 || no_shrink) return 0;
-        for (int i = 0; i < nrows; ++i) {
-            const int t = fpc * c + i / 24, q = i % 24;
-            if (t >= T || q >= 23) continue;
-            for (int k = kc * 64; k < kc * 64 + 64; ++k)
-                if (m_fin[(size_t)(t * 23 + q) * H + perm[k]] != 0.f) return i & ~15;
-        }
-        return nrows - 16;   // (a K-chunk this chunk reads only for the ordering rule below: smallest legal record)
     };
 
     // ---- GEMM source tables (effective matrices are built in sorted hidden order) ----
@@ -450,133 +395,58 @@ int build_fused(nfb_flow* f, Layer& L, cudaStream_t st) {
         NFB_TRY(add_gemm(n.wf, n.mf, H, n_chunks * crow, H, fr, perm, fs));
     }
 
-    // ---- step table + record list (same order) ----
-    memset(F.blk_sig, 3, sizeof(F.blk_sig));
+    // ---- step table + record list (same order).  A record carries the same K-chunk of two output slices, one per
+    //      consumer warpgroup of the kernel: hidden GEMMs split their 64-column slices in two halves ([0, half) and
+    //      [half, ns)), the final layer deals its chunks alternately.  K-chunks ascend (the accumulation order is part
+    //      of the validated numerics); K-chunk 0 is always kept, so that every slice has a first record that initialises
+    //      its accumulator; a K-chunk only one of the two slices reaches is skipped by the other warpgroup. ----
     std::vector<FusedStep> steps;
     size_t off = 0;
-    // slab_r0[s]: first row (absolute, multiple of 16, >= row0; -1 = no row) the K=16 slab s of this K-chunk reaches
-    auto add = [&](FusedPack::Gemm& g, int row0, int nrows, int kc, int col, int first, int wait_hi,
-                   int signal_lo, const int* slab_r0 = nullptr) {
-        FusedStep s{};
-        s.n8 = (uint8_t)(nrows / 8);
-        static const bool no_slab = getenv("NFB_NO_SLAB_SHRINK") != nullptr;   // (A/B measurements)
-        for (int j = 0; j < 4; ++j) {
-            int r = (slab_r0 && !no_slab) ? slab_r0[j] : row0;
-            if (r >= 0 && r < row0) r = row0;
-            if (first && j == 0) r = row0;                       // the overwriting MMA initialises every column
-            s.dr[j] = r < 0 ? 0xFF : (uint8_t)((r - row0) / 8);
-            if (r >= 0 && nrows - (r - row0) < 16) s.dr[j] = (uint8_t)((nrows - 16) / 8);
+    // rows [row_a, row_a + nrows) for warpgroup 0 and (row_b >= 0) [row_b, row_b + nrows) for warpgroup 1
+    auto add_pair = [&](FusedPack::Gemm& g, int row_a, int row_b, int nrows, const std::vector<bool>& need_a,
+                        const std::vector<bool>& need_b, bool onto) {
+        const int tot = row_b >= 0 ? 2 * nrows : nrows;
+        std::vector<int> kcs;
+        for (size_t kc = 0; kc < need_a.size(); ++kc)
+            if (kc == 0 || need_a[kc] || (row_b >= 0 && need_b[kc])) kcs.push_back((int)kc);
+        for (size_t i = 0; i < kcs.size(); ++i) {
+            const int kc = kcs[i];
+            FusedStep st{};
+            st.bytes16 = (uint16_t)(tot * 16);
+            st.n8 = (uint8_t)(nrows / 8);
+            st.kc = (uint8_t)kc;
+            st.flags = (uint8_t)(((i == 0 && !onto) ? kStepFirst : 0) | (i + 1 == kcs.size() ? kStepLast : 0) |
+                                 ((kc > 0 && !need_a[kc]) ? kStepSkip0 : 0) |
+                                 ((row_b < 0 || (kc > 0 && !need_b[kc])) ? kStepSkip1 : 0));
+            steps.push_back(st);
+            g.recs.push_back(FusedPack::Rec{row_a, nrows, kc, off, off + (size_t)tot * 128});
+            if (row_b >= 0)
+                g.recs.push_back(FusedPack::Rec{row_b, nrows, kc, off + (size_t)nrows * 128, off + (size_t)(tot + nrows) * 128});
+            off += (size_t)tot * 256;
         }
-        if (s.dr[0] == 0xFF && s.dr[1] == 0xFF && s.dr[2] == 0xFF && s.dr[3] == 0xFF) s.dr[0] = (uint8_t)((nrows - 16) / 8);
-        static const bool no_merge = getenv("NFB_NO_MERGE") != nullptr;          // (A/B measurements)
-        if (nrows * 256 <= 32768 && !no_merge) {
-            // both tiles fit one ring slot: ONE record, 12 MMAs (the issuer's per-record sequence costs ~700 cycles
-            // whatever the record holds; the shrinking N of the block-triangular layers made it the bound)
-            s.bytes16 = (uint16_t)(nrows * 16);
-            s.a0 = (uint8_t)kc; s.a1 = (uint8_t)(4 + kc); s.a2 = (uint8_t)kc;
-            s.ctl = make_ctl(col, first, wait_hi, signal_lo);
-            steps.push_back(s);  // W_hi x {A_hi, A_lo}, W_lo x {A_hi}
-        } else {
-            s.bytes16 = (uint16_t)(nrows * 8);
-            s.a0 = (uint8_t)kc; s.a1 = (uint8_t)(4 + kc); s.a2 = 0xFF;
-            s.ctl = make_ctl(col, first, wait_hi, 0);
-            steps.push_back(s);  // W_hi x {A_hi, A_lo}
-            s.a1 = 0xFF;
-            s.ctl = make_ctl(col, 0, 0, signal_lo);
-            steps.push_back(s);  // W_lo x {A_hi}
-        }
-        FusedPack::Rec r{row0, nrows, kc, off, off + (size_t)nrows * 128};
-        off += (size_t)nrows * 256;
-        g.recs.push_back(r);
     };
+    const int half = (kcs_h + 1) / 2;
     for (int ph = 0; ph < n_hidden; ++ph) {
-        const int region = (ph & 1) ? 256 : 0;
         const bool accum_onto = (ph > 0 && (ph & 1) == 0);  // second GEMM of a residual block: h += ...
         const int kcs = (ph == 0) ? 1 : kcs_h;
-        FusedPack::Gemm& g = F.gemms[ph];
-        int last = 0;
-        std::vector<int> r0s(kcs, 0);
-        for (int kc = 0; kc < kcs; ++kc) {
-            r0s[kc] = (ph == 0 || kc == 0) ? 0 : hidden_row0(kc);
-            if (r0s[kc] < H) last = kc;
-        }
-        // Output chunk j (rows [64 j, 64 j + 64) of this GEMM = A K-chunk j of the next one) is final once the last
-        // K-chunk whose records reach those rows has been accumulated: fin(j).  Unmasked nets: the last K-chunk.
-        const int ochunks = H / 64;
-        std::vector<int> fin(ochunks, last);
-        for (int j = 0; j < ochunks; ++j) {
-            int fj = 0;
-            for (int kc = 0; kc <= last; ++kc) if (r0s[kc] < 64 * (j + 1)) fj = kc;
-            fin[j] = fj;
-            static const bool no_early = getenv("NFB_NO_EARLY_EPI") != nullptr;  // (A/B measurements)
-            F.blk_sig[ph * 4 + j] = (unsigned char)((fj >= last || fj > 2 || no_early) ? 3 : fj);
-        }
-        for (int kc = 0; kc < kcs; ++kc) {
-            const int r0 = r0s[kc];
-            if (r0 >= H) continue;
-            int sig = kc == last ? 1 : 0;
-            if (kc < last && kc <= 2)
-                for (int j = 0; j < ochunks; ++j) if (F.blk_sig[ph * 4 + j] == kc) sig = 4 + kc;
-            // every hi record is the first reader of A K-chunk kc in this phase: wait a_ready[kc]
-            int sr[4] = {r0, r0, r0, r0};
-            if (ph > 0) for (int s4 = 0; s4 < 4; ++s4) sr[s4] = hidden_row0_slab(kc, s4);
-            add(g, r0, H - r0, kc, region + r0, (kc == 0 && !accum_onto) ? 1 : 0, 1, sig, sr);
+        auto need = [&](int j) {
+            std::vector<bool> v(kcs);
+            for (int kc = 0; kc < kcs; ++kc) v[kc] = ph == 0 || hidden_needs(j, kc);
+            return v;
+        };
+        for (int q = 0; q < half; ++q) {
+            const int jb = q + half < kcs_h ? q + half : -1;
+            add_pair(F.gemms[ph], 64 * q, jb >= 0 ? 64 * jb : -1, 64, need(q), jb >= 0 ? need(jb) : need(q), accum_onto);
         }
     }
-    {
-        FusedPack::Gemm& g = F.gemms[n_hidden];
-        bool a_waited[4] = {false, false, false, false};
-        // Which K-chunks does each chunk need (MADE masks)?  Processing slot 0 writes TMEM buffer 1 (columns 256..),
-        // slot 1 is the first writer of buffer 0 = the residual stream's columns, which the LAST hidden epilogue is
-        // still reading: before its first MMA the issuer must have passed a_ready[last K-chunk] (the epilogue converts
-        // the chunks in order, so that arrival means it has read everything).  (A short first chunk with nothing
-        // enforcing this is a real race: found on hardware in round 1.)  Round 2b: slot 0 takes the LIGHTEST chunk
-        // (features 0..F-1 of a MADE net need K-chunk 0 only) so that the spline evaluators start ~2 k cycles after the
-        // last hidden GEMM instead of waiting ~8 k for a dense chunk; the first record of slot 1 carries wait code 5 =
-        // a_ready[LAST K-chunk of the phase] + chunk buffer 0 free (its own K-chunk 0 was announced to slot 0 already).
-        // (K-chunks stay in ascending order: the accumulation order is part of the validated numerics.)
-        std::vector<std::vector<int>> need_of(n_chunks);
-        for (int c = 0; c < n_chunks; ++c)
-            for (int kc = 0; kc < kcs_h; ++kc)
-                if (kc == 0 || c == n_chunks - 1 || final_needs(c, kc)) need_of[c].push_back(kc);
-        // light, heavy, light, heavy, ...: chunk 0, the last chunk (every K-chunk), then alternate low / high chunks
-        std::vector<int> order;
-        for (int lo = 0, hi = n_chunks - 1; lo <= hi;) {
-            order.push_back(lo++);
-            if (lo <= hi) order.push_back(hi--);
-        }
-        F.chunk_order = order;
-        for (int ci = 0; ci < n_chunks; ++ci) {
-            const int c = order[ci];
-            const int b = (ci + 1) & 1;  // two TMEM chunk buffers (columns 0.. and 256..); slot 0 uses the second
-            const std::vector<int>& need = need_of[c];
-            // live rows of the chunk: the last one usually holds fewer than F features -- no MMA work for the padding
-            const int live = std::min(fpc, T - fpc * c);
-            const int nrows = std::min(crow, (live * 24 + 15) / 16 * 16);
-            for (size_t j = 0; j < need.size(); ++j) {
-                const int kc = need[j];
-                int wait = 0;
-                if (j == 0) {
-                    if (!a_waited[kc] && ci > 0) return NFB_OK;       // (slot 0 always reads K-chunk 0: cannot happen)
-                    if (ci == 0) wait = 6;                            // a_ready[kc] + chunk buffer 1 free
-                    else if (ci == 1 && !a_waited[kcs_h - 1]) {       // a_ready[last K-chunk] + chunk buffer 0 free
-                        wait = 5;
-                        a_waited[kcs_h - 1] = true;
-                    } else wait = 2 + b;                              // chunk buffer free
-                } else if (!a_waited[kc]) wait = 1;                   // first reader of this A K-chunk
-                a_waited[kc] = true;
-                const int r0 = j == 0 ? 0 : final_row0(c, kc, nrows);   // (the first record initialises every column)
-                int sr[4];
-                for (int s4 = 0; s4 < 4; ++s4) {
-                    const int rs = final_row0_slab(c, kc, s4, nrows);
-                    sr[s4] = rs < 0 ? -1 : c * crow + rs;
-                }
-                add(g, c * crow + r0, nrows - r0, kc, chunk_col_host(b) + r0, j == 0 ? 1 : 0, wait,
-                    j + 1 == need.size() ? 2 + b : 0, sr);
-            }
-        }
+    for (int c = 0; c < n_chunks; c += 2) {
+        auto need = [&](int cc) {
+            std::vector<bool> v(kcs_h);
+            for (int kc = 0; kc < kcs_h; ++kc) v[kc] = final_needs(cc, kc);
+            return v;
+        };
+        add_pair(F.gemms[n_hidden], c * crow, (c + 1) * crow, crow, need(c), need(c + 1), false);
     }
-    if (steps.size() + 3 > 256) return NFB_OK;  // step table would not fit in shared memory
     F.steps_host = steps;
     F.n_steps = (int)steps.size();
     F.D = L.D; F.H = H; F.n_hidden = n_hidden; F.T = T; F.F = fpc; F.n_chunks = n_chunks; F.tail = L.tail;
@@ -616,7 +486,7 @@ int build_fused(nfb_flow* f, Layer& L, cudaStream_t st) {
 //   weights of GEMM g    = effective weight * 2^pw[g]
 //   true GEMM output     = accumulator * 2^-(pa[g]+pw[g]) / u_row  (applied by the epilogue, exact)
 // pa[g] comes from a GUARANTEED bound on the activation (infinity-norm chain below: no input can overflow fp16),
-// pw[g] from max |w|.  GEMMs 0, 2, 4, ... accumulate onto the residual stream in TMEM and therefore share
+// pw[g] from max |w|.  GEMMs 0, 2, 4, ... accumulate onto the residual stream (in registers) and therefore share
 // pa + pw.  For inputs that are post-ReLU (>= 0) the bound uses max(sum w+, sum w-) per row instead of sum |w|.
 // Values far below the bound lose nothing that matters: fp16 subnormals keep the ABSOLUTE error at 2^-25 of the
 // scaled range.  Validated offline against the fp64 oracle by tools/numerics_emul2.py (worst row of the 32-layer
@@ -774,14 +644,7 @@ int repack_fused(nfb_flow* f, Layer& L, cudaStream_t st, Layer* Ufold = nullptr)
     plan_scales(F.n_hidden, nm, bmax, F.b_in0, F.pa, F.pw, Ufold ? fold_nm.data() : nullptr, fold_bmax, &F.pw_fold);
     if (getenv("NFB_DEBUG_PACK"))
         fprintf(stderr, "[nfb pack] fold: U=%p pair_ok=%d pw_fold=%d pa0=%d pw0=%d\n", (void*)Ufold, (int)F.pair_ok, F.pw_fold, F.pa[0], F.pw[0]);
-    if (Ufold && F.pw_fold > -100) {
-        NFB_TRY(F.fold_recs.reserve((size_t)H * 256));
-        NFB_TRY(launch_pack_record(F.fold_G.as<float>(), 64, 0, H, 0, pow2f(F.pw_fold), F.fold_recs.as<uint8_t>(),
-                                   F.fold_recs.as<uint8_t>() + (size_t)H * 128, st));
-        F.fold_ok = true;
-    }
-    for (int gi = 0; gi < ng; ++gi) {
-        auto& g = F.gemms[gi];
+    for (auto& g : F.gemms) {
         if (g.recs_dev.p == nullptr && !g.recs.empty()) {   // the record table of a GEMM is static: uploaded once
             std::vector<PackRec> tab;
             for (auto& r : g.recs) {
@@ -790,11 +653,21 @@ int repack_fused(nfb_flow* f, Layer& L, cudaStream_t st, Layer* Ufold = nullptr)
             }
             NFB_TRY(g.recs_dev.upload(tab));
         }
+    }
+    if (Ufold && F.pw_fold > -100) {   // the folded matrix takes the place of GEMM 0: same records (build_fused)
+        auto& g0 = F.gemms[0];
+        NFB_TRY(F.fold_recs.reserve((size_t)H * 256));
+        NFB_TRY(launch_pack_records(F.fold_G.as<float>(), 64, g0.recs_dev.as<PackRec>(), (int)g0.recs.size(), g0.max_rows,
+                                    pow2f(F.pw_fold), F.fold_recs.as<uint8_t>(), st));
+        F.fold_ok = true;
+    }
+    for (int gi = 0; gi < ng; ++gi) {
+        auto& g = F.gemms[gi];
         NFB_TRY(launch_pack_records(f->E.as<float>() + eoff[gi], g.k_pad, g.recs_dev.as<PackRec>(), (int)g.recs.size(), g.max_rows,
                                     pow2f(F.pw[gi]), F.wstream.as<uint8_t>(), st));
     }
     const int crow = F.F * 24;
-    std::vector<float> bfin, bf((size_t)(F.n_chunks + 1) * crow, 0.f);  // +1 chunk: the bias prefetch runs one chunk ahead
+    std::vector<float> bfin, bf((size_t)F.n_chunks * crow, 0.f);
     R.get(o_bf, (size_t)n.out, bfin);
     for (int i = 0; i < F.n_chunks * crow; ++i) {
         const int t = F.F * (i / crow) + (i % crow) / 24, q = (i % crow) % 24;
@@ -823,8 +696,6 @@ int repack_fused(nfb_flow* f, Layer& L, cudaStream_t st, Layer* Ufold = nullptr)
         Lh.tr_idx[k] = (unsigned char)(k < (int)F.tr_idx.size() ? F.tr_idx[k] : 0);
         Lh.id_idx[k] = (unsigned char)(k < (int)F.id_idx.size() ? F.id_idx[k] : 0);
     }
-    for (int k = 0; k < 16; ++k) Lh.chunk_order[k] = (unsigned char)(k < (int)F.chunk_order.size() ? F.chunk_order[k] : 0);
-    memcpy(Lh.blk_sig, F.blk_sig, sizeof(Lh.blk_sig));
     Lh.a_sc[0] = 1.f; Lh.a_inv[0] = 1.f;
     for (int gi = 0; gi < ng; ++gi) {
         Lh.a_sc[1 + gi] = pow2f(F.pa[gi]);
@@ -902,29 +773,22 @@ int repack_lu(nfb_flow* f, Layer& L, cudaStream_t st, bool packed_already = fals
     return NFB_OK;
 }
 
+// the LU map in front of a block: one 64-row record W_hi | W_lo, all four products (the map transforms z itself, ~2^-22)
+FusedStep lu_step() {
+    FusedStep s{};
+    s.bytes16 = 64 * 16; s.n8 = 8; s.kc = 0; s.flags = kStepFirst | kStepLast | kStepQuad | kStepSkip1;
+    return s;
+}
+
 int build_pair(nfb_flow* f, Layer& R, Layer& U, cudaStream_t st) {
     FusedPack& F = R.fused;
     F.pair_ok = false;
     if (!F.ok || U.D != R.D || U.D > 64) return NFB_OK;
-    if (F.n_steps + 2 > 256) return NFB_OK;
-    std::vector<FusedStep> steps;
-    auto mk = [&](int a0, int a1, int a2, int first, int wait, int signal) {
-        FusedStep s{};
-        s.bytes16 = 64 * 16; s.n8 = 8; s.a0 = (uint8_t)a0; s.a1 = (uint8_t)a1; s.a2 = (uint8_t)a2;
-        s.ctl = make_ctl(256, first, wait, signal);
-        steps.push_back(s);
-    };
-    mk(0, 4, 0x80, 1, 1, 7);     // one record: W_hi x {A_hi, A_lo}, W_lo x {A_hi, A_lo}  (4 terms: the map transforms z
-                                 // itself, ~2^-22); signals lu_full
+    std::vector<FusedStep> steps(1, lu_step());
     steps.insert(steps.end(), F.steps_host.begin(), F.steps_host.end());
     F.pair_steps = (int)steps.size();
     NFB_TRY(F.pair_steps_dev.upload(steps));
-    {   // folded variant: GEMM 0 of the block reads the LU stage's A operand (already waited for by the LU records)
-        std::vector<FusedStep> sf = steps;
-        sf[1].ctl = (uint16_t)(sf[1].ctl & ~(7u << 10));
-        NFB_TRY(F.pair_steps_fold_dev.upload(sf));
-        NFB_TRY(F.in_idx_dev.upload(F.in_idx));
-    }
+    NFB_TRY(F.in_idx_dev.upload(F.in_idx));   // (LU fold, repack_fused)
     NFB_TRY(F.pair_wstream.reserve(2 * 8192 + F.rqs_bytes));
     std::vector<int> sr(64), sc(64, -1);
     for (int i = 0; i < 64; ++i) sr[i] = i < U.D ? i : -1;
@@ -962,7 +826,6 @@ int repack_pair(nfb_flow* f, Layer& R, Layer& U, cudaStream_t st) {
         NFB_CUDA(cudaMemcpyAsync(F.pair_wstream.as<uint8_t>() + 2 * 8192, F.fold_recs.p, (size_t)F.H * 256,
                                  cudaMemcpyDeviceToDevice, st));   // (stream-ordered after the copy of the block's records)
         Lp.fold_lu = 1;
-        Lp.steps = F.pair_steps_fold_dev.as<FusedStep>();
         for (int ph = 0; ph < F.n_hidden; ph += 2)   // b0 (+ W0 b_lu) is part of every pre-summed residual bias
             for (int j = 0; j < F.H; ++j) Lp.bias_h[ph * 256 + j] += F.fold_delta_host[j];
     }
@@ -981,15 +844,8 @@ int build_fwd_unit(nfb_flow* f, Layer& R, Layer* U) {
     F.fwd_ok = false;
     if (!F.ok || (R.kind != L_COUPLED_RQS && R.kind != L_AR_RQS)) return NFB_OK;
     if (!U) { F.fwd_ok = true; return NFB_OK; }  // first block of the stack: no LU in front of it
-    if (U->D != R.D || U->D > 64 || F.n_steps + 2 > 256) return NFB_OK;
-    std::vector<FusedStep> steps;
-    auto mk = [&](int a0, int a1, int a2, int first, int wait, int signal) {
-        FusedStep s{};
-        s.bytes16 = 64 * 16; s.n8 = 8; s.a0 = (uint8_t)a0; s.a1 = (uint8_t)a1; s.a2 = (uint8_t)a2;
-        s.ctl = make_ctl(256, first, wait, signal);
-        steps.push_back(s);
-    };
-    mk(0, 4, 0x80, 1, 1, 7);     // same 4-term record as the density pair (build_pair)
+    if (U->D != R.D || U->D > 64) return NFB_OK;
+    std::vector<FusedStep> steps(1, lu_step());
     steps.insert(steps.end(), F.steps_host.begin(), F.steps_host.end());
     NFB_TRY(F.fwd_steps_dev.upload(steps));
     NFB_TRY(F.fwd_wstream.reserve(2 * 8192 + F.rqs_bytes));
@@ -1039,8 +895,6 @@ int launch_fused_layer(nfb_flow* f, Layer& R, Layer* U, const float* zin, float*
     p.zin = zin; p.zout = zout; p.logq = logq; p.rows = rows; p.accumulate = accumulate;
     p.progress = nullptr;
     p.err = f->err.as<int>();
-    p.poll_all = getenv("NFB_POLL_LANE0") == nullptr;
-    p.prof = f->prof.p ? f->prof.as<long long>() : nullptr;
     NFB_TRY(launch_fused_rqs(p, f->sm_count, sample, st));
     f->launches++;
     return NFB_OK;
@@ -1050,7 +904,7 @@ int launch_fused_layer(nfb_flow* f, Layer& R, Layer* U, const float* zin, float*
 // pre-filled (accumulate semantics); zout may alias zin.
 int launch_fused_stack(nfb_flow* f, const float* zin, float* zout, float* logq, long long rows, cudaStream_t st,
                        int sample = 0, long long z_stride = 0) {
-    const long long n_tiles = (rows + 127) / 128;
+    const long long n_tiles = (rows + kFusedTileRows - 1) / kFusedTileRows;
     NFB_TRY(f->progress.reserve((size_t)(n_tiles + 1) * sizeof(int)));   // + the unit ticket counter
     NFB_CUDA(cudaMemsetAsync(f->progress.p, 0, (size_t)(n_tiles + 1) * sizeof(int), st));
     FusedParams p{};
@@ -1086,8 +940,6 @@ int launch_fused_stack(nfb_flow* f, const float* zin, float* zout, float* logq, 
         p.wave_tpg = tpg;
     }
     p.err = f->err.as<int>();
-    p.poll_all = getenv("NFB_POLL_LANE0") == nullptr;
-    p.prof = f->prof.p ? f->prof.as<long long>() : nullptr;
     NFB_TRY(launch_fused_rqs(p, f->sm_count, sample, st));
     f->launches += 2;  // memset + kernel
     return NFB_OK;
@@ -1502,7 +1354,7 @@ int nfb_flow_create(nfb_flow_t** out, int32_t features) {
     NFB_CHECK(n > 0, NFB_ERR_CUDA, "nfb_flow_create: no CUDA device (this library has no CPU path)");
     nfb_flow* f = new nfb_flow();
     f->D = features;
-    int sm = 148;
+    int sm = 132;
     if (nfb_device_info(&sm, nullptr, nullptr) == NFB_OK) f->sm_count = sm;
     int rc = f->err.reserve(16);
     if (rc) { delete f; return rc; }
@@ -1733,7 +1585,7 @@ int nfb_flow_finalize(nfb_flow_t* f, int32_t use_tensor_cores, void* stream) {
     f->use_tc = use_tensor_cores != 0;
     int major = 0;
     NFB_TRY(nfb_device_info(nullptr, &major, nullptr));
-    if (major != 10) f->use_tc = false;  // tcgen05 exists on sm_100 only; the fp32 kernels still run
+    if (major != 9) f->use_tc = false;  // wgmma exists on sm_90 only; the fp32 kernels still run
     const int n = (int)f->layers.size();
     // per-layer static prep
     for (auto& Lp : f->layers) {
@@ -1957,7 +1809,7 @@ int h2d_prepare(nfb_flow* f, int64_t rows, int* gated) {
     return NFB_OK;
 }
 int h2d_copies(nfb_flow* f, const float* x_host, float* xd, int64_t rows, int gate) {
-    const int64_t per = ((rows + kH2dChunks - 1) / kH2dChunks + 127) / 128 * 128;  // whole tiles per chunk
+    const int64_t per = ((rows + kH2dChunks - 1) / kH2dChunks + kFusedTileRows - 1) / kFusedTileRows * kFusedTileRows;  // whole tiles
     int64_t done = 0;
     for (int c = 0; c < kH2dChunks && done < rows; ++c) {
         const int64_t n = std::min(per, rows - done);
@@ -2014,14 +1866,6 @@ int nfb_flow_forward_kld_host(nfb_flow_t* f, const float* x_host, int64_t rows, 
     if (rc) return rc;
     NFB_CUDA(cudaMemcpyAsync(loss_host, f->loss.p, 4, cudaMemcpyDeviceToHost, 0));
     NFB_CUDA(cudaStreamSynchronize(0));
-    return NFB_OK;
-}
-
-/* debug-only (not part of the ABI header): phase timestamps of CTA 0's first tile */
-__attribute__((visibility("default"))) int nfb_debug_profile(nfb_flow_t* f, int enable, long long* out128) {
-    if (!f) return NFB_ERR_ARG;
-    if (enable) { NFB_TRY(f->prof.reserve(2048 * 8)); NFB_CUDA(cudaMemset(f->prof.p, 0, 2048 * 8)); return NFB_OK; }
-    if (f->prof.p && out128) NFB_CUDA(cudaMemcpy(out128, f->prof.p, 2048 * 8, cudaMemcpyDeviceToHost));
     return NFB_OK;
 }
 

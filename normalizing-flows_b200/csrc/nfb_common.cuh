@@ -1,5 +1,5 @@
-// nfb_common.cuh -- shared device helpers for the normflows-b200 kernels (sm_100a only).
-// PTX wrappers for mbarrier / bulk-copy (TMA) / tcgen05 + error plumbing for the C-ABI.
+// nfb_common.cuh -- shared device helpers for the normflows-b200 kernels (sm_90a).
+// PTX wrappers for mbarrier / bulk-copy (TMA) / wgmma + error plumbing for the C-ABI.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -47,9 +47,8 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
-// One lane of a fully-converged warp.  Issuing tcgen05.mma / cp.async.bulk under this predicate
-// (instead of `lane == 0`) lets ptxas keep the operands in uniform registers; with a plain lane test
-// it wraps every UTCHMMA in an ELECT/BRA.U.ANY waterfall loop (~17 dependent instructions per MMA).
+// One lane of a fully-converged warp.  Issuing cp.async.bulk under this predicate (instead of `lane == 0`) lets
+// ptxas keep the operands in uniform registers.
 __device__ __forceinline__ bool elect_one_sync() {
     uint32_t pred = 0;
     asm volatile(
@@ -88,17 +87,21 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
         : "memory");
     return ok != 0;
 }
-// Bounded wait: a protocol bug must never hang the GPU box.  On timeout the kernel records
-// the barrier id in *err and traps; the host sees a launch failure instead of a dead device.
+// A wait that can never end (a protocol bug) records `tag` in *err and traps: the host sees a launch failure instead
+// of a hung device.  Out of line: a trap inlined into a warp-specialised kernel keeps ptxas from giving its consumer
+// warps the registers setmaxnreg hands them.
+static __device__ __noinline__ void fail_timeout(int* err, int tag) {
+    if (err) atomicExch(err, tag);
+    __threadfence_system();
+    asm volatile("trap;");
+}
+
+// Bounded wait (~2 s): a protocol bug must never hang the device.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int* err, int tag) {
     if (mbar_try_wait(bar, parity)) return;
     long long t0 = clock64();
     while (!mbar_try_wait(bar, parity)) {
-        if (clock64() - t0 > 4000000000LL) {  // ~2 s
-            if (err) atomicExch(err, tag);
-            __threadfence_system();
-            asm volatile("trap;");
-        }
+        if (clock64() - t0 > 4000000000LL) fail_timeout(err, tag);
     }
 }
 
@@ -108,11 +111,7 @@ __device__ __forceinline__ void mbar_wait_warp(uint32_t bar, uint32_t parity, in
     if ((threadIdx.x & 31) == 0 && !mbar_try_wait(bar, parity)) {
         long long t0 = clock64();
         while (!mbar_try_wait(bar, parity)) {
-            if (clock64() - t0 > 4000000000LL) {
-                if (err) atomicExch(err, tag);
-                __threadfence_system();
-                asm volatile("trap;");
-            }
+            if (clock64() - t0 > 4000000000LL) fail_timeout(err, tag);
         }
     }
     __syncwarp();
@@ -133,165 +132,102 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
 }
 
 // ----------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// wgmma (sm_90a): one warpgroup (4 consecutive warps, the first a multiple of 4) multiplies a [64 x 16] A tile by a
+// [16 x N] B tile from shared memory into fp32 accumulators held in its registers.  Accumulator register i of lane l
+// in warp w of the group holds row 16 w + l / 4 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 (l % 4) + (i & 1).
 // ----------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem),
-                 "r"(ncols)
-                 : "memory");
+// K-major SWIZZLE_128B canonical tile (rows of 128 B = 64 16-bit elements, 8-row groups 1024 B apart) or, with
+// lbo16 / sbo16 set accordingly, the MN-major one (64-wide MN blocks LBO apart, 8-row k groups SBO apart).
+// desc: [0,14) addr >> 4 | [16,30) LBO >> 4 | [32,46) SBO >> 4 | [62,64) layout = 1 (SWIZZLE_128B)
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr, uint32_t lbo16 = 1, uint32_t sbo16 = 64) {
+    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)lbo16 << 16) | ((uint64_t)sbo16 << 32) | (1ull << 62);
 }
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// orders this thread's register / shared-memory writes before the warpgroup's next wgmma
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-                 : "memory");
+// keeps the compiler from moving accesses to an accumulator across a wgmma that is still in flight
+template <int R> __device__ __forceinline__ void wgmma_hold(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tc_fence_before() {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_wait_ld() {
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 covers bf16 inputs with fp32 accumulate.
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                          uint32_t idesc, uint32_t accumulate) {
+// D (+)= A * B^T, A [64 x 16] and B [N x 16] both K-major (TA / TB = 1: MN-major); scale_d = 0 overwrites D;
+// on = 0: no operation (a predicate, which must be the same for the whole warpgroup, instead of a branch: ptxas
+// serialises the wgmma of a warpgroup when one sits in a branch it cannot prove warp-uniform)
+__device__ __forceinline__ void wgmma_f16_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t scale_d, uint32_t on = 1) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "{\n\t.reg .pred p, q;\n\tsetp.ne.b32 p, %34, 0;\n\tsetp.ne.b32 q, %35, 0;\n\t"
+        "@q wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{"
+        "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31"
+        "}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a), "l"(b), "r"(scale_d), "r"(on));
 }
-// Same, with the A operand read from tensor memory (128 lanes x 8 columns of packed bf16 pairs per
-// K=16 step) -- no shared-memory traffic for A.
-__device__ __forceinline__ void umma_bf16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc,
-                                             uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_f16_n48(float (&d)[24], uint64_t a, uint64_t b, uint32_t scale_d, uint32_t on = 1) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "{\n\t.reg .pred p, q;\n\tsetp.ne.b32 p, %26, 0;\n\tsetp.ne.b32 q, %27, 0;\n\t"
+        "@q wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 "
+        "{"
+        "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+        "%16,%17,%18,%19,%20,%21,%22,%23"
+        "}, %24, %25, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+        : "l"(a), "l"(b), "r"(scale_d), "r"(on));
 }
-__device__ __forceinline__ void tc_wait_st() {
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
+template <int TA = 0, int TB = 0>
+__device__ __forceinline__ void wgmma_bf16_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t scale_d, uint32_t on = 1) {
+    asm volatile(
+        "{\n\t.reg .pred p, q;\n\tsetp.ne.b32 p, %34, 0;\n\tsetp.ne.b32 q, %37, 0;\n\t"
+        "@q wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{"
+        "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31"
+        "}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB), "r"(on));
 }
-#define NFB_TMEM_ST16(addr, v)                                                           \
-    asm volatile(                                                                        \
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "                                  \
-        "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"                      \
-        ::"r"(addr), "r"((v)[0]), "r"((v)[1]), "r"((v)[2]), "r"((v)[3]), "r"((v)[4]),    \
-          "r"((v)[5]), "r"((v)[6]), "r"((v)[7]), "r"((v)[8]), "r"((v)[9]), "r"((v)[10]), \
-          "r"((v)[11]), "r"((v)[12]), "r"((v)[13]), "r"((v)[14]), "r"((v)[15])           \
-        : "memory")
-// mbarrier arrives when all tcgen05.mma issued so far by this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-                 : "memory");
+template <int TA = 0, int TB = 0>
+__device__ __forceinline__ void wgmma_bf16_n128(float (&d)[64], uint64_t a, uint64_t b, uint32_t scale_d, uint32_t on = 1) {
+    asm volatile(
+        "{\n\t.reg .pred p, q;\n\tsetp.ne.b32 p, %66, 0;\n\tsetp.ne.b32 q, %69, 0;\n\t"
+        "@q wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{"
+        "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+        "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+        "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63"
+        "}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+          "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB), "r"(on));
 }
 
-// ---- CTA pairs (cluster of 2, tcgen05 cta_group::2): one M=256 MMA spans both SMs; each CTA stages HALF of B ----
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
+// warpgroup-wide register budget changes (the whole warpgroup executes them): a producer warpgroup hands registers to
+// the consumer warpgroups of the same CTA
+template <int N> __device__ __forceinline__ void setmaxnreg_dec() {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
 }
-__device__ __forceinline__ uint32_t cluster_id_x() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r));
-    return r;
+template <int N> __device__ __forceinline__ void setmaxnreg_inc() {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
 }
-__device__ __forceinline__ uint32_t cluster_nctaid_x() {  // number of clusters along x
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%nclusterid.x;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cta address of THIS CTA -> shared::cluster address of the same offset in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_rank(uint32_t smem_addr, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
-    return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish2() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma2_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrives on the barrier at this shared-memory offset in BOTH CTAs of the pair when the MMAs issued so far are done
-__device__ __forceinline__ void umma2_commit_mc(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(bar), "h"((uint16_t)3)
-                 : "memory");
-}
-
-// K-major, SWIZZLE_128B canonical tile: rows of 128 B (64 bf16), 8-row groups 1024 B apart.
-// desc: [0,14) addr>>4 | [16,30) LBO>>4 (=1, ignored for swizzled K-major) | [32,46) SBO>>4 (=64)
-//       | [46,48) version=1 (sm_100) | [61,64) layout=2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) |
-           (2ull << 61);
-}
-// fp16 operands (a_format = b_format = 0): the split-precision GEMMs of the fused spline kernel (11-bit mantissas:
-// hi + lo carries 22-23 bits of an fp32 value, against 16-17 for a bf16 pair)
-__host__ __device__ constexpr uint32_t umma_idesc_f16(uint32_t m, uint32_t n) {
-    return (1u << 4) | ((n >> 3) << 17) | ((m >> 4) << 24);
-}
-// instruction descriptor: c=f32 (bit4), a=bf16 (bit7), b=bf16 (bit10), K-major A and B,
-// N>>3 at [17,23), M>>4 at [24,29)
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(uint32_t m, uint32_t n) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((n >> 3) << 17) | ((m >> 4) << 24);
-}
-
-#define NFB_TMEM_LD8(addr, v)                                                            \
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];" \
-                 : "=r"((v)[0]), "=r"((v)[1]), "=r"((v)[2]), "=r"((v)[3]), "=r"((v)[4]),   \
-                   "=r"((v)[5]), "=r"((v)[6]), "=r"((v)[7])                                \
-                 : "r"(addr))
-#define NFB_TMEM_LD16(addr, v)                                                           \
-    asm volatile(                                                                        \
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "                                        \
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"                \
-        : "=r"((v)[0]), "=r"((v)[1]), "=r"((v)[2]), "=r"((v)[3]), "=r"((v)[4]), "=r"((v)[5]), \
-          "=r"((v)[6]), "=r"((v)[7]), "=r"((v)[8]), "=r"((v)[9]), "=r"((v)[10]), "=r"((v)[11]), \
-          "=r"((v)[12]), "=r"((v)[13]), "=r"((v)[14]), "=r"((v)[15])                     \
-        : "r"(addr))
-#define NFB_TMEM_LD32(addr, v)                                                           \
-    asm volatile(                                                                        \
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "                                        \
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"                        \
-        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"       \
-        : "=r"((v)[0]), "=r"((v)[1]), "=r"((v)[2]), "=r"((v)[3]), "=r"((v)[4]), "=r"((v)[5]), \
-          "=r"((v)[6]), "=r"((v)[7]), "=r"((v)[8]), "=r"((v)[9]), "=r"((v)[10]), "=r"((v)[11]), \
-          "=r"((v)[12]), "=r"((v)[13]), "=r"((v)[14]), "=r"((v)[15]), "=r"((v)[16]),      \
-          "=r"((v)[17]), "=r"((v)[18]), "=r"((v)[19]), "=r"((v)[20]), "=r"((v)[21]),      \
-          "=r"((v)[22]), "=r"((v)[23]), "=r"((v)[24]), "=r"((v)[25]), "=r"((v)[26]),      \
-          "=r"((v)[27]), "=r"((v)[28]), "=r"((v)[29]), "=r"((v)[30]), "=r"((v)[31])       \
-        : "r"(addr))
 
 // ----------------------------------------------------------------------------------------
 // bf16 split helpers: v ~= hi + lo (+ lo2), each term a bf16 (round-to-nearest-even)
@@ -308,9 +244,6 @@ __device__ __forceinline__ uint32_t pack_f16x2(float lo_elem, float hi_elem) {
 }
 __device__ __forceinline__ float2 unpack_f16x2(uint32_t h) {  // .x = lower half, .y = upper half
     return __half22float2(*reinterpret_cast<const __half2*>(&h));
-}
-__device__ __forceinline__ float bf16_round(float v) {
-    return __bfloat162float(__float2bfloat16_rn(v));
 }
 
 __device__ __forceinline__ float warp_sum(float v) {

@@ -1,43 +1,31 @@
 // nfb_conv_tc.cu -- stride-1 "same" convolution of the Glow conditioner (nets/cnn.py:33-61, ConvNet2d) as an
-// implicit GEMM on the sm_100a tensor core.
+// implicit GEMM on the sm_90a tensor core (wgmma).
 //
 //   y[b, n, h, w] = act( sum_{c,kh,kw} W[n, c, kh, kw] x[b, c0+c, h+kh-p, w+kw-p] + bias[n] )
-//   M = B*H*W pixels (128 per CTA = the 128 TMEM lanes), N = cout (<= 256, one accumulator), K in chunks of 64.
+//   M = B*H*W pixels (128 per work unit), N = cout in tiles of NT = 64 or 128 columns, K in chunks of 64.
 //   K order: k = cb*(T*16) + tap*16 + ci for channel c = 16 cb + ci and tap = kh*k + kw (T = k*k), i.e. blocks
 //   of 16 channels, tap-major inside a block.  A 16-wide group of k is then ONE tap of 16 consecutive channels:
-//   one bounds check and one base address per group, the 16 loads differ by the plane stride only (3 instead of
-//   ~20 instructions per gathered element), while all T taps of a channel block stay within 2-3 chunks, so the
-//   shifted re-reads of the same 16 planes hit L1.  Channels are zero-padded to a multiple of 16.
+//   one bounds check and one base address per group, the 16 loads differ by the plane stride only, while all T taps
+//   of a channel block stay within 2-3 chunks, so the shifted re-reads of the same 16 planes hit L1.  Channels are
+//   zero-padded to a multiple of 16.
 //
 // Numerics: the same split-bf16 scheme as the spline conditioner (a*w ~= a_hi*w_hi + a_lo*w_hi + a_hi*w_lo,
-// fp32 accumulation in TMEM, weights packed with the accumulate-truncation gain, see nfb_api.cu kAccStepGain).
+// fp32 accumulation, weights packed with the accumulate-truncation gain, see nfb_api.cu kAccStepGain).
 //
-// Roles (576 threads, persistent: CTA b takes 128-pixel tiles b, b+grid, ...):
-//   warps 0-15 builders, 4 per SM sub-partition: thread = (pixel, quarter of the K-chunk).  Per K-chunk it gathers
-//              16 im2col values of its pixel (consecutive lanes = consecutive pixels -> coalesced; the taps of a
-//              channel hit L1) -- the loads of chunk k+1 are issued before chunk k is converted -- splits them to
-//              bf16 hi/lo and stores two 16-byte chunks per tile straight into the SWIZZLE_128B A tiles (3-6
-//              stages, as many as the weight ring leaves room for).  The epilogue of tile i-1 (TMEM -> bias ->
-//              LeakyReLU -> NCHW store, coalesced per channel) runs AFTER tile i has been built, so it overlaps
-//              tile i's MMAs; the accumulator is double-buffered in TMEM.
-//   warp 16    one elected lane streams the packed weight records ([n_pad x 64] hi | lo, pre-swizzled) with
-//              1-D bulk TMA into a 2-slot ring.
-//   warp 17    one elected lane issues 12 tcgen05.mma (M=128, N=n_pad, K=16) per chunk; tcgen05.commit frees the
-//              A stage and the weight slot; owns the TMEM allocation.
+// Structure (256 threads = two warpgroups, persistent over (pixel tile, n tile) units): thread = (pixel, half of the
+// K-chunk) gathers 32 im2col values per chunk (consecutive threads = consecutive pixels -> coalesced; the taps of a
+// channel hit L1), splits them to bf16 hi/lo into the SWIZZLE_128B A tile of a two-stage ring while the previous
+// chunk is on the tensor core; thread 0 streams the pre-packed weight record of the chunk ([NT x 64] hi | lo) with
+// 1-D bulk TMA.  Warpgroup w multiplies pixels [64 w, 64 w + 64); the epilogue (bias, LeakyReLU, NCHW store,
+// coalesced per channel) goes through a shared-memory staging tile.
 #include "nfb_kernels.h"
 
 namespace nfb {
 
 namespace {
-constexpr int kCtBuildWarps = 16;
-constexpr int kCtThreads = 32 * kCtBuildWarps + 64;
-constexpr int kCtMaxStages = 6;
+constexpr int kCtThreads = 256;
 constexpr uint32_t kCtTileA = 16384;   // [128 x 64] bf16
-constexpr uint32_t kCtStage = 2 * kCtTileA;  // hi | lo
-constexpr uint32_t kCtBarBytes = 32 * 8;
 constexpr uint32_t kCtSmemMax = 232448;
-constexpr int kCtMaxSlots = 8;
-enum { CB_AFULL = 0, CB_AEMPTY = 6, CB_WFULL = 12, CB_WEMPTY = 20, CB_ACCFULL = 28, CB_ACCEMPTY = 30 };
 
 __device__ __forceinline__ uint32_t ct_chunk_off(int r, int c8) {
     return (r >> 3) * 1024 + (r & 7) * 128 + ((c8 ^ (r & 7)) << 4);
@@ -45,228 +33,182 @@ __device__ __forceinline__ uint32_t ct_chunk_off(int r, int c8) {
 __device__ __forceinline__ void ct_st_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
     asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
+__device__ __forceinline__ void ct_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kCtThreads) : "memory"); }
+constexpr int ct_n_tile(int n_pad) { return n_pad > 64 ? 128 : 64; }
 }  // namespace
 
 struct ConvTcParams {
     const float* x; float* y; const float* bias; const uint8_t* wstream;
-    long long M; int ctot, c0, cin, H, W, cout, ks, n_pad, k_chunks, stages, w_slots; uint32_t slot_bytes; float leaky; int* err;
+    long long M; int ctot, c0, cin, H, W, cout, ks, n_tiles, k_chunks; float leaky; int* err;
 };
 
-// shared memory: [stages x (A hi | A lo)] [w_slots x weight slot] [barriers] [tmem ptr]
+template <int NT>
 __global__ void __launch_bounds__(kCtThreads, 1) conv_tc_kernel(const ConvTcParams p) {
     extern __shared__ __align__(1024) uint8_t smem[];
+    constexpr int NREG = NT / 2;
+    constexpr uint32_t b_tile = (uint32_t)NT * 128u;
+    constexpr uint32_t stage_bytes = 2 * kCtTileA + 2 * b_tile;   // A hi | A lo | W hi | W lo
+    constexpr int kStgLd = NT + 1;
     const uint32_t sbase = smem_u32(smem);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int S = p.stages;
-    const uint32_t offW = (uint32_t)S * kCtStage;
-    const int WS = p.w_slots;
-    const uint32_t offBars = offW + (uint32_t)WS * p.slot_bytes;
-    const uint32_t bars = sbase + offBars;
-    auto bar = [bars](int i) { return bars + 8u * i; };
-    const uint32_t tcols = p.n_pad <= 32 ? 32u : p.n_pad <= 64 ? 64u : p.n_pad <= 128 ? 128u : 256u;
-
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < kCtMaxStages; ++i) {
-            mbar_init(bar(CB_AFULL + i), kCtBuildWarps);  // one arrive per builder warp
-            mbar_init(bar(CB_AEMPTY + i), 1);             // tcgen05.commit
-        }
-        for (int i = 0; i < kCtMaxSlots; ++i) {
-            mbar_init(bar(CB_WFULL + i), 1);              // expect_tx
-            mbar_init(bar(CB_WEMPTY + i), 1);             // tcgen05.commit
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(bar(CB_ACCFULL + i), 1);            // tcgen05.commit
-            mbar_init(bar(CB_ACCEMPTY + i), kCtBuildWarps);
-        }
+    const int bt = threadIdx.x, wg = bt >> 7, warp = (bt >> 5) & 3, lane = bt & 31;
+    const uint32_t bars = sbase + 2 * stage_bytes;   // [0, 2): weight record of stage s landed
+    float* stg = reinterpret_cast<float*>(smem + 2 * stage_bytes + 64);
+    if (bt == 0) {
+        mbar_init(bars, 1);
+        mbar_init(bars + 8, 1);
         fence_mbar_init();
     }
-    if (warp == kCtBuildWarps + 1) {
-        tmem_alloc(sbase + offBars + kCtBarBytes, 2 * tcols);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *reinterpret_cast<volatile uint32_t*>(smem + offBars + kCtBarBytes);
     const int KC = p.k_chunks;
-    const uint32_t rec_bytes = (uint32_t)p.n_pad * 256u;  // hi + lo
-    const long long n_tiles = (p.M + 127) / 128;
+    const long long m_tiles = (p.M + 127) / 128;
+    const long long n_units = m_tiles * p.n_tiles;
+    const int HW = p.H * p.W, pad = p.ks >> 1, ks = p.ks, kk2 = ks * ks;
+    const int r = bt & 127, half = bt >> 7;   // A-tile row (pixel) and half of the K-chunk this thread gathers
+    const int inv_ks = 65536 / ks + 1;        // tap / ks for tap < 25
 
-    if (warp == kCtBuildWarps) {
-        // ------------------------------ weight producer ------------------------------------
-        uint32_t ws = 0, ws_use = 0;  // ring position over all tiles of this CTA
-        for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x)
-            for (int kc = 0; kc < KC; ++kc) {
-                if (ws_use > 0) mbar_wait(bar(CB_WEMPTY + ws), (ws_use - 1) & 1u, p.err, 700 + ws);
-                if (elect_one_sync()) {
-                    mbar_expect_tx(bar(CB_WFULL + ws), rec_bytes);
-                    bulk_g2s(sbase + offW + ws * p.slot_bytes, p.wstream + (size_t)kc * rec_bytes, rec_bytes,
-                             bar(CB_WFULL + ws));
-                }
-                __syncwarp();
-                if (++ws == (uint32_t)WS) { ws = 0; ++ws_use; }
-            }
-    } else if (warp == kCtBuildWarps + 1) {
-        // ------------------------------ MMA issuer ------------------------------------------
-        const uint32_t idesc = umma_idesc_bf16(128, (uint32_t)p.n_pad);
-        uint32_t ws = 0, ws_use = 0, st = 0, st_use = 0, it = 0;
-        for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x, ++it) {
-            const uint32_t ab = it & 1u;  // accumulator buffer
-            if (it >= 2) mbar_wait(bar(CB_ACCEMPTY + ab), ((it >> 1) - 1) & 1u, p.err, 750 + ab);
-            const uint32_t d = tmem + ab * tcols;
-            for (int kc = 0; kc < KC; ++kc) {
-                mbar_wait(bar(CB_AFULL + st), st_use & 1u, p.err, 710 + st);
-                mbar_wait(bar(CB_WFULL + ws), ws_use & 1u, p.err, 720 + ws);
-                tc_fence_after();
-                if (elect_one_sync()) {
-                    const uint64_t a_hi = umma_desc_sw128(sbase + st * kCtStage);
-                    const uint64_t a_lo = umma_desc_sw128(sbase + st * kCtStage + kCtTileA);
-                    const uint64_t w_hi = umma_desc_sw128(sbase + offW + ws * p.slot_bytes);
-                    const uint64_t w_lo = umma_desc_sw128(sbase + offW + ws * p.slot_bytes + (uint32_t)p.n_pad * 128u);
+    struct Pos { long long u, mt; int nt, kc; };
+    auto unit_pos = [&](long long u, int kc) {
+        Pos q;
+        q.u = u; q.kc = kc;
+        q.mt = u / p.n_tiles;
+        q.nt = (int)(u - q.mt * p.n_tiles);
+        return q;
+    };
+    // the two 16-wide k groups G = 4 kc + 2 half + {0, 1} of this thread: one tap of channel block cb each
+    float v[2][16];
+    auto gather = [&](const Pos& q) {
+        const long long m = q.mt * 128 + r;
+        const bool live = m < p.M;
+        const long long bi = live ? m / HW : 0;
+        const int pix = live ? (int)(m - bi * HW) : 0;
+        const int h = pix / p.W, w = pix - h * p.W;
+        const float* xb = p.x + (bi * p.ctot + p.c0) * (long long)HW;
 #pragma unroll
-                    for (int j = 0; j < 4; ++j) umma_bf16(d, a_hi + 2 * j, w_hi + 2 * j, idesc, (kc | j) ? 1u : 0u);
+        for (int g = 0; g < 2; ++g) {
+            const int G = 4 * q.kc + 2 * half + g;
+            const int cb = G / kk2, tap = G - cb * kk2;
+            const int kh = (tap * inv_ks) >> 16, kw = tap - kh * ks;
+            const int hh = h + kh - pad, ww = w + kw - pad;
+            const bool ok = live && hh >= 0 && hh < p.H && ww >= 0 && ww < p.W;
+            const int cbase = cb * 16;
+            const int nvalid = ok ? p.cin - cbase : 0;  // channels of this block that exist (<= 0: none)
+            const float* src = xb + ((cbase * p.H + hh) * p.W + ww);  // one pointer, stepped by the plane stride
 #pragma unroll
-                    for (int j = 0; j < 4; ++j) umma_bf16(d, a_lo + 2 * j, w_hi + 2 * j, idesc, 1u);
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) umma_bf16(d, a_hi + 2 * j, w_lo + 2 * j, idesc, 1u);
-                    umma_commit(bar(CB_AEMPTY + st));
-                    umma_commit(bar(CB_WEMPTY + ws));
-                    if (kc == KC - 1) umma_commit(bar(CB_ACCFULL + ab));
-                }
-                __syncwarp();
-                if (++st == (uint32_t)S) { st = 0; ++st_use; }
-                if (++ws == (uint32_t)WS) { ws = 0; ++ws_use; }
+            for (int j = 0; j < 16; ++j) {
+                v[g][j] = 0.f;
+                if (j < nvalid) v[g][j] = __ldg(src);
+                src += HW;
             }
         }
-    } else {
-        // ------------------------------ im2col builders / epilogue -------------------------
-        const int q = warp & 3, wh = warp >> 2;  // TMEM lane quadrant, K-quarter / column group
-        const int r = q * 32 + lane;             // tile row = TMEM lane
-        const int HW = p.H * p.W, pad = p.ks >> 1, ks = p.ks, kk2 = ks * ks;
-        const uint32_t tlane = tmem + ((uint32_t)(q * 32) << 16);
-        uint32_t st = 0, st_use = 0, it = 0;
-
-        auto epilogue = [&](long long tile, uint32_t i) {
-            const uint32_t ab = i & 1u;
-            mbar_wait(bar(CB_ACCFULL + ab), (i >> 1) & 1u, p.err, 740 + ab);
-            tc_fence_after();
-            const long long m = tile * 128 + r;
-            const bool live = m < p.M;
-            const long long bi = live ? m / HW : 0;
-            const int pix = live ? (int)(m - bi * HW) : 0;
-            float* yb = p.y + bi * (long long)p.cout * HW + pix;
-            for (int n0 = wh * 16; n0 < p.n_pad; n0 += 64) {
-                uint32_t acc[16];
-                NFB_TMEM_LD16(tlane + ab * tcols + n0, acc);
-                tc_wait_ld();
+    };
+    uint32_t full_use[2] = {0, 0};
+    auto emit = [&](const Pos& q, int s) {   // weight record by TMA, A chunk split into the stage
+        const uint32_t sa = sbase + s * stage_bytes;
+        if (bt == 0) {
+            mbar_expect_tx(bars + 8 * s, 2 * b_tile);
+            bulk_g2s(sa + 2 * kCtTileA, p.wstream + ((size_t)q.nt * KC + q.kc) * (2 * b_tile), 2 * b_tile, bars + 8 * s);
+        }
 #pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const int n = n0 + j;
-                    if (live && n < p.cout) {
-                        float v = __uint_as_float(acc[j]) + (p.bias ? __ldg(p.bias + n) : 0.f);
-                        if (p.leaky >= 0.f) v = v >= 0.f ? v : v * p.leaky;
-                        yb[(long long)n * HW] = v;
-                    }
+        for (int g = 0; g < 2; ++g)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                uint32_t hi[4], lo[4];
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const float a = v[g][8 * e + 2 * i], b = v[g][8 * e + 2 * i + 1];
+                    hi[i] = pack_bf16x2(a, b);
+                    lo[i] = pack_bf16x2(a - __uint_as_float(hi[i] << 16), b - __uint_as_float(hi[i] & 0xffff0000u));
                 }
+                const uint32_t off = ct_chunk_off(r, 4 * half + 2 * g + e);
+                ct_st_v4(sa + off, hi[0], hi[1], hi[2], hi[3]);
+                ct_st_v4(sa + kCtTileA + off, lo[0], lo[1], lo[2], lo[3]);
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(bar(CB_ACCEMPTY + ab));
+        fence_proxy_async_smem();
+    };
+    auto mma_chunk = [&](float (&acc)[NREG], int s, bool first) {
+        const uint32_t sa = sbase + s * stage_bytes;
+        const uint64_t ah = wgmma_desc(sa + wg * 8192u), al = wgmma_desc(sa + kCtTileA + wg * 8192u);
+        const uint64_t bh = wgmma_desc(sa + 2 * kCtTileA), bl = wgmma_desc(sa + 2 * kCtTileA + b_tile);
+        auto mma = [&](uint64_t a, uint64_t b, uint32_t sd) {
+            if constexpr (NT == 64) wgmma_bf16_n64(acc, a, b, sd);
+            else wgmma_bf16_n128(acc, a, b, sd);
         };
-
-        long long prev_tile = -1;
-        for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x, ++it) {
-            const long long m = t * 128 + r;
-            const bool live = m < p.M;
-            const long long bi = live ? m / HW : 0;
-            const int pix = live ? (int)(m - bi * HW) : 0;
-            const int h = pix / p.W, w = pix - h * p.W;
-            const float* xb = p.x + (bi * p.ctot + p.c0) * (long long)HW;
-            // this thread's 16 k indices of chunk kc = group G = 4 kc + wh: one tap of channel block cb.  The
-            // calls come in increasing kc, so (cb, tap) is carried along instead of divided out each time, and
-            // the 16 loads use one 32-bit offset stepped by the plane stride.
-            int g_cb = ks == 1 ? wh : wh / kk2, g_tap = ks == 1 ? 0 : wh % kk2;
-            const int inv_ks = 65536 / ks + 1;  // tap / ks for tap < 25
-            auto gather = [&](float (&v)[16]) {
-                const int kh = (g_tap * inv_ks) >> 16, kw = g_tap - kh * ks;
-                const int hh = h + kh - pad, ww = w + kw - pad;
-                const bool ok = live && hh >= 0 && hh < p.H && ww >= 0 && ww < p.W;
-                const int cbase = g_cb * 16;
-                const int nvalid = ok ? p.cin - cbase : 0;  // channels of this block that exist (<= 0: none)
-                const float* src = xb + ((cbase * p.H + hh) * p.W + ww);  // one pointer, stepped by the plane stride
+        wgmma_fence();
 #pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    v[j] = 0.f;
-                    if (j < nvalid) v[j] = __ldg(src);
-                    src += HW;
-                }
-                if (ks == 1) g_cb += 4;
-                else { g_tap += 4; while (g_tap >= kk2) { g_tap -= kk2; ++g_cb; } }
-            };
-            auto emit = [&](const float (&v)[16]) {  // split, store into the next free A stage, publish
-                if (st_use > 0) mbar_wait(bar(CB_AEMPTY + st), (st_use - 1) & 1u, p.err, 730 + st);
-                const uint32_t t_hi = sbase + st * kCtStage, t_lo = t_hi + kCtTileA;
+        for (int j = 0; j < 4; ++j) mma(ah + 2 * j, bh + 2 * j, (first && j == 0) ? 0u : 1u);
 #pragma unroll
-                for (int g = 0; g < 2; ++g) {
-                    uint32_t hi[4], lo[4];
+        for (int j = 0; j < 4; ++j) mma(al + 2 * j, bh + 2 * j, 1u);
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        const float a = v[8 * g + 2 * i], b = v[8 * g + 2 * i + 1];
-                        hi[i] = pack_bf16x2(a, b);
-                        lo[i] = pack_bf16x2(a - __uint_as_float(hi[i] << 16), b - __uint_as_float(hi[i] & 0xffff0000u));
-                    }
-                    const uint32_t off = ct_chunk_off(r, wh * 2 + g);
-                    ct_st_v4(t_hi + off, hi[0], hi[1], hi[2], hi[3]);
-                    ct_st_v4(t_lo + off, lo[0], lo[1], lo[2], lo[3]);
-                }
-                fence_proxy_async_smem();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(bar(CB_AFULL + st));
-                if (++st == (uint32_t)S) { st = 0; ++st_use; }
-            };
-            // three register sets in rotation: the loads of chunks k+1 and k+2 are in flight while chunk k is
-            // converted (the gathers come from HBM/L2 at ~2 k cycles; one chunk of work is ~0.6 k)
-            float a0[16], a1[16], a2[16];
-            gather(a0);
-            if (KC > 1) gather(a1);
-            for (int kc = 0; kc < KC; kc += 3) {
-                if (kc + 2 < KC) gather(a2);
-                emit(a0);
-                if (kc + 1 < KC) {
-                    if (kc + 3 < KC) gather(a0);
-                    emit(a1);
-                }
-                if (kc + 2 < KC) {
-                    if (kc + 4 < KC) gather(a1);
-                    emit(a2);
+        for (int j = 0; j < 4; ++j) mma(ah + 2 * j, bl + 2 * j, 1u);
+        wgmma_commit();
+    };
+    auto epilogue = [&](const Pos& q, const float (&acc)[NREG]) {
+        const int r0 = 64 * wg + 16 * warp + (lane >> 2);
+#pragma unroll
+        for (int i = 0; i < NREG; ++i)
+            stg[(r0 + ((i & 2) ? 8 : 0)) * kStgLd + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1)] = acc[i];
+        ct_bar_sync();
+        const long long m = q.mt * 128 + r;
+        if (m < p.M) {
+            const long long bi = m / HW;
+            const int pix = (int)(m - bi * HW);
+            float* yb = p.y + bi * (long long)p.cout * HW + pix;
+            for (int j = half; j < NT; j += 2) {   // consecutive threads: consecutive pixels of one channel
+                const int n = q.nt * NT + j;
+                if (n < p.cout) {
+                    float val = stg[r * kStgLd + j] + (p.bias ? __ldg(p.bias + n) : 0.f);
+                    if (p.leaky >= 0.f) val = val >= 0.f ? val : val * p.leaky;
+                    yb[(long long)n * HW] = val;
                 }
             }
-            if (prev_tile >= 0) epilogue(prev_tile, it - 1);  // overlaps this tile's MMAs
-            prev_tile = t;
         }
-        if (prev_tile >= 0) epilogue(prev_tile, it - 1);
+        ct_bar_sync();   // the staging tile is reused by the next unit
+    };
+
+    if ((long long)blockIdx.x >= n_units) return;
+    float acc[NREG];
+    Pos cur = unit_pos(blockIdx.x, 0);
+    gather(cur);
+    emit(cur, 0);
+    ct_bar_sync();
+    for (int s = 0;; s ^= 1) {
+        Pos nxt = cur;
+        if (++nxt.kc == KC) nxt = unit_pos(cur.u + gridDim.x, 0);
+        const bool has_next = nxt.u < n_units;
+        if (has_next) gather(nxt);   // in flight during this chunk's MMAs
+        mbar_wait(bars + 8 * s, full_use[s] & 1u, p.err, 710 + s);
+        ++full_use[s];
+        mma_chunk(acc, s, cur.kc == 0);
+        if (has_next) emit(nxt, s ^ 1);   // (stage s ^ 1 was read by the previous chunk: complete, see below)
+        wgmma_wait<0>();
+        wgmma_hold(acc);
+        ct_bar_sync();   // both warpgroups are done with stage s, and stage s ^ 1 holds the next chunk
+        if (cur.kc == KC - 1) epilogue(cur, acc);
+        if (!has_next) break;
+        cur = nxt;
     }
-    __syncthreads();
-    if (warp == kCtBuildWarps + 1) tmem_dealloc(tmem, 2 * tcols);
 }
 
-// weights [cout, cin, k, k] fp32 -> per K-chunk record [n_pad x 64] hi | lo, SWIZZLE_128B, K in the kernel's order
-__global__ void conv_pack_kernel(const float* __restrict__ w, int cout, int cin, int T, int n_pad, int k_chunks,
+// weights [cout, cin, k, k] fp32 -> one record per (n tile, K-chunk): [NT x 64] hi | lo, SWIZZLE_128B, K in the kernel's
+// order
+__global__ void conv_pack_kernel(const float* __restrict__ w, int cout, int cin, int T, int NT, int n_tiles, int k_chunks,
                                  float gain, uint8_t* __restrict__ out) {
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const long long total = (long long)k_chunks * n_pad * 64;
+    const long long total = (long long)k_chunks * n_tiles * NT * 64;
     if (idx >= total) return;
     const int kk = (int)(idx & 63);
-    const int n = (int)((idx >> 6) % n_pad);
-    const int kc = (int)(idx / ((long long)n_pad * 64));
+    const long long rowg = idx >> 6;                  // row of the padded [n_tiles * NT] weight matrix, chunk-major
+    const int kc = (int)(rowg / ((long long)n_tiles * NT));
+    const int ng = (int)(rowg - (long long)kc * n_tiles * NT);
+    const int nt = ng / NT, n = ng - nt * NT;
     const int G = kc * 4 + (kk >> 4), ci = kk & 15;
     const int cb = G / T, tap = G - cb * T, c = cb * 16 + ci;
-    const float v = (n < cout && c < cin) ? w[((long long)n * cin + c) * T + tap] * gain : 0.f;
+    const float v = (ng < cout && c < cin) ? w[((long long)ng * cin + c) * T + tap] * gain : 0.f;
     const size_t off = (size_t)(n >> 3) * 1024 + (n & 7) * 128 + (((kk >> 3) ^ (n & 7)) << 4) + (kk & 7) * 2;
-    uint8_t* rec = out + (size_t)kc * n_pad * 256;
+    uint8_t* rec = out + ((size_t)nt * k_chunks + kc) * NT * 256;
     const __nv_bfloat16 hi = __float2bfloat16_rn(v);
     *reinterpret_cast<__nv_bfloat16*>(rec + off) = hi;
-    *reinterpret_cast<__nv_bfloat16*>(rec + (size_t)n_pad * 128 + off) = __float2bfloat16_rn(v - __bfloat162float(hi));
+    *reinterpret_cast<__nv_bfloat16*>(rec + (size_t)NT * 128 + off) = __float2bfloat16_rn(v - __bfloat162float(hi));
 }
 
 bool conv_tc_supported(int cin, int cout, int ks) {
@@ -275,46 +217,46 @@ bool conv_tc_supported(int cin, int cout, int ks) {
     return (ks == 1 || ks == 3 || ks == 5) && cout >= 1 && cout <= 256 && (cout > 64 || K > 64);
 }
 
+template <int NT>
+int launch_conv_tc_t(const ConvTcParams& p, cudaStream_t st) {
+    static PerDevice per_dev;  // attribute + SM count of the device this launch goes to (not the first one seen)
+    constexpr uint32_t smem = 2 * (2 * kCtTileA + 2 * (uint32_t)NT * 128u) + 64 + 128 * (NT + 1) * 4;
+    static_assert(smem <= kCtSmemMax, "conv_tc: shared memory");
+    const int sm_count = per_dev.ensure([] {
+        return cudaFuncSetAttribute(conv_tc_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    });
+    if (sm_count < 0) return NFB_ERR_CUDA;
+    const long long n_units = (p.M + 127) / 128 * p.n_tiles;
+    const unsigned grid = (unsigned)(n_units < sm_count ? n_units : sm_count);
+    conv_tc_kernel<NT><<<grid, kCtThreads, smem, st>>>(p);
+    return NFB_OK;
+}
+
 int launch_conv2d_tc(const float* x, int ctot, int c0, const float* w, const float* bias, float* y, long long B,
                      int cin, int H, int W, int cout, int ks, float leaky, float gain_per_step, int* err,
                      cudaStream_t st) {
-    static PerDevice per_dev;  // attribute + SM count of the device this launch goes to (not the first one seen)
-    const int sm_count = per_dev.ensure([] {
-        return cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kCtSmemMax);
-    });
-    if (sm_count < 0) return NFB_ERR_CUDA;
     const long long M = B * H * W;
     if (M == 0) return NFB_OK;
     const int T = ks * ks;
     const int groups = (cin + 15) / 16 * T;  // 16-wide k groups: (channel block, tap)
     const int k_chunks = (groups + 3) / 4;
-    const int n_pad = (cout + 15) / 16 * 16;
-    const size_t bytes = (size_t)k_chunks * n_pad * 256;
+    const int NT = ct_n_tile(cout);
+    const int n_tiles = (cout + NT - 1) / NT;
+    const size_t bytes = (size_t)k_chunks * n_tiles * NT * 256;
     void* scratch = nullptr;
     NFB_CUDA(cudaMallocAsync(&scratch, bytes, st));  // stream-ordered: freed after the kernel that reads it
-    const long long total = (long long)k_chunks * n_pad * 64;
+    const long long total = (long long)k_chunks * n_tiles * NT * 64;
     const float gain = 1.f + gain_per_step * (float)(3 * 4 * k_chunks);
-    conv_pack_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(w, cout, cin, T, n_pad, k_chunks, gain,
+    conv_pack_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(w, cout, cin, T, NT, n_tiles, k_chunks, gain,
                                                                       static_cast<uint8_t*>(scratch));
     ConvTcParams p{};
     p.x = x; p.y = y; p.bias = bias; p.wstream = static_cast<const uint8_t*>(scratch);
     p.M = M; p.ctot = ctot; p.c0 = c0; p.cin = cin; p.H = H; p.W = W; p.cout = cout; p.ks = ks;
-    p.n_pad = n_pad; p.k_chunks = k_chunks; p.leaky = leaky; p.err = err;
-    p.slot_bytes = ((uint32_t)n_pad * 256u + 1023u) & ~1023u;
-    // weight ring: up to 128 KB / 8 slots (small-N records are latency-, not bandwidth-limited); A stages: the rest
-    int w_slots = (int)(131072u / p.slot_bytes);
-    w_slots = w_slots < 2 ? 2 : (w_slots > kCtMaxSlots ? kCtMaxSlots : w_slots);
-    const uint32_t fixed = (uint32_t)w_slots * p.slot_bytes + kCtBarBytes + 16;
-    int stages = (int)((kCtSmemMax - fixed) / kCtStage);
-    stages = stages > kCtMaxStages ? kCtMaxStages : stages;  // 3 at N = 256, 6 at N <= 64
-    p.stages = stages;
-    p.w_slots = w_slots;
-    const uint32_t smem = (uint32_t)stages * kCtStage + fixed;
-    const long long n_tiles = (M + 127) / 128;
-    const unsigned grid = (unsigned)(n_tiles < sm_count ? n_tiles : sm_count);
-    conv_tc_kernel<<<grid, kCtThreads, smem, st>>>(p);
+    p.n_tiles = n_tiles; p.k_chunks = k_chunks; p.leaky = leaky; p.err = err;
+    int rc = NT == 64 ? launch_conv_tc_t<64>(p, st) : launch_conv_tc_t<128>(p, st);
     const cudaError_t e = cudaGetLastError();
     cudaFreeAsync(scratch, st);
+    if (rc) return rc;
     if (e != cudaSuccess) {
         nfb_set_error("conv_tc launch: %s", cudaGetErrorString(e));
         return NFB_ERR_CUDA;

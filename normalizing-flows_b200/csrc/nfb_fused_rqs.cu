@@ -1,6 +1,6 @@
-// nfb_fused_rqs.cu -- one fused sm_100a kernel per neural-spline coupling block.
+// nfb_fused_rqs.cu -- the fused sm_90a kernel of the neural-spline coupling blocks (one block, or a whole stack).
 //
-// Per 128-row tile, without leaving the SM:
+// Per 64-row tile, without leaving the SM:
 //   [LULinearPermute.inverse  (flows/mixing.py:560-563)]      x  = z[:,perm] (LU)^T + b
 //   conditioner  MADE (nets/made.py:296-304) or ResidualNet (nets/resnet.py:92-104)
 //   RQ spline    (utils/splines.py:16-219) on every transformed feature
@@ -9,62 +9,60 @@
 // z is read once and written once per block; the [B, T*(3K-1)] parameter tensor the reference
 // materialises never exists.
 //
-// Tensor-core numerics: every GEMM runs as a split-fp16 product on tcgen05 (fp32 accumulate in TMEM), operands
+// Tensor-core numerics: every GEMM runs as a split-fp16 product on wgmma (fp32 accumulation in registers), operands
 // scaled by powers of two (nfb_api.cu plan_scales):
 //   a*w ~= a_hi*w_hi + a_lo*w_hi + a_hi*w_lo     (conditioner layers; ~2^-22 relative per product)
 //   all four terms for the LU linear map that transforms z itself.
 // Plain bf16/tf32 fail the rtol 1e-4 log_prob bar (SURVEY 7.2); this is why.
 //
-// Structure (576 threads, 1 CTA/SM, persistent over (layer, tile) work units of the whole stack):
-//   warp 16  weight producer: 1-D bulk TMA (cp.async.bulk -> UBLKCP) of pre-swizzled fp16 records
-//            from the packed weight stream (L2 resident) into a 2 x 32 KB ring.
-//   warp 17  MMA issuer: walks the same step table, one elected lane issues tcgen05.mma
-//            (M=128, N<=256, K=16) and commits to mbarriers; owns the 512-column TMEM alloc.
-//   warps 0-15 epilogue (4 per SM sub-partition = 4 column groups x 4 TMEM lane quadrants):
-//            TMEM -> registers (tcgen05.ld 32x32b, software-pipelined one K-chunk ahead), bias/ReLU, fp16 hi/lo split
-//            back into the swizzled A-operand tiles; the final layer arrives in 240-column chunks (10 features
-//            x 24) through a 2-deep TMEM ring and is consumed by the spline evaluator while the
-//            tensor core produces the next chunk.
-// The residual stream h lives in TMEM columns [0,256) and is updated by accumulating the second
-// GEMM of each residual block straight onto it (h += W2 relu(...)); biases are pre-summed on the
-// host side of the packer.  Shared memory: A operand 128 KB (hi|lo x K=256), weight ring 64 KB,
-// x/y tile 32 KB (XOR-swizzled, conflict-free column access).
-// Round 2b measured three alternatives to this ring (byte-granular ring, hi|lo "mixed" records, a third slot with the
-// x tile parked in L2) -- all slower; the GEMM phases sit at the shared-memory bound of SS-mode operands
-// (profiles/r02b_ring_experiments.md).  Kept from that work: the pipelined TMEM loads of the hidden epilogues, the
-// LU fold (first conditioner GEMM issued together with the LU stage), the early log_q fetch, row maxima by shuffle.
+// Structure (384 threads, 1 CTA/SM, persistent over (layer, tile) work units of the whole stack):
+//   warp 8     weight producer: 1-D bulk TMA (cp.async.bulk) of pre-swizzled fp16 records from the packed weight stream
+//              (read from L2) into a 3 x 32 KB ring.  A record is one W_hi tile and its W_lo twin for one K-chunk: the
+//              output slices of BOTH consumer warpgroups stacked (rows [0, 8 n8) for warpgroup 0, [8 n8, 16 n8) for 1).
+//              Its warpgroup gives its registers to the consumers (setmaxnreg); warps 9-11 exit.
+//   warps 0-7  two warpgroups; each issues the wgmma (M = the 64 rows of the tile, K = 16) of its half of every record
+//              and runs its epilogues.  A hidden GEMM's output columns are split between them (warpgroup w: 64-column
+//              slices [w h, w h + h), h = ceil(H / 128)), so the whole output -- and the conditioner's residual stream,
+//              64 x H fp32 -- lives in registers (2 x 32 per thread each) and ONE A-operand buffer suffices: both
+//              warpgroups finish the GEMM, then overwrite its input with its output (bias, ReLU, fp16 hi/lo split).  The
+//              second GEMM of each residual block accumulates straight onto the residual stream (h += W2 relu(...));
+//              the biases are pre-summed by the packer.  The final layer is computed two features (N = 48) per
+//              warpgroup at a time and staged through shared memory, so that each thread evaluates one (row, feature)
+//              spline; the two warpgroups drift apart by up to the ring depth, so one's splines overlap the other's
+//              products.
+// Shared memory: A operand 64 KB (hi|lo x K=256), weight ring 96 KB, x/y tile 16 KB (XOR-swizzled, conflict-free
+// column access), final-layer staging 2 x 13 KB.
+#include <type_traits>
+
 #include "nfb_kernels.h"
 #include "nfb_spline.cuh"
 
 namespace nfb {
 
-constexpr int kNG = 4;                         // epilogue column groups (warps per TMEM lane quadrant)
-constexpr int kEpiWarps = 4 * kNG;             // 16 epilogue warps: 4 per SM sub-partition (latency hiding by TLP)
-constexpr int kEpiThreads = 32 * kEpiWarps;    // 512
-constexpr int kFusedThreads = kEpiThreads + 64;  // + TMA producer warp + MMA issuer warp
-constexpr int kGC = 64 / kNG;                  // columns of a 64-column K-chunk handled per thread (16)
-constexpr uint32_t kTileA = 16384;             // one [128 x 64] fp16 SW128 tile
-constexpr uint32_t kSlotBytes = 32768;         // one record = up to [256 rows x 64 K] fp16
-constexpr uint32_t kSlots = 2;                 // (a third slot was measured: no gain, profiles/r02b_ring_experiments.md)
-constexpr uint32_t kOffA = 0;
-constexpr uint32_t kOffW = 131072;
-constexpr uint32_t kOffX = kOffW + kSlots * kSlotBytes;  // 196608: x/y tile
-constexpr uint32_t kOffMisc = kOffX + 32768;             // 229376: log-det partials [kNG-1][128], row maxima [128]
-constexpr uint32_t kOffRowMax = kOffMisc + (kNG - 1) * 128 * 4;
-constexpr uint32_t kOffBars = kOffMisc + 2048;           // 231424
-constexpr uint32_t kNumBars = 24;
-constexpr uint32_t kOffTmemPtr = kOffBars + kNumBars * 8;  // 231616
-constexpr uint32_t kOffUnitQ = kOffTmemPtr + 16;           // claimed work units, 4-deep (producer -> MMA issuer, epilogue)
-constexpr uint32_t kFusedSmem = kOffUnitQ + 16;            // 231648 <= 232448
+constexpr int kRows = kFusedTileRows;             // 64
+constexpr int kCons = 256;                        // the consumer warpgroups (warps 0-7)
+constexpr int kFusedThreads = kCons + 128;        // + the producer warpgroup (warp 8 streams the weights)
+// Register budget: the producer warpgroup gives most of its registers to the two consumer warpgroups (setmaxnreg), so
+// that the residual-stream halves, the GEMM accumulators and the spline evaluation stay in registers:
+// 128 x 24 + 256 x 240 <= 64 K, and per SM sub-partition (3 warps) 2 x 240 x 32 + 24 x 32 <= 16 K.
+constexpr int kProducerRegs = 24, kConsumerRegs = 240;
+constexpr uint32_t kTileA = 8192;                 // one [64 x 64] fp16 SW128 tile
+constexpr uint32_t kSlotBytes = 32768;            // one record: [<= 128 rows x 64 K] hi + lo
+constexpr uint32_t kSlots = 3;
+constexpr uint32_t kOffW = 8 * kTileA;                      // 65536: after the A operand (hi K-chunks 0..3 | lo 0..3)
+constexpr uint32_t kOffX = kOffW + kSlots * kSlotBytes;     // 163840: x/y tile
+constexpr int kStgLd = 52;                                  // final-layer staging row stride (floats)
+constexpr uint32_t kStgBytes = kRows * kStgLd * 4;
+constexpr uint32_t kOffStg = kOffX + kRows * 64 * 4;        // 180224: one staging tile per warpgroup
+constexpr uint32_t kOffMisc = kOffStg + 2 * kStgBytes;      // log-det partials [3][64], row exponents [64]
+constexpr uint32_t kOffBars = kOffMisc + 4 * kRows * 4;
+constexpr uint32_t kNumBars = 10;
+constexpr uint32_t kOffUnitQ = kOffBars + kNumBars * 8;     // claimed work units (layer, tile), 4-deep
+constexpr uint32_t kFusedSmem = kOffUnitQ + 32;
 static_assert(kFusedSmem <= 232448, "shared memory budget");
+static_assert(2 * kFusedFeaturesPerChunk * 24 * 64 * 4 <= (int)kSlotBytes, "final-layer record must fit a ring slot");
 
-// barrier indices
-constexpr int kBarWFull = 0 /* +slot */, kBarWEmpty = 3 /* +slot */, kBarAReady = 6 /* +kc, 4 */, kBarAccFull = 10,
-              kBarCFull = 11 /* +b, 2 */, kBarCEmpty = 13 /* +b, 2 */, kBarLuFull = 15, kBarAccBlk = 16 /* +kc, 3 */,
-              kBarUnit = 19 /* +slot, 4 */;
-// TMEM column of final-layer chunk buffer i
-// (both accumulator regions are dead once the last hidden epilogue has run: one buffer in each)
-__device__ __forceinline__ uint32_t chunk_col(int i) { return (uint32_t)i * 256u; }
+constexpr int kBarWFull = 0 /* +slot */, kBarWEmpty = 3 /* +slot */, kBarUnit = 6 /* +slot, 4 */;
 
 __device__ __forceinline__ uint32_t xs_index(int r, int c) { return r * 64 + (c ^ (r & 31)); }
 
@@ -78,17 +76,21 @@ __device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t
     asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d)
                  : "memory");
 }
-__device__ __forceinline__ void epi_bar_sync() {  // the 512 epilogue threads only
-    asm volatile("bar.sync 1, %0;" ::"n"(kEpiThreads) : "memory");
+__device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) {
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
 }
-// tcgen05.wait::ld that also names the 16 destination registers of the load it completes, so that the compiler
-// cannot schedule arithmetic on them above the wait (the load's asm statement "returns" before the data has landed)
-#define NFB_TMEM_WAIT16(v)                                                                                     \
-    asm volatile("tcgen05.wait::ld.sync.aligned;"                                                              \
-                 : "+r"((v)[0]), "+r"((v)[1]), "+r"((v)[2]), "+r"((v)[3]), "+r"((v)[4]), "+r"((v)[5]),         \
-                   "+r"((v)[6]), "+r"((v)[7]), "+r"((v)[8]), "+r"((v)[9]), "+r"((v)[10]), "+r"((v)[11]),       \
-                   "+r"((v)[12]), "+r"((v)[13]), "+r"((v)[14]), "+r"((v)[15])                                  \
-                 :: "memory")
+__device__ __forceinline__ void cons_bar_sync() {  // both consumer warpgroups
+    asm volatile("bar.sync 1, %0;" ::"n"(kCons) : "memory");
+}
+__device__ __forceinline__ void wg_bar_sync(int wg) {  // one consumer warpgroup
+    asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+}
+// mbarrier arrive by one thread of the warpgroup, as a predicated instruction: a branch around it would make ptxas
+// serialise the warpgroup's wgmma
+__device__ __forceinline__ void mbar_arrive_if(uint32_t bar, bool pred) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %1, 0;\n\t@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}"
+                 ::"r"(bar), "r"((uint32_t)pred) : "memory");
+}
 
 // split 8 consecutive fp32 values (already in the GEMM's scaled units) into fp16 hi / lo chunks and store them at
 // the same chunk offset of the two A tiles.  hi + lo reproduces the value to ~2^-23 relative (11 + 11 bits + sign).
@@ -104,27 +106,52 @@ __device__ __forceinline__ void split_store8(const float* v, uint32_t t0, uint32
     st_shared_v4(t0 + off, h[0], h[1], h[2], h[3]);
     st_shared_v4(t1 + off, l[0], l[1], l[2], l[3]);
 }
+// a value every lane of the warp holds, broadcast from lane 0 so that ptxas can prove it warp-uniform: a wgmma under
+// a branch it cannot prove uniform is serialised
+template <typename T> __device__ __forceinline__ T uniform(T v) {
+    return (T)__shfl_sync(0xffffffffu, (int)v, 0);
+}
 // 2^e as a float, e in [-126, 127]
 __device__ __forceinline__ float pow2i(int e) { return __uint_as_float((uint32_t)(127 + e) << 23); }
+
+// the products of one record: acc (+)= A[K-chunk] W^T as W_hi A_hi + W_hi A_lo + W_lo A_hi (+ W_lo A_lo), four K=16
+// slabs each, in that order (first: the first product overwrites the accumulator; on = 0: none)
+template <int NREG, bool QUAD>
+__device__ __forceinline__ void mma_record(float (&acc)[NREG], uint32_t a_hi, uint32_t a_lo, uint32_t w_hi, uint32_t w_lo,
+                                           bool first, uint32_t on) {
+    const uint64_t ah = wgmma_desc(a_hi), al = wgmma_desc(a_lo), bh = wgmma_desc(w_hi), bl = wgmma_desc(w_lo);
+    auto mma = [&](uint64_t a, uint64_t b, uint32_t sd) {
+        if constexpr (NREG == 32) wgmma_f16_n64(acc, a, b, sd, on);
+        else wgmma_f16_n48(acc, a, b, sd, on);
+    };
+    uint32_t sd = first ? 0u : 1u;
+#pragma unroll
+    for (int s = 0; s < 4; ++s) { mma(ah + 2 * s, bh + 2 * s, sd); sd = 1u; }
+#pragma unroll
+    for (int s = 0; s < 4; ++s) mma(al + 2 * s, bh + 2 * s, 1u);
+#pragma unroll
+    for (int s = 0; s < 4; ++s) mma(ah + 2 * s, bl + 2 * s, 1u);
+    if constexpr (QUAD) {
+#pragma unroll
+        for (int s = 0; s < 4; ++s) mma(al + 2 * s, bl + 2 * s, 1u);
+    }
+}
 
 // SAMPLE = false: density direction (Flow.inverse of every layer: x -> z, core.py:70-85).
 // SAMPLE = true : sampling direction of coupling-layer stacks (Flow.forward: z -> x, core.py:40-55): the unit is
 //   still "LU map, then spline block" -- the packer hands it the INVERSE LU map of the previous layer -- but the
 //   unconditional spline runs first and in its inverse branch, the conditioner sees its result, and the
 //   conditional spline is inverted (Coupling.inverse, neural_spline/coupling.py:100-128).
-// (The CTA-pair / cta_group::2 schedule of round 2a was measured 2-3 % slower and removed: profiles/r02_pair_vs_single.md;
-//  so were "mixed" hi|lo weight records and a byte-granular ring: profiles/r02b_ring_experiments.md.)
-// PROF = true: clock64 stamps of CTA 0's first unit (nfb_debug_profile); compiled out of the production instantiation --
-//   the MMA issuer's per-record sequence is on the critical path of every GEMM phase.
-template <bool SAMPLE, bool PROF>
+template <bool SAMPLE>
 __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const FusedParams p) {
     extern __shared__ __align__(1024) uint8_t smem[];
     const uint32_t sbase = smem_u32(smem);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = uniform((int)(threadIdx.x >> 5)), lane = threadIdx.x & 31;
     float* xs = reinterpret_cast<float*>(smem + kOffX);
-    const uint32_t bars = sbase + kOffBars;
     float* ldsum = reinterpret_cast<float*>(smem + kOffMisc);
-    float* rowmax = reinterpret_cast<float*>(smem + kOffRowMax);
+    int* rowexp = reinterpret_cast<int*>(smem + kOffMisc + 3 * kRows * 4);
+    float* rowmax = reinterpret_cast<float*>(smem + kOffStg);  // (the staging tiles are free while a tile is loaded)
+    const uint32_t bars = sbase + kOffBars;
     auto bar = [bars](int i) { return bars + 8u * i; };
 
     if ((sbase & 1023u) != 0) {
@@ -134,62 +161,41 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
     if (threadIdx.x == 0) {
         for (int i = 0; i < (int)kSlots; ++i) {
             mbar_init(bar(kBarWFull + i), 1);
-            mbar_init(bar(kBarWEmpty + i), 1);
+            mbar_init(bar(kBarWEmpty + i), 2);   // one arrival per consumer warpgroup
         }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(bar(kBarCFull + i), 1);
-            mbar_init(bar(kBarCEmpty + i), kEpiWarps);
-        }
-        for (int i = 0; i < 4; ++i) mbar_init(bar(kBarAReady + i), kEpiWarps);
-        mbar_init(bar(kBarAccFull), 1);
-        mbar_init(bar(kBarLuFull), 1);
-        for (int i = 0; i < 3; ++i) mbar_init(bar(kBarAccBlk + i), 1);
         for (int i = 0; i < 4; ++i) mbar_init(bar(kBarUnit + i), 1);
         fence_mbar_init();
     }
-    if (warp == kEpiWarps + 1) {
-        tmem_alloc(sbase + kOffTmemPtr, 512);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *reinterpret_cast<volatile uint32_t*>(smem + kOffTmemPtr);
 
-    const long long n_tiles = (p.rows + 127) / 128;
-    // Unit index -> (layer, tile).  Default: layer-major.  Host batch in flight (wave_order): the tiles are split into
-    // groups in arrival order and the (layer, group) elements are walked DIAGONALLY -- (l, g) sorted by l + g, then g -- so
-    // that the first groups move through the layers while the later groups' rows are still on the PCIe bus; every element
-    // still comes after (l - 1, g), so claiming in increasing order stays deadlock-free.  wave_order[2 e] = layer |
-    // group << 8, wave_order[2 e + 1] = first unit index of element e; each role walks it with its own cursor (the units
-    // a role sees are increasing).  Every unit is a real tile -- an empty unit would let the producer lap the unit queue.
-    const long long n_units = n_tiles * p.n_layers;
-    auto decode = [&](long long u, int& cursor, int& layer, long long& tile) {
-        if (!p.wave_order) {
-            layer = (int)(u / n_tiles);
-            tile = u - (long long)layer * n_tiles;
-            return;
-        }
-        while (cursor + 1 < p.wave_elems && u >= (long long)__ldg(p.wave_order + 2 * (cursor + 1) + 1)) ++cursor;
-        const uint32_t w = __ldg(p.wave_order + 2 * cursor);
-        layer = (int)(w & 0xffu);
-        tile = (long long)(w >> 8) * p.wave_tpg + (u - (long long)__ldg(p.wave_order + 2 * cursor + 1));
-    };
-    // Which unit a CTA works on next is decided by its producer warp and handed to the MMA issuer and the epilogue warps
-    // through a 4-deep queue in shared memory.  With a ticket counter (whole-stack launches) units are CLAIMED in
-    // increasing order from a global atomic: a unit's dependency (layer - 1, same tile) has a smaller index, so it was
-    // claimed earlier by a CTA that is running -- no co-residency of the whole grid is assumed (ADVICE r1: with the static
-    // b, b + grid, ... assignment a CTA that never gets scheduled would starve the others), and faster CTAs take more
-    // units.  Without a counter (single-layer launches: no dependencies) the static assignment is used.
-    volatile int* unit_q = reinterpret_cast<volatile int*>(smem + kOffUnitQ);
-    auto next_unit = [&](uint32_t i) -> long long {   // consumer side: the i-th unit of this CTA, -1 = no more
-        mbar_wait(bar(kBarUnit + (i & 3u)), (i >> 2) & 1u, p.err, 600 + (int)(i & 3u));
-        return (long long)unit_q[i & 3u];
-    };
-
-    // Warp roles: the SM arbiter favours high warp ids, so the two latency-critical single-lane roles
-    // (TMA producer, MMA issuer) sit above the epilogue warps (0..kEpiWarps-1).
-    if (warp == kEpiWarps) {
+    volatile int* unit_q = reinterpret_cast<volatile int*>(smem + kOffUnitQ);   // [4][layer, tile]
+    if (warp >= kCons / 32) {
+        setmaxnreg_dec<kProducerRegs>();
+        if (warp != kCons / 32) return;
+        const long long n_tiles = (p.rows + kRows - 1) / kRows;
+        // Unit index -> (layer, tile).  Default: layer-major.  Host batch in flight (wave_order): the tiles are split into
+        // groups in arrival order and the (layer, group) elements are walked DIAGONALLY -- (l, g) sorted by l + g, then g -- so
+        // that the first groups move through the layers while the later groups' rows are still on the PCIe bus; every element
+        // still comes after (l - 1, g), so claiming in increasing order stays deadlock-free.  wave_order[2 e] = layer |
+        // group << 8, wave_order[2 e + 1] = first unit index of element e; each role walks it with its own cursor (the units
+        // a role sees are increasing).  Every unit is a real tile -- an empty unit would let the producer lap the unit queue.
+        const long long n_units = n_tiles * p.n_layers;
+        auto decode = [&](long long u, int& cursor, int& layer, long long& tile) {
+            if (!p.wave_order) {
+                layer = (int)(u / n_tiles);
+                tile = u - (long long)layer * n_tiles;
+                return;
+            }
+            while (cursor + 1 < p.wave_elems && u >= (long long)__ldg(p.wave_order + 2 * (cursor + 1) + 1)) ++cursor;
+            const uint32_t w = __ldg(p.wave_order + 2 * cursor);
+            layer = (int)(w & 0xffu);
+            tile = (long long)(w >> 8) * p.wave_tpg + (u - (long long)__ldg(p.wave_order + 2 * cursor + 1));
+        };
+        // Which unit a CTA works on next is decided by its producer warp and handed to the consumers, decoded to (layer,
+        // tile), through a 4-deep queue in shared memory.  With a ticket counter (whole-stack launches) units are CLAIMED in increasing order from a global
+        // atomic: a unit's dependency (layer - 1, same tile) has a smaller index, so it was claimed earlier by a CTA that is
+        // running -- no co-residency of the whole grid is assumed, and faster CTAs take more units.  Without a counter
+        // (single-layer launches: no dependencies) the static assignment is used.
         // ------------------------------ weight producer -----------------------------------
         // whole warp walks the table (warp-uniform control flow); one elected lane issues the copy
         uint32_t slot = 0, par = 0;
@@ -204,20 +210,21 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
                 u = (long long)blockIdx.x + (long long)ui * gridDim.x;
             }
             const bool more = u < n_units;
+            int ulayer = -1;
+            long long utile = 0;
+            if (more) decode(u, wcur, ulayer, utile);
             if (lane == 0) {
-                unit_q[ui & 3u] = more ? (int)u : -1;
+                unit_q[2 * (ui & 3u)] = ulayer;
+                unit_q[2 * (ui & 3u) + 1] = (int)utile;
                 mbar_arrive(bar(kBarUnit + (ui & 3u)));   // (release: the queue entry is visible to whoever passes the wait)
             }
             __syncwarp();
             if (!more) break;
-            int ulayer;
-            long long utile;
-            decode(u, wcur, ulayer, utile);
             const FusedLayer& L = p.layers[ulayer];
-            const FusedStep* steps = L.steps;  // global (L2-resident); the producer only needs the size
+            const FusedStep* steps = L.steps;  // global (L2-resident)
             const int n_steps = L.n_steps;
-            // autoregressive sampling (SAMPLE, ar_passes = D): the LU records are streamed once, the block's D times
-            const int lu_steps = L.has_lu ? 1 : 0;  // (hi and lo tile of the LU map travel as one record)
+            // autoregressive sampling (SAMPLE, ar_passes = D): the LU record is streamed once, the block's D times
+            const int lu_steps = L.has_lu ? 1 : 0;
             const int reps = (SAMPLE && L.ar_passes > 0) ? L.ar_passes : 1;
             const int total = n_steps ? lu_steps + reps * (n_steps - lu_steps) : 0;
             const uint32_t lu_bytes = L.has_lu ? 2u * 8192u : 0u;
@@ -241,330 +248,251 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
                 if (++slot == kSlots) { slot = 0; par ^= 1; }
             }
         }
-    } else if (warp == kEpiWarps + 1) {
-        // ------------------------------ MMA issuer ----------------------------------------
-        // Warp-uniform loop; the MMAs of one weight record are issued by one elected lane from
-        // descriptors that differ only by an add on the 14-bit address field (16-byte units).
-        uint32_t slot = 0, wpar = 0, apar = 0, cebits = 0;
-        const uint64_t adesc0 = umma_desc_sw128(sbase + kOffA);
-        const uint64_t bdesc0 = umma_desc_sw128(sbase + kOffW);
-        constexpr uint32_t kIdesc0 = umma_idesc_f16(128, 0);
-        int wcur = 0;
-        for (uint32_t ui = 0;; ++ui) {
-            const long long u = next_unit(ui);
-            if (u < 0) break;
-            const bool prof_unit = PROF && p.prof && ui == 0 && blockIdx.x == 0;
-            int ulayer;
-            long long utile;
-            decode(u, wcur, ulayer, utile);
-            const FusedLayer& L = p.layers[ulayer];
-            const uint4* steps = reinterpret_cast<const uint4*>(L.steps);  // 16-byte entries, L2-resident
-            const int n_steps = L.n_steps;
-            const int lu_steps = L.has_lu ? 1 : 0;  // (hi and lo tile of the LU map travel as one record)
-            const int reps = (SAMPLE && L.ar_passes > 0) ? L.ar_passes : 1;
-            const int total = n_steps ? lu_steps + reps * (n_steps - lu_steps) : 0;
-            union { uint4 raw; FusedStep s; } cur, nx;
-            cur.raw = __ldg(steps);
-            int sidx = 0;
-            for (int s = 0; s < total; ++s) {
+        return;
+    }
+
+    // ------------------------------ consumer warpgroups -----------------------------------
+    setmaxnreg_inc<kConsumerRegs>();
+    const int et = threadIdx.x;                    // 0..255
+    const int wg = uniform(et >> 7);               // consumer warpgroup
+    const int wl = warp & 3;                       // warp within the warpgroup
+    const int ra = 16 * wl + (lane >> 2);          // accumulator rows of this thread: ra, ra + 8
+    const int rb = ra + 8;
+    const int cq = 2 * (lane & 3);                 // first of its two columns in every 8-column group
+    const uint32_t aA = sbase;                     // the A operand
+    const uint32_t skip_bit = wg ? kStepSkip1 : kStepSkip0;
+    float* stg = reinterpret_cast<float*>(smem + kOffStg + wg * kStgBytes);
+    uint32_t slot = 0, wpar = 0;
+
+    for (uint32_t ui = 0;; ++ui) {
+        mbar_wait(bar(kBarUnit + (ui & 3u)), (ui >> 2) & 1u, p.err, 600 + (int)(ui & 3u));
+        const int layer = uniform(unit_q[2 * (ui & 3u)]);
+        const long long tile = uniform(unit_q[2 * (ui & 3u) + 1]);
+        if (layer < 0) break;
+        const FusedLayer& L = p.layers[layer];
+        const int D = L.D, ns = uniform(L.H >> 6), half = (ns + 1) >> 1;
+        const int n_steps = uniform(L.n_steps), lu_steps = uniform(L.has_lu ? 1 : 0);
+        const int n_hidden = uniform(L.n_hidden), n_pairs = uniform(L.n_chunks >> 1);
+        int sidx = 0;
+        // The records of one output slice (until the one flagged last): this warpgroup's half of each goes into acc
+        // (live: the warpgroup has a slice here; a record's skip bit: its half is all zero).  Every record is waited
+        // for and handed back by both warpgroups; a slot is handed back as soon as the products that read it have
+        // completed (an empty wgmma group stands in for a skipped half, so the group count stays uniform).
+        auto run_slice = [&](auto& acc, bool live, auto quad) {
+            int prev = -1;
+            for (;;) {
+                union { uint2 raw; FusedStep s; } st;
+                st.raw = __ldg(reinterpret_cast<const uint2*>(L.steps) + sidx);
+                st.raw.x = uniform(st.raw.x);
+                st.raw.y = uniform(st.raw.y);
                 sidx = sidx + 1 == n_steps ? lu_steps : sidx + 1;
-                nx.raw = __ldg(steps + sidx);  // prefetch one entry ahead (wraps to the block's first step)
-                const FusedStep st = cur.s;
-                const uint32_t ctl = st.ctl;
-                if (prof_unit && s < 380 && lane == 0) p.prof[512 + s] = clock64();  // debug: step reached
-                const uint32_t wcode = (ctl >> 10) & 7u, scode = (ctl >> 13) & 7u;
-                if (wcode == 1 || wcode == 5 || wcode == 6) {  // first use of A-operand K-chunk kc in this phase
-                    // (code 5: the LAST K-chunk of the final layer's A operand, whatever chunk the record itself reads)
-                    const uint32_t kc = wcode == 5 ? (uint32_t)(L.H >> 6) - 1u : st.a0 & 3u;
-                    mbar_wait(bar(kBarAReady + kc), (apar >> kc) & 1u, p.err, 200 + kc);
-                    apar ^= 1u << kc;
-                }
-                if (wcode >= 2) {
-                    const uint32_t i = wcode == 6 ? 1u : (wcode == 5 ? 0u : wcode - 2);  // processing slot 0 uses buffer 1
-                    mbar_wait(bar(kBarCEmpty + i), ((cebits >> i) & 1u) ^ 1u, p.err, 210 + i);
-                    cebits ^= 1u << i;
-                }
-                if (prof_unit && s < 380 && lane == 0) p.prof[896 + s] = clock64();  // debug: operands (A / chunk) ready
                 mbar_wait(bar(kBarWFull + slot), wpar, p.err, 220 + slot);
-                tc_fence_after();
-                if (prof_unit && s < 380 && lane == 0) p.prof[128 + s] = clock64();  // debug: issue time
-                if (elect_one_sync()) {
-                    const uint32_t d = tmem + (ctl & 511u);
-                    const uint64_t bd = bdesc0 + (uint64_t)(slot * (kSlotBytes >> 4));
-                    uint32_t accum = ((ctl >> 9) & 1u) ^ 1u;
-                    // Per K=16 slab s the record's rows [8 dr[s], 8 n8) are multiplied (block-triangular MADE matrices: a
-                    // later slab reaches fewer rows; dr = 0xFF: no row at all): D columns, B rows and the MMA's N shift
-                    // together.  (Unmasked nets: dr = 0 everywhere.)
-                    uint32_t dcol[4], nsl[4];
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const uint32_t dr = st.dr[j];
-                        dcol[j] = dr == 0xFFu ? 0xFFFFFFFFu : dr * 8u;
-                        nsl[j] = kIdesc0 | (((uint32_t)st.n8 - (dr == 0xFFu ? 0u : dr)) << 17);
-                    }
-                    // A tile t < 4: hi part of K-chunk t; 4 + t: lo part.  Four K=16 slabs per tile.
-                    auto issue4 = [&](uint32_t code, uint64_t b) {
-                        const uint64_t ad = adesc0 + (uint64_t)(code * (kTileA >> 4));
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            if (dcol[j] != 0xFFFFFFFFu) {
-                                // 8 dr rows of the [N x 64] SW128 tile = dr KB = 64 dr descriptor units
-                                umma_bf16(d + dcol[j], ad + 2 * j, b + 2 * j + (uint64_t)(dcol[j] * 8u), nsl[j], accum);
-                                accum = 1u;
-                            }
-                        }
-                    };
-                    issue4(st.a0, bd);                       // W_hi tile x A tiles a0 (, a1)
-                    if (st.a1 != 0xFF) issue4(st.a1, bd);
-                    if (st.a2 != 0xFF) {                     // merged record: the W_lo tile follows the W_hi tile
-                        const uint64_t bd2 = bd + (uint64_t)st.n8 * 64u;   // n8 * 8 rows * 128 B, in 16-byte units
-                        issue4(st.a2 & 7u, bd2);
-                        if (st.a2 & 0x80u) issue4((st.a2 & 7u) + 4u, bd2);   // (LU map: all four terms)
-                    }
-                    if (prof_unit && s < 380) p.prof[1280 + s] = clock64();  // debug: MMAs of this record issued
-                    umma_commit(bar(kBarWEmpty + slot));
-                    if (scode == 1) umma_commit(bar(kBarAccFull));
-                    else if (scode == 7) umma_commit(bar(kBarLuFull));
-                    else if (scode >= 4) umma_commit(bar(kBarAccBlk + (scode - 4)));
-                    else if (scode >= 2) umma_commit(bar(kBarCFull + (scode - 2)));
-                    if (prof_unit && s < 380) p.prof[1664 + s] = clock64();  // debug: commits issued
-                }
-                __syncwarp();
+                const uint32_t w = sbase + kOffW + slot * kSlotBytes + (uint32_t)wg * st.s.n8 * 1024u;
+                const uint32_t kc = st.s.kc;
+                wgmma_fence();
+                mma_record<sizeof(acc) / sizeof(float), decltype(quad)::value>(
+                    acc, aA + kc * kTileA, aA + (4 + kc) * kTileA, w, w + ((uint32_t)st.s.bytes16 << 3),
+                    (st.s.flags & kStepFirst) != 0, (uint32_t)(live && !(st.s.flags & skip_bit)));
+                wgmma_commit();
+                wgmma_wait<1>();   // the previous record's products are complete: hand its slot back
+                mbar_arrive_if(bar(kBarWEmpty + (prev < 0 ? 0 : prev)), prev >= 0 && (et & 127) == 0);
+                prev = (int)slot;
                 if (++slot == kSlots) { slot = 0; wpar ^= 1; }
-                cur.raw = nx.raw;
+                if (st.s.flags & kStepLast) break;
+            }
+            wgmma_wait<0>();
+            wgmma_hold(acc);
+            mbar_arrive_if(bar(kBarWEmpty + prev), (et & 127) == 0);
+        };
+        using NoQuad = std::integral_constant<bool, false>;
+
+        // layers >= 1 update z in place (z_stride = 0) or, for the training pass, every layer writes its own
+        // buffer zout + layer * z_stride so that the backward finds each layer's input
+        float* zdst = p.zout + (long long)layer * p.z_stride;
+        const float* zsrc = layer == 0 ? p.zin : p.zout + (long long)(layer - 1) * p.z_stride;
+        const long long row0 = tile * kRows;
+        const int r = et & (kRows - 1);           // row of the per-row work (splines, log-det) of this thread
+        const int rq = et >> 6;                   // ... and its quarter of the 256 threads
+        const long long grow = row0 + r;
+        const bool row_live = grow < p.rows;
+
+        // ---- layer-to-layer dependency: this tile's rows must have left layer-1 (any CTA) ----
+        if (layer > 0) {
+            if (lane == 0) {  // one lane per warp spins (keeps the warp converged for the .aligned ops below)
+                const int* flag = p.progress + tile;
+                int seen;
+                const long long t0 = clock64();
+                do {
+                    asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(seen) : "l"(flag) : "memory");
+                    if (seen < layer && clock64() - t0 > 4000000000LL) fail_timeout(p.err, 500);
+                } while (seen < layer);
+            }
+            __syncwarp();
+            {   // every thread performs its own acquire of the (now set) flag before touching the rows
+                int seen;
+                asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(seen) : "l"(p.progress + tile) : "memory");
+                if (seen < layer) fail_timeout(p.err, 501);
             }
         }
-    } else {
-        // ------------------------------ epilogue warps ------------------------------------
-        const int et = threadIdx.x;            // 0..kEpiThreads-1
-        const int q = warp & 3;                // TMEM lane quadrant this warp may touch
-        const int wh = warp >> 2;              // column group 0..kNG-1
-        const int r = q * 32 + lane;           // tile row owned by this thread
-        const uint32_t tlane = tmem + ((uint32_t)(q * 32) << 16);
-        const uint32_t aA = sbase + kOffA;
-        uint32_t afpar = 0, lupar = 0, cfbits = 0, blkpar = 0;
-        // epilogue-side waits: every thread polls (default; measured 3-4 % faster than one polling lane per warp)
-        auto ewait = [&](uint32_t b, uint32_t parity, int tag) {
-            if (p.poll_all) mbar_wait(b, parity, p.err, tag);
-            else mbar_wait_warp(b, parity, p.err, tag);
-        };
-        long long* prof = (PROF && p.prof && blockIdx.x == 0 && et == 0) ? p.prof : nullptr;
-        int pi = 0;
-#define NFB_STAMP() do { if (PROF && prof && pi < 126) prof[pi++] = clock64(); } while (0)
-
-        int wcur = 0;
-        for (uint32_t ui = 0;; ++ui) {
-            const long long u = next_unit(ui);
-            if (u < 0) break;
-            int layer;
-            long long tile;
-            decode(u, wcur, layer, tile);
-            const FusedLayer& L = p.layers[layer];
-            const int D = L.D, H = L.H;
-            // layers >= 1 update z in place (z_stride = 0) or, for the training pass, every layer writes its own
-            // buffer zout + layer * z_stride so that the backward finds each layer's input
-            float* zdst = p.zout + (long long)layer * p.z_stride;
-            const float* zsrc = layer == 0 ? p.zin : p.zout + (long long)(layer - 1) * p.z_stride;
-            const long long row0 = tile * 128;
-            const long long grow = row0 + r;          // this thread's global row
-            const bool row_live = grow < p.rows;
-            if (ui != 0) prof = nullptr;
-            float ru = 1.f, ruinv = 1.f;  // this row's power-of-two unit (set after the tile load)
-
-            // ---- layer-to-layer dependency: this tile's rows must have left layer-1 (any CTA) ----
-            if (layer > 0) {
-                if (lane == 0) {  // one lane per warp spins (keeps the warp converged for the .aligned ops below)
-                    const int* flag = p.progress + tile;
-                    int seen;
-                    const long long t0 = clock64();
-                    do {
-                        asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(seen) : "l"(flag) : "memory");
-                        if (seen < layer && clock64() - t0 > 4000000000LL) {
-                            if (p.err) atomicExch(p.err, 500);
-                            asm volatile("trap;");
-                        }
-                    } while (seen < layer);
-                }
-                __syncwarp();
-                {   // every thread performs its own acquire of the (now set) flag before touching the rows
-                    int seen;
-                    asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(seen) : "l"(p.progress + tile) : "memory");
-                    if (seen < layer) { if (p.err) atomicExch(p.err, 501); asm volatile("trap;"); }
-                }
-            }
-            // ---- host batch still in flight (nfb_api.cu h2d_prepare / h2d_copies): layer-0 tiles wait for their rows ----
-            if (layer == 0 && p.in_ready) {
-                const int need = (int)min(row0 + 128, p.rows);
-                if (lane == 0) {
-                    int seen;
-                    const long long t0 = clock64();
-                    do {
-                        asm volatile("ld.acquire.sys.global.s32 %0, [%1];" : "=r"(seen) : "l"(p.in_ready) : "memory");
-                        if (seen < need && clock64() - t0 > 20000000000LL) {  // ~10 s: the copy never came
-                            if (p.err) atomicExch(p.err, 510);
-                            asm volatile("trap;");
-                        }
-                    } while (seen < need);
-                }
-                __syncwarp();
-                {   // every thread acquires the (now sufficient) counter itself before reading the rows
-                    int seen;
+        // ---- host batch still in flight (nfb_api.cu h2d_prepare / h2d_copies): layer-0 tiles wait for their rows ----
+        if (layer == 0 && p.in_ready) {
+            const int need = (int)min(row0 + kRows, p.rows);
+            if (lane == 0) {
+                int seen;
+                const long long t0 = clock64();
+                do {
                     asm volatile("ld.acquire.sys.global.s32 %0, [%1];" : "=r"(seen) : "l"(p.in_ready) : "memory");
-                    if (seen < need) { if (p.err) atomicExch(p.err, 511); asm volatile("trap;"); }
+                    if (seen < need && clock64() - t0 > 20000000000LL) fail_timeout(p.err, 510);  // ~10 s: no copy
+                } while (seen < need);
+            }
+            __syncwarp();
+            {   // every thread acquires the (now sufficient) counter itself before reading the rows
+                int seen;
+                asm volatile("ld.acquire.sys.global.s32 %0, [%1];" : "=r"(seen) : "l"(p.in_ready) : "memory");
+                if (seen < need) fail_timeout(p.err, 511);
+            }
+        }
+        // this row's running log_q (only this tile's units touch it): fetched now, used at the end of the unit
+        float lq_old = 0.f;
+        if (rq == 0 && row_live && (layer > 0 || p.accumulate)) lq_old = __ldcg(p.logq + grow);
+        // ---- load z tile -> xs (coalesced global, swizzled shared) ----
+        if (D == 64) {
+            float4 v[kRows * 16 / kCons];
+#pragma unroll
+            for (int k = 0; k < kRows * 16 / kCons; ++k) {
+                const int i4 = et + k * kCons, rr = i4 >> 4;
+                const long long gr = row0 + rr;
+                v[k] = gr < p.rows ? __ldcg(reinterpret_cast<const float4*>(zsrc + gr * 64) + (i4 & 15))
+                                   : make_float4(0.f, 0.f, 0.f, 0.f);
+            }
+#pragma unroll
+            for (int k = 0; k < kRows * 16 / kCons; ++k) {
+                const int i4 = et + k * kCons, rr = i4 >> 4, c0 = (i4 & 15) * 4;
+                xs[xs_index(rr, c0)] = v[k].x;
+                xs[xs_index(rr, c0 + 1)] = v[k].y;
+                xs[xs_index(rr, c0 + 2)] = v[k].z;
+                xs[xs_index(rr, c0 + 3)] = v[k].w;
+                // max |z| of row rr: its 64 values sit in the 16 consecutive lanes of this half-warp
+                float m = fmaxf(fmaxf(fabsf(v[k].x), fabsf(v[k].y)), fmaxf(fabsf(v[k].z), fabsf(v[k].w)));
+                m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+                m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+                m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
+                m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 8));
+                if ((et & 15) == 0) rowmax[rr] = m;
+            }
+        } else {
+            for (int i = et; i < kRows * D; i += kCons) {
+                const int rr = i / D, cc = i - rr * D;
+                const long long gr = row0 + rr;
+                xs[xs_index(rr, cc)] = gr < p.rows ? __ldcg(zsrc + gr * D + cc) : 0.f;
+            }
+        }
+        cons_bar_sync();
+        // Row unit u = 2^-e, e = clamp(floor(log2 max|x_row|) + 1, 0, 40): |x| u < 1 for every input of the row, so every
+        // fp16 operand of this unit stays inside the static bounds the packer derived (nfb_api.cu plan_scales) whatever
+        // the magnitude of the data; u = 1 for ordinary rows (|x| < 1 .. 2).
+        auto set_row_exp = [&](float zmax) {
+            int e = (int)((__float_as_uint(zmax) >> 23) & 0xffu) - 126;
+            rowexp[r] = max(0, min(40, e));
+        };
+        if (rq == 0) {
+            float zmax = 0.f;
+            if (D == 64) zmax = rowmax[r];
+            else
+                for (int c = 0; c < D; ++c) zmax = fmaxf(zmax, fabsf(xs[xs_index(r, c)]));
+            set_row_exp(zmax);
+        }
+        cons_bar_sync();
+        auto ru = [&](int row) { return pow2i(-rowexp[row]); };
+        auto ruinv = [&](int row) { return pow2i(rowexp[row]); };
+        auto get_x = [&](int c) -> float { return xs[xs_index(r, c)]; };
+        auto put_y = [&](int c, float y) { xs[xs_index(r, c)] = y; };
+        // A[:, 0:64] (K-chunk 0): fp16 hi/lo split of value(row, k) * u_row * sc; thread = (row, quarter of k)
+        const int ar = et >> 2, aq = et & 3;
+        auto store_a = [&](auto value, float sc_base) {
+            const float sc = sc_base * ru(ar);
+            float v[16];
+#pragma unroll
+            for (int j = 0; j < 16; ++j) v[j] = value(aq * 16 + j) * sc;
+#pragma unroll
+            for (int g = 0; g < 2; ++g) split_store8(v + 8 * g, aA, aA + 4 * kTileA, a_chunk_off(ar, 2 * aq + g));
+            fence_proxy_async_smem();
+            cons_bar_sync();
+        };
+        // conditioner input: column in_idx[k] of the (LU-transformed) row
+        auto build_a_net = [&]() {
+            store_a([&](int k) {
+                const int c = L.in_idx[k];
+                return c >= 0 ? xs[xs_index(ar, c)] : 0.f;
+            }, L.a_sc[1]);
+        };
+        float ladsum = 0.f;
+        // fold_lu (density direction): the packer multiplied the first conditioner matrix into the LU map, so the first
+        // hidden GEMM reads the SAME A operand as the LU stage (the split of z)
+        const bool folded = uniform(!SAMPLE && L.has_lu && L.fold_lu);
+        if (lu_steps) {
+            store_a([&](int k) { return k < D ? xs[xs_index(ar, k)] : 0.f; }, L.a_sc[0]);
+            float acc[32];
+            run_slice(acc, wg == 0, std::integral_constant<bool, true>());   // (no half for warpgroup 1)
+            if (wg == 0) {
+                // x' = acc + b (this thread: rows ra / rb, two columns of every 8-column group)
+                const float ia = L.a_inv[0] * ruinv(ra), ib = L.a_inv[0] * ruinv(rb);
+#pragma unroll
+                for (int i = 0; i < 32; ++i) {
+                    const int c = 8 * (i >> 2) + cq + (i & 1);
+                    const int rr = (i & 2) ? rb : ra;
+                    if (c < D) xs[xs_index(rr, c)] = fmaf(acc[i], (i & 2) ? ib : ia, __ldg(L.bias_lu + c));
                 }
             }
-            NFB_STAMP();  // [0] tile start
-            // this row's running log_q (only this tile's units touch it): fetched now, used at the end of the unit
-            float lq_old = 0.f;
-            if (wh == 0 && row_live && (layer > 0 || p.accumulate)) lq_old = __ldcg(p.logq + grow);
-            // ---- load z tile -> xs (coalesced global, swizzled shared) ----
+            cons_bar_sync();   // x' of the whole tile is visible to both warpgroups
+        }
+        auto store_tile = [&]() {  // xs -> global, coalesced
             if (D == 64) {
-                float4 v[2048 / kEpiThreads];
 #pragma unroll
-                for (int k = 0; k < 2048 / kEpiThreads; ++k) {
-                    const int i4 = et + k * kEpiThreads, rr = i4 >> 4;
+                for (int k = 0; k < kRows * 16 / kCons; ++k) {
+                    const int i4 = et + k * kCons, rr = i4 >> 4, c0 = (i4 & 15) * 4;
                     const long long gr = row0 + rr;
-                    v[k] = gr < p.rows ? __ldcg(reinterpret_cast<const float4*>(zsrc + gr * 64) + (i4 & 15))
-                                       : make_float4(0.f, 0.f, 0.f, 0.f);
-                }
-#pragma unroll
-                for (int k = 0; k < 2048 / kEpiThreads; ++k) {
-                    const int i4 = et + k * kEpiThreads, rr = i4 >> 4, c0 = (i4 & 15) * 4;
-                    xs[xs_index(rr, c0)] = v[k].x;
-                    xs[xs_index(rr, c0 + 1)] = v[k].y;
-                    xs[xs_index(rr, c0 + 2)] = v[k].z;
-                    xs[xs_index(rr, c0 + 3)] = v[k].w;
-                    // max |z| of row rr: its 64 values sit in the 16 consecutive lanes of this half-warp
-                    float m = fmaxf(fmaxf(fabsf(v[k].x), fabsf(v[k].y)), fmaxf(fabsf(v[k].z), fabsf(v[k].w)));
-                    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
-                    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
-                    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
-                    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 8));
-                    if ((et & 15) == 0) rowmax[rr] = m;
+                    const float4 v = make_float4(xs[xs_index(rr, c0)], xs[xs_index(rr, c0 + 1)],
+                                                 xs[xs_index(rr, c0 + 2)], xs[xs_index(rr, c0 + 3)]);
+                    if (gr < p.rows) __stcg(reinterpret_cast<float4*>(zdst + gr * 64) + (i4 & 15), v);
                 }
             } else {
-                for (int i = et; i < 128 * D; i += kEpiThreads) {
+                for (int i = et; i < kRows * D; i += kCons) {
                     const int rr = i / D, cc = i - rr * D;
                     const long long gr = row0 + rr;
-                    xs[xs_index(rr, cc)] = gr < p.rows ? __ldcg(zsrc + gr * D + cc) : 0.f;
+                    if (gr < p.rows) __stcg(zdst + gr * D + cc, xs[xs_index(rr, cc)]);
                 }
             }
-            epi_bar_sync();
-            {   // Row unit u = 2^-e, e = clamp(floor(log2 max|x_row|) + 1, 0, 40): |x| u < 1 for every input of the
-                // row, so every fp16 operand of this unit stays inside the static bounds the packer derived
-                // (nfb_api.cu plan_scales) whatever the magnitude of the data; u = 1 for ordinary rows (|x| < 1 .. 2).
-                float zmax = 0.f;
-                if (D == 64) zmax = rowmax[r];
-                else
-                    for (int c = 0; c < D; ++c) zmax = fmaxf(zmax, fabsf(xs[xs_index(r, c)]));
-                int e = (int)((__float_as_uint(zmax) >> 23) & 0xffu) - 126;
-                e = max(0, min(40, e));
-                ru = pow2i(-e);
-                ruinv = pow2i(e);
-            }
-            NFB_STAMP();  // [1] load done
-            auto get_x = [&](int c) -> float { return xs[xs_index(r, c)]; };
-            auto put_y = [&](int c, float y) { xs[xs_index(r, c)] = y; };
-            // A[:, k] for k in [wh*kGC, (wh+1)*kGC): fp16 hi/lo split of v[k], in units of u * a_sc
-            auto store_a = [&](const float* v) {
-    #pragma unroll
-                for (int g = 0; g < kGC / 8; ++g) split_store8(v + 8 * g, aA, aA + 4 * kTileA, a_chunk_off(r, wh * (kGC / 8) + g));
-                fence_proxy_async_smem();
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(bar(kBarAReady + 0));
-            };
-            // conditioner input: column in_idx[k] of the (LU-transformed) row
-            auto build_a_net = [&]() {
-                const float sc = ru * L.a_sc[1];
-                float v[kGC];
-    #pragma unroll
-                for (int j = 0; j < kGC; ++j) {
-                    const int c = L.in_idx[wh * kGC + j];
-                    v[j] = c >= 0 ? get_x(c) * sc : 0.f;
-                }
-                store_a(v);
-            };
-            float ladsum = 0.f;
-            // fold_lu (density direction): the packer multiplied the first conditioner matrix into the LU map, so the
-            // first hidden GEMM reads the SAME A operand as the LU stage (the split of z) and both are in flight at once;
-            // the LU result is only needed as spline input and is collected while hidden GEMM 0 runs.
-            const bool folded = !SAMPLE && L.has_lu && L.fold_lu;
-            if (L.has_lu) {
-                {
-                    const float sc = ru * L.a_sc[0];
-                    float v[kGC];
-    #pragma unroll
-                    for (int j = 0; j < kGC; ++j) v[j] = wh * kGC + j < D ? xs[xs_index(r, wh * kGC + j)] * sc : 0.f;
-                    store_a(v);
-                }
-                NFB_STAMP();  // build_a(lu) done
-                ewait(bar(kBarLuFull), lupar, 300);
-                NFB_STAMP();  // LU gemm done
-                lupar ^= 1;
-                tc_fence_after();
-                // x' = acc + b  (64 columns at TMEM col 256; this thread: kGC of them)
-                uint32_t acc[kGC];
-                NFB_TMEM_LD16(tlane + 256 + wh * kGC, acc);
-                NFB_TMEM_WAIT16(acc);
-                // (this thread built the LU stage's A from exactly these elements of xs: no other reader to wait for)
-#pragma unroll
-                for (int j = 0; j < kGC; ++j) {
-                    const int c = wh * kGC + j;
-                    if (c < D) xs[xs_index(r, c)] = fmaf(__uint_as_float(acc[j]), L.a_inv[0] * ruinv, __ldg(L.bias_lu + c));
-                }
-                tc_fence_before();  // (folded: hidden GEMM 1 overwrites columns 256.. once every warp has passed epilogue 0)
-                epi_bar_sync();     // x' of the whole row is visible to the CTA
-            }
-            auto store_tile = [&]() {  // xs -> global, coalesced
-                if (D == 64) {
-#pragma unroll
-                    for (int k = 0; k < 2048 / kEpiThreads; ++k) {
-                        const int i4 = et + k * kEpiThreads, rr = i4 >> 4, c0 = (i4 & 15) * 4;
-                        const long long gr = row0 + rr;
-                        const float4 v = make_float4(xs[xs_index(rr, c0)], xs[xs_index(rr, c0 + 1)],
-                                                     xs[xs_index(rr, c0 + 2)], xs[xs_index(rr, c0 + 3)]);
-                        if (gr < p.rows) __stcg(reinterpret_cast<float4*>(zdst + gr * 64) + (i4 & 15), v);
-                    }
-                } else {
-                    for (int i = et; i < 128 * D; i += kEpiThreads) {
-                        const int rr = i / D, cc = i - rr * D;
-                        const long long gr = row0 + rr;
-                        if (gr < p.rows) __stcg(zdst + gr * D + cc, xs[xs_index(rr, cc)]);
-                    }
-                }
-            };
-            // ---- autoregressive block, sampling direction (flows/affine/autoregressive.py:29-38): D conditioner
-            // passes over a running output that starts at zero; every pass inverts the spline on the SAME input S
-            // (this tile after the LU stage) with parameters computed from the current output; after pass j the
-            // first j features are exact.  S is parked in this tile's rows of `zout` (L2) and read back per element,
-            // the running output lives in xs, and nothing else leaves the SM between passes.
-            const bool arsamp = SAMPLE && L.ar_passes > 0;
-            const int reps = arsamp ? L.ar_passes : 1;
-            if (arsamp) {
-                store_tile();
+        };
+        // ---- autoregressive block, sampling direction (flows/affine/autoregressive.py:29-38): D conditioner
+        // passes over a running output that starts at zero; every pass inverts the spline on the SAME input S
+        // (this tile after the LU stage) with parameters computed from the current output; after pass j the
+        // first j features are exact.  S is parked in this tile's rows of `zout` (L2) and read back per element,
+        // the running output lives in xs, and nothing else leaves the SM between passes.
+        const bool arsamp = uniform(SAMPLE && L.ar_passes > 0);
+        const int reps = uniform(arsamp ? L.ar_passes : 1);
+        if (arsamp) {
+            store_tile();
+            if (rq == 0) {
                 float zmax = L.tail;  // |output| <= max(|S|, tail): bound of every pass's conditioner input
                 for (int c = 0; c < D; ++c) zmax = fmaxf(zmax, fabsf(xs[xs_index(r, c)]));
-                int e = (int)((__float_as_uint(zmax) >> 23) & 0xffu) - 126;
-                e = max(0, min(40, e));
-                ru = pow2i(-e);
-                ruinv = pow2i(e);
-                epi_bar_sync();  // every thread has scanned its row; S is in L2 for every thread of the CTA
-                for (int i = et; i < 128 * 64; i += kEpiThreads) xs[i] = 0.f;
-                epi_bar_sync();
+                set_row_exp(zmax);
             }
-            for (int rep = 0; rep < reps; ++rep) {
+            cons_bar_sync();  // every row is scanned; S is in L2 for every thread of the CTA
+            for (int i = et; i < kRows * 64; i += kCons) xs[i] = 0.f;
+            cons_bar_sync();
+        }
+        for (int rep = 0; rep < reps; ++rep) {
             if (rep > 0) {
                 ladsum = 0.f;     // the log-det of the last pass is the layer's (autoregressive.py:36-38)
-                epi_bar_sync();   // the previous pass's outputs (all column groups) are in xs
+                cons_bar_sync();  // the previous pass's outputs (every thread's) are in xs
             }
             // ---- unconditional spline on the identity features (coupled layer only).
             // density: the conditioner input is taken from the RAW values first (Coupling.forward,
-            //   neural_spline/coupling.py:80-92) and the spline then runs while the tensor core is busy;
-            // sampling: the inverse spline comes first and the conditioner sees its output (:100-128).
+            //   neural_spline/coupling.py:80-92) and the spline then runs; sampling: the inverse spline comes first and
+            //   the conditioner sees its output (:100-128).
             auto uncond = [&]() {
-                const int per = (L.n_id + kNG - 1) / kNG;
-                for (int i = wh * per; i < min(L.n_id, (wh + 1) * per); ++i) {
+                for (int i = rq; i < L.n_id; i += kCons / kRows) {
                     const int c = L.id_idx[i];
                     const float* tb = L.uncond + i * 23;
                     auto acc = [tb](int k) { return __ldg(tb + k); };
@@ -576,203 +504,144 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
             };
             if (SAMPLE && L.n_id > 0) {
                 uncond();
-                epi_bar_sync();  // build_a reads this row's columns written by the other column groups
+                cons_bar_sync();  // build_a reads this row's columns written by the other threads
             }
-            if (!folded) {
-                build_a_net();
-                NFB_STAMP();  // net input A built
-            }
-            if (!SAMPLE && L.n_id > 0) {
-                if (!folded) epi_bar_sync();  // every warp has read the raw identity columns of this row into A
-                uncond();
-            }
+            if (!folded) build_a_net();   // (ends with a barrier: every thread has read its raw identity columns)
+            if (!SAMPLE && L.n_id > 0) uncond();
 
-            // ---- hidden layers ----
-            for (int ph = 0; ph < L.n_hidden; ++ph) {
-                const uint32_t region = (ph & 1) ? 256u : 0u;
-                const bool relu = ph + 1 < L.n_hidden;
-                const float inv = L.a_inv[1 + ph] * ruinv;   // accumulator -> true value
-                const float sc = L.a_sc[2 + ph] * ru;       // true value -> the next GEMM's A units
-                // K-chunk order: all column groups convert the same 64 columns, then release that slice of
-                // the next A operand so the next GEMM's kc-step can start while the rest is converted.
-                // Block-triangular (MADE) layers: output chunk j is FINAL as soon as the last K-chunk that reaches
-                // its rows has been accumulated (blk_sig: the barrier that says so; 3 = the whole GEMM), so the chunks
-                // are converted while the tensor core is still working on the later K-chunks of the same GEMM and the
-                // next GEMM follows without a gap.  The TMEM load of chunk kc + 1 is issued before chunk kc is
-                // converted whenever its barrier has already been passed.
-                const int nkc = H >> 6;
-                uint32_t acc[2][kGC];
-                uint32_t waited = 0;
-                bool loading = false;
-                const uint32_t sig4 = *reinterpret_cast<const uint32_t*>(L.blk_sig + ph * 4);  // this phase's four entries
+            // ---- hidden layers: warpgroup wg owns the 64-column slices [wg half, wg half + half) of every output ----
+            float hres[2][32];   // its part of the residual stream h
+            for (int ph = 0; ph < n_hidden; ++ph) {
+                const bool t_phase = (ph & 1) != 0;   // first GEMM of a residual block: its own accumulator
+                const bool relu = ph + 1 < n_hidden;
+                float tacc[2][32];
 #pragma unroll
-                for (int kc = 0; kc < 4; ++kc) {
-                    if (kc < nkc) {
-                        const uint32_t sg = (sig4 >> (8 * kc)) & 3u;
-                        if (!((waited >> sg) & 1u)) {
-                            if (sg == 3u) { ewait(bar(kBarAccFull), afpar, 310 + ph); afpar ^= 1; }
-                            else { ewait(bar(kBarAccBlk + sg), (blkpar >> sg) & 1u, 320 + (int)sg); blkpar ^= 1u << sg; }
-                            tc_fence_after();
-                            waited |= 1u << sg;
-                            if (kc == 0) NFB_STAMP();  // first output chunk of hidden gemm ph available
-                        }
-                        const int c0 = kc * 64 + wh * kGC;
-                        if (!loading) NFB_TMEM_LD16(tlane + region + c0, acc[kc & 1]);
-                        const float4* bf = reinterpret_cast<const float4*>(L.bias_h + ph * 256 + c0);  // warp-uniform
-                        float bv[kGC];
-#pragma unroll
-                        for (int j = 0; j < kGC / 4; ++j) {
-                            const float4 q4 = __ldg(bf + j);
-                            bv[4 * j] = q4.x; bv[4 * j + 1] = q4.y; bv[4 * j + 2] = q4.z; bv[4 * j + 3] = q4.w;
-                        }
-                        NFB_TMEM_WAIT16(acc[kc & 1]);
-                        loading = false;
-                        if (kc + 1 < nkc && ((waited >> ((sig4 >> (8 * kc + 8)) & 3u)) & 1u)) {
-                            NFB_TMEM_LD16(tlane + region + c0 + 64, acc[(kc + 1) & 1]);
-                            loading = true;
-                        }
-                        float v[kGC];
-#pragma unroll
-                        for (int j = 0; j < kGC; ++j) {
-                            float t = fmaf(__uint_as_float(acc[kc & 1][j]), inv, bv[j]);
-                            v[j] = (relu ? fmaxf(t, 0.f) : t) * sc;
-                        }
-                        const uint32_t thi = aA + kc * kTileA, tlo = aA + (4 + kc) * kTileA;
-#pragma unroll
-                        for (int j = 0; j < kGC / 8; ++j)
-                            split_store8(v + 8 * j, thi, tlo, a_chunk_off(r, wh * (kGC / 8) + j));
-                        fence_proxy_async_smem();
-                        if (kc + 1 >= nkc) tc_fence_before();  // (the last TMEM read of this phase is complete)
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive(bar(kBarAReady + kc));
+                for (int q = 0; q < 2; ++q) {
+                    if (q < half) {
+                        const bool live = wg * half + q < ns;
+                        if (t_phase) run_slice(tacc[q], live, NoQuad());
+                        else run_slice(hres[q], live, NoQuad());
                     }
                 }
-                NFB_STAMP();  // hidden epilogue ph done
-            }
-
-            // ---- final layer chunks -> spline ----
-            // chunk = F features x 24 columns (N = 24 F <= 240).  The F features are dealt round-robin to the kNG
-            // column groups (feature f of the chunk -> group f % kNG); one evaluation at a time per thread,
-            // latency is hidden by the four warps per SM sub-partition.
-            const float inv_f = L.a_inv[1 + L.n_hidden] * ruinv;
-            for (int ci = 0; ci < L.n_chunks; ++ci) {
-                // Processing slot 0 -> buffer 1 (columns 256..): the last hidden epilogue is still reading the
-                // residual stream (columns 0..255) when the first final-layer MMAs start.  The packer makes the
-                // first record of slot 1 wait for a_ready[last K-chunk] (= the epilogue has finished reading
-                // columns 0..255) before it overwrites buffer 0 (nfb_api.cu build_fused).
-                const int b = (ci + 1) & 1;
-                const int c = L.chunk_order[ci];
-                // rotate the deal by the chunk index: with F = 10 the groups get 3,3,2,2 features of a chunk, and
-                // a fixed deal would give groups 0/1 half as much work again as groups 2/3 over the tile
-                const int f0 = (wh + ci) & (kNG - 1);
-                ewait(bar(kBarCFull + b), (cfbits >> b) & 1u, 400 + b);
-                cfbits ^= 1u << b;
-                tc_fence_after();
-                NFB_STAMP();  // chunk c available
-                const uint32_t ta = tlane + chunk_col(b);
+                cons_bar_sync();   // every product of this GEMM has read the A operand: overwrite it with the output
+                const float inv_a = L.a_inv[1 + ph] * ruinv(ra), inv_b = L.a_inv[1 + ph] * ruinv(rb);
+                const float sc_a = L.a_sc[2 + ph] * ru(ra), sc_b = L.a_sc[2 + ph] * ru(rb);
+                // output slice j: bias, ReLU, scale to the next GEMM's units, fp16 hi/lo -> A K-chunk j
+                auto epilogue = [&](const float (&acc)[32], int j) {
+                    const float* bias = L.bias_h + ph * 256 + 64 * j;
 #pragma unroll
-                for (int j = 0; j < 3; ++j) {
-                    const int f = f0 + j * kNG;
-                    if (f < L.F) {
-                    const int t = c * L.F + f;
-                    uint32_t pr[24];
-                    NFB_TMEM_LD16(ta + f * 24, pr);
-                    NFB_TMEM_LD8(ta + f * 24 + 16, pr + 16);
-                    const float4* bp = reinterpret_cast<const float4*>(L.bias_f + t * 24);  // warp-uniform
-                    float bv[24];
+                    for (int g = 0; g < 8; ++g) {
+                        const float2 b2 = __ldg(reinterpret_cast<const float2*>(bias + 8 * g + cq));
 #pragma unroll
-                    for (int jj = 0; jj < 6; ++jj) {
-                        const float4 q4 = __ldg(bp + jj);
-                        bv[4 * jj] = q4.x; bv[4 * jj + 1] = q4.y; bv[4 * jj + 2] = q4.z; bv[4 * jj + 3] = q4.w;
-                    }
-                    tc_wait_ld();
-                    if (f + kNG >= L.F) {  // all of this thread's columns are in registers: free the buffer
-                        tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive(bar(kBarCEmpty + b));
-                    }
-                    if (t < L.T) {
-                        // the packer folded log2(e) (and the layer's 1/sqrt(H)) into the w/h columns and biases
-                        float lw[8], lh[8], dd[8];
-#pragma unroll
-                        for (int jj = 0; jj < 8; ++jj) {
-                            lw[jj] = fmaf(__uint_as_float(pr[jj]), inv_f, bv[jj]);
-                            lh[jj] = fmaf(__uint_as_float(pr[8 + jj]), inv_f, bv[8 + jj]);
-                            dd[jj] = fmaf(__uint_as_float(pr[16 + jj]), inv_f, bv[16 + jj]);
+                        for (int hb = 0; hb < 2; ++hb) {
+                            const int rr = hb ? rb : ra;
+                            float v0 = fmaf(acc[4 * g + 2 * hb], hb ? inv_b : inv_a, b2.x);
+                            float v1 = fmaf(acc[4 * g + 2 * hb + 1], hb ? inv_b : inv_a, b2.y);
+                            if (relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+                            v0 *= hb ? sc_b : sc_a;
+                            v1 *= hb ? sc_b : sc_a;
+                            const uint32_t hi = pack_f16x2(v0, v1);
+                            const float2 hf = unpack_f16x2(hi);
+                            const uint32_t off = (rr >> 3) * 1024 + (rr & 7) * 128 + ((g ^ (rr & 7)) << 4) + cq * 2;
+                            st_shared_b32(aA + j * kTileA + off, hi);
+                            st_shared_b32(aA + (4 + j) * kTileA + off, pack_f16x2(v0 - hf.x, v1 - hf.y));
                         }
-                        const int col = L.tr_idx[t];
-                        float y, l;
-                        float xin = get_x(col);
-                        if (arsamp) xin = row_live ? __ldcg(zdst + grow * D + col) : 0.f;
-                        rqs_core<8, SAMPLE>(xin, lw, lh, [&dd](int k) { return dd[k]; }, L.tail, y, l);
-                        put_y(col, y);
-                        ladsum += l;
                     }
+                };
+#pragma unroll
+                for (int q = 0; q < 2; ++q) {
+                    const int j = wg * half + q;   // output slice = A K-chunk j of the next GEMM
+                    if (q < half && j < ns) {
+                        if (t_phase) epilogue(tacc[q], j);
+                        else epilogue(hres[q], j);
                     }
                 }
-                if (f0 >= L.F) {  // (F < kNG: this group had no feature in the chunk) still release the buffer
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(bar(kBarCEmpty + b));
-                }
-                NFB_STAMP();  // chunk c consumed
+                fence_proxy_async_smem();
+                cons_bar_sync();   // the next GEMM's A operand is complete
             }
 
-            }  // passes
-            NFB_STAMP();  // last spline done
-            // ---- log-det reduction across the column groups, then store ----
-            if (wh > 0) ldsum[(wh - 1) * 128 + r] = ladsum;
-            epi_bar_sync();
-            if (wh == 0 && row_live) {
-                float tot = ladsum + (L.lu_logdet ? __ldg(L.lu_logdet) : 0.f);
+            // ---- final layer: record c = chunks 2c (warpgroup 0) and 2c + 1 (warpgroup 1), kFusedFeaturesPerChunk
+            //      features (x 24 columns) each -> staging -> one spline per thread ----
+            const float inv_f = L.a_inv[1 + n_hidden] * ruinv(r);
+            const int f = (et >> 6) & 1;   // feature of the warpgroup's chunk this thread evaluates (for row r)
+            for (int ci = 0; ci < n_pairs; ++ci) {
+                float acc[kFusedFeaturesPerChunk * 12];
+                run_slice(acc, true, NoQuad());
 #pragma unroll
-                for (int g = 0; g < kNG - 1; ++g) tot += ldsum[g * 128 + r];
-                __stcg(p.logq + grow, tot + lq_old);
+                for (int i = 0; i < kFusedFeaturesPerChunk * 12; i += 2) {
+                    const int c = 8 * (i >> 2) + cq;
+                    *reinterpret_cast<float2*>(stg + ((i & 2) ? rb : ra) * kStgLd + c) = make_float2(acc[i], acc[i + 1]);
+                }
+                wg_bar_sync(wg);
+                const int t = (2 * ci + wg) * L.F + f;
+                if (t < L.T) {
+                    // the packer folded log2(e) (and the layer's 1/sqrt(H)) into the w/h columns and biases
+                    const float4* sp = reinterpret_cast<const float4*>(stg + r * kStgLd + 24 * f);
+                    const float4* bp = reinterpret_cast<const float4*>(L.bias_f + t * 24);
+                    float pv[24];
+#pragma unroll
+                    for (int q = 0; q < 6; ++q) {
+                        const float4 s4 = sp[q], b4 = __ldg(bp + q);
+                        pv[4 * q] = fmaf(s4.x, inv_f, b4.x);
+                        pv[4 * q + 1] = fmaf(s4.y, inv_f, b4.y);
+                        pv[4 * q + 2] = fmaf(s4.z, inv_f, b4.z);
+                        pv[4 * q + 3] = fmaf(s4.w, inv_f, b4.w);
+                    }
+                    float lw[8], lh[8], dd[8];
+#pragma unroll
+                    for (int q = 0; q < 8; ++q) { lw[q] = pv[q]; lh[q] = pv[8 + q]; dd[q] = pv[16 + q]; }
+                    const int col = L.tr_idx[t];
+                    float y, l;
+                    float xin = get_x(col);
+                    if (arsamp) xin = row_live ? __ldcg(zdst + grow * D + col) : 0.f;
+                    rqs_core<8, SAMPLE>(xin, lw, lh, [&dd](int k) { return dd[k]; }, L.tail, y, l);
+                    put_y(col, y);
+                    ladsum += l;
+                }
+                wg_bar_sync(wg);   // the staging tile is free again
             }
-            store_tile();
-            // publish this tile: each thread makes ITS OWN global stores visible device-wide, then the barrier,
-            // then one thread releases the flag (a fence by thread 0 alone would not cover stores that other
-            // warps still have in flight to L2)
-            if (p.progress) __threadfence();
-            epi_bar_sync();
-            if (p.progress && et == 0) {
-                __threadfence();
-                asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p.progress + tile), "r"(layer + 1) : "memory");
-            }
-            NFB_STAMP();  // tile stored
-            if (PROF && prof) prof[127] = pi;
+            cons_bar_sync();   // (AR sampling: every output of this pass is in xs before the next pass reads it)
+        }  // passes
+        // ---- log-det reduction over the four threads of each row, then store ----
+        if (rq > 0) ldsum[(rq - 1) * kRows + r] = ladsum;
+        cons_bar_sync();
+        if (rq == 0 && row_live) {
+            const float tot = ladsum + ldsum[r] + ldsum[kRows + r] + ldsum[2 * kRows + r] +
+                              (L.lu_logdet ? __ldg(L.lu_logdet) : 0.f);
+            __stcg(p.logq + grow, tot + lq_old);
+        }
+        store_tile();
+        // publish this tile: each thread makes ITS OWN global stores visible device-wide, then the barrier,
+        // then one thread releases the flag (a fence by thread 0 alone would not cover stores that other
+        // warps still have in flight to L2)
+        if (p.progress) __threadfence();
+        cons_bar_sync();
+        if (p.progress && et == 0) {
+            __threadfence();
+            asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p.progress + tile), "r"(layer + 1) : "memory");
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == kEpiWarps + 1) tmem_dealloc(tmem, 512);
 }
 
 int launch_fused_rqs(const FusedParams& p, int sm_count, int sample, cudaStream_t st) {
     static PerDevice per_dev;  // the opt-in shared-memory size is a per-device function attribute
     const int dev_sms = per_dev.ensure([] {
-        cudaError_t e = cudaSuccess;
-        const void* fns[4] = {(const void*)fused_rqs_kernel<false, false>, (const void*)fused_rqs_kernel<true, false>,
-                              (const void*)fused_rqs_kernel<false, true>, (const void*)fused_rqs_kernel<true, true>};
-        for (int i = 0; i < 4 && e == cudaSuccess; ++i)
-            e = cudaFuncSetAttribute(fns[i], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFusedSmem);
+        cudaError_t e = cudaFuncSetAttribute(fused_rqs_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             (int)kFusedSmem);
+        if (e == cudaSuccess)
+            e = cudaFuncSetAttribute(fused_rqs_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFusedSmem);
         return e;
     });
     if (dev_sms < 0) return NFB_ERR_CUDA;
     if (sm_count <= 0 || sm_count > dev_sms) sm_count = dev_sms;  // co-residency bound of the CURRENT device
     NFB_CHECK(p.n_layers >= 1 && (p.n_layers == 1 || p.progress), NFB_ERR_ARG, "fused rqs: bad layer list");
-    const long long n_tiles = (p.rows + 127) / 128;
+    const long long n_tiles = (p.rows + kRows - 1) / kRows;
     if (n_tiles == 0) return NFB_OK;
     const long long n_units = n_tiles * p.n_layers;
     // every CTA must be resident (units wait on flags published by other CTAs): grid <= #SMs, 1 CTA/SM
     const unsigned grid = (unsigned)(n_units < sm_count ? n_units : sm_count);
-    if (p.prof) {   // instrumented build (nfb_debug_profile)
-        if (sample) fused_rqs_kernel<true, true><<<grid, kFusedThreads, kFusedSmem, st>>>(p);
-        else fused_rqs_kernel<false, true><<<grid, kFusedThreads, kFusedSmem, st>>>(p);
-    } else {
-        if (sample) fused_rqs_kernel<true, false><<<grid, kFusedThreads, kFusedSmem, st>>>(p);
-        else fused_rqs_kernel<false, false><<<grid, kFusedThreads, kFusedSmem, st>>>(p);
-    }
+    if (sample) fused_rqs_kernel<true><<<grid, kFusedThreads, kFusedSmem, st>>>(p);
+    else fused_rqs_kernel<false><<<grid, kFusedThreads, kFusedSmem, st>>>(p);
     NFB_LAUNCH_CHECK();
     return NFB_OK;
 }
@@ -824,19 +693,6 @@ __global__ void swizzle_split_kernel(const float* __restrict__ E, int n_pad, int
     }
 }
 
-// one record pair: rows [row0, row0+nrows) x K-chunk kc of E (times the GEMM's power-of-two weight scale) -> fp16 hi and
-// lo swizzled tiles (nrows*128 B each)
-__global__ void pack_record_kernel(const float* __restrict__ E, int k_pad, int row0, int nrows, int kc, float scale,
-                                         uint8_t* __restrict__ out_hi, uint8_t* __restrict__ out_lo) {
-    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= nrows * 64) return;
-    const int rr = idx >> 6, kk = idx & 63;
-    const float v = E[(size_t)(row0 + rr) * k_pad + kc * 64 + kk] * scale;
-    const size_t off = (size_t)(rr >> 3) * 1024 + (rr & 7) * 128 + (((kk >> 3) ^ (rr & 7)) << 4) + (kk & 7) * 2;
-    const __half h = __float2half_rn(v);
-    *reinterpret_cast<__half*>(out_hi + off) = h;
-    *reinterpret_cast<__half*>(out_lo + off) = __float2half_rn(v - __half2float(h));
-}
 // all records of one GEMM in ONE launch: blockIdx.y = record (table entry), blockIdx.x = 256-element slice of it
 __global__ void pack_records_kernel(const float* __restrict__ E, int k_pad, const PackRec* __restrict__ recs, float scale,
                                     uint8_t* __restrict__ base) {
@@ -859,14 +715,6 @@ int launch_pack_records(const float* E, int k_pad, const PackRec* recs_dev, int 
     NFB_LAUNCH_CHECK();
     return NFB_OK;
 }
-int launch_pack_record(const float* E, int k_pad, int row0, int nrows, int kc, float scale, uint8_t* out_hi,
-                       uint8_t* out_lo, cudaStream_t st) {
-    NFB_CHECK(nrows > 0 && nrows % 8 == 0, NFB_ERR_ARG, "pack_record: bad row count %d", nrows);
-    pack_record_kernel<<<(nrows * 64 + 255) / 256, 256, 0, st>>>(E, k_pad, row0, nrows, kc, scale, out_hi, out_lo);
-    NFB_LAUNCH_CHECK();
-    return NFB_OK;
-}
-
 // LU fold: G[i, c] = gain * sum_k E0[i, k] Elu[in_idx[k], c],  delta[i] = sum_k E0[i, k] blu[in_idx[k]]
 // (E0: [H x 64] first conditioner matrix in sorted hidden order, column k <-> conditioner input k = x'[in_idx[k]];
 //  Elu: [64 x 64] with x' = Elu z + blu).  fp64 accumulation, one block per row i.

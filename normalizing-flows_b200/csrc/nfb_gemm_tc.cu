@@ -1,4 +1,4 @@
-// nfb_gemm_tc.cu -- general fp32-in / fp32-out GEMM on the sm_100a tensor core, for the TRAINING pass of the
+// nfb_gemm_tc.cu -- general fp32-in / fp32-out GEMM on the sm_90a tensor core (wgmma), for the TRAINING pass of the
 // neural-spline stacks (recompute of the conditioner activations, dgrad, wgrad; SURVEY 8f-1).
 //
 //   C[M x N] (+)= op_a(A) [M x K] * op_b(B)^T [N x K]           (fp32 row-major operands in global memory)
@@ -9,50 +9,37 @@
 //   dgrad    gX = gY W    : A = gY [B x N']  K-major,  B = W  [N' x Kin] MN-major (the GEMM's N is W's column)
 //   wgrad    dW = gY^T X  : A = gY [B x N']  MN-major, B = X  [B x Kin]  MN-major (reduction over the batch)
 // MN-major operands use the canonical SWIZZLE_128B MN-major shared-memory layout (64 MN elements per 128-byte row,
-// 8 k-rows per 1024-byte atom; LBO = stride between 64-wide MN blocks, SBO = stride between 8-row k groups) and
-// the a_major / b_major bits of the tcgen05 instruction descriptor; nothing is transposed in memory.
+// 8 k-rows per 1024-byte atom; LBO = stride between 64-wide MN blocks, SBO = stride between 8-row k groups) and the
+// transpose operands of wgmma; nothing is transposed in memory.
 //
-// Numerics: split-bf16, fp32 accumulation in TMEM: a*b ~= a_hi*b_hi + a_lo*b_hi + a_hi*b_lo (~2^-17 relative per
-// product; bf16 keeps fp32's exponent range, so gradients of any magnitude need no scaling).  NFB_GEMM_TERMS=1
-// selects the single-pass bf16 product (measurement only).
+// Numerics: split-bf16, fp32 accumulation: a*b ~= a_hi*b_hi + a_lo*b_hi + a_hi*b_lo (~2^-17 relative per product;
+// bf16 keeps fp32's exponent range, so gradients of any magnitude need no scaling).  NFB_GEMM_TERMS=1 selects the
+// single-pass bf16 product (measurement only).
 //
-// Roles (576 threads, persistent over work units (m tile, n tile, k split)):
-//   warps 0-15 builders + epilogue: load fp32 from global (float4 when aligned, guarded scalars otherwise), apply the
-//              optional ReLU on load, split to bf16 hi/lo and write 16-byte chunks into the swizzled A and B stages;
-//              the epilogue of unit i-1 (TMEM -> bias / ReLU-mask / residual -> store or red.add) runs after unit i
-//              has been built, under unit i's MMAs (accumulator double-buffered in TMEM).
-//   warp 16    idle (kept so that warp 17 is the MMA issuer as in the other tcgen05 kernels)
-//   warp 17    one elected lane issues 12 (or 4) tcgen05.mma (M=128, N=n_tile, K=16) per 64-wide K chunk;
-//              tcgen05.commit frees the stage; owns the TMEM allocation.
+// Structure (256 threads = two warpgroups, persistent over work units (m tile, n tile, k split)): every thread loads
+// fp32 from global (float4 when aligned, guarded scalars otherwise), applies the optional ReLU on load, splits to bf16
+// hi/lo and writes 16-byte chunks into the swizzled A and B tiles of a two-stage ring; warpgroup w multiplies rows
+// [64 w, 64 w + 64) of the 128-row tile by the whole n tile (wgmma, accumulator in registers) while the next K-chunk
+// is loaded and converted.  The epilogue goes through a shared-memory staging tile so that bias / ReLU-mask / residual
+// loads and the stores (or red.add) are contiguous.
 #include "nfb_kernels.h"
 
 namespace nfb {
 
 namespace {
-constexpr int kGtBuildWarps = 16;
-constexpr int kGtBuildThreads = 32 * kGtBuildWarps;
-constexpr int kGtThreads = kGtBuildThreads + 64;
+constexpr int kGtThreads = 256;
 constexpr uint32_t kGtTileA = 16384;            // [128 x 64] bf16
 constexpr uint32_t kGtSmemMax = 232448;
-constexpr uint32_t kGtBarBytes = 16 * 8;
-constexpr int kGtMaxStages = 4;
-enum { GB_FULL = 0, GB_EMPTY = 4, GB_ACCFULL = 8, GB_ACCEMPTY = 10 };
-
 __device__ __forceinline__ void gt_st_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
     asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
-// shared-memory matrix descriptor, SWIZZLE_128B, explicit leading / stride byte offsets (16-byte units)
-__device__ __forceinline__ uint64_t gt_desc(uint32_t smem_addr, uint32_t lbo16, uint32_t sbo16) {
-    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)lbo16 << 16) | ((uint64_t)sbo16 << 32) | (1ull << 46) |
-           (2ull << 61);
-}
+__device__ __forceinline__ void gt_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kGtThreads) : "memory"); }
 }  // namespace
 
 struct GemmTcParams {
     const float* A; const float* B; float* C;
     long long lda, ldb, ldc;
     long long M; int N; long long K;
-    int a_mn, b_mn;          // 1: the operand's M/N dimension is the contiguous one (element (i,k) at base[k*ld + i])
     int a_relu, b_relu;      // max(x, 0) applied while loading
     const float* bias;       // [N] or null: added to every row
     const float* mask;       // [M x N] (ld = ldmask) or null: v *= (mask > 0)      (ReLU derivative)
@@ -62,47 +49,34 @@ struct GemmTcParams {
     long long ldres;
     int relu_out;            // v = max(v, 0) before the store
     int atomic_out;          // red.global.add instead of a store (split-K partials; C must be pre-zeroed)
-    int n_tile;              // multiple of 16, <= 256
     int k_splits;            // >= 1
     long long k_per_split;   // multiple of 64
-    int stages, terms;       // pipeline depth; 3 = split-bf16, 1 = plain bf16
+    int terms;               // 3 = split-bf16, 1 = plain bf16
     const uint8_t* b_packed; // optional: B pre-split to bf16 hi | lo tiles in the stage layout, one record per
                              // (n tile, K chunk): streamed by bulk TMA instead of being converted by the builders
     int* err;
 };
 
-template <bool PACKED>
+// NT: n tile (64 or 128); AMN / BMN: the operand's M / N dimension is the contiguous one (element (i, k) at
+// base[k * ld + i]); PACKED: B comes pre-packed (b_packed)
+template <int NT, int AMN, int BMN, bool PACKED>
 __global__ void __launch_bounds__(kGtThreads, 1) gemm_tc_kernel(const GemmTcParams p) {
     extern __shared__ __align__(1024) uint8_t smem[];
+    constexpr int NREG = NT / 2;
+    constexpr uint32_t b_tile = (uint32_t)NT * 128u;             // one [NT x 64] bf16 tile
+    constexpr uint32_t stage_bytes = 2 * kGtTileA + 2 * b_tile;  // A hi | A lo | B hi | B lo
+    constexpr int kStgLd = NT + 4;
     const uint32_t sbase = smem_u32(smem);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int S = p.stages;
-    const int NT = p.n_tile;
-    const uint32_t b_tile = (uint32_t)NT * 128u;             // one [NT x 64] bf16 tile
-    const uint32_t stage_bytes = 2 * kGtTileA + 2 * b_tile;  // A hi | A lo | B hi | B lo
-    const uint32_t offBars = (uint32_t)S * stage_bytes;
-    const uint32_t bars = sbase + offBars;
-    auto bar = [bars](int i) { return bars + 8u * i; };
-
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < kGtMaxStages; ++i) {
-            mbar_init(bar(GB_FULL + i), kGtBuildWarps + (PACKED ? 1 : 0));  // (+ the TMA producer's expect_tx)
-            mbar_init(bar(GB_EMPTY + i), 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(bar(GB_ACCFULL + i), 1);
-            mbar_init(bar(GB_ACCEMPTY + i), kGtBuildWarps);
-        }
+    const int bt = threadIdx.x, wg = bt >> 7, warp = (bt >> 5) & 3, lane = bt & 31;
+    const uint32_t offBars = 2 * stage_bytes;
+    float* stg = reinterpret_cast<float*>(smem + offBars + 64);   // epilogue staging tile [128][kStgLd]
+    const uint32_t bars = sbase + offBars;   // [0, 2): B stage full (PACKED)
+    if (bt == 0) {
+        mbar_init(bars, 1);
+        mbar_init(bars + 8, 1);
         fence_mbar_init();
     }
-    if (warp == kGtBuildWarps + 1) {
-        tmem_alloc(sbase + offBars + kGtBarBytes, 512);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *reinterpret_cast<volatile uint32_t*>(smem + offBars + kGtBarBytes);
 
     const long long m_tiles = (p.M + 127) / 128;
     const int n_tiles = (p.N + NT - 1) / NT;
@@ -110,280 +84,202 @@ __global__ void __launch_bounds__(kGtThreads, 1) gemm_tc_kernel(const GemmTcPara
     // units are K-split-major: the CTAs that run at the same time work on the SAME k range of different output tiles,
     // so an operand slab that several tiles share (the activations of a weight gradient) is re-read from L2, not HBM
     const long long n_units = n_out_tiles * p.k_splits;
+    const bool a_al = (p.lda % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.A) & 15) == 0);
+    const bool b_al = (p.ldb % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.B) & 15) == 0);
 
-    if (PACKED && warp == kGtBuildWarps) {
-        // ------------------------------ B producer (pre-packed operand) ----------------------
-        const int kc_total = (int)((p.K + 63) / 64);
-        const uint32_t rec = 2 * b_tile;
-        uint32_t st = 0, st_use = 0;
-        for (long long u = blockIdx.x; u < n_units; u += gridDim.x) {
-            const long long tile = u % n_out_tiles;
-            const int nt = (int)(tile % n_tiles);
-            for (int kc = 0; kc < kc_total; ++kc) {  // (k_splits == 1 with a packed operand)
-                if (st_use > 0) mbar_wait(bar(GB_EMPTY + st), (st_use - 1) & 1u, p.err, 860 + st);
-                if (elect_one_sync()) {
-                    mbar_expect_tx(bar(GB_FULL + st), rec);
-                    bulk_g2s(sbase + st * stage_bytes + 2 * kGtTileA, p.b_packed + ((size_t)nt * kc_total + kc) * rec, rec,
-                             bar(GB_FULL + st));
-                }
-                __syncwarp();
-                if (++st == (uint32_t)S) { st = 0; ++st_use; }
-            }
+    // One operand tile = R "rows" of the GEMM's M/N dimension x 64 k, from a row-major fp32 matrix, handled in groups
+    // of 8 contiguous source elements (one 16-byte bf16 chunk of the swizzled tile):
+    //   K-major : element (i, k) at src[(i0+i)*ld + k0+k]; group g = (row = g>>3, 16-byte chunk c8 = g&7)
+    //   MN-major: element (i, k) at src[(k0+k)*ld + i0+i]; group g = (k row = g / (R/8), chunk cm = g % (R/8))
+    auto load_group = [&](const float* src, long long ld, int mn, bool al, long long i0, long long i_end, long long k0,
+                          long long k_end, int R, int g, float (&v)[8], uint32_t& off) {
+        long long row, col, row_end, col_end;
+        if (!mn) {
+            const int i = g >> 3, c8 = g & 7;
+            row = i0 + i; col = k0 + c8 * 8; row_end = i_end; col_end = k_end;
+            off = (uint32_t)((i >> 3) * 1024 + (i & 7) * 128 + ((c8 ^ (i & 7)) << 4));
+        } else {
+            const int per = R >> 3;
+            const int kr = g / per, cm = g - kr * per;
+            row = k0 + kr; col = i0 + cm * 8; row_end = k_end; col_end = i_end;
+            off = (uint32_t)((cm >> 3) * 8192 + (kr >> 3) * 1024 + (kr & 7) * 128 + (((cm & 7) ^ (kr & 7)) << 4));
         }
-    } else if (warp == kGtBuildWarps + 1) {
-        // ------------------------------ MMA issuer ------------------------------------------
-        const uint32_t idesc = umma_idesc_bf16(128, (uint32_t)NT) | ((uint32_t)p.a_mn << 15) | ((uint32_t)p.b_mn << 16);
-        // K-major: 8-row groups 1024 B apart, a K=16 step is 32 B further along the row.
-        // MN-major: 64-wide MN blocks 8192 B apart (LBO), 8-row k groups 1024 B apart (SBO), a K=16 step = 2 groups.
-        const uint32_t a_lbo = p.a_mn ? 512u : 1u, b_lbo = p.b_mn ? 512u : 1u;
-        const uint32_t a_step = p.a_mn ? 128u : 2u, b_step = p.b_mn ? 128u : 2u;  // descriptor address units (16 B)
-        uint32_t st = 0, st_use = 0, it = 0;
-        for (long long u = blockIdx.x; u < n_units; u += gridDim.x, ++it) {
-            const int ks = (int)(u / n_out_tiles);
-            const long long k0 = (long long)ks * p.k_per_split;
-            const long long k1 = k0 + p.k_per_split < p.K ? k0 + p.k_per_split : p.K;
-            const int KC = (int)((k1 - k0 + 63) / 64);
-            const uint32_t ab = it & 1u;
-            if (it >= 2) mbar_wait(bar(GB_ACCEMPTY + ab), ((it >> 1) - 1) & 1u, p.err, 850 + ab);
-            const uint32_t d = tmem + ab * 256u;
-            for (int kc = 0; kc < KC; ++kc) {
-                mbar_wait(bar(GB_FULL + st), st_use & 1u, p.err, 810 + st);
-                tc_fence_after();
-                if (elect_one_sync()) {
-                    const uint32_t sa = sbase + st * stage_bytes;
-                    const uint64_t a_hi = gt_desc(sa, a_lbo, 64), a_lo = gt_desc(sa + kGtTileA, a_lbo, 64);
-                    const uint64_t b_hi = gt_desc(sa + 2 * kGtTileA, b_lbo, 64);
-                    const uint64_t b_lo = gt_desc(sa + 2 * kGtTileA + b_tile, b_lbo, 64);
+        if (row < row_end && col + 8 <= col_end && al) {
+            const float4* s4 = reinterpret_cast<const float4*>(src + row * ld + col);
+            const float4 x0 = __ldg(s4), x1 = __ldg(s4 + 1);
+            v[0] = x0.x; v[1] = x0.y; v[2] = x0.z; v[3] = x0.w; v[4] = x1.x; v[5] = x1.y; v[6] = x1.z; v[7] = x1.w;
+        } else {
 #pragma unroll
-                    for (int j = 0; j < 4; ++j)
-                        umma_bf16(d, a_hi + (uint64_t)(a_step * j), b_hi + (uint64_t)(b_step * j), idesc, (kc | j) ? 1u : 0u);
-                    if (p.terms == 3) {
-#pragma unroll
-                        for (int j = 0; j < 4; ++j)
-                            umma_bf16(d, a_lo + (uint64_t)(a_step * j), b_hi + (uint64_t)(b_step * j), idesc, 1u);
-#pragma unroll
-                        for (int j = 0; j < 4; ++j)
-                            umma_bf16(d, a_hi + (uint64_t)(a_step * j), b_lo + (uint64_t)(b_step * j), idesc, 1u);
-                    }
-                    umma_commit(bar(GB_EMPTY + st));
-                    if (kc == KC - 1) umma_commit(bar(GB_ACCFULL + ab));
-                }
-                __syncwarp();
-                if (++st == (uint32_t)S) { st = 0; ++st_use; }
-            }
+            for (int j = 0; j < 8; ++j)
+                v[j] = (row < row_end && col + j < col_end) ? __ldg(src + row * ld + col + j) : 0.f;
         }
-    } else if (warp < kGtBuildWarps) {
-        // ------------------------------ builders / epilogue -----------------------------------
-        const int bt = threadIdx.x;              // 0..511
-        const int q = warp & 3, wh = warp >> 2;  // TMEM lane quadrant, column group
-        const int r = q * 32 + lane;             // accumulator row this thread reads in the epilogue
-        const uint32_t tlane = tmem + ((uint32_t)(q * 32) << 16);
-        const bool a_al = (p.lda % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.A) & 15) == 0);
-        const bool b_al = (p.ldb % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.B) & 15) == 0);
-        uint32_t st = 0, st_use = 0, it = 0;
-
-        // One operand tile = R "rows" of the GEMM's M/N dimension x 64 k, from a row-major fp32 matrix, handled in
-        // groups of 8 contiguous source elements (one 16-byte bf16 chunk of the swizzled tile):
-        //   K-major : element (i, k) at src[(i0+i)*ld + k0+k]; group g = (row = g>>3, 16-byte chunk c8 = g&7)
-        //   MN-major: element (i, k) at src[(k0+k)*ld + i0+i]; group g = (k row = g / (R/8), chunk cm = g % (R/8))
-        // A thread owns up to 2 groups of A and 4 of B per K chunk.  ALL their global loads are issued first (12
-        // independent LDG.128 in flight per thread, and before the wait for the stage to be free), then converted and
-        // stored: one memory round trip per chunk instead of one per group.
-        auto load_group = [&](const float* src, long long ld, int mn, bool al, long long i0, long long i_end, long long k0,
-                              long long k_end, int R, int g, float (&v)[8], uint32_t& off) {
-            long long row, col, row_end, col_end;
-            if (!mn) {
-                const int i = g >> 3, c8 = g & 7;
-                row = i0 + i; col = k0 + c8 * 8; row_end = i_end; col_end = k_end;
-                off = (uint32_t)((i >> 3) * 1024 + (i & 7) * 128 + ((c8 ^ (i & 7)) << 4));
-            } else {
-                const int per = R >> 3;
-                const int kr = g / per, cm = g - kr * per;
-                row = k0 + kr; col = i0 + cm * 8; row_end = k_end; col_end = i_end;
-                off = (uint32_t)((cm >> 3) * 8192 + (kr >> 3) * 1024 + (kr & 7) * 128 + (((cm & 7) ^ (kr & 7)) << 4));
-            }
-            if (row < row_end && col + 8 <= col_end && al) {
-                const float4* s4 = reinterpret_cast<const float4*>(src + row * ld + col);
-                const float4 x0 = __ldg(s4), x1 = __ldg(s4 + 1);
-                v[0] = x0.x; v[1] = x0.y; v[2] = x0.z; v[3] = x0.w; v[4] = x1.x; v[5] = x1.y; v[6] = x1.z; v[7] = x1.w;
-            } else {
+    };
+    auto store_group = [&](const float (&v)[8], int relu, uint32_t t_hi, uint32_t t_lo, uint32_t off) {
+        uint32_t hi[4], lo[4];
 #pragma unroll
-                for (int j = 0; j < 8; ++j)
-                    v[j] = (row < row_end && col + j < col_end) ? __ldg(src + row * ld + col + j) : 0.f;
-            }
-        };
-        auto store_group = [&](const float (&v)[8], int relu, uint32_t t_hi, uint32_t t_lo, uint32_t off) {
-            uint32_t hi[4], lo[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                float a = v[2 * i], b = v[2 * i + 1];
-                if (relu) { a = fmaxf(a, 0.f); b = fmaxf(b, 0.f); }
-                hi[i] = pack_bf16x2(a, b);
-                lo[i] = pack_bf16x2(a - __uint_as_float(hi[i] << 16), b - __uint_as_float(hi[i] & 0xffff0000u));
-            }
-            gt_st_v4(t_hi + off, hi[0], hi[1], hi[2], hi[3]);
-            gt_st_v4(t_lo + off, lo[0], lo[1], lo[2], lo[3]);
-        };
-
-        // Epilogue through shared memory.  tcgen05.ld hands every thread one ROW of the accumulator (lane = row), so a
-        // direct global access would touch 32 different cache lines per warp instruction (measured: ~33 k cycles per
-        // 128 x 256 tile).  Instead each 64-column slab is parked in a [128][65] fp32 staging tile, and after a barrier
-        // thread t processes (row t / 16 + 32 j, columns 4 (t % 16) ..): bias / mask / residual loads and the store (or
-        // red.add) are then 256 contiguous bytes per 16 lanes.
-        float* stg = reinterpret_cast<float*>(smem + offBars + kGtBarBytes + 16);
-        auto epi_sync = [] { asm volatile("bar.sync 1, %0;" ::"n"(kGtBuildThreads) : "memory"); };
-        auto epilogue = [&](long long u, uint32_t i) {
-            const uint32_t ab = i & 1u;
-            mbar_wait_warp(bar(GB_ACCFULL + ab), (i >> 1) & 1u, p.err, 840 + ab);
-            tc_fence_after();
-            const long long tile = u % n_out_tiles;
-            const long long mt = tile / n_tiles;
-            const int nt = (int)(tile - mt * n_tiles);
-            const bool vec_ok = (p.ldc % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0) && !p.atomic_out;
-            for (int cb = 0; cb < NT; cb += 64) {
-                const int c0 = cb + wh * 16;
-                if (c0 < NT) {
-                    uint32_t acc[16];
-                    NFB_TMEM_LD16(tlane + ab * 256u + c0, acc);
-                    tc_wait_ld();
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) stg[r * 65 + wh * 16 + j] = __uint_as_float(acc[j]);
-                }
-                epi_sync();
-                const int cq = (bt & 15) * 4;            // first of this thread's 4 columns inside the slab
-                const int n0 = nt * NT + cb + cq;
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const int rr = (bt >> 4) + 32 * j;
-                    const long long m = mt * 128 + rr;
-                    if (m >= p.M || cb + cq >= NT || n0 >= p.N) continue;
-                    float v[4];
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) v[q] = stg[rr * 65 + cq + q];
-                    const bool full = n0 + 4 <= p.N;
-                    if (p.bias) {
-#pragma unroll
-                        for (int q = 0; q < 4; ++q) if (n0 + q < p.N) v[q] += __ldg(p.bias + n0 + q);
-                    }
-                    if (p.mask) {
-#pragma unroll
-                        for (int q = 0; q < 4; ++q)
-                            if (n0 + q < p.N) v[q] = __ldg(p.mask + m * p.ldmask + n0 + q) > 0.f ? v[q] : 0.f;
-                    }
-                    if (p.mulm) {
-#pragma unroll
-                        for (int q = 0; q < 4; ++q) if (n0 + q < p.N) v[q] *= __ldg(p.mulm + m * p.ldmask + n0 + q);
-                    }
-                    if (p.resid) {
-#pragma unroll
-                        for (int q = 0; q < 4; ++q) if (n0 + q < p.N) v[q] += __ldg(p.resid + m * p.ldres + n0 + q);
-                    }
-                    if (p.relu_out) {
-#pragma unroll
-                        for (int q = 0; q < 4; ++q) v[q] = fmaxf(v[q], 0.f);
-                    }
-                    float* dst = p.C + m * p.ldc + n0;
-                    if (p.atomic_out) {
-#pragma unroll
-                        for (int q = 0; q < 4; ++q) if (n0 + q < p.N) atomicAdd(dst + q, v[q]);
-                    } else if (full && vec_ok) {
-                        *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
-                    } else {
-#pragma unroll
-                        for (int q = 0; q < 4; ++q) if (n0 + q < p.N) dst[q] = v[q];
-                    }
-                }
-                epi_sync();  // the staging tile is reused by the next slab
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(bar(GB_ACCEMPTY + ab));
-        };
-
-        // The builders walk this CTA's K chunks as ONE stream across unit boundaries.  With a pre-packed B operand a
-        // thread only owns two A groups per chunk (16 registers), so the loads of chunk j+1 are issued BEFORE chunk j is
-        // converted and stored: the HBM latency of the activation stream (~2 k cycles) is then hidden behind one
-        // chunk's worth of work instead of being exposed once per chunk.
-        struct Pos { long long u, mt, k0, k1; int nt, kc, KC; };
-        auto unit_pos = [&](long long u, int kc) {
-            Pos q;
-            q.u = u; q.kc = kc;
-            const int ks = (int)(u / n_out_tiles);
-            const long long tile = u % n_out_tiles;
-            q.mt = tile / n_tiles;
-            q.nt = (int)(tile - q.mt * n_tiles);
-            q.k0 = (long long)ks * p.k_per_split;
-            q.k1 = q.k0 + p.k_per_split < p.K ? q.k0 + p.k_per_split : p.K;
-            q.KC = (int)((q.k1 - q.k0 + 63) / 64);
-            return q;
-        };
-        const int nb_groups = NT * 8;  // B groups per chunk (A: 1024)
-        constexpr bool packed = PACKED;
-        float va[2][8], vb[4][8], na[2][8];
-        uint32_t oa[2], ob[4], noa[2];
-        auto load_a = [&](const Pos& q, float (&v)[2][8], uint32_t (&o)[2]) {
-#pragma unroll
-            for (int i = 0; i < 2; ++i)
-                load_group(p.A, p.lda, p.a_mn, a_al, q.mt * 128, p.M, q.k0 + (long long)q.kc * 64, q.k1, 128,
-                           bt + i * kGtBuildThreads, v[i], o[i]);
-        };
-        long long prev = -1;
-        Pos cur{};
-        if ((long long)blockIdx.x < n_units) {
-            cur = unit_pos(blockIdx.x, 0);
-            load_a(cur, va, oa);
+        for (int i = 0; i < 4; ++i) {
+            float a = v[2 * i], b = v[2 * i + 1];
+            if (relu) { a = fmaxf(a, 0.f); b = fmaxf(b, 0.f); }
+            hi[i] = pack_bf16x2(a, b);
+            lo[i] = pack_bf16x2(a - __uint_as_float(hi[i] << 16), b - __uint_as_float(hi[i] & 0xffff0000u));
         }
-        for (bool more = (long long)blockIdx.x < n_units; more;) {
-            Pos nxt = cur;
-            if (++nxt.kc == cur.KC) nxt = unit_pos(cur.u + gridDim.x, 0);
-            const bool has_next = nxt.u < n_units;
-            if (packed && has_next) load_a(nxt, na, noa);  // prefetch: in flight during this chunk's convert / store
-            if (!packed) {
+        gt_st_v4(t_hi + off, hi[0], hi[1], hi[2], hi[3]);
+        gt_st_v4(t_lo + off, lo[0], lo[1], lo[2], lo[3]);
+    };
+
+    struct Pos { long long u, mt, k0, k1; int nt, kc, KC; };
+    auto unit_pos = [&](long long u, int kc) {
+        Pos q;
+        q.u = u; q.kc = kc;
+        const int ks = (int)(u / n_out_tiles);
+        const long long tile = u % n_out_tiles;
+        q.mt = tile / n_tiles;
+        q.nt = (int)(tile - q.mt * n_tiles);
+        q.k0 = (long long)ks * p.k_per_split;
+        q.k1 = q.k0 + p.k_per_split < p.K ? q.k0 + p.k_per_split : p.K;
+        q.KC = (int)((q.k1 - q.k0 + 63) / 64);
+        return q;
+    };
+    constexpr int kAG = 1024 / kGtThreads;              // A groups per thread and chunk (4)
+    constexpr int kBG = NT * 8 / kGtThreads;            // B groups per thread and chunk (2 or 4)
+    float va[kAG][8], vb[kBG][8];
+    uint32_t oa[kAG], ob[kBG];
+    auto load_chunk = [&](const Pos& q) {
 #pragma unroll
-                for (int i = 0; i < 4; ++i)
-                    if (bt + i * kGtBuildThreads < nb_groups)
-                        load_group(p.B, p.ldb, p.b_mn, b_al, (long long)cur.nt * NT, p.N, cur.k0 + (long long)cur.kc * 64,
-                                   cur.k1, NT, bt + i * kGtBuildThreads, vb[i], ob[i]);
-            }
-            const uint32_t sa = sbase + st * stage_bytes;
-            if (st_use > 0) mbar_wait(bar(GB_EMPTY + st), (st_use - 1) & 1u, p.err, 830 + st);  // (loads in flight)
+        for (int i = 0; i < kAG; ++i)
+            load_group(p.A, p.lda, AMN, a_al, q.mt * 128, p.M, q.k0 + (long long)q.kc * 64, q.k1, 128, bt + i * kGtThreads,
+                       va[i], oa[i]);
+        if (!PACKED) {
 #pragma unroll
-            for (int i = 0; i < 2; ++i) store_group(va[i], p.a_relu, sa, sa + kGtTileA, oa[i]);
-            if (!packed) {
+            for (int i = 0; i < kBG; ++i)
+                load_group(p.B, p.ldb, BMN, b_al, (long long)q.nt * NT, p.N, q.k0 + (long long)q.kc * 64, q.k1, NT,
+                           bt + i * kGtThreads, vb[i], ob[i]);
+        }
+    };
+    uint32_t full_use[2] = {0, 0};
+    auto store_chunk = [&](const Pos& q, int s) {
+        const uint32_t sa = sbase + s * stage_bytes;
+        if (PACKED && bt == 0) {
+            const int kc_total = (int)((p.K + 63) / 64);   // (k_splits == 1 with a packed operand)
+            mbar_expect_tx(bars + 8 * s, 2 * b_tile);
+            bulk_g2s(sa + 2 * kGtTileA, p.b_packed + ((size_t)q.nt * kc_total + q.kc) * (2 * b_tile), 2 * b_tile, bars + 8 * s);
+        }
 #pragma unroll
-                for (int i = 0; i < 4; ++i)
-                    if (bt + i * kGtBuildThreads < nb_groups)
-                        store_group(vb[i], p.b_relu, sa + 2 * kGtTileA, sa + 2 * kGtTileA + b_tile, ob[i]);
-            }
-            fence_proxy_async_smem();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(bar(GB_FULL + st));
-            if (++st == (uint32_t)S) { st = 0; ++st_use; }
-            if (cur.kc == cur.KC - 1) {  // unit complete: the previous unit's epilogue overlaps this unit's MMAs
-                if (prev >= 0) epilogue(prev, it - 1);
-                prev = cur.u;
-                ++it;
-            }
-            if (has_next) {
-                if (packed) {
+        for (int i = 0; i < kAG; ++i) store_group(va[i], p.a_relu, sa, sa + kGtTileA, oa[i]);
+        if (!PACKED) {
 #pragma unroll
-                    for (int i = 0; i < 2; ++i) {
-                        oa[i] = noa[i];
+            for (int i = 0; i < kBG; ++i) store_group(vb[i], p.b_relu, sa + 2 * kGtTileA, sa + 2 * kGtTileA + b_tile, ob[i]);
+        }
+        fence_proxy_async_smem();
+    };
+
+    // wgmma descriptors.  K-major: 8-row groups 1024 B apart, a K=16 step is 32 B further along the row.  MN-major:
+    // 64-wide MN blocks 8192 B apart (LBO), 8-row k groups 1024 B apart (SBO), a K=16 step = 2 groups.
+    constexpr uint32_t a_lbo = AMN ? 512u : 1u, b_lbo = BMN ? 512u : 1u;
+    constexpr uint32_t a_step = AMN ? 128u : 2u, b_step = BMN ? 128u : 2u;   // descriptor address units (16 B)
+    // this warpgroup's 64 rows: 8 row groups further (K-major) or the second 64-wide M block (MN-major): 8 KB either way
+    const uint32_t a_wg = (uint32_t)wg * 8192u;
+    auto mma_chunk = [&](float (&acc)[NREG], int s, bool first) {
+        const uint32_t sa = sbase + s * stage_bytes;
+        const uint64_t ah = wgmma_desc(sa + a_wg, a_lbo), al = wgmma_desc(sa + kGtTileA + a_wg, a_lbo);
+        const uint64_t bh = wgmma_desc(sa + 2 * kGtTileA, b_lbo), bl = wgmma_desc(sa + 2 * kGtTileA + b_tile, b_lbo);
+        auto mma = [&](uint64_t a, uint64_t b, uint32_t sd) {
+            if constexpr (NT == 64) wgmma_bf16_n64<AMN, BMN>(acc, a, b, sd);
+            else wgmma_bf16_n128<AMN, BMN>(acc, a, b, sd);
+        };
+        wgmma_fence();
 #pragma unroll
-                        for (int j = 0; j < 8; ++j) va[i][j] = na[i][j];
-                    }
+        for (int j = 0; j < 4; ++j) mma(ah + a_step * j, bh + b_step * j, (first && j == 0) ? 0u : 1u);
+        if (p.terms == 3) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) mma(al + a_step * j, bh + b_step * j, 1u);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) mma(ah + a_step * j, bl + b_step * j, 1u);
+        }
+        wgmma_commit();
+    };
+
+    const bool vec_ok = (p.ldc % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0) && !p.atomic_out;
+    auto epilogue = [&](const Pos& q, const float (&acc)[NREG]) {
+        // accumulator register i: row 16 warp + lane / 4 (+ 8), column 8 (i / 4) + 2 (lane % 4) (+ 1)
+        const int r0 = 64 * wg + 16 * warp + (lane >> 2);
+#pragma unroll
+        for (int i = 0; i < NREG; i += 2) {
+            const int c = 8 * (i >> 2) + 2 * (lane & 3);
+            *reinterpret_cast<float2*>(stg + (r0 + ((i & 2) ? 8 : 0)) * kStgLd + c) = make_float2(acc[i], acc[i + 1]);
+        }
+        gt_bar_sync();
+        const int cq = (bt & 15) * 4;   // this thread's 4 columns inside a 64-column slab
+        for (int cb = 0; cb < NT; cb += 64) {
+            const int n0 = q.nt * NT + cb + cq;
+#pragma unroll 2
+            for (int j = 0; j < 8; ++j) {
+                const int rr = (bt >> 4) + 16 * j;
+                const long long m = q.mt * 128 + rr;
+                if (m >= p.M || n0 >= p.N) continue;
+                float v[4];
+#pragma unroll
+                for (int t = 0; t < 4; ++t) v[t] = stg[rr * kStgLd + cb + cq + t];
+                const bool full = n0 + 4 <= p.N;
+                if (p.bias) {
+#pragma unroll
+                    for (int t = 0; t < 4; ++t) if (n0 + t < p.N) v[t] += __ldg(p.bias + n0 + t);
+                }
+                if (p.mask) {
+#pragma unroll
+                    for (int t = 0; t < 4; ++t)
+                        if (n0 + t < p.N) v[t] = __ldg(p.mask + m * p.ldmask + n0 + t) > 0.f ? v[t] : 0.f;
+                }
+                if (p.mulm) {
+#pragma unroll
+                    for (int t = 0; t < 4; ++t) if (n0 + t < p.N) v[t] *= __ldg(p.mulm + m * p.ldmask + n0 + t);
+                }
+                if (p.resid) {
+#pragma unroll
+                    for (int t = 0; t < 4; ++t) if (n0 + t < p.N) v[t] += __ldg(p.resid + m * p.ldres + n0 + t);
+                }
+                if (p.relu_out) {
+#pragma unroll
+                    for (int t = 0; t < 4; ++t) v[t] = fmaxf(v[t], 0.f);
+                }
+                float* dst = p.C + m * p.ldc + n0;
+                if (p.atomic_out) {
+#pragma unroll
+                    for (int t = 0; t < 4; ++t) if (n0 + t < p.N) atomicAdd(dst + t, v[t]);
+                } else if (full && vec_ok) {
+                    *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
                 } else {
-                    load_a(nxt, va, oa);
+#pragma unroll
+                    for (int t = 0; t < 4; ++t) if (n0 + t < p.N) dst[t] = v[t];
                 }
             }
-            cur = nxt;
-            more = has_next;
         }
-        if (prev >= 0) epilogue(prev, it - 1);
+        gt_bar_sync();  // the staging tile is reused by the next unit
+    };
+
+    // The CTA walks its K chunks as ONE stream across unit boundaries: while the tensor core multiplies chunk i, the
+    // global loads of chunk i + 1 are in flight and then converted into the other stage.
+    if ((long long)blockIdx.x >= n_units) return;
+    float acc[NREG];
+    Pos cur = unit_pos(blockIdx.x, 0);
+    load_chunk(cur);
+    store_chunk(cur, 0);
+    gt_bar_sync();
+    for (int s = 0;; s ^= 1) {
+        Pos nxt = cur;
+        if (++nxt.kc == cur.KC) nxt = unit_pos(cur.u + gridDim.x, 0);
+        const bool has_next = nxt.u < n_units;
+        if (has_next) load_chunk(nxt);
+        if (PACKED) { mbar_wait(bars + 8 * s, full_use[s] & 1u, p.err, 810 + s); ++full_use[s]; }
+        mma_chunk(acc, s, cur.kc == 0);
+        if (has_next) store_chunk(nxt, s ^ 1);   // (stage s ^ 1 was read by the previous chunk: complete, see below)
+        wgmma_wait<0>();
+        wgmma_hold(acc);
+        gt_bar_sync();   // both warpgroups are done with stage s, and stage s ^ 1 holds the next chunk
+        if (cur.kc == cur.KC - 1) epilogue(cur, acc);
+        if (!has_next) break;
+        cur = nxt;
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == kGtBuildWarps + 1) tmem_dealloc(tmem, 512);
 }
 
 // Pre-pack a B operand (weights: reused by every 128-row tile of the batch) into bf16 hi | lo records in the exact stage
@@ -429,10 +325,10 @@ __global__ void gemm_pack_b_kernel(const float* __restrict__ B, long long ldb, i
     *reinterpret_cast<uint4*>(rec + b_tile + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
 }
 
+// n tile: 128 columns (one B tile is reused by the whole 128-row A tile) or 64 for narrow products
 int gemm_tc_n_tile(long long N, int b_mn) {
-    int nt = N >= 256 ? 256 : (int)((N + 15) / 16 * 16);
-    if (b_mn) nt = (nt + 63) / 64 * 64;
-    return nt;
+    (void)b_mn;
+    return N > 64 ? 128 : 64;
 }
 size_t gemm_tc_packed_b_bytes(long long N, long long K, int b_mn) {
     const int nt = gemm_tc_n_tile(N, b_mn);
@@ -450,13 +346,35 @@ int launch_gemm_pack_b(const float* B, long long ldb, int b_mn, long long N, lon
 // -------------------------------------------------------------------------------------------------------------
 // host side
 // -------------------------------------------------------------------------------------------------------------
+template <int NT, int AMN, int BMN, bool PACKED>
+int launch_gemm_tc_t(const GemmTcParams& p, long long n_units, cudaStream_t st) {
+    static PerDevice per_dev;
+    constexpr uint32_t stage_bytes = 2 * kGtTileA + 2 * (uint32_t)NT * 128u;
+    constexpr uint32_t smem = 2 * stage_bytes + 64 + 128 * (NT + 4) * 4;
+    static_assert(smem <= kGtSmemMax, "gemm_tc: shared memory");
+    const int sm_count = per_dev.ensure([] {
+        return cudaFuncSetAttribute(gemm_tc_kernel<NT, AMN, BMN, PACKED>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    (int)smem);
+    });
+    if (sm_count < 0) return NFB_ERR_CUDA;
+    const unsigned grid = (unsigned)(n_units < sm_count ? n_units : sm_count);
+    gemm_tc_kernel<NT, AMN, BMN, PACKED><<<grid, kGtThreads, smem, st>>>(p);
+    NFB_LAUNCH_CHECK();
+    return NFB_OK;
+}
+template <int NT, int AMN, int BMN>
+int launch_gemm_tc_p(const GemmTcParams& p, long long n_units, cudaStream_t st) {
+    return p.b_packed ? launch_gemm_tc_t<NT, AMN, BMN, true>(p, n_units, st) : launch_gemm_tc_t<NT, AMN, BMN, false>(p, n_units, st);
+}
+template <int NT>
+int launch_gemm_tc_n(const GemmTcParams& p, int a_mn, int b_mn, long long n_units, cudaStream_t st) {
+    if (!a_mn) return b_mn ? launch_gemm_tc_p<NT, 0, 1>(p, n_units, st) : launch_gemm_tc_p<NT, 0, 0>(p, n_units, st);
+    return b_mn ? launch_gemm_tc_p<NT, 1, 1>(p, n_units, st) : launch_gemm_tc_p<NT, 1, 0>(p, n_units, st);
+}
+
 int launch_gemm_tc(const GemmTcArgs& a, int* err, cudaStream_t st) {
     static PerDevice per_dev;
-    const int sm_count = per_dev.ensure([] {
-        cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kGtSmemMax);
-        if (e != cudaSuccess) return e;
-        return cudaFuncSetAttribute(gemm_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kGtSmemMax);
-    });
+    const int sm_count = per_dev.ensure([] { return cudaSuccess; });
     if (sm_count < 0) return NFB_ERR_CUDA;
     NFB_CHECK(a.A && a.B && a.C, NFB_ERR_ARG, "gemm_tc: null operand");
     if (a.M <= 0 || a.N <= 0) return NFB_OK;
@@ -464,15 +382,12 @@ int launch_gemm_tc(const GemmTcArgs& a, int* err, cudaStream_t st) {
     static const int terms = [] { const char* e = getenv("NFB_GEMM_TERMS"); return (e && atoi(e) == 1) ? 1 : 3; }();
     GemmTcParams p{};
     p.A = a.A; p.B = a.B; p.C = a.C; p.lda = a.lda; p.ldb = a.ldb; p.ldc = a.ldc;
-    p.M = a.M; p.N = (int)a.N; p.K = a.K; p.a_mn = a.a_mn; p.b_mn = a.b_mn; p.a_relu = a.a_relu; p.b_relu = a.b_relu;
+    p.M = a.M; p.N = (int)a.N; p.K = a.K; p.a_relu = a.a_relu; p.b_relu = a.b_relu;
     p.bias = a.bias; p.mask = a.mask; p.mulm = a.mulm; p.ldmask = a.ldmask; p.resid = a.resid; p.ldres = a.ldres;
     p.relu_out = a.relu_out; p.terms = terms; p.err = err;
-    // n tile: as wide as possible (one B tile is reused by the whole 128-row A tile), multiple of 16.  MN-major B needs
-    // whole 64-wide blocks.
     const int nt = gemm_tc_n_tile(a.N, a.b_mn);
-    p.n_tile = nt;
     const long long m_tiles = (a.M + 127) / 128;
-    const int n_tiles = (a.N + nt - 1) / nt;
+    const int n_tiles = (int)((a.N + nt - 1) / nt);
     // split K only when there are too few output tiles to fill the machine (weight gradients: K = batch)
     int ks = 1;
     const long long tiles = m_tiles * n_tiles;
@@ -490,19 +405,8 @@ int launch_gemm_tc(const GemmTcArgs& a, int* err, cudaStream_t st) {
     if (ks > 1) NFB_CHECK(!a.bias && !a.mask && !a.resid && !a.relu_out, NFB_ERR_ARG, "gemm_tc: split-K with a non-linear epilogue");
     if (ks > 1 && !a.accumulate)  // the partial products are added with red.global.add: start from zero
         NFB_CUDA(cudaMemset2DAsync(a.C, (size_t)a.ldc * 4, 0, (size_t)a.N * 4, (size_t)a.M, st));
-    const uint32_t stage_bytes = 2 * kGtTileA + 2 * (uint32_t)nt * 128u;
-    constexpr uint32_t kStgBytes = 128 * 65 * 4;  // epilogue staging tile
-    int stages = (int)((kGtSmemMax - kGtBarBytes - 16 - kStgBytes) / stage_bytes);
-    stages = stages > kGtMaxStages ? kGtMaxStages : stages;
-    NFB_CHECK(stages >= 2, NFB_ERR_STATE, "gemm_tc: stage does not fit");
-    p.stages = stages;
-    const uint32_t smem = (uint32_t)stages * stage_bytes + kGtBarBytes + 16 + kStgBytes;
     const long long n_units = tiles * ks;
-    const unsigned grid = (unsigned)(n_units < sm_count ? n_units : sm_count);
-    if (p.b_packed) gemm_tc_kernel<true><<<grid, kGtThreads, smem, st>>>(p);
-    else gemm_tc_kernel<false><<<grid, kGtThreads, smem, st>>>(p);
-    NFB_LAUNCH_CHECK();
-    return NFB_OK;
+    return nt == 64 ? launch_gemm_tc_n<64>(p, a.a_mn, a.b_mn, n_units, st) : launch_gemm_tc_n<128>(p, a.a_mn, a.b_mn, n_units, st);
 }
 
 }  // namespace nfb

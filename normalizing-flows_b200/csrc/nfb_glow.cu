@@ -5,8 +5,8 @@
 // 1x1 convolution W' = (P L U) diag(exp(-s)), b' = -W' t at pack time (`glow_fold_kernel`) and run through
 // the same implicit-GEMM kernel as the ConvNet2d conditioner (nets/cnn.py:33-61: 3x3 -> 1x1 -> 3x3 with
 // LeakyReLU).  The coupling epilogue applies shift/scale (interleaved channels, coupling.py:152-160) and
-// reduces log|det| per sample.  Plain fp32 FFMA tiles for now (parity first); the tcgen05 implicit-GEMM
-// version is future work (DESIGN.md section 7).
+// reduces log|det| per sample.  Conditioner-sized convolutions run on the wgmma implicit GEMM (nfb_conv_tc.cu);
+// the small maps stay on the plain fp32 FFMA tiles below.
 #include <cstdlib>
 #include "nfb_kernels.h"
 
@@ -118,13 +118,13 @@ int launch_conv2d(const float* x, int ctot, int c0, const float* w, const float*
     NFB_CHECK(c0 >= 0 && c0 + cin <= ctot, NFB_ERR_ARG, "conv2d: channel slice out of range");
     const long long M = B * H * W;
     if (M == 0 || cout == 0) return NFB_OK;
-    // conditioner-sized convolutions run on the tensor core (sm_100 only; NFB_CONV_FP32=1 forces this kernel)
+    // conditioner-sized convolutions run on the tensor core (sm_90 only; NFB_CONV_FP32=1 forces this kernel)
     static const bool tc = [] {
         int dev = 0, major = 0;
         if (getenv("NFB_CONV_FP32")) return false;
         if (cudaGetDevice(&dev) != cudaSuccess) return false;
         cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-        return major == 10;
+        return major == 9;
     }();
     if (ks == 1 && cin <= 64 && cout <= 64) {
         const unsigned g = (unsigned)((M + 255) / 256);

@@ -3,10 +3,10 @@
 //   * rqs_shared_kernel    RQ-spline with per-feature parameters shared over the batch
 //                          (PiecewiseRationalQuadraticCDF, neural_spline/coupling.py:221-253)
 //   * linear_kernel        Y = act(X[:,idx]) W^T + b (+R), fp32 FFMA tiles (conditioner nets of
-//                          shapes the fused tcgen05 kernel does not cover)
+//                          shapes the fused tensor-core kernel does not cover)
 //   * pack / log-det / base-density / reduction helpers
 // The flagship shapes run through nfb_fused_rqs.cu instead; these kernels are the same
-// arithmetic in plain fp32 and serve every other shape.  sm_100a only.
+// arithmetic in plain fp32 and serve every other shape.  Built for sm_90a.
 #include "nfb_kernels.h"
 #include "nfb_spline.cuh"
 
@@ -400,8 +400,8 @@ __global__ void lu_pack_kernel(const float* __restrict__ lower_e, const float* _
                                float* __restrict__ Winv, float* __restrict__ logabsdet) {
     lu_pack_block(lower_e, upper_e, udiag, eps, n, Wout, Winv, logabsdet);
 }
-// every LU layer of a flow in ONE launch, one block per layer (a 32-layer stack spent 3.9 ms per repack in 32 serialised
-// single-block launches: profiles/r02b_launches_bench_steps2.csv of the packing phase)
+// every LU layer of a flow in ONE launch, one block per layer (32 serialised single-block launches dominated the
+// packing phase of a 32-layer stack)
 __global__ void lu_pack_batched_kernel(const LuPackArgs* __restrict__ args) {
     const LuPackArgs a = args[blockIdx.x];
     lu_pack_block(a.lower_e, a.upper_e, a.udiag, a.eps, a.n, a.W, a.Winv, a.logabsdet);

@@ -134,21 +134,25 @@ size_t affine_op_size();
 int launch_affine_stack(const void* ops_dev, int n_ops, const float* zin, float* zout, float* logq,
                         long long rows, int d, int accumulate, int direction, cudaStream_t st);
 
-// ---- fused tcgen05 neural-spline block (nfb_fused_rqs.cu) ----
-struct __align__(16) FusedStep {
-    uint16_t bytes16;    // weight record size / 16
-    uint8_t n8;          // MMA N / 8 (rows of the record's tile(s))
-    uint8_t a0, a1, a2;  // A-operand tiles to multiply the record's (first) tile with: a0 and (unless 0xFF) a1; tile t < 4 =
-                         //   hi part of K-chunk t, 4 + t = lo part.  a2 != 0xFF: MERGED record -- a second [N x 64] tile (W_lo)
-                         //   follows the first (W_hi) and is multiplied with A tile a2 & 7 (and, bit 7 set, with its lo twin)
-    uint16_t ctl;        // [0,9) TMEM column | [9] first (overwrite) | [10,13) wait | [13,16) signal
-    uint8_t dr[4];       // per K=16 slab: the slab reaches the tile's rows [8 dr, 8 n8) only (dr even; 0xFF: none)
-    uint8_t pad_[4];
+// ---- fused neural-spline block (nfb_fused_rqs.cu) ----
+constexpr int kFusedTileRows = 64;          // rows of a work unit (the M of one wgmma)
+constexpr int kFusedFeaturesPerChunk = 2;   // spline features per final-layer record (N = 24 per feature)
+// One weight record of the packed stream: a W_hi tile followed by its W_lo twin, multiplied with K-chunk kc of the A
+// operand.  Each tile stacks the [8 n8 x 64] halves of the two consumer warpgroups of the fused kernel (warpgroup 0's
+// output slice, then warpgroup 1's).  The records of a slice are consecutive; the slices come in the order the kernel
+// consumes them (LU map, hidden GEMMs slice by slice, final-layer chunks).
+enum { kStepFirst = 1,    // first record of its slice: overwrites the accumulator
+       kStepLast = 2,     // last record of its slice: the slice's epilogue follows
+       kStepQuad = 4,     // four products (W_lo A_lo as well): the LU map, which transforms z itself
+       kStepSkip0 = 8,    // warpgroup 0's half is all zero (MADE mask): no products
+       kStepSkip1 = 16 }; // the same for warpgroup 1
+struct __align__(8) FusedStep {
+    uint16_t bytes16;    // record size / 16
+    uint8_t n8;          // rows of each warpgroup's half of a tile / 8 (MMA N / 8)
+    uint8_t kc;          // A-operand K-chunk
+    uint8_t flags;       // kStep*
+    uint8_t pad_[3];
 };
-// wait codes : 0 none, 1 a_ready[kc], 2+i chunk_empty[i], 5 a_ready[H/64 - 1] + chunk_empty[0],
-//              6 a_ready[kc] + chunk_empty[1]   (kc = a0 & 3)
-// signal codes: 0 none, 1 acc_full, 2+i chunk_full[i] (i < 2), 4+kc acc_blk[kc] (kc < 3: the output chunks whose last
-//               contributing K-chunk is kc are final), 7 lu_full
 
 // One fused [LULinearPermute +] spline block, packed.  Device-resident (uploaded at pack time): the kernel
 // reads it through a pointer so that ONE persistent launch can walk a whole stack of blocks.
@@ -166,16 +170,13 @@ struct FusedLayer {
     signed char in_idx[64];    // conditioner input column per k (-1 = zero pad)
     unsigned char tr_idx[64];  // transformed feature columns
     unsigned char id_idx[64];  // identity feature columns (coupled layer)
-    unsigned char chunk_order[16];  // final-layer chunks in processing order (first one reads every K-chunk)
-    alignas(4) unsigned char blk_sig[7 * 4];   // [hidden phase][output chunk] -> barrier that announces the chunk: 0..2 = acc_blk[kc]
-                                    // (block-triangular MADE layer: final after K-chunk kc), 3 = acc_full (whole GEMM)
     // fp16 operand scaling (all powers of two; nfb_api.cu plan_scales): index 0 = LU stage, 1 + g = GEMM g of the
     // conditioner (g = n_hidden: final layer).  A operand = true value * u_row * a_sc; true value = acc * a_inv / u_row.
     float a_sc[10], a_inv[10];
     alignas(16) float bias_h[7 * 256];   // [n_hidden <= 7][256], residual biases pre-summed along the stream
-    alignas(16) float bias_f[82 * 24];   // [(n_chunks+1)*F <= 82][24] final-layer bias in chunk/column order
+    alignas(16) float bias_f[64 * 24];   // [n_chunks * F <= 64][24] final-layer bias in chunk/column order
 };
-// Launch arguments.  Work units are (layer, 128-row tile) pairs in layer-major order; unit (l, t) may start
+// Launch arguments.  Work units are (layer, kFusedTileRows-row tile) pairs in layer-major order; unit (l, t) may start
 // once progress[t] >= l.  Rows of a tile are private to it, so layers l >= 1 update `zout` in place.
 struct FusedParams {
     const FusedLayer* layers;  // [n_layers], in application order
@@ -194,8 +195,6 @@ struct FusedParams {
     const int* in_ready;       // optional: number of rows of `zin` that have landed (chunked H2D in flight, written
                                // by the copy engine); layer-0 tiles wait for their rows.  null = all resident
     int* err;
-    int poll_all;              // every epilogue thread polls its mbarrier (1, default) or one lane per warp (0: NFB_POLL_LANE0)
-    long long* prof;           // optional [128] clock64 stamps (debug)
 };
 int launch_fused_rqs(const FusedParams& p, int sm_count, int sample, cudaStream_t st);
 int launch_fold_lu(const float* E0, const float* Elu, const float* blu, const int* in_idx, int H, int d, float gain,
@@ -241,8 +240,8 @@ int launch_glu_residual(const float* h, const float* t, const float* c, long lon
 int launch_rowdot(const float* a, const float* b, long long rows, int d, float c, int accumulate, float* out,
                   cudaStream_t st);
 
-// tcgen05 fp32 accumulation truncates: relative loss per K=16 MMA step, compensated at pack time (nfb_api.cu)
-constexpr float kAccStepGain = 2.9e-8f;
+// tensor-core fp32 accumulation truncates: relative loss per K=16 MMA step, compensated at pack time (nfb_api.cu)
+constexpr float kAccStepGain = 2.4e-8f;
 // implicit-GEMM convolution on the tensor core (csrc/nfb_conv_tc.cu)
 bool conv_tc_supported(int cin, int cout, int ks);
 int launch_conv2d_tc(const float* x, int ctot, int c0, const float* w, const float* bias, float* y, long long B,
@@ -254,8 +253,6 @@ int launch_build_effective(const float* W, const float* M, int src_cols, const i
 struct PackRec { int row0, nrows, kc, pad_; unsigned long long off_hi, off_lo; };  // one weight record of a GEMM
 int launch_pack_records(const float* E, int k_pad, const PackRec* recs_dev, int n_recs, int max_rows, float scale,
                         uint8_t* base, cudaStream_t st);
-int launch_pack_record(const float* E, int k_pad, int row0, int nrows, int kc, float scale, uint8_t* out_hi,
-                       uint8_t* out_lo, cudaStream_t st);
 int launch_swizzle_split(const float* E, int n_pad, int k_pad, int rows_per_rec, int nsplit, float scale,
                          uint8_t* out, cudaStream_t st);
 int launch_matrix_norms(const float* E, int n, int k, float* out3, cudaStream_t st);

@@ -1,4 +1,4 @@
-"""normflows-b200: the coupling-stack hot path of `normflows` as hand-written sm_100a CUDA kernels
+"""normflows-b200: the coupling-stack hot path of `normflows` as hand-written sm_90a (H100) CUDA kernels
 behind the reference's `nf.NormalizingFlow` / `nf.flows.*` nn.Module API.
 
     import normflows as nf            # this package; sys.path entry: <repo>/normalizing-flows_b200

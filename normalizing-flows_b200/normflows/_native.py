@@ -47,7 +47,7 @@ def require_cuda_f32(t, what="input"):
         raise TypeError(f"{what} must be a torch.Tensor")
     if not t.is_cuda:
         raise RuntimeError(
-            f"{what} is on {t.device}: normflows-b200 runs the transform stack as sm_100a CUDA kernels "
+            f"{what} is on {t.device}: normflows-b200 runs the transform stack as sm_90a CUDA kernels "
             "only; there is no CPU/eager fallback. Move the model and data to a CUDA device.")
     if t.dtype != torch.float32:
         raise RuntimeError(f"{what} has dtype {t.dtype}; the CUDA path computes in float32 only")

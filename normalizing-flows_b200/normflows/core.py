@@ -4,7 +4,7 @@ Same public surface: forward, forward_and_log_det, inverse, inverse_and_log_det,
 log_prob, save, load.  Where the reference loops over layers in Python and accumulates `log_q` with a
 tiny kernel per layer (core.py:96-102), this class hands the whole stack to one `nfb_flow` so that
 log-det accumulation happens in kernel epilogues and adjacent layers fuse
-([LULinearPermute + spline block] -> one tcgen05 kernel).  If any layer is not a `NativeFlow`, it
+([LULinearPermute + spline block] -> one tensor-core kernel).  If any layer is not a `NativeFlow`, it
 falls back to the reference's per-layer loop over whatever the layers implement."""
 import torch
 from torch import nn

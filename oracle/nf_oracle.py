@@ -7,12 +7,12 @@ imports it.  Only `tests/`, `__graft_entry__.smoke()` and `bench.py`'s
 `cpu_baseline` / `--impl reference` leg may import it.
 
 Pinned against the real reference: `tests/golden/make_golden.py` imports the
-reference package from /root/reference, dumps state_dicts + inputs + outputs
+reference package from its checkout (oracle/reference.py), dumps state_dicts + inputs + outputs
 (fp64 and fp32) to `tests/golden/*.npz`, and `tests/test_oracle_golden.py`
 replays every fixture through this file (fp64: rtol 1e-12, fp32: rtol 2e-5).
 
 Every function cites the reference file:line it restates (paths relative to
-/root/reference/normflows/).  The restatement is mask-free: where the reference
+the reference's normflows/ package).  The restatement is mask-free: where the reference
 uses boolean-mask indexing (utils/splines.py:40-41,77-95) it evaluates every
 element and selects with `where`, which is the formulation the CUDA kernels use.
 

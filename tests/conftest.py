@@ -1,7 +1,7 @@
 """pytest config: the `gpu` marker + import paths.
 
-`-m "not gpu"` runs here on CPU (oracle vs golden vectors, host logic, C-ABI symbol
-check); `-m gpu` runs on the B200 box and calls through the C-ABI library."""
+`-m "not gpu"` runs without a GPU (oracle vs golden vectors, host logic, C-ABI symbol
+check); `-m gpu` needs an H100 and calls through the C-ABI library."""
 import json
 import os
 import sys
@@ -19,15 +19,20 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100: the library is built for sm_90a)")
 
 
 def load_golden(name):
-    """-> (spec, sd, arrays) from tests/golden/<name>.npz (minted from the reference)."""
+    """-> (spec, sd, arrays) from tests/golden/<name>.npz (minted from the reference).  A golden whose weights are too
+    large to store carries a rebuild recipe and digests instead (tests/helpers.py state_dict_from_recipe)."""
     f = np.load(os.path.join(GOLDEN, name + ".npz"), allow_pickle=False)
-    sd = {k[4:]: f[k] for k in f.files if k.startswith("sd__")}
+    if "sd_recipe" in f.files:
+        from helpers import state_dict_from_recipe
+        sd = state_dict_from_recipe(json.loads(str(f["sd_recipe"])), json.loads(str(f["sd_sha256"])))
+    else:
+        sd = {k[4:]: f[k] for k in f.files if k.startswith("sd__")}
     spec = json.loads(str(f["spec"])) if "spec" in f.files else None
-    arr = {k: f[k] for k in f.files if not k.startswith("sd__") and k != "spec"}
+    arr = {k: f[k] for k in f.files if not k.startswith("sd__") and k not in ("spec", "sd_recipe", "sd_sha256")}
     return spec, sd, arr
 
 

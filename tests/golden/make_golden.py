@@ -1,15 +1,18 @@
-"""Mint golden vectors from the REAL reference (normflows 1.7.3 at /root/reference).
-
-Run in the build container only (the GPU box has no /root/reference):
+"""Mint golden vectors from the REAL reference (normflows 1.7.3): a checkout of it at $NORMFLOWS_REFERENCE or next to
+this repository (oracle/reference.py finds it).  Needs no GPU:
     python tests/golden/make_golden.py
 Writes tests/golden/<case>.npz, each holding:
-    spec (json string), sd__<key> (state_dict arrays), x, [y], and for fp64 & fp32:
+    spec (json string), sd__<key> (state_dict arrays) -- or, for models too large to store, sd_recipe (how
+    tests/helpers.py state_dict_from_recipe rebuilds the state_dict with this package's constructors, which draw from
+    torch's generator exactly like the reference's) and sd_sha256 (digests that check the rebuild) --, x, [y], and for
+    fp64 & fp32:
     log_prob, z, kld, per-layer log_det (ld__<i>) in the density direction, and
     fwd_z / fwd_ld (forward_and_log_det of the latent = sampling direction).
 The reference ships no golden vectors (SURVEY.md section 4), so these files are what
 pins the oracle (oracle/nf_oracle.py) and the CUDA path to the reference.
 torch version used is recorded in each file.
 """
+import hashlib
 import json
 import os
 import sys
@@ -17,10 +20,37 @@ import sys
 import numpy as np
 import torch
 
-sys.path.insert(0, "/root/reference")
+HERE = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
+from oracle import reference  # noqa: E402
+
+if reference.source() is None:
+    sys.exit("make_golden.py: no checkout of the reference (set NORMFLOWS_REFERENCE)")
+sys.path.insert(0, os.path.dirname(reference.source()))
 import normflows as nf  # noqa: E402  (the reference)
 
-HERE = os.path.dirname(os.path.abspath(__file__))
+assert os.path.dirname(nf.__file__) == reference.source(), nf.__file__
+
+
+def sha256(a):
+    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
+
+
+def save_parts(name, out, max_bytes=900_000):
+    """np.savez_compressed into <name>.npz, continued in <name>.2.npz, ... so that no file exceeds max_bytes
+    (fp64 vectors do not compress; tests/helpers.py load_npz_parts reads them back as one dict)."""
+    keys, part = list(out), 1
+    while keys:
+        take = []
+        while keys:
+            take.append(keys.pop(0))
+            fn = os.path.join(HERE, name + ("" if part == 1 else f".{part}") + ".npz")
+            np.savez_compressed(fn, **{k: out[k] for k in take})
+            if os.path.getsize(fn) > max_bytes and len(take) > 1:
+                keys.insert(0, take.pop())
+                np.savez_compressed(fn, **{k: out[k] for k in take})
+                break
+        part += 1
 
 
 def perturb(model, sigma, seed):
@@ -31,13 +61,17 @@ def perturb(model, sigma, seed):
             p.add_(sigma * torch.randn(p.shape, generator=g, dtype=p.dtype))
 
 
-def dump(name, model, spec, x, y=None, sampling=True, extra=None):
+def dump(name, model, spec, x, y=None, sampling=True, extra=None, recipe=None):
     out = {"spec": json.dumps(spec), "torch_version": torch.__version__,
            "x": x.numpy().astype(np.float64)}
     if y is not None:
         out["y"] = y.numpy()
-    for k, v in model.state_dict().items():
-        out["sd__" + k] = v.detach().numpy()  # float32 params are stored exactly; .double() models are casts of these
+    if recipe is None:
+        for k, v in model.state_dict().items():
+            out["sd__" + k] = v.detach().numpy()  # float32 params are stored exactly; .double() models are casts of these
+    else:
+        out["sd_recipe"] = json.dumps(recipe)
+        out["sd_sha256"] = json.dumps({k: sha256(v.detach().numpy()) for k, v in model.state_dict().items()})
     for tag, dt in (("f64", torch.float64), ("f32", torch.float32)):
         m = model.to(dt)
         xx = x.to(dt)
@@ -76,6 +110,8 @@ def dump(name, model, spec, x, y=None, sampling=True, extra=None):
 
 
 def nsf(kind, d, layers, hidden, blocks, seed, sigma, tail_bound=3.0, bins=8, lu_identity=True):
+    """Constructors under torch.manual_seed(seed), then perturb(sigma, seed + 1); tests/helpers.py nsf_model repeats
+    this recipe with this package's classes."""
     torch.manual_seed(seed)
     flows, spec = [], []
     for i in range(layers):
@@ -234,9 +270,7 @@ def main():
     case_spline_edges()
     # the survey's sanity anchors (SURVEY.md 8c.2) are re-derived by tests from these files
     for kind in ("ar", "coupled"):
-        m, spec = nsf(kind, 64, 2, 256, 2, seed=0, sigma=0.05)
-        x = torch.randn(48, 64, generator=torch.Generator().manual_seed(1234)) * 1.5
-        dump(f"nsf_{kind}_d64_h256_l2", m, spec, x, sampling=(kind == "coupled"))
+        case_nsf64(kind)
         m, spec = nsf(kind, 5, 3, 128, 2, seed=20, sigma=0.1, lu_identity=False)
         x = torch.randn(64, 5, generator=torch.Generator().manual_seed(21)) * 1.5
         dump(f"nsf_{kind}_d5_h128_l3", m, spec, x)
@@ -248,8 +282,20 @@ def main():
     case_glow()
 
 
+def case_nsf64(kind):
+    """The flagship block shape, 2 layers (5 MB of weights): stored as a rebuild recipe + digests.
+        python tests/golden/make_golden.py nsf64"""
+    recipe = {"builder": "nsf", "kind": kind, "d": 64, "layers": 2, "hidden": 256, "blocks": 2, "seed": 0, "sigma": 0.05}
+    m, spec = nsf(kind, 64, 2, 256, 2, seed=0, sigma=0.05)
+    x = torch.randn(48, 64, generator=torch.Generator().manual_seed(1234)) * 1.5
+    dump(f"nsf_{kind}_d64_h256_l2", m, spec, x, sampling=(kind == "coupled"), recipe=recipe)
+
+
 if __name__ == "__main__" and len(sys.argv) == 1:
     main()
+if __name__ == "__main__" and len(sys.argv) > 1 and sys.argv[1] == "nsf64":
+    case_nsf64("ar")
+    case_nsf64("coupled")
 if __name__ == "__main__" and len(sys.argv) > 1 and sys.argv[1] == "glow":
     case_glow()
 
@@ -292,7 +338,7 @@ def case_grads():
         for k, p in m.named_parameters():
             if p.grad is not None:
                 out["grad__" + k] = p.grad.numpy()
-        np.savez_compressed(os.path.join(HERE, f"grads_nsf_{kind}_d5_h128_l3.npz"), **out)
+        save_parts(f"grads_nsf_{kind}_d5_h128_l3", out)
         print("wrote grads", kind, len(out))
 
 
@@ -655,3 +701,55 @@ def case_spline_circular():
 
 if __name__ == "__main__" and len(sys.argv) > 1 and sys.argv[1] == "spline_circular":
     case_spline_circular()
+
+
+def case_glow_c3():
+    """BASELINE config 3 at its real shape (examples/glow.ipynb cell 2 verbatim: L=3, K=16, hidden 256, 3x32x32, 10
+    classes; 48 Glow blocks, 8 M parameters), fp64 on 64 images.  Constructors under torch.manual_seed(0), the
+    ActNorm data-dependent init on the batch, then every parameter moved off its init by 0.02 randn (seed 2).  Stored:
+    the entries the data-dependent init set (a few KB), digests of the whole state_dict and of the inputs, and the
+    reference's log_prob; tests/helpers_glow.py glow_c3_state_dict rebuilds the rest.
+        python tests/golden/make_golden.py glow_c3"""
+    def build():
+        torch.manual_seed(0)
+        L, K, hidden, shape, ncls = 3, 16, 256, (3, 32, 32), 10
+        q0, merges, flows = [], [], []
+        for i in range(L):
+            flows_ = []
+            for j in range(K):
+                flows_ += [nf.flows.GlowBlock(shape[0] * 2 ** (L + 1 - i), hidden, split_mode="channel", scale=True)]
+            flows_ += [nf.flows.Squeeze()]
+            flows += [flows_]
+            if i > 0:
+                merges += [nf.flows.Merge()]
+                ls = (shape[0] * 2 ** (L - i), shape[1] // 2 ** (L - i), shape[2] // 2 ** (L - i))
+            else:
+                ls = (shape[0] * 2 ** (L + 1), shape[1] // 2 ** L, shape[2] // 2 ** L)
+            q0 += [nf.distributions.ClassCondDiagGaussian(ls, ncls)]
+        return nf.MultiscaleFlow(q0, flows, merges).double()
+    batch = 64
+    model = build()
+    g = torch.Generator().manual_seed(1)
+    x = torch.rand(batch, 3, 32, 32, generator=g)
+    y = torch.randint(10, (batch,), generator=g)
+    with torch.no_grad():
+        model.log_prob(x.double(), y)  # ActNorm data-dependent init
+        perturb(model, 0.02, 2)
+        lp = model.log_prob(x.double(), y)
+    sd = {k: v.detach() for k, v in model.state_dict().items()}
+    # the entries the data-dependent init changed (perturb() moves every parameter: compare against init + the same draw)
+    again = build()
+    perturb(again, 0.02, 2)
+    moved = {k: v.detach() for k, v in again.state_dict().items()}
+    out = {"torch_version": torch.__version__, "log_prob_f64": lp.numpy(), "x_sha256": sha256(x.numpy()),
+           "y_sha256": sha256(y.numpy()), "sd_sha256": json.dumps({k: sha256(v.numpy()) for k, v in sd.items()})}
+    for k, v in sd.items():
+        if not torch.equal(v, moved[k]):
+            out["init__" + k] = v.numpy()
+    np.savez_compressed(os.path.join(HERE, "glow_c3.npz"), **out)
+    print("wrote glow_c3", sum(1 for k in out if k.startswith("init__")), "data-initialised entries; log_prob",
+          lp[:3].numpy())
+
+
+if __name__ == "__main__" and len(sys.argv) > 1 and sys.argv[1] == "glow_c3":
+    case_glow_c3()

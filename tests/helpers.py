@@ -1,4 +1,8 @@
 """Shared test helpers: build OUR modules from a golden `spec` and load the reference state_dict."""
+import glob
+import hashlib
+import os
+
 import numpy as np
 import torch
 
@@ -63,3 +67,53 @@ def annotate_spec(spec, sd):
 def rel_err(a, b):
     a, b = np.asarray(a, dtype=np.float64), np.asarray(b, dtype=np.float64)
     return np.max(np.abs(a - b) / (np.abs(b) + 1e-12))
+
+
+def sha256(a):
+    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
+
+
+def check_digests(sd, digests, what):
+    """sd must be bit-identical to the arrays the golden was minted from (digests: key -> sha256)."""
+    assert set(sd) == set(digests), f"{what}: state_dict keys differ from the golden's"
+    bad = [k for k in sd if sha256(sd[k]) != digests[k]]
+    assert not bad, f"{what}: rebuilt entries differ from the reference's: {bad[:5]}"
+
+
+def nsf_model(kind, d, layers, hidden, blocks, seed, sigma, tail_bound=3.0, bins=8, lu_identity=True):
+    """tests/golden/make_golden.py nsf() with this package's classes: constructors under torch.manual_seed(seed) (they
+    draw from torch's generator exactly like the reference's), then every parameter moved by sigma * randn (seed + 1)."""
+    torch.manual_seed(seed)
+    flows = []
+    for i in range(layers):
+        if kind == "ar":
+            flows += [nf.flows.AutoregressiveRationalQuadraticSpline(d, blocks, hidden, num_bins=bins, tail_bound=tail_bound)]
+        else:
+            flows += [nf.flows.CoupledRationalQuadraticSpline(d, blocks, hidden, num_bins=bins, tail_bound=tail_bound,
+                                                             reverse_mask=bool(i % 2))]
+        flows += [nf.flows.LULinearPermute(d, identity_init=lu_identity)]
+    model = nf.NormalizingFlow(nf.distributions.DiagGaussian(d, trainable=False), flows)
+    g = torch.Generator().manual_seed(seed + 1)
+    with torch.no_grad():
+        for p in model.parameters():
+            p.add_(sigma * torch.randn(p.shape, generator=g, dtype=p.dtype))
+    return model
+
+
+def state_dict_from_recipe(recipe, digests):
+    """The state_dict of a golden stored as a rebuild recipe (make_golden.py dump(recipe=...)), checked bit for bit."""
+    r = dict(recipe)
+    assert r.pop("builder") == "nsf", recipe
+    sd = {k: v.detach().numpy() for k, v in nsf_model(**r).state_dict().items()}
+    check_digests(sd, digests, f"nsf recipe {recipe}")
+    return sd
+
+
+def load_npz_parts(path):
+    """<stem>.npz and its continuations <stem>.2.npz, ... (make_golden.py save_parts) as one dict."""
+    stem = path[:-4]
+    out = {}
+    for fn in [path] + sorted(glob.glob(stem + ".[0-9].npz")):
+        f = np.load(fn, allow_pickle=False)
+        out.update({k: f[k] for k in f.files})
+    return out

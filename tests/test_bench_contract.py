@@ -1,6 +1,7 @@
 """bench.py contract checks that need no GPU: the reference arm (`--impl reference`, the unmodified reference
-package from baseline/_ref on the host cores; the oracle port only if that copy is absent) must print ONE JSON line carrying the same metric / unit / workload as the GPU arm plus the keys the driver
-reads; ranks other than 0 print nothing."""
+package from oracle/_ref on the host cores; the oracle port only if that copy is absent) must print ONE JSON line
+carrying the same metric / unit / workload as the GPU arm plus the keys a reader of the line relies on; ranks other
+than 0 print nothing."""
 import json
 import os
 import subprocess

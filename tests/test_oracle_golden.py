@@ -2,10 +2,13 @@
 tests/golden/ was produced by tests/golden/make_golden.py importing normflows 1.7.3.
 fp64 must agree to round-off (the restatement is the same arithmetic); fp32 to a few ulp-ish
 multiples because numpy/OpenBLAS and ATen/MKL order their sums differently."""
+import os
+
 import numpy as np
 import pytest
 
-from conftest import load_golden
+from conftest import GOLDEN, load_golden
+from helpers import load_npz_parts
 from oracle import nf_oracle as O
 
 NF_CASES = ["nsf_ar_d64_h256_l2", "nsf_ar_d5_h128_l3", "nsf_ar_d2_h32_l2_k4",
@@ -117,11 +120,11 @@ def test_gradient_oracle_matches_reference_autograd(kind):
     gradients minted from the reference's own autograd in fp64 (make_golden.py grads): every parameter + input."""
     from oracle import nf_oracle_grad as G
     spec, sd, _ = load_golden(f"nsf_{kind}_d5_h128_l3")
-    g = np.load(f"tests/golden/grads_nsf_{kind}_d5_h128_l3.npz")
+    g = load_npz_parts(os.path.join(GOLDEN, f"grads_nsf_{kind}_d5_h128_l3.npz"))
     loss, grads, gx = G.forward_kld_grads(spec, sd, g["x"].astype(np.float64))
     assert loss == pytest.approx(float(g["kld"]), rel=1e-6)  # the reference accumulates log_q in fp32 (core.py:96)
     np.testing.assert_allclose(gx, g["grad__x"], rtol=1e-9, atol=1e-12)
-    names = [k[6:] for k in g.files if k.startswith("grad__") and k != "grad__x"]
+    names = [k[6:] for k in g if k.startswith("grad__") and k != "grad__x"]
     assert len(names) >= 48 and set(names) == set(grads)
     for n in names:
         np.testing.assert_allclose(grads[n], g["grad__" + n], rtol=1e-9, atol=1e-12, err_msg=n)

@@ -3,8 +3,8 @@
       batch 4096, forward_kld
   C3  Glow (examples/glow.ipynb cell 2): L=3, K=16, hidden 256, 3x32x32 images, batch 1024, forward_kld
   C2' the Coupled RQ-NSF variant of the bench line (SURVEY 8d reports both)
-Device-resident inputs, CUDA events, median of the timed calls.  Writes one JSON line per configuration.
-Run on the GPU box:  python tools/bench_configs.py > gpurun_out/configs.json"""
+Device-resident inputs, CUDA events, median of the timed calls.  Prints one JSON line per configuration:
+    python tools/bench_configs.py [c1 c2 c3 c5]"""
 import json
 import os
 import sys
@@ -69,7 +69,7 @@ def glow():
     y = torch.randint(ncls, (1024,)).cuda()
     m.forward_kld(x, y)  # ActNorm init
     ms = timed(lambda: m.forward_kld(x, y), warmup=2, iters=8)
-    return {"config": "C3 Glow L=3 K=16 hidden 256, 3x32x32, batch 1024, forward_kld (one nfb_glow_block call per GlowBlock: folded 1x1 conv, fused tcgen05 conditioner, tap-form coupling)",
+    return {"config": "C3 Glow L=3 K=16 hidden 256, 3x32x32, batch 1024, forward_kld (one nfb_glow_block call per GlowBlock: folded 1x1 conv, fused wgmma conditioner, tap-form coupling)",
             "ms": ms, "images_per_s": 1024 / ms * 1e3, "tflops_algorithmic": 1.303e9 * 1024 / ms / 1e9}
 
 

@@ -102,39 +102,6 @@ elif mode == "time":
                 traceback.print_exc()
 print("done", mode, flush=True)
 
-if mode == "prof":
-    import ctypes as C
-    from normflows import _lib as L
-    B = int(sys.argv[2]) if len(sys.argv) > 2 else 65536
-    for kind in ("ar",):
-        m = rand_model(kind, 2)
-        x = (torch.randn(B, 64) * 1.5).cuda()
-        m.forward_kld(x); torch.cuda.synchronize()
-        h = m._stack()._h
-        lib = L.lib()
-        lib.nfb_debug_profile.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-        lib.nfb_debug_profile(h, 1, None)
-        m.forward_kld(x); torch.cuda.synchronize()
-        buf = (C.c_longlong * 2048)()
-        lib.nfb_debug_profile(h, 0, buf)
-        n = buf[127]
-        t = [buf[i] - buf[0] for i in range(n)]
-        print(f"prof {kind}: {n} stamps (cycles since tile start; deltas)")
-        print("  abs  :", t)
-        print("  delta:", [t[i] - t[i - 1] for i in range(1, n)])
-        mm = [buf[128 + i] - buf[0] for i in range(380) if buf[128 + i]]
-        print(f"  mma issue times ({len(mm)} steps):", mm)
-        reach = [buf[512 + i] - buf[0] for i in range(len(mm))]
-        opnd = [buf[896 + i] - buf[0] for i in range(len(mm))]
-        print("  step reached      :", reach)
-        print("  waited for A/chunk:", [opnd[i] - reach[i] for i in range(len(mm))])
-        print("  waited for weights:", [mm[i] - opnd[i] for i in range(len(mm))])
-        issued = [buf[1280 + i] - buf[0] for i in range(len(mm))]
-        comm = [buf[1664 + i] - buf[0] for i in range(len(mm))]
-        print("  MMA issue took    :", [issued[i] - mm[i] for i in range(len(mm))])
-        print("  commits took      :", [comm[i] - issued[i] for i in range(len(mm))])
-        print("  to next step      :", [reach[i + 1] - comm[i] for i in range(len(mm) - 1)])
-
 if mode == "spline":
     import ctypes as C
     from normflows import _lib as L
@@ -153,7 +120,7 @@ if mode == "spline":
         ms = timeit(run, n=11, warm=3)
         byt = B * T * (P * 4 + 8) + B * 8
         print(f"spline standalone inverse={inv}: {ms*1e3:.1f} us  {byt/ms/1e6:.1f} GB/s  "
-              f"frac of 6580 = {byt/ms/1e6/6580.3:.3f}", flush=True)
+              f"of the H100 SXM data sheet's 3350 = {byt/ms/1e6/3350:.3f}", flush=True)
 
 if mode == "stackdbg":
     spec, sd, a = load_golden("nsf_ar_d64_h256_l2")

@@ -3,8 +3,10 @@ and measure the log_prob error of the 32-layer bench model on chosen rows.  Ever
 stays in fp64, so the numbers isolate the operand-split error of each candidate scheme.
     python tools/numerics_emul.py [row_lo row_hi]
 """
+import os
 import sys
-sys.path[:0] = ["/root/repo", "/root/repo/normalizing-flows_b200"]
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path[:0] = [ROOT, os.path.join(ROOT, "normalizing-flows_b200")]
 import numpy as np, torch, bench
 from oracle import nf_oracle as O
 

@@ -1,8 +1,10 @@
 """Offline emulation of the PLANNED fp16-split numerics of the fused kernel (per-row power-of-two unit u = 2^-e_r from
 the row's input magnitude, static per-GEMM power-of-two scales from guaranteed infinity-norm bounds, 3-term 2-way
 fp16 split for conditioner GEMMs, 4-term for the LU map), inside the fp64 oracle.  CPU only."""
+import os
 import sys
-sys.path[:0] = ["/root/repo", "/root/repo/normalizing-flows_b200"]
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path[:0] = [ROOT, os.path.join(ROOT, "normalizing-flows_b200")]
 import numpy as np, torch, bench
 from oracle import nf_oracle as O
 
@@ -44,7 +46,7 @@ def plan(norms, bmaxs, b_in0):
     bounds_in.append(B_h)  # final layer input
     pa = [14 - cl2(b) for b in bounds_in]
     pw = [13 - cl2(nm[1]) for nm in norms]
-    # GEMMs that accumulate onto the residual stream in TMEM (0, 2, 4, ...) share pa + pw
+    # GEMMs that accumulate onto the residual stream (0, 2, 4, ...) share pa + pw
     hs = [0] + list(range(2, n - 1, 2))
     P = min(pa[i] + pw[i] for i in hs)
     for i in hs:
