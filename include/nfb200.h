@@ -209,6 +209,41 @@ int nfb_class_cond_diag_gaussian_log_prob(const float* z_dev, const int64_t* y_d
                                           const float* log_scale_dev, float* log_q_dev, int64_t batch,
                                           int32_t dim, int32_t num_classes, int32_t accumulate, void* stream);
 
+/* ---- training pass of the image path (`MultiscaleFlow.forward_kld(x, y).backward()`, examples/glow.ipynb cell 4) ----
+ * Adjoints of the density-direction operators above; g_* are gradients of a scalar loss. */
+
+/* Weight / bias gradient of nfb_conv2d: gw[n, c, kh, kw] (+)= sum_{b,h,w} gy[b, n, h, w] x[b, c0+c, h+kh-k/2, w+kw-k/2]
+ * and gb[n] (+)= sum_{b,h,w} gy[b, n, h, w] (gw or gb may be NULL); k = 1, 3 or 5.  Tensor core (split bf16, fp32
+ * accumulation over pixel splits of <= 2048 pixels, splits summed in fp64): deterministic. */
+int nfb_conv2d_wgrad(const float* x_dev, int32_t x_channels, int32_t c0, const float* gy_dev, float* gw_dev, float* gb_dev,
+                     int64_t batch, int32_t cin, int32_t height, int32_t width, int32_t cout, int32_t ksize,
+                     int32_t accumulate, void* stream);
+/* Data gradient of nfb_conv2d (w [cout, cin, k, k]): gx [B, cin, H, W] (+)= conv2d(gy, w rotated by 180 degrees with
+ * in/out swapped); mask_act (optional, [B, cin, H, W]) multiplies the result by LeakyReLU'(mask_act) =
+ * (mask_act > 0 ? 1 : mask_slope) -- the post-activation tensor of the layer input suffices for slope >= 0. */
+int nfb_conv2d_dgrad(const float* gy_dev, const float* w_dev, float* gx_dev, int64_t batch, int32_t cin, int32_t height,
+                     int32_t width, int32_t cout, int32_t ksize, const float* mask_act_dev, float mask_slope,
+                     int32_t accumulate, void* stream);
+/* Adjoint of nfb_affine_coupling_image in the density direction: z = the coupling's input [B, C, H, W], param its
+ * conditioner output, g_out [B, C, H, W], g_log_det [B] (may be NULL).  Writes the z2 channels of g_z [B, C, H, W]
+ * (its z1 channels are left to the caller) and g_param [B, (scale?2:1)*n2, H, W] in param's interleaved layout. */
+int nfb_affine_coupling_image_backward(const float* z_dev, const float* param_dev, const float* g_out_dev,
+                                       const float* g_log_det_dev, float* g_z_dev, float* g_param_dev, int64_t batch,
+                                       int32_t channels, int32_t hw, int32_t scale, int32_t scale_map, int32_t split_mode,
+                                       void* stream);
+/* Adjoint of a diagonal-Gaussian density with parameter tables (DiagGaussian, ClassCondDiagGaussian, GlowBase;
+ * distributions/base.py): element i of a sample uses entry i / group of loc / log_scale [dim / group, num_classes] in
+ * column y[b] (y NULL: num_classes = 1).  g_z [B, dim] (may be NULL) is overwritten; g_loc / g_log_scale (may be NULL)
+ * receive the batch sums, formed deterministically (per-sample partials, fixed-order reduction). */
+int nfb_gaussian_table_log_prob_backward(const float* z_dev, const int64_t* y_dev, const float* loc_dev,
+                                         const float* log_scale_dev, const float* g_log_q_dev, float* g_z_dev,
+                                         float* g_loc_dev, float* g_log_scale_dev, int64_t batch, int32_t dim,
+                                         int32_t group, int32_t num_classes, void* stream);
+/* Adjoint of nfb_logit_transform in the density direction (NFB_INVERSE): g_in = dy/dx g_out + d log_det/dx g_log_det
+ * (g_out or g_log_det may be NULL). */
+int nfb_logit_transform_backward(const float* in_dev, const float* g_out_dev, const float* g_log_det_dev, float* g_in_dev,
+                                 int64_t batch, int64_t inner, float alpha, void* stream);
+
 /* ---- layer parameter descriptors (device pointers into the caller's parameters) ---- */
 
 /* A residual conditioner: nets/resnet.py:53-104 ResidualNet (mask pointers NULL) or

@@ -1296,6 +1296,44 @@ int nfb_class_cond_diag_gaussian_log_prob(const float* z, const int64_t* y, cons
                                    num_classes, accumulate, S(stream));
 }
 
+int nfb_conv2d_wgrad(const float* x, int32_t x_channels, int32_t c0, const float* gy, float* gw, float* gb, int64_t batch,
+                     int32_t cin, int32_t height, int32_t width, int32_t cout, int32_t ksize, int32_t accumulate,
+                     void* stream) {
+    NFB_CHECK(x && gy, NFB_ERR_ARG, "nfb_conv2d_wgrad: null pointer");
+    return launch_conv2d_wgrad(x, x_channels, c0, gy, gw, gb, batch, cin, height, width, cout, ksize, accumulate, 0,
+                               S(stream));
+}
+int nfb_conv2d_dgrad(const float* gy, const float* w, float* gx, int64_t batch, int32_t cin, int32_t height, int32_t width,
+                     int32_t cout, int32_t ksize, const float* mask_act, float mask_slope, int32_t accumulate,
+                     void* stream) {
+    NFB_CHECK(gy && w && gx, NFB_ERR_ARG, "nfb_conv2d_dgrad: null pointer");
+    return launch_conv2d_dgrad(gy, w, gx, batch, cin, height, width, cout, ksize, mask_act, mask_slope, accumulate,
+                               S(stream));
+}
+int nfb_affine_coupling_image_backward(const float* z, const float* param, const float* g_out, const float* g_log_det,
+                                       float* g_z, float* g_param, int64_t batch, int32_t channels, int32_t hw,
+                                       int32_t scale, int32_t scale_map, int32_t split_mode, void* stream) {
+    NFB_CHECK(z && param && g_out && g_z && g_param, NFB_ERR_ARG, "nfb_affine_coupling_image_backward: null pointer");
+    NFB_CHECK(scale_map >= 0 && scale_map <= 2, NFB_ERR_UNSUPPORTED, "This scale map is not implemented.");
+    NFB_CHECK(split_mode == 0 || split_mode == 1, NFB_ERR_UNSUPPORTED, "split mode is not implemented.");
+    return launch_coupling_image_bwd(z, param, g_out, g_log_det, g_z, g_param, batch, channels, hw, scale, scale_map,
+                                     split_mode, S(stream));
+}
+int nfb_gaussian_table_log_prob_backward(const float* z, const int64_t* y, const float* loc, const float* log_scale,
+                                         const float* g_log_q, float* g_z, float* g_loc, float* g_log_scale, int64_t batch,
+                                         int32_t dim, int32_t group, int32_t num_classes, void* stream) {
+    NFB_CHECK(z && loc && log_scale && g_log_q, NFB_ERR_ARG, "nfb_gaussian_table_log_prob_backward: null pointer");
+    NFB_CHECK(y || num_classes == 1, NFB_ERR_ARG, "nfb_gaussian_table_log_prob_backward: labels needed for num_classes > 1");
+    return launch_gauss_table_bwd(z, reinterpret_cast<const long long*>(y), loc, log_scale, g_log_q, g_z, g_loc,
+                                  g_log_scale, batch, dim, group, num_classes, S(stream));
+}
+int nfb_logit_transform_backward(const float* in, const float* g_out, const float* g_log_det, float* g_in, int64_t batch,
+                                 int64_t inner, float alpha, void* stream) {
+    NFB_CHECK(in && g_in, NFB_ERR_ARG, "nfb_logit_transform_backward: null pointer");
+    NFB_CHECK(alpha >= 0.f && alpha < 0.5f, NFB_ERR_ARG, "Logit: alpha must be in [0, 0.5)");
+    return launch_logit_bwd(in, g_out, g_log_det, g_in, batch, inner, alpha, S(stream));
+}
+
 int nfb_swish(const float* x, float beta_softplus, int64_t n, float* a, float* da, void* stream) {
     NFB_CHECK(x && a, NFB_ERR_ARG, "nfb_swish: null pointer");
     return launch_swish(x, beta_softplus, n, a, da, S(stream));

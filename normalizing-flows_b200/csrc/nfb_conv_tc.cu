@@ -40,6 +40,7 @@ constexpr int ct_n_tile(int n_pad) { return n_pad > 64 ? 128 : 64; }
 struct ConvTcParams {
     const float* x; float* y; const float* bias; const uint8_t* wstream;
     long long M; int ctot, c0, cin, H, W, cout, ks, n_tiles, k_chunks; float leaky; int* err;
+    const float* mask; float mask_slope; int accumulate;   // data-gradient epilogue (see launch_conv2d)
 };
 
 template <int NT>
@@ -158,6 +159,9 @@ __global__ void __launch_bounds__(kCtThreads, 1) conv_tc_kernel(const ConvTcPara
                 if (n < p.cout) {
                     float val = stg[r * kStgLd + j] + (p.bias ? __ldg(p.bias + n) : 0.f);
                     if (p.leaky >= 0.f) val = val >= 0.f ? val : val * p.leaky;
+                    const long long yo = bi * (long long)p.cout * HW + (long long)n * HW + pix;
+                    if (p.mask) val *= __ldg(p.mask + yo) > 0.f ? 1.f : p.mask_slope;
+                    if (p.accumulate) val += yb[(long long)n * HW];
                     yb[(long long)n * HW] = val;
                 }
             }
@@ -234,7 +238,7 @@ int launch_conv_tc_t(const ConvTcParams& p, cudaStream_t st) {
 
 int launch_conv2d_tc(const float* x, int ctot, int c0, const float* w, const float* bias, float* y, long long B,
                      int cin, int H, int W, int cout, int ks, float leaky, float gain_per_step, int* err,
-                     cudaStream_t st) {
+                     cudaStream_t st, const float* mask, float mask_slope, int accumulate) {
     const long long M = B * H * W;
     if (M == 0) return NFB_OK;
     const int T = ks * ks;
@@ -253,6 +257,7 @@ int launch_conv2d_tc(const float* x, int ctot, int c0, const float* w, const flo
     p.x = x; p.y = y; p.bias = bias; p.wstream = static_cast<const uint8_t*>(scratch);
     p.M = M; p.ctot = ctot; p.c0 = c0; p.cin = cin; p.H = H; p.W = W; p.cout = cout; p.ks = ks;
     p.n_tiles = n_tiles; p.k_chunks = k_chunks; p.leaky = leaky; p.err = err;
+    p.mask = mask; p.mask_slope = mask_slope; p.accumulate = accumulate;
     int rc = NT == 64 ? launch_conv_tc_t<64>(p, st) : launch_conv_tc_t<128>(p, st);
     const cudaError_t e = cudaGetLastError();
     cudaFreeAsync(scratch, st);

@@ -17,7 +17,7 @@ namespace nfb {
 __global__ void __launch_bounds__(256)
 conv2d_kernel(const float* __restrict__ x, int ctot, int c0, const float* __restrict__ w,
               const float* __restrict__ bias, float* __restrict__ y, long long B, int cin, int H, int W,
-              int cout, int ks, float leaky) {
+              int cout, int ks, float leaky, const float* __restrict__ mask, float mslope, int accumulate) {
     __shared__ float As[16][64 + 1];
     __shared__ float Bs[16][64 + 1];
     const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
@@ -74,7 +74,10 @@ conv2d_kernel(const float* __restrict__ x, int ctot, int c0, const float* __rest
             if (n >= cout) continue;
             float v = acc[i][j] + (bias ? bias[n] : 0.f);
             if (leaky >= 0.f) v = v >= 0.f ? v : v * leaky;
-            y[(bi * cout + n) * HW + pix] = v;
+            const long long yo = (bi * cout + n) * HW + pix;
+            if (mask) v *= mask[yo] > 0.f ? 1.f : mslope;
+            if (accumulate) v += y[yo];
+            y[yo] = v;
         }
     }
 }
@@ -86,7 +89,7 @@ template <int CMAX>
 __global__ void __launch_bounds__(256)
 conv1x1_small_kernel(const float* __restrict__ x, int ctot, int c0, const float* __restrict__ w,
                      const float* __restrict__ bias, float* __restrict__ y, long long M, int cin, int HW, int cout,
-                     float leaky) {
+                     float leaky, const float* __restrict__ mask, float mslope, int accumulate) {
     __shared__ float ws[CMAX * CMAX];
     __shared__ float bs[CMAX];
     for (int i = threadIdx.x; i < cout * cin; i += 256) ws[i] = w[i];
@@ -108,12 +111,16 @@ conv1x1_small_kernel(const float* __restrict__ x, int ctot, int c0, const float*
         for (int c = 0; c < CMAX; ++c)
             if (c < cin) acc = fmaf(wr[c], v[c], acc);
         if (leaky >= 0.f) acc = acc >= 0.f ? acc : acc * leaky;
+        const long long yo = (bi * cout + n) * (long long)HW + pix;
+        if (mask) acc *= mask[yo] > 0.f ? 1.f : mslope;
+        if (accumulate) acc += yp[(long long)n * HW];
         yp[(long long)n * HW] = acc;
     }
 }
 
 int launch_conv2d(const float* x, int ctot, int c0, const float* w, const float* bias, float* y, long long B,
-                  int cin, int H, int W, int cout, int ks, float leaky, cudaStream_t st) {
+                  int cin, int H, int W, int cout, int ks, float leaky, cudaStream_t st, const float* mask,
+                  float mask_slope, int accumulate) {
     NFB_CHECK(ks == 1 || ks == 3 || ks == 5, NFB_ERR_UNSUPPORTED, "conv2d: kernel size %d", ks);
     NFB_CHECK(c0 >= 0 && c0 + cin <= ctot, NFB_ERR_ARG, "conv2d: channel slice out of range");
     const long long M = B * H * W;
@@ -129,18 +136,23 @@ int launch_conv2d(const float* x, int ctot, int c0, const float* w, const float*
     if (ks == 1 && cin <= 64 && cout <= 64) {
         const unsigned g = (unsigned)((M + 255) / 256);
         if (cin <= 16 && cout <= 16)
-            conv1x1_small_kernel<16><<<g, 256, 0, st>>>(x, ctot, c0, w, bias, y, M, cin, H * W, cout, leaky);
+            conv1x1_small_kernel<16><<<g, 256, 0, st>>>(x, ctot, c0, w, bias, y, M, cin, H * W, cout, leaky, mask,
+                                                          mask_slope, accumulate);
         else if (cin <= 32 && cout <= 32)
-            conv1x1_small_kernel<32><<<g, 256, 0, st>>>(x, ctot, c0, w, bias, y, M, cin, H * W, cout, leaky);
+            conv1x1_small_kernel<32><<<g, 256, 0, st>>>(x, ctot, c0, w, bias, y, M, cin, H * W, cout, leaky, mask,
+                                                          mask_slope, accumulate);
         else
-            conv1x1_small_kernel<64><<<g, 256, 0, st>>>(x, ctot, c0, w, bias, y, M, cin, H * W, cout, leaky);
+            conv1x1_small_kernel<64><<<g, 256, 0, st>>>(x, ctot, c0, w, bias, y, M, cin, H * W, cout, leaky, mask,
+                                                          mask_slope, accumulate);
         NFB_LAUNCH_CHECK();
         return NFB_OK;
     }
     if (tc && conv_tc_supported(cin, cout, ks))
-        return launch_conv2d_tc(x, ctot, c0, w, bias, y, B, cin, H, W, cout, ks, leaky, kAccStepGain, nullptr, st);
+        return launch_conv2d_tc(x, ctot, c0, w, bias, y, B, cin, H, W, cout, ks, leaky, kAccStepGain, nullptr, st, mask,
+                                mask_slope, accumulate);
     dim3 grid((unsigned)((M + 63) / 64), (unsigned)((cout + 63) / 64));
-    conv2d_kernel<<<grid, 256, 0, st>>>(x, ctot, c0, w, bias, y, B, cin, H, W, cout, ks, leaky);
+    conv2d_kernel<<<grid, 256, 0, st>>>(x, ctot, c0, w, bias, y, B, cin, H, W, cout, ks, leaky, mask, mask_slope,
+                                        accumulate);
     NFB_LAUNCH_CHECK();
     return NFB_OK;
 }
@@ -600,6 +612,177 @@ int launch_tap_shift_add(const float* Y, const float* bias, float* out, long lon
     const long long n = B * cout * H * W;
     if (n == 0) return NFB_OK;
     tap_shift_add_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(Y, bias, out, B, cout, H, W, ks);
+    NFB_LAUNCH_CHECK();
+    return NFB_OK;
+}
+
+// -----------------------------------------------------------------------------------------
+// Training pass of the image path (density direction): adjoints of the operators above.
+// -----------------------------------------------------------------------------------------
+
+// Data gradient of a stride-1 "same" k x k convolution: gx = conv(gy, w') with w'[c, n, kh, kw] = w[n, c, k-1-kh, k-1-kw]
+// (in/out swapped, taps rotated by 180 degrees), i.e. the forward convolution kernels with the epilogue options
+// mask (LeakyReLU' of the layer input's stored activation) and accumulate.
+__global__ void conv_rot180_kernel(const float* __restrict__ w, float* __restrict__ wr, int cout, int cin, int ks) {
+    const int T = ks * ks;
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (long long)cout * cin * T) return;
+    const int tap = (int)(i % T), c = (int)((i / T) % cin), n = (int)(i / ((long long)T * cin));
+    wr[((long long)c * cout + n) * T + (T - 1 - tap)] = w[i];
+}
+int launch_conv2d_dgrad(const float* gy, const float* w, float* gx, long long B, int cin, int H, int W, int cout, int ks,
+                        const float* mask, float mask_slope, int accumulate, cudaStream_t st) {
+    NFB_CHECK(ks == 1 || ks == 3 || ks == 5, NFB_ERR_UNSUPPORTED, "conv2d_dgrad: kernel size %d", ks);
+    if (B * H * W == 0 || cin == 0) return NFB_OK;
+    const long long n = (long long)cout * cin * ks * ks;
+    void* wr = nullptr;
+    NFB_CUDA(cudaMallocAsync(&wr, (size_t)n * sizeof(float), st));
+    conv_rot180_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(w, static_cast<float*>(wr), cout, cin, ks);
+    const int rc = launch_conv2d(gy, cout, 0, static_cast<const float*>(wr), nullptr, gx, B, cout, H, W, cin, ks, -1.f, st,
+                                 mask, mask_slope, accumulate);
+    cudaFreeAsync(wr, st);
+    return rc;
+}
+
+// Adjoint of coupling_image_kernel in the density direction (direction 0; coupling.py:149-171), one block per sample.
+// z: the coupling's input [B, C, HW]; param [B, np*n2, HW] (shift 0::2, scale 1::2); g_out [B, C, HW]; g_ld [B] or NULL.
+// Writes the z2 channels of g_z (the z1 channels are the caller's: they pass through and feed the conditioner) and g_param.
+__global__ void __launch_bounds__(256)
+coupling_image_bwd_kernel(const float* __restrict__ z, const float* __restrict__ param, const float* __restrict__ g_out,
+                          const float* __restrict__ g_ld, float* __restrict__ g_z, float* __restrict__ g_param, int C,
+                          int HW, int scale, int smap, int inv_split) {
+    const long long b = blockIdx.x;
+    const int h = (C + 1) / 2;
+    const int o2 = inv_split ? 0 : h, n2 = inv_split ? h : C - h;
+    const int np = scale ? 2 : 1;
+    const float gl = g_ld ? g_ld[b] : 0.f;
+    for (int i = threadIdx.x; i < n2 * HW; i += 256) {
+        const int c = i / HW, pix = i - c * HW;
+        const long long zi = (b * C + o2 + c) * HW + pix;
+        const float go = g_out[zi];
+        if (!scale) {
+            g_z[zi] = go;
+            g_param[(b * n2 + c) * HW + pix] = -go;
+            continue;
+        }
+        const long long ps = (b * np * n2 + 2 * c) * HW + pix, pc = ps + HW;
+        const float d = z[zi] - param[ps], sc = param[pc];
+        float f, gsc;   // out = d * f;  d out / d sc and d ld / d sc folded into gsc
+        if (smap == 0) {
+            f = expf(-sc);
+            gsc = -go * d * f - gl;
+        } else {
+            const float sg = 1.f / (1.f + expf(-(sc + 2.f)));
+            if (smap == 1) {   // out = d sg, ld += log sg
+                f = sg;
+                gsc = (go * d * sg + gl) * (1.f - sg);
+            } else {           // out = d / sg, ld -= log sg
+                f = 1.f / sg;
+                gsc = -(go * d * f + gl) * (1.f - sg);
+            }
+        }
+        g_z[zi] = go * f;
+        g_param[ps] = -go * f;
+        g_param[pc] = gsc;
+    }
+}
+int launch_coupling_image_bwd(const float* z, const float* param, const float* g_out, const float* g_ld, float* g_z,
+                              float* g_param, long long B, int C, int HW, int scale, int smap, int inv_split,
+                              cudaStream_t st) {
+    if (B == 0) return NFB_OK;
+    coupling_image_bwd_kernel<<<(unsigned)B, 256, 0, st>>>(z, param, g_out, g_ld, g_z, g_param, C, HW, scale, smap,
+                                                           inv_split);
+    NFB_LAUNCH_CHECK();
+    return NFB_OK;
+}
+
+// Adjoint of the diagonal-Gaussian densities of the image bases (DiagGaussian, ClassCondDiagGaussian, GlowBase):
+//   log_q[b] = -d/2 log 2pi - sum_i ( ls[e(i), y_b] + (z[b, i] - loc[e(i), y_b])^2 / (2 exp(2 ls)) ),  e(i) = i / group,
+// tables [dim / group, ncls] (ncls = 1 and y = NULL: one table).  g_z[b, i] = -g[b] t / sigma (t = (z - loc) / sigma);
+// the table gradients are deterministic: per-(sample, entry) partial sums, then a fixed-order sum over the batch per
+// (entry, class) -- no float atomics.
+__global__ void gauss_table_bwd_rows_kernel(const float* __restrict__ z, const long long* __restrict__ y,
+                                            const float* __restrict__ loc, const float* __restrict__ log_scale,
+                                            const float* __restrict__ g_lq, float* __restrict__ g_z,
+                                            float* __restrict__ part, long long B, int dim, int group, int ncls) {
+    const int E = dim / group;
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= B * E) return;
+    const long long b = idx / E;
+    const int e = (int)(idx - b * E);
+    const int cls = y ? (int)y[b] : 0;
+    const float mu = loc[(long long)e * ncls + cls], ls = log_scale[(long long)e * ncls + cls];
+    const float inv = expf(-ls), g = g_lq[b];
+    float pl = 0.f, ps = 0.f;
+    for (int j = 0; j < group; ++j) {
+        const long long i = b * dim + (long long)e * group + j;
+        const float t = (z[i] - mu) * inv;
+        if (g_z) g_z[i] = -g * t * inv;
+        pl += t * inv;
+        ps += t * t - 1.f;
+    }
+    part[idx] = g * pl;
+    part[B * E + idx] = g * ps;
+}
+__global__ void gauss_table_bwd_sum_kernel(const float* __restrict__ part, const long long* __restrict__ y,
+                                           float* __restrict__ g_loc, float* __restrict__ g_log_scale, long long B,
+                                           int E, int ncls) {
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= E * ncls) return;
+    const int e = idx / ncls, k = idx - e * ncls;
+    double sl = 0.0, ss = 0.0;
+    for (long long b = 0; b < B; ++b) {
+        if (y && (int)y[b] != k) continue;
+        sl += part[b * E + e];
+        ss += part[B * E + b * E + e];
+    }
+    if (g_loc) g_loc[idx] = (float)sl;
+    if (g_log_scale) g_log_scale[idx] = (float)ss;
+}
+int launch_gauss_table_bwd(const float* z, const long long* y, const float* loc, const float* log_scale,
+                           const float* g_lq, float* g_z, float* g_loc, float* g_log_scale, long long B, int dim,
+                           int group, int ncls, cudaStream_t st) {
+    NFB_CHECK(group >= 1 && dim % group == 0 && ncls >= 1, NFB_ERR_ARG, "gauss_table_bwd: bad table shape");
+    const int E = dim / group;
+    if (B == 0) {
+        if (g_loc) NFB_CUDA(cudaMemsetAsync(g_loc, 0, (size_t)E * ncls * sizeof(float), st));
+        if (g_log_scale) NFB_CUDA(cudaMemsetAsync(g_log_scale, 0, (size_t)E * ncls * sizeof(float), st));
+        return NFB_OK;
+    }
+    void* part = nullptr;
+    NFB_CUDA(cudaMallocAsync(&part, (size_t)2 * B * E * sizeof(float), st));
+    gauss_table_bwd_rows_kernel<<<(unsigned)((B * E + 255) / 256), 256, 0, st>>>(
+        z, y, loc, log_scale, g_lq, g_z, static_cast<float*>(part), B, dim, group, ncls);
+    gauss_table_bwd_sum_kernel<<<(unsigned)((E * ncls + 255) / 256), 256, 0, st>>>(
+        static_cast<const float*>(part), y, g_loc, g_log_scale, B, E, ncls);
+    const cudaError_t e = cudaGetLastError();
+    cudaFreeAsync(part, st);
+    if (e != cudaSuccess) {
+        nfb_set_error("gauss_table_bwd launch: %s", cudaGetErrorString(e));
+        return NFB_ERR_CUDA;
+    }
+    return NFB_OK;
+}
+
+// Adjoint of Logit.inverse (logit_kernel, direction NFB_INVERSE): u = alpha + beta x, y = log u - log(1 - u),
+// log_det = n log beta - sum(log u + log(1 - u)):
+//   g_x = beta / (u (1 - u)) * (g_y - g_ld (1 - 2 u))
+__global__ void logit_bwd_kernel(const float* __restrict__ in, const float* __restrict__ g_out,
+                                 const float* __restrict__ g_ld, float* __restrict__ g_in, long long B, long long inner,
+                                 float alpha) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= B * inner) return;
+    const float beta = 1.f - 2.f * alpha;
+    const float u = alpha + beta * in[i];
+    const float gl = g_ld ? g_ld[i / inner] : 0.f;
+    const float go = g_out ? g_out[i] : 0.f;
+    g_in[i] = beta / (u * (1.f - u)) * (go - gl * (1.f - 2.f * u));
+}
+int launch_logit_bwd(const float* in, const float* g_out, const float* g_ld, float* g_in, long long B, long long inner,
+                     float alpha, cudaStream_t st) {
+    const long long n = B * inner;
+    if (n == 0) return NFB_OK;
+    logit_bwd_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(in, g_out, g_ld, g_in, B, inner, alpha);
     NFB_LAUNCH_CHECK();
     return NFB_OK;
 }

@@ -73,8 +73,11 @@ int launch_sum(const float* v, long long n, double scale, double* scratch, float
                double* out_sum, cudaStream_t st);
 
 // ---- image-shaped Glow pieces (nfb_glow.cu) ----
+// mask (optional, [B, cout, H, W]): multiply the output by LeakyReLU'(mask) = (mask > 0 ? 1 : mask_slope);
+// accumulate: y += result instead of y = result (both used by the data gradient, off for the forward callers)
 int launch_conv2d(const float* x, int ctot, int c0, const float* w, const float* bias, float* y, long long B,
-                  int cin, int H, int W, int cout, int ks, float leaky, cudaStream_t st);
+                  int cin, int H, int W, int cout, int ks, float leaky, cudaStream_t st, const float* mask = nullptr,
+                  float mask_slope = 0.f, int accumulate = 0);
 int launch_glow_fold(const float* P, const float* L, const float* U, const float* sign_S, const float* log_S,
                      const float* s, const float* t, int C, int HW, float* w_out, float* b_out, float* logdet,
                      cudaStream_t st);
@@ -104,6 +107,20 @@ int launch_logit(const float* in, float* out, float* logdet, long long B, long l
                  int accumulate, cudaStream_t st);
 int launch_class_cond_gauss(const float* z, const long long* y, const float* loc, const float* log_scale,
                             float* logq, long long B, int dim, int ncls, int accumulate, cudaStream_t st);
+
+// ---- training pass of the image path (nfb_glow.cu, nfb_conv_wgrad.cu) ----
+int launch_conv2d_dgrad(const float* gy, const float* w, float* gx, long long B, int cin, int H, int W, int cout, int ks,
+                        const float* mask, float mask_slope, int accumulate, cudaStream_t st);
+int launch_conv2d_wgrad(const float* x, int ctot, int c0, const float* gy, float* gw, float* gb, long long B, int cin,
+                        int H, int W, int cout, int ks, int accumulate, int max_chunks_per_split, cudaStream_t st);
+int launch_coupling_image_bwd(const float* z, const float* param, const float* g_out, const float* g_ld, float* g_z,
+                              float* g_param, long long B, int C, int HW, int scale, int smap, int inv_split,
+                              cudaStream_t st);
+int launch_gauss_table_bwd(const float* z, const long long* y, const float* loc, const float* log_scale,
+                           const float* g_lq, float* g_z, float* g_loc, float* g_log_scale, long long B, int dim,
+                           int group, int ncls, cudaStream_t st);
+int launch_logit_bwd(const float* in, const float* g_out, const float* g_ld, float* g_in, long long B, long long inner,
+                     float alpha, cudaStream_t st);
 
 // ---- small-dimension affine stack (nfb_affine.cu) ----
 constexpr int kAffMaxD = 16;
@@ -246,7 +263,7 @@ constexpr float kAccStepGain = 2.4e-8f;
 bool conv_tc_supported(int cin, int cout, int ks);
 int launch_conv2d_tc(const float* x, int ctot, int c0, const float* w, const float* bias, float* y, long long B,
                      int cin, int H, int W, int cout, int ks, float leaky, float gain_per_step, int* err,
-                     cudaStream_t st);
+                     cudaStream_t st, const float* mask = nullptr, float mask_slope = 0.f, int accumulate = 0);
 int launch_build_effective(const float* W, const float* M, int src_cols, const int* src_row,
                            const int* src_col, const float* row_scale, float* E, int n_pad,
                            int k_pad, float gain, cudaStream_t st);

@@ -111,6 +111,11 @@ SYMBOLS = {
     "nfb_copy_channels": (C.c_int, [_VP, _VP, _I64, _I32, _I32, _I32, _I32, _VP]),
     "nfb_paste_channels": (C.c_int, [_VP, _VP, _I64, _I32, _I32, _I32, _I32, _VP]),
     "nfb_class_cond_diag_gaussian_log_prob": (C.c_int, [_VP, _VP, _VP, _VP, _VP, _I64, _I32, _I32, _I32, _VP]),
+    "nfb_conv2d_wgrad": (C.c_int, [_VP, _I32, _I32, _VP, _VP, _VP, _I64, _I32, _I32, _I32, _I32, _I32, _I32, _VP]),
+    "nfb_conv2d_dgrad": (C.c_int, [_VP, _VP, _VP, _I64, _I32, _I32, _I32, _I32, _I32, _VP, _F, _I32, _VP]),
+    "nfb_affine_coupling_image_backward": (C.c_int, [_VP] * 6 + [_I64, _I32, _I32, _I32, _I32, _I32, _VP]),
+    "nfb_gaussian_table_log_prob_backward": (C.c_int, [_VP] * 8 + [_I64, _I32, _I32, _I32, _VP]),
+    "nfb_logit_transform_backward": (C.c_int, [_VP, _VP, _VP, _VP, _I64, _I64, _F, _VP]),
     "nfb_flow_create": (C.c_int, [C.POINTER(_VP), _I32]),
     "nfb_flow_destroy": (C.c_int, [_VP]),
     "nfb_flow_add_ar_rqs": (C.c_int, [_VP, C.POINTER(ArRqsDesc)]),

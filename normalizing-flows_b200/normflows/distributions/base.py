@@ -5,6 +5,7 @@ import torch
 from torch import nn
 
 from .. import _lib as L
+from .._image_autograd import gaussian_table_log_prob, wants_grad
 from .._native import require_cuda_f32
 
 
@@ -50,11 +51,16 @@ class DiagGaussian(BaseDistribution):
     def log_prob(self, z, context=None):
         z = require_cuda_f32(z)
         ls = self._log_scale().contiguous()
-        out = torch.empty(z.shape[0], dtype=torch.float32, device=z.device)
-        with torch.cuda.device(z.device):
-            L.check(L.lib().nfb_diag_gaussian_log_prob(L.ptr(z), L.ptr(self.loc), L.ptr(ls), L.ptr(out),
-                                                       z.shape[0], self.d, 0, L.stream_ptr()))
-        return out
+
+        def run():
+            out = torch.empty(z.shape[0], dtype=torch.float32, device=z.device)
+            with torch.cuda.device(z.device):
+                L.check(L.lib().nfb_diag_gaussian_log_prob(L.ptr(z), L.ptr(self.loc), L.ptr(ls), L.ptr(out),
+                                                           z.shape[0], self.d, 0, L.stream_ptr()))
+            return out
+        if wants_grad(self, z) and z.shape[0]:
+            return gaussian_table_log_prob(run, z, self.loc.reshape(self.d, 1), ls.reshape(self.d, 1), None, 1)
+        return run()
 
 
 class ClassCondDiagGaussian(BaseDistribution):
@@ -99,13 +105,19 @@ class ClassCondDiagGaussian(BaseDistribution):
             y = torch.argmax(y, dim=1)  # one-hot rows (base.py:336-337 accepts both)
         y = y.to(device=z.device, dtype=torch.int64).contiguous()
         ls = self._log_scale().contiguous()  # temperature annealing: log_scale + log T (base.py:318-319,339-340)
-        out = torch.empty(z.shape[0], dtype=torch.float32, device=z.device)
-        if z.shape[0]:
-            with torch.cuda.device(z.device):
-                L.check(L.lib().nfb_class_cond_diag_gaussian_log_prob(
-                    L.ptr(z), L.ptr(y), L.ptr(self.loc), L.ptr(ls), L.ptr(out), z.shape[0], self.d,
-                    self.num_classes, 0, L.stream_ptr()))
-        return out
+
+        def run():
+            out = torch.empty(z.shape[0], dtype=torch.float32, device=z.device)
+            if z.shape[0]:
+                with torch.cuda.device(z.device):
+                    L.check(L.lib().nfb_class_cond_diag_gaussian_log_prob(
+                        L.ptr(z), L.ptr(y), L.ptr(self.loc), L.ptr(ls), L.ptr(out), z.shape[0], self.d,
+                        self.num_classes, 0, L.stream_ptr()))
+            return out
+        if wants_grad(self, z) and z.shape[0]:
+            K = self.num_classes
+            return gaussian_table_log_prob(run, z, self.loc.reshape(self.d, K), ls.reshape(self.d, K), y, 1)
+        return run()
 
 
 class ConditionalDiagGaussian(BaseDistribution):
@@ -175,9 +187,9 @@ class GlowBase(BaseDistribution):
             self.log_scale_cc = nn.Parameter(torch.zeros(num_classes, shape[0]))
         self.temperature = None
 
-    def _channel_params(self):
+    def _channel_params(self, differentiable=False):
         """([C] or [K, C]) mean and log-scale per channel (per class), base.py:397-424 / 438-461."""
-        with torch.no_grad():
+        with torch.set_grad_enabled(differentiable and torch.is_grad_enabled()):
             loc = (self.loc * torch.exp(self.loc_logs * self.logscale_factor)).reshape(1, -1)
             ls = (self.log_scale * torch.exp(self.log_scale_logs * self.logscale_factor)).reshape(1, -1)
             if self.class_cond:
@@ -209,6 +221,15 @@ class GlowBase(BaseDistribution):
 
     def log_prob(self, z, y=None):
         z = require_cuda_f32(z)
+        if wants_grad(self, z) and z.shape[0]:
+            # tables [C, K]: element i of a sample uses channel i // num_pix
+            loc_d, ls_d = self._channel_params(differentiable=True)
+            yy = self._labels(y).to(device=z.device, dtype=torch.int64).contiguous() if self.class_cond else None
+            return gaussian_table_log_prob(lambda: self._log_prob_native(z, y), z, loc_d.t(), ls_d.t(), yy,
+                                           self.num_pix)
+        return self._log_prob_native(z, y)
+
+    def _log_prob_native(self, z, y):
         loc, ls = self._channel_params()
         out = torch.empty(z.shape[0], dtype=torch.float32, device=z.device)
         if not z.shape[0]:

@@ -10,6 +10,7 @@ import torch
 from torch import nn
 
 from .. import _lib as L
+from .._image_autograd import GlowBlockInverseFn, SplitChannelsFn, SqueezeFn, wants_grad
 from .._native import require_cuda_f32
 from ..nets.cnn import ConvNet2d
 from .affine import ActNorm, AffineCoupling, Merge, Split
@@ -69,6 +70,18 @@ class Invertible1x1Conv(Flow):
                 ldc = (hw * (sv.double().sum() - logabsdet)).float()
         return w, b.contiguous(), ldc
 
+    def folded_torch(self, s, t, hw):
+        """Differentiable restatement of `folded(NFB_INVERSE, s, t, hw)` (the gradient chain of the training pass)."""
+        sv, tv = s.reshape(-1), t.reshape(-1)
+        if self.use_lu:
+            lo = torch.tril(self.L, -1) + self.eye
+            up = torch.triu(self.U, 1) + torch.diag(self.sign_S * torch.exp(self.log_S))
+            Wm, logabsdet = self.P @ lo @ up, self.log_S.sum()
+        else:
+            Wm, logabsdet = self.W, torch.linalg.slogdet(self.W)[1]
+        w = Wm * torch.exp(-sv)[None, :]
+        return w, -(w @ tv), hw * (logabsdet - sv.sum())
+
     def _conv1x1(self, z, direction):
         z = require_cuda_f32(z)
         if z.dim() != 4 or z.shape[1] != self.num_channels:
@@ -110,11 +123,15 @@ class Squeeze(Flow):
         return self._run(z, L.NFB_FORWARD)
 
     def inverse(self, z):
+        if wants_grad(self, z):
+            return SqueezeFn.apply(self, z, L.NFB_INVERSE), 0
         return self._run(z, L.NFB_INVERSE)
 
 
 def split_channels(z, mode="channel"):
     """Split.forward (reshape.py:27-31): contiguous copies of the two channel chunks."""
+    if torch.is_grad_enabled() and z.requires_grad:
+        return SplitChannelsFn.apply(z, mode)
     z = require_cuda_f32(z)
     B, C, H, W = z.shape
     h = (C + 1) // 2
@@ -285,6 +302,11 @@ class GlowBlock(Flow):
         return out, ld
 
     def inverse(self, z):
+        if wants_grad(self, z):
+            return GlowBlockInverseFn.apply(self, z, *self.parameters())
+        return self._inverse_native(z)
+
+    def _inverse_native(self, z):
         z = require_cuda_f32(z)
         if z.dim() != 4 or z.shape[1] != self.channels:
             raise ValueError("Expected an NCHW tensor with {} channels.".format(self.channels))
@@ -308,3 +330,44 @@ class GlowBlock(Flow):
             c0, cin = (0, h) if self.split_mode == "channel" else (h, C - h)
             self._coupling(out, out, c0, cin, ld, ldc, L.NFB_INVERSE)
         return out, ld
+
+    def _inverse_backward(self, z, g_out, g_ld):
+        """Adjoint of the density direction: recompute the folded 1x1 output and the conditioner's activations, then
+        coupling adjoint -> conditioner dgrad / wgrad -> 1x1 dgrad / wgrad (all CUDA), and the gradients of the folded
+        w [C, C], b [C] and log-det constant mapped to Invertible1x1Conv / ActNorm parameters by torch autograd over the
+        fold.  Returns (g_z, {id(parameter): gradient})."""
+        lib = L.lib()
+        conv, an = self.flows[1], self.flows[2]
+        pm = self.flows[0].flows[1].param_map
+        B, C, H, W = z.shape
+        HW, dev = H * W, z.device
+        h = (C + 1) // 2
+        c0, cin = (0, h) if self.split_mode == "channel" else (h, C - h)
+        grads = {}
+        with torch.cuda.device(dev):
+            st = L.stream_ptr()
+            w, b, _ = self._folded("_nfb_fold", lib.nfb_glow_fold_actnorm_conv1x1, HW, dev)
+            mid = torch.empty_like(z)
+            L.check(lib.nfb_conv2d(L.ptr(z), C, 0, L.ptr(w), L.ptr(b), L.ptr(mid), B, C, H, W, C, 1, -1.0, st))
+            acts = pm.native_activations(mid, c0, cin)
+            param = acts[-1]
+            g_mid = torch.empty_like(z)
+            g_param = torch.empty_like(param)
+            L.check(lib.nfb_affine_coupling_image_backward(
+                L.ptr(mid), L.ptr(param), L.ptr(g_out), L.ptr(g_ld), L.ptr(g_mid), L.ptr(g_param), B, C, HW,
+                int(bool(self.scale)), _MAPS[self.scale_map], 0 if self.split_mode == "channel" else 1, st))
+            g_z1 = torch.empty(B, cin, H, W, device=dev)   # z1 passes through the coupling and feeds the conditioner
+            L.check(lib.nfb_copy_channels(L.ptr(g_out), L.ptr(g_z1), B, C, c0, cin, HW, st))
+            grads.update(pm.native_backward(mid, c0, cin, acts, g_param, g_z1))
+            L.check(lib.nfb_paste_channels(L.ptr(g_z1), L.ptr(g_mid), B, C, c0, cin, HW, st))
+            gz = torch.empty_like(z)
+            L.check(lib.nfb_conv2d_dgrad(L.ptr(g_mid), L.ptr(w), L.ptr(gz), B, C, H, W, C, 1, None, 0.0, 0, st))
+            gw, gb = torch.empty(C, C, device=dev), torch.empty(C, device=dev)
+            L.check(lib.nfb_conv2d_wgrad(L.ptr(z), C, 0, L.ptr(g_mid), L.ptr(gw), L.ptr(gb), B, C, H, W, C, 1, 0, st))
+        srcs = [p for p in conv._sources() + (an.s, an.t) if isinstance(p, nn.Parameter) and p.requires_grad]
+        if srcs:
+            with torch.enable_grad():
+                outs = [(o, g) for o, g in zip(conv.folded_torch(an.s, an.t, HW), (gw, gb, g_ld.sum())) if o.requires_grad]
+                gs = torch.autograd.grad([o for o, _ in outs], srcs, [g for _, g in outs], allow_unused=True)
+            grads.update({id(p): g for p, g in zip(srcs, gs)})
+        return gz, grads

@@ -116,6 +116,83 @@ class ConvNet2d(nn.Module):
                 cur, cur_tot, cur_c0 = y, conv.out_channels, 0
         return cur
 
+    def _folded_layers(self, differentiable=False):
+        """[(conv, w, b, act)] per convolution with a following ActNorm folded in (w * exp(s), b = t), as apply_native
+        runs them; act = LeakyReLU slope, or -1.0 for the last layer.  differentiable=True: w / b keep autograd history
+        to the parameters (the gradient chain of the training pass)."""
+        import torch
+        from ..utils.nn import ActNorm
+        mods = list(self.net)
+        out = []
+        for j, conv in enumerate(mods):
+            if not isinstance(conv, nn.Conv2d):
+                continue
+            an = mods[j + 1].actNorm if j + 1 < len(mods) and isinstance(mods[j + 1], ActNorm) else None
+            w, b = conv.weight, conv.bias
+            if an is not None:
+                w = conv.weight * torch.exp(an.s.reshape(-1))[:, None, None, None]
+                b = an.t.reshape(-1)
+            if not differentiable:
+                w, b = w.detach().contiguous(), b.detach().contiguous()
+            out.append((conv, w, b, -1.0 if conv is mods[-1] else float(self.leaky)))
+        return out
+
+    def native_activations(self, x, c0, cin):
+        """Training-pass recompute of the conditioner on x[:, c0:c0+cin] layer by layer (nfb_conv2d): the list of every
+        layer's output (post-activation); the last one is the parameter tensor.  ActNorm must be initialised.  For the
+        Glow shape the forward ran the fused kernel with the tap-form coupling instead: the recomputed activations and
+        parameter tensor are the same sums rounded in a different order (~1e-5 relative), so the adjoint is taken at
+        values within that of the forward's; a ReLU whose input lies that close to 0 may take the other branch."""
+        import torch
+        B, ctot, H, W = x.shape
+        acts, cur, cur_tot, cur_c0 = [], x, ctot, c0
+        for conv, w, b, act in self._folded_layers():
+            y = torch.empty(B, conv.out_channels, H, W, device=x.device, dtype=torch.float32)
+            L.check(L.lib().nfb_conv2d(L.ptr(cur), cur_tot, cur_c0, L.ptr(w), L.ptr(b), L.ptr(y), B, conv.in_channels,
+                                       H, W, conv.out_channels, conv.kernel_size[0], act, L.stream_ptr()))
+            acts.append(y)
+            cur, cur_tot, cur_c0 = y, conv.out_channels, 0
+        return acts
+
+    def native_backward(self, x, c0, cin, acts, g_out, g_x):
+        """Adjoint of native_activations: g_out = gradient of the last output; the input gradient is ACCUMULATED into
+        g_x [B, cin, H, W].  LeakyReLU' comes from the stored post-activation tensors.  Returns {id(parameter): grad};
+        folded ActNorm gradients go back to (weight, s, t) by torch autograd over the fold."""
+        import torch
+        lib = L.lib()
+        B, ctot, H, W = x.shape
+        layers = self._folded_layers()
+        geff = [None] * len(layers)
+        g = g_out
+        for i in range(len(layers) - 1, -1, -1):
+            conv, w, b, _ = layers[i]
+            k, ci, co = conv.kernel_size[0], conv.in_channels, conv.out_channels
+            inp, itot, ic0 = (x, ctot, c0) if i == 0 else (acts[i - 1], acts[i - 1].shape[1], 0)
+            gw, gb = torch.empty_like(w), torch.empty(co, device=x.device)
+            L.check(lib.nfb_conv2d_wgrad(L.ptr(inp), itot, ic0, L.ptr(g), L.ptr(gw), L.ptr(gb), B, ci, H, W, co, k, 0,
+                                         L.stream_ptr()))
+            geff[i] = (gw, gb)
+            if i > 0:
+                gi = torch.empty_like(acts[i - 1])
+                L.check(lib.nfb_conv2d_dgrad(L.ptr(g), L.ptr(w), L.ptr(gi), B, ci, H, W, co, k, L.ptr(acts[i - 1]),
+                                             float(self.leaky), 0, L.stream_ptr()))
+                g = gi
+            else:
+                L.check(lib.nfb_conv2d_dgrad(L.ptr(g), L.ptr(w), L.ptr(g_x), B, ci, H, W, co, k, None, 0.0, 1,
+                                             L.stream_ptr()))
+        params = [p for p in self.parameters() if p.requires_grad]
+        if not params:
+            return {}
+        with torch.enable_grad():
+            outs, gs = [], []
+            for (conv, w, b, _), (gw, gb) in zip(self._folded_layers(differentiable=True), geff):
+                for t, gt in ((w, gw), (b, gb)):
+                    if t.requires_grad:
+                        outs.append(t)
+                        gs.append(gt)
+            got = torch.autograd.grad(outs, params, gs, allow_unused=True)
+        return {id(p): gp for p, gp in zip(params, got)}
+
     def _packed_conditioner(self, c1, c2, c3, cin, hid, cout):
         """bf16 hi | lo records of the three convolutions in the fused kernel's layout (csrc/nfb_glow_fused.cu), cached per
         parameter version (and packed-weight generation): round 2a re-packed them on every call (5.5 % of a Glow pass)."""

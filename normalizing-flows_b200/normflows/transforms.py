@@ -4,6 +4,7 @@ reduction, csrc/nfb_glow.cu `logit_kernel`)."""
 import torch
 
 from . import _lib as L
+from ._image_autograd import LogitInverseFn, wants_grad
 from ._native import require_cuda_f32
 from .flows.base import Flow
 
@@ -28,6 +29,8 @@ class Logit(Flow):
         return self._run(z, L.NFB_FORWARD)
 
     def inverse(self, z):
+        if wants_grad(self, z):
+            return LogitInverseFn.apply(self, z)
         return self._run(z, L.NFB_INVERSE)
 
 
