@@ -13,7 +13,8 @@ from . import _lib as L
 
 
 def wants_grad(module, *tensors):
-    """Same criterion as NormalizingFlow._wants_grad: grad enabled, and an input or a parameter requires grad."""
+    """Grad enabled, and an input or a parameter of the module requires grad: the module's call goes through its
+    autograd.Function (NormalizingFlow.log_prob uses the same test)."""
     if not torch.is_grad_enabled():
         return False
     return any(t is not None and t.requires_grad for t in tensors) or any(p.requires_grad for p in module.parameters())
@@ -89,13 +90,12 @@ class SplitChannelsFn(torch.autograd.Function):
 
 
 class GaussianTableFn(torch.autograd.Function):
-    """log_q[b] of a diagonal Gaussian whose element i of a sample uses entry i // group of the tables
-    loc / log_scale [dim // group, num_classes] (column y[b]).  `run` computes the forward value exactly as the no-grad
-    path does; backward is nfb_gaussian_table_log_prob_backward."""
+    """gaussian_table_log_prob with gradients: the forward runs the no-grad path on the same tables; backward is
+    nfb_gaussian_table_log_prob_backward.  y: empty = one table column."""
 
     @staticmethod
-    def forward(ctx, run, z, loc, log_scale, y, group):
-        out = run()
+    def forward(ctx, z, loc, log_scale, y, group):
+        out = gaussian_table_log_prob(z, loc, log_scale, y if y.numel() else None, group)
         ctx.group = group
         ctx.save_for_backward(z, loc, log_scale, y)
         return out
@@ -106,22 +106,40 @@ class GaussianTableFn(torch.autograd.Function):
         B = z.shape[0]
         dim = z.numel() // max(B, 1)
         ncls = loc.shape[1]
-        gz = torch.empty_like(z) if ctx.needs_input_grad[1] else None
-        gl = torch.empty(loc.shape, device=z.device) if ctx.needs_input_grad[2] else None   # contiguous [E, K]
-        gs = torch.empty(ls.shape, device=z.device) if ctx.needs_input_grad[3] else None
+        gz = torch.empty_like(z) if ctx.needs_input_grad[0] else None
+        gl = torch.empty(loc.shape, device=z.device) if ctx.needs_input_grad[1] else None   # contiguous [E, K]
+        gs = torch.empty(ls.shape, device=z.device) if ctx.needs_input_grad[2] else None
         # contiguous copies held by name: a temporary freed inside the call could hand its memory to the next one
         loc, ls, g = loc.contiguous(), ls.contiguous(), g.contiguous().float()
         with torch.cuda.device(z.device):
             L.check(L.lib().nfb_gaussian_table_log_prob_backward(
                 L.ptr(z), L.ptr(y if y.numel() else None), L.ptr(loc), L.ptr(ls), L.ptr(g), L.ptr(gz), L.ptr(gl),
                 L.ptr(gs), B, dim, ctx.group, ncls, L.stream_ptr()))
-        return None, gz, gl, gs, None, None
+        return gz, gl, gs, None, None
 
 
-def gaussian_table_log_prob(run, z, loc, log_scale, y, group):
-    """Apply GaussianTableFn; y None = one table column."""
-    yy = y if y is not None else torch.empty(0, dtype=torch.int64, device=z.device)
-    return GaussianTableFn.apply(run, z, loc, log_scale, yy, group)
+def gaussian_table_log_prob(z, loc, log_scale, y, group):
+    """log_q[b] of a diagonal Gaussian whose element i of a sample uses entry i // group of the tables
+    loc / log_scale [E, K], column y[b] (y None: K = 1).  The density kernel (nfb_diag_gaussian_log_prob for K = 1,
+    nfb_class_cond_diag_gaussian_log_prob otherwise) reads one entry per element, so tables with group > 1 are expanded
+    first; through GaussianTableFn when a gradient is wanted."""
+    if torch.is_grad_enabled() and any(t.requires_grad for t in (z, loc, log_scale)) and z.shape[0]:
+        yy = y if y is not None else torch.empty(0, dtype=torch.int64, device=z.device)
+        return GaussianTableFn.apply(z, loc, log_scale, yy, group)
+    B, K = z.shape[0], loc.shape[1]
+    if group > 1:
+        loc, log_scale = loc.repeat_interleave(group, dim=0), log_scale.repeat_interleave(group, dim=0)
+    loc, log_scale = loc.detach().contiguous(), log_scale.detach().contiguous()   # held by name until the kernel has run
+    out = torch.empty(B, dtype=torch.float32, device=z.device)
+    if B:
+        with torch.cuda.device(z.device):
+            if K == 1:
+                L.check(L.lib().nfb_diag_gaussian_log_prob(L.ptr(z), L.ptr(loc), L.ptr(log_scale), L.ptr(out), B,
+                                                           loc.shape[0], 0, L.stream_ptr()))
+            else:
+                L.check(L.lib().nfb_class_cond_diag_gaussian_log_prob(L.ptr(z), L.ptr(y), L.ptr(loc), L.ptr(log_scale),
+                                                                      L.ptr(out), B, loc.shape[0], K, 0, L.stream_ptr()))
+    return out
 
 
 class LogitInverseFn(torch.autograd.Function):

@@ -20,7 +20,8 @@ _VERSION = operator.attrgetter("_version")
 #   * every torch optimizer step (global post-hook below),
 #   * load_state_dict / train() / eval() on a NormalizingFlow (core.py),
 #   * an explicit `normflows.invalidate_packed_weights()` (or `model.repack()`),
-# which is the documented call after any other out-of-band `.data` mutation.
+# which is the documented call after any other out-of-band `.data` mutation.  `cached` below applies this to the
+# image path's caches; FlowHandle keeps its own split signature.
 _GENERATION = [0]
 
 
@@ -32,6 +33,17 @@ def invalidate_packed_weights():
 
 def generation():
     return _GENERATION[0]
+
+
+def cached(owner, key, tensors, extra, build):
+    """build() once per parameter version: the value is kept in owner.__dict__[key] under the signature of `tensors`
+    ((data_ptr, _version) each), `extra` and the generation, and rebuilt when that signature changes."""
+    sig = tuple((t.data_ptr(), t._version) for t in tensors) + tuple(extra) + (_GENERATION[0],)
+    hit = owner.__dict__.get(key)
+    if hit is None or hit[0] != sig:
+        hit = (sig, build())
+        owner.__dict__[key] = hit
+    return hit[1]
 
 
 try:  # torch >= 2.0

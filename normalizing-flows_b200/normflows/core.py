@@ -10,6 +10,7 @@ import torch
 from torch import nn
 
 from . import _lib as L
+from ._image_autograd import wants_grad
 from ._native import FlowHandle
 from .distributions.base import DiagGaussian
 from .flows.base import NativeFlow
@@ -32,8 +33,6 @@ class NormalizingFlow(nn.Module):
         layers = list(self.flows)
         if (h is None or h.layers != layers or h.base is not base
                 or h.use_tc != NativeFlow.use_tensor_cores):
-            for f in layers:  # data-dependent inits must have happened before packing
-                pass
             h = FlowHandle(layers, base, NativeFlow.use_tensor_cores)
             self.__dict__["_nfb_stack"] = h
         return h
@@ -102,14 +101,11 @@ class NormalizingFlow(nn.Module):
             log_det = log_det + ld
         return x, log_det
 
-    def _wants_grad(self, x):
-        return torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters()))
-
     def log_prob(self, x):
         h = self._stack()
         self._run_pending_inits(x, inverse=True)
         if h is not None and h.base is not None and x.dim() == 2:
-            if self._wants_grad(x):  # forward on the CUDA kernels, backward via _autograd (interim, SURVEY 8f-1)
+            if wants_grad(self, x):  # forward on the CUDA kernels, backward via _autograd (interim, SURVEY 8f-1)
                 from ._autograd import DensityFn
                 return DensityFn.apply(self, x, *self.parameters())
             return h.log_prob(x)
@@ -119,7 +115,7 @@ class NormalizingFlow(nn.Module):
     def forward_kld(self, x):
         h = self._stack()
         self._run_pending_inits(x, inverse=True)
-        if h is not None and h.base is not None and x.dim() == 2 and not self._wants_grad(x):
+        if h is not None and h.base is not None and x.dim() == 2 and not wants_grad(self, x):
             return h.forward_kld(x)
         return -torch.mean(self.log_prob(x))
 

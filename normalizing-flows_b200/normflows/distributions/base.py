@@ -5,8 +5,18 @@ import torch
 from torch import nn
 
 from .. import _lib as L
-from .._image_autograd import gaussian_table_log_prob, wants_grad
+from .._image_autograd import gaussian_table_log_prob
 from .._native import require_cuda_f32
+
+
+def _tempered(log_scale, temperature):
+    """Temperature annealing: log_scale + log T (base.py:318-319, 339-340)."""
+    return log_scale if temperature is None else log_scale + np.log(temperature)
+
+
+def _labels(y, device):
+    """int64 class indices on `device`; one-hot rows select their class (base.py:336-337, 403-411)."""
+    return (y if y.dim() == 1 else torch.argmax(y, dim=1)).to(device=device, dtype=torch.int64).contiguous()
 
 
 class BaseDistribution(nn.Module):
@@ -36,13 +46,10 @@ class DiagGaussian(BaseDistribution):
             self.register_buffer("log_scale", torch.zeros(1, *shape))
         self.temperature = None
 
-    def _log_scale(self):
-        return self.log_scale if self.temperature is None else self.log_scale + np.log(self.temperature)
-
     def forward(self, num_samples=1, context=None):
         # sampling from the base is off the hot path (core.py:167-180): plain torch RNG
         eps = torch.randn((num_samples,) + self.shape, dtype=self.loc.dtype, device=self.loc.device)
-        ls = self._log_scale()
+        ls = _tempered(self.log_scale, self.temperature)
         z = self.loc + torch.exp(ls) * eps
         log_p = -0.5 * self.d * np.log(2 * np.pi) - torch.sum(ls + 0.5 * eps ** 2,
                                                               list(range(1, self.n_dim + 1)))
@@ -50,17 +57,8 @@ class DiagGaussian(BaseDistribution):
 
     def log_prob(self, z, context=None):
         z = require_cuda_f32(z)
-        ls = self._log_scale().contiguous()
-
-        def run():
-            out = torch.empty(z.shape[0], dtype=torch.float32, device=z.device)
-            with torch.cuda.device(z.device):
-                L.check(L.lib().nfb_diag_gaussian_log_prob(L.ptr(z), L.ptr(self.loc), L.ptr(ls), L.ptr(out),
-                                                           z.shape[0], self.d, 0, L.stream_ptr()))
-            return out
-        if wants_grad(self, z) and z.shape[0]:
-            return gaussian_table_log_prob(run, z, self.loc.reshape(self.d, 1), ls.reshape(self.d, 1), None, 1)
-        return run()
+        ls = _tempered(self.log_scale, self.temperature)
+        return gaussian_table_log_prob(z, self.loc.reshape(self.d, 1), ls.reshape(self.d, 1), None, 1)
 
 
 class ClassCondDiagGaussian(BaseDistribution):
@@ -77,9 +75,6 @@ class ClassCondDiagGaussian(BaseDistribution):
         self.log_scale = nn.Parameter(torch.zeros(*shape, num_classes))
         self.temperature = None
 
-    def _log_scale(self):
-        return self.log_scale if self.temperature is None else self.log_scale + np.log(self.temperature)
-
     def forward(self, num_samples=1, y=None):
         """distributions/base.py:302-325: z = loc[..., y] + exp(log_scale[..., y]) * eps and its log-density.
         The random draws (labels, eps) and the per-class parameter gather are torch device ops (plumbing; the
@@ -87,37 +82,20 @@ class ClassCondDiagGaussian(BaseDistribution):
         dev = self.loc.device
         if y is not None:
             num_samples = len(y)
-            if y.dim() != 1:
-                y = torch.argmax(y, dim=1)
-            y = y.to(device=dev, dtype=torch.int64)
+            y = _labels(y, dev)
         else:
             y = torch.randint(self.num_classes, (num_samples,), device=dev)
         with torch.no_grad():
             eps = torch.randn((num_samples,) + self.shape, dtype=self.loc.dtype, device=dev)
             loc = self.loc.detach().movedim(-1, 0)[y]
-            log_scale = self._log_scale().detach().movedim(-1, 0)[y]
+            log_scale = _tempered(self.log_scale, self.temperature).detach().movedim(-1, 0)[y]
             z = (loc + torch.exp(log_scale) * eps).contiguous()
         return z, self.log_prob(z, y)
 
     def log_prob(self, z, y):
         z = require_cuda_f32(z)
-        if y.dim() != 1:
-            y = torch.argmax(y, dim=1)  # one-hot rows (base.py:336-337 accepts both)
-        y = y.to(device=z.device, dtype=torch.int64).contiguous()
-        ls = self._log_scale().contiguous()  # temperature annealing: log_scale + log T (base.py:318-319,339-340)
-
-        def run():
-            out = torch.empty(z.shape[0], dtype=torch.float32, device=z.device)
-            if z.shape[0]:
-                with torch.cuda.device(z.device):
-                    L.check(L.lib().nfb_class_cond_diag_gaussian_log_prob(
-                        L.ptr(z), L.ptr(y), L.ptr(self.loc), L.ptr(ls), L.ptr(out), z.shape[0], self.d,
-                        self.num_classes, 0, L.stream_ptr()))
-            return out
-        if wants_grad(self, z) and z.shape[0]:
-            K = self.num_classes
-            return gaussian_table_log_prob(run, z, self.loc.reshape(self.d, K), ls.reshape(self.d, K), y, 1)
-        return run()
+        K, ls = self.num_classes, _tempered(self.log_scale, self.temperature)
+        return gaussian_table_log_prob(z, self.loc.reshape(self.d, K), ls.reshape(self.d, K), _labels(y, z.device), 1)
 
 
 class ConditionalDiagGaussian(BaseDistribution):
@@ -187,65 +165,33 @@ class GlowBase(BaseDistribution):
             self.log_scale_cc = nn.Parameter(torch.zeros(num_classes, shape[0]))
         self.temperature = None
 
-    def _channel_params(self, differentiable=False):
-        """([C] or [K, C]) mean and log-scale per channel (per class), base.py:397-424 / 438-461."""
-        with torch.set_grad_enabled(differentiable and torch.is_grad_enabled()):
-            loc = (self.loc * torch.exp(self.loc_logs * self.logscale_factor)).reshape(1, -1)
-            ls = (self.log_scale * torch.exp(self.log_scale_logs * self.logscale_factor)).reshape(1, -1)
-            if self.class_cond:
-                loc = loc + self.loc_cc
-                ls = ls + self.log_scale_cc
-            if self.temperature is not None:
-                ls = ls + np.log(self.temperature)
-        return loc, ls
-
-    @staticmethod
-    def _labels(y):
-        return y if y.dim() == 1 else torch.argmax(y, dim=1)   # one-hot rows select their class (base.py:403-411)
+    def _channel_params(self):
+        """([1, C] or [K, C]) mean and log-scale per channel (per class), base.py:397-424 / 438-461."""
+        loc = (self.loc * torch.exp(self.loc_logs * self.logscale_factor)).reshape(1, -1)
+        ls = (self.log_scale * torch.exp(self.log_scale_logs * self.logscale_factor)).reshape(1, -1)
+        if self.class_cond:
+            loc = loc + self.loc_cc
+            ls = ls + self.log_scale_cc
+        return loc, _tempered(ls, self.temperature)
 
     def forward(self, num_samples=1, y=None):
         dev = self.loc.device
-        loc, ls = self._channel_params()
-        if self.class_cond:
-            if y is not None:
-                num_samples = len(y)
-                y = self._labels(y).to(device=dev, dtype=torch.int64)
-            else:
-                y = torch.randint(self.num_classes, (num_samples,), device=dev)
-            loc, ls = loc[y], ls[y]                                         # [B, C]
         view = (-1, self.shape[0]) + (1,) * (self.n_dim - 1)
         with torch.no_grad():
+            loc, ls = self._channel_params()
+            if self.class_cond:
+                if y is not None:
+                    num_samples = len(y)
+                    y = _labels(y, dev)
+                else:
+                    y = torch.randint(self.num_classes, (num_samples,), device=dev)
+                loc, ls = loc[y], ls[y]                                     # [B, C]
             eps = torch.randn((num_samples,) + self.shape, dtype=self.loc.dtype, device=dev)
             z = (loc.reshape(view) + torch.exp(ls.reshape(view)) * eps).contiguous()
         return z, self.log_prob(z, y)
 
     def log_prob(self, z, y=None):
         z = require_cuda_f32(z)
-        if wants_grad(self, z) and z.shape[0]:
-            # tables [C, K]: element i of a sample uses channel i // num_pix
-            loc_d, ls_d = self._channel_params(differentiable=True)
-            yy = self._labels(y).to(device=z.device, dtype=torch.int64).contiguous() if self.class_cond else None
-            return gaussian_table_log_prob(lambda: self._log_prob_native(z, y), z, loc_d.t(), ls_d.t(), yy,
-                                           self.num_pix)
-        return self._log_prob_native(z, y)
-
-    def _log_prob_native(self, z, y):
-        loc, ls = self._channel_params()
-        out = torch.empty(z.shape[0], dtype=torch.float32, device=z.device)
-        if not z.shape[0]:
-            return out
-        with torch.cuda.device(z.device):
-            if self.class_cond:
-                y = self._labels(y).to(device=z.device, dtype=torch.int64).contiguous()
-                # [dim, K] tables: every pixel of channel c carries the channel's value
-                lt = loc.t().repeat_interleave(self.num_pix, dim=0).contiguous()
-                st = ls.t().repeat_interleave(self.num_pix, dim=0).contiguous()
-                L.check(L.lib().nfb_class_cond_diag_gaussian_log_prob(L.ptr(z), L.ptr(y), L.ptr(lt), L.ptr(st), L.ptr(out),
-                                                                      z.shape[0], self.d, self.num_classes, 0,
-                                                                      L.stream_ptr()))
-            else:
-                lt = loc.reshape(-1).repeat_interleave(self.num_pix).contiguous()
-                st = ls.reshape(-1).repeat_interleave(self.num_pix).contiguous()
-                L.check(L.lib().nfb_diag_gaussian_log_prob(L.ptr(z), L.ptr(lt), L.ptr(st), L.ptr(out), z.shape[0], self.d,
-                                                           0, L.stream_ptr()))
-        return out
+        loc, ls = self._channel_params()   # tables [C, K]: element i of a sample uses channel i // num_pix
+        return gaussian_table_log_prob(z, loc.t(), ls.t(), _labels(y, z.device) if self.class_cond else None,
+                                       self.num_pix)

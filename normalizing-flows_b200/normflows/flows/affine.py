@@ -160,12 +160,13 @@ class AffineCoupling(Flow):
         self.scale, self.scale_map = scale, scale_map
 
 
-class AffineCouplingBlock(NativeFlow):
-    _MAPS = {"exp": 0, "sigmoid": 1, "sigmoid_inv": 2}
+_MAPS = {"exp": 0, "sigmoid": 1, "sigmoid_inv": 2}   # scale-map enum of the coupling kernels (include/nfb200.h)
 
+
+class AffineCouplingBlock(NativeFlow):
     def __init__(self, param_map, scale=True, scale_map="exp", split_mode="channel"):
         super().__init__()
-        if scale_map not in self._MAPS:
+        if scale_map not in _MAPS:
             raise NotImplementedError("This scale map is not implemented.")
         if not isinstance(param_map, MLP):
             raise NotImplementedError("AffineCouplingBlock on the CUDA path takes a nets.MLP param_map")
@@ -180,7 +181,7 @@ class AffineCouplingBlock(NativeFlow):
     def _native_add(self, handle, features):
         d = L.AffineCouplingDesc()
         d.features, d.scale = features, int(bool(self.scale))
-        d.scale_map = self._MAPS[self.scale_map]
+        d.scale_map = _MAPS[self.scale_map]
         d.split_mode = 0 if self.split_mode == "channel" else 1
         d.param_map = mlp_desc(self.flows[1].param_map)
         L.check(L.lib().nfb_flow_add_affine_coupling(handle, C.byref(d)))

@@ -11,12 +11,16 @@ from torch import nn
 
 from .. import _lib as L
 from .._image_autograd import GlowBlockInverseFn, SplitChannelsFn, SqueezeFn, wants_grad
-from .._native import require_cuda_f32
+from .._native import cached, require_cuda_f32
 from ..nets.cnn import ConvNet2d
-from .affine import ActNorm, AffineCoupling, Merge, Split
+from .affine import _MAPS, ActNorm, AffineCoupling, Merge, Split
 from .base import Flow
 
-_MAPS = {"exp": 0, "sigmoid": 1, "sigmoid_inv": 2}
+
+def _pointwise(x, w, b, out):
+    """out = w x + b at every pixel of the NCHW tensor x: the folded 1x1 convolution, C -> C channels."""
+    B, C, H, W = x.shape
+    L.check(L.lib().nfb_conv2d(L.ptr(x), C, 0, L.ptr(w), L.ptr(b), L.ptr(out), B, C, H, W, C, 1, -1.0, L.stream_ptr()))
 
 
 class Invertible1x1Conv(Flow):
@@ -92,8 +96,7 @@ class Invertible1x1Conv(Flow):
         out = torch.empty_like(z)
         if B:
             with torch.cuda.device(z.device):
-                L.check(L.lib().nfb_conv2d(L.ptr(z), C, 0, L.ptr(w), L.ptr(b), L.ptr(out), B, C, H, W, C, 1, -1.0,
-                                           L.stream_ptr()))
+                _pointwise(z, w, b, out)
         return out, ldc  # 0-dim log-det like the reference (broadcasts in log_q += log_det)
 
     def forward(self, z):
@@ -183,122 +186,89 @@ class GlowBlock(Flow):
             raise NotImplementedError("Mode " + split_mode + " is not implemented.")
         if channels < 2:
             raise NotImplementedError("GlowBlock with a single channel is not on the CUDA path")
-        num_param = 2 if scale else 1
-        if split_mode == "channel":
-            ch = ((channels + 1) // 2, hidden_channels, hidden_channels, num_param * (channels // 2))
-        else:
-            ch = (channels // 2, hidden_channels, hidden_channels, num_param * ((channels + 1) // 2))
-        param_map = ConvNet2d(ch, (3, 1, 3), leaky, init_zeros, actnorm=net_actnorm)
+        h = (channels + 1) // 2
+        # the conditioner reads channels [c0, c0 + cin); the coupling transforms the other ones
+        self._c0, self._cin = (0, h) if split_mode == "channel" else (h, channels - h)
+        param_map = ConvNet2d((self._cin, hidden_channels, hidden_channels, (2 if scale else 1) * (channels - self._cin)),
+                              (3, 1, 3), leaky, init_zeros, actnorm=net_actnorm)
         block = Flow()
         block.flows = nn.ModuleList([Split(split_mode), AffineCoupling(param_map, scale, scale_map),
                                      Merge(split_mode)])
         self.flows = nn.ModuleList([block, Invertible1x1Conv(channels, use_lu), ActNorm((channels, 1, 1))])
         self.channels, self.scale, self.scale_map, self.split_mode = channels, scale, scale_map, split_mode
+        # (scale, scale map, split mode) enums of the coupling kernels
+        self._modes = (int(bool(scale)), _MAPS[scale_map], 0 if split_mode == "channel" else 1)
 
-    def _folded(self, key, fn, hw, dev):
+    def _param_map(self):
+        return self.flows[0].flows[1].param_map
+
+    def _folded(self, direction, hw, dev):
         """Folded 1x1 convolution (weights, bias, per-sample log-det constant) of ActNorm + Invertible1x1Conv for
-        one direction; depends on the parameters only, so it is rebuilt when one of them changes
-        ((data_ptr, _version) signature, like _native.FlowHandle), not on every call."""
+        one direction, rebuilt when one of the parameters changes, not on every call."""
         conv, an = self.flows[1], self.flows[2]
-        src = conv._sources() + (an.s, an.t)
-        from .._native import generation
-        sig = tuple((t.data_ptr(), t._version) for t in src) + (hw, dev, generation())
-        cache = self.__dict__.get(key)
-        if cache is None or cache[0] != sig:
-            direction = L.NFB_INVERSE if fn is L.lib().nfb_glow_fold_actnorm_conv1x1 else L.NFB_FORWARD
-            w, b, ldc = conv.folded(direction, an.s, an.t, hw, dev)
-            cache = (sig, w, b, ldc)
-            self.__dict__[key] = cache
-        return cache[1], cache[2], cache[3]
+        return cached(self, "_nfb_fold_fwd" if direction == L.NFB_FORWARD else "_nfb_fold",
+                      conv._sources() + (an.s, an.t), (hw, dev), lambda: conv.folded(direction, an.s, an.t, hw, dev))
 
     def _one_call(self, z, out, scratch, ld, w, b, ldc, direction):
         """The whole block through nfb_glow_block (one C-ABI call: folded 1x1 convolution, fused conditioner, tap-form
-        coupling) when the conditioner has the Glow shape; False = not applicable, the caller takes the step-by-step path."""
-        lib = L.lib()
+        coupling) when the conditioner has the Glow shape and the sample fits the tap-form coupling; False = not
+        applicable, the caller takes the step-by-step path."""
         B, C, H, W = z.shape
-        pm = self.flows[0].flows[1].param_map
-        h = (C + 1) // 2
-        cin = h if self.split_mode == "channel" else C - h
-        if not (pm._glow_shape(cin) and lib.nfb_affine_coupling_image_taps_supported(C, H, W, int(bool(self.scale)))):
+        pm = self._param_map()
+        if not (pm.glow_shape(self._cin) and L.lib().nfb_affine_coupling_image_taps_supported(C, H, W, self._modes[0])):
             return False
         c1, c2, c3 = pm.conv_layers()
-        cout, hid = c3.out_channels, c1.out_channels
         with torch.cuda.device(z.device):
-            packed = pm._packed_conditioner(c1, c2, c3, cin, hid, cout)
-            yt = torch.empty(B, 9 * cout, H, W, device=z.device, dtype=torch.float32)
-            L.check(lib.nfb_glow_block(L.ptr(z), L.ptr(out), L.ptr(scratch) if scratch is not None else None, L.ptr(yt),
-                                       L.ptr(ld), L.ptr(w), L.ptr(b), L.ptr(ldc), L.ptr(packed), L.ptr(c1.bias),
-                                       L.ptr(c2.bias), L.ptr(c3.bias), B, C, H, W, hid, int(bool(self.scale)),
-                                       _MAPS[self.scale_map], 0 if self.split_mode == "channel" else 1,
-                                       float(pm.leaky), direction, L.stream_ptr()))
+            packed = pm._packed_conditioner(self._cin)
+            yt = torch.empty(B, 9 * c3.out_channels, H, W, device=z.device, dtype=torch.float32)
+            L.check(L.lib().nfb_glow_block(L.ptr(z), L.ptr(out), L.ptr(scratch), L.ptr(yt), L.ptr(ld), L.ptr(w), L.ptr(b),
+                                           L.ptr(ldc), L.ptr(packed), L.ptr(c1.bias), L.ptr(c2.bias), L.ptr(c3.bias),
+                                           B, C, H, W, c1.out_channels, *self._modes, float(pm.leaky), direction,
+                                           L.stream_ptr()))
         return True
 
-    def _coupling(self, src, dst, c0, cin, ld, ldc, direction):
-        """Conditioner on src[:, c0:c0+cin], then the affine coupling in place on the other half of dst, log-det into ld.
-        Glow-shaped conditioners hand their output over in tap form (no summed parameter tensor); other shapes go
-        through apply_native + nfb_affine_coupling_image."""
-        lib = L.lib()
-        B, C, H, W = dst.shape
-        pm = self.flows[0].flows[1].param_map
-        args = (B, C)
-        tail = (int(bool(self.scale)), _MAPS[self.scale_map], 0 if self.split_mode == "channel" else 1, direction, 0,
-                L.stream_ptr())
-        taps = pm.apply_native_taps(src, c0, cin) if lib.nfb_affine_coupling_image_taps_supported(
-            C, H, W, int(bool(self.scale))) else None
-        if taps is not None:
-            yt, bias = taps
-            L.check(lib.nfb_affine_coupling_image_taps(L.ptr(dst), L.ptr(yt), L.ptr(bias), L.ptr(ld), L.ptr(ldc), *args,
-                                                       H, W, *tail))
-        else:
-            param = pm.apply_native(src, c0, cin)
-            L.check(lib.nfb_affine_coupling_image(L.ptr(dst), L.ptr(param), L.ptr(ld), L.ptr(ldc), *args, H * W, *tail))
+    def _coupling(self, z, param, ld, ldc, direction):
+        """nfb_affine_coupling_image in place on the transformed half of z, given the conditioner's output param;
+        ld / ldc None: no log-det."""
+        B, C, H, W = z.shape
+        L.check(L.lib().nfb_affine_coupling_image(L.ptr(z), L.ptr(param), L.ptr(ld), L.ptr(ldc), B, C, H * W,
+                                                  *self._modes, direction, 0, L.stream_ptr()))
 
-    def forward(self, z):
-        """Sampling direction (glow.py:72-77): coupling block, then Invertible1x1Conv.forward, then ActNorm.forward."""
+    def _check(self, z):
         z = require_cuda_f32(z)
         if z.dim() != 4 or z.shape[1] != self.channels:
             raise ValueError("Expected an NCHW tensor with {} channels.".format(self.channels))
+        return z
+
+    def forward(self, z):
+        """Sampling direction (glow.py:72-77): coupling block, then Invertible1x1Conv.forward, then ActNorm.forward."""
+        z = self._check(z)
         an = self.flows[2]
         B, C, H, W = z.shape
         dev = z.device
-        lib = L.lib()
         out = torch.empty_like(z)
         ld = torch.empty(B, device=dev)
         if B == 0:
             return out, ld
-        h = (C + 1) // 2
-        c0, cin = (0, h) if self.split_mode == "channel" else (h, C - h)
         if an._done():
-            w, b, ldc = self._folded("_nfb_fold_fwd", lib.nfb_glow_fold_conv1x1_actnorm_forward, H * W, dev)
+            w, b, ldc = self._folded(L.NFB_FORWARD, H * W, dev)
             if self._one_call(z, out, torch.empty_like(z), ld, w, b, ldc, L.NFB_FORWARD):
                 return out, ld
         mid = z.clone()  # the coupling kernel works in place on the transformed half
         with torch.cuda.device(dev):
-            # (initialised ActNorm: the conditioner's output stays in tap form and the coupling sums it on the fly)
-            param = self.flows[0].flows[1].param_map.apply_native(z, c0, cin) if not an._done() else None
+            param = self._param_map().apply_native(z, self._c0, self._cin)
             if not an._done():
                 # data-dependent init in the sampling direction sees the output of the 1x1 convolution
-                # (normalization.py:19-29); run the first two layers, initialise, then fold
-                w0, b0, _ = self._folded("_nfb_fold_fwd_init", lib.nfb_glow_fold_conv1x1_actnorm_forward, H * W, dev)
+                # (normalization.py:19-29): run the first two layers on a copy, initialise, then fold again
+                w0, b0, _ = self._folded(L.NFB_FORWARD, H * W, dev)
                 tmp = mid.clone()
-                L.check(lib.nfb_affine_coupling_image(
-                    L.ptr(tmp), L.ptr(param), None, None, B, C, H * W, int(bool(self.scale)),
-                    _MAPS[self.scale_map], 0 if self.split_mode == "channel" else 1, L.NFB_FORWARD, 0,
-                    L.stream_ptr()))
+                self._coupling(tmp, param, None, None, L.NFB_FORWARD)
                 pre = torch.empty_like(z)
-                L.check(lib.nfb_conv2d(L.ptr(tmp), C, 0, L.ptr(w0), L.ptr(b0), L.ptr(pre), B, C, H, W, C, 1, -1.0,
-                                       L.stream_ptr()))
+                _pointwise(tmp, w0, b0, pre)
                 an._data_init(pre, "forward")
-            w, b, ldc = self._folded("_nfb_fold_fwd", lib.nfb_glow_fold_conv1x1_actnorm_forward, H * W, dev)
-            if param is None:
-                self._coupling(z, mid, c0, cin, ld, ldc, L.NFB_FORWARD)
-            else:
-                L.check(lib.nfb_affine_coupling_image(
-                    L.ptr(mid), L.ptr(param), L.ptr(ld), L.ptr(ldc), B, C, H * W, int(bool(self.scale)),
-                    _MAPS[self.scale_map], 0 if self.split_mode == "channel" else 1, L.NFB_FORWARD, 0,
-                    L.stream_ptr()))
-            L.check(lib.nfb_conv2d(L.ptr(mid), C, 0, L.ptr(w), L.ptr(b), L.ptr(out), B, C, H, W, C, 1, -1.0,
-                                   L.stream_ptr()))
+            w, b, ldc = self._folded(L.NFB_FORWARD, H * W, dev)
+            self._coupling(mid, param, ld, ldc, L.NFB_FORWARD)
+            _pointwise(mid, w, b, out)
         return out, ld
 
     def inverse(self, z):
@@ -307,28 +277,22 @@ class GlowBlock(Flow):
         return self._inverse_native(z)
 
     def _inverse_native(self, z):
-        z = require_cuda_f32(z)
-        if z.dim() != 4 or z.shape[1] != self.channels:
-            raise ValueError("Expected an NCHW tensor with {} channels.".format(self.channels))
-        conv, an = self.flows[1], self.flows[2]
+        z = self._check(z)
+        an = self.flows[2]
         if not an._done():
             an._data_init(z, "inverse")
         B, C, H, W = z.shape
-        dev = z.device
-        lib = L.lib()
         out = torch.empty_like(z)
-        ld = torch.empty(B, device=dev)
+        ld = torch.empty(B, device=z.device)
         if B == 0:
             return out, ld
-        w, b, ldc = self._folded("_nfb_fold", lib.nfb_glow_fold_actnorm_conv1x1, H * W, dev)
+        w, b, ldc = self._folded(L.NFB_INVERSE, H * W, z.device)
         if self._one_call(z, out, None, ld, w, b, ldc, L.NFB_INVERSE):
             return out, ld
-        with torch.cuda.device(dev):
-            L.check(lib.nfb_conv2d(L.ptr(z), C, 0, L.ptr(w), L.ptr(b), L.ptr(out), B, C, H, W, C, 1, -1.0,
-                                   L.stream_ptr()))
-            h = (C + 1) // 2
-            c0, cin = (0, h) if self.split_mode == "channel" else (h, C - h)
-            self._coupling(out, out, c0, cin, ld, ldc, L.NFB_INVERSE)
+        with torch.cuda.device(z.device):
+            _pointwise(z, w, b, out)
+            param = self._param_map().apply_native(out, self._c0, self._cin)
+            self._coupling(out, param, ld, ldc, L.NFB_INVERSE)
         return out, ld
 
     def _inverse_backward(self, z, g_out, g_ld):
@@ -338,24 +302,23 @@ class GlowBlock(Flow):
         fold.  Returns (g_z, {id(parameter): gradient})."""
         lib = L.lib()
         conv, an = self.flows[1], self.flows[2]
-        pm = self.flows[0].flows[1].param_map
+        pm = self._param_map()
         B, C, H, W = z.shape
         HW, dev = H * W, z.device
-        h = (C + 1) // 2
-        c0, cin = (0, h) if self.split_mode == "channel" else (h, C - h)
+        c0, cin = self._c0, self._cin
         grads = {}
         with torch.cuda.device(dev):
             st = L.stream_ptr()
-            w, b, _ = self._folded("_nfb_fold", lib.nfb_glow_fold_actnorm_conv1x1, HW, dev)
+            w, b, _ = self._folded(L.NFB_INVERSE, HW, dev)
             mid = torch.empty_like(z)
-            L.check(lib.nfb_conv2d(L.ptr(z), C, 0, L.ptr(w), L.ptr(b), L.ptr(mid), B, C, H, W, C, 1, -1.0, st))
+            _pointwise(z, w, b, mid)
             acts = pm.native_activations(mid, c0, cin)
             param = acts[-1]
             g_mid = torch.empty_like(z)
             g_param = torch.empty_like(param)
             L.check(lib.nfb_affine_coupling_image_backward(
                 L.ptr(mid), L.ptr(param), L.ptr(g_out), L.ptr(g_ld), L.ptr(g_mid), L.ptr(g_param), B, C, HW,
-                int(bool(self.scale)), _MAPS[self.scale_map], 0 if self.split_mode == "channel" else 1, st))
+                *self._modes, st))
             g_z1 = torch.empty(B, cin, H, W, device=dev)   # z1 passes through the coupling and feeds the conditioner
             L.check(lib.nfb_copy_channels(L.ptr(g_out), L.ptr(g_z1), B, C, c0, cin, HW, st))
             grads.update(pm.native_backward(mid, c0, cin, acts, g_param, g_z1))

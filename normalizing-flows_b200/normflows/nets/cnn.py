@@ -1,9 +1,11 @@
 """ConvNet2d parameter container (reference: normflows/nets/cnn.py:5-63): Conv2d / LeakyReLU stack with
 `padding = k // 2`, last conv optionally zero-initialised; same `net.<i>` state_dict keys.  The convolutions
 run in csrc/nfb_glow.cu (`nfb_conv2d`)."""
+import torch
 from torch import nn
 
 from .. import _lib as L
+from .._native import cached
 
 
 class ConvNet2d(nn.Module):
@@ -31,119 +33,90 @@ class ConvNet2d(nn.Module):
     def conv_layers(self):
         return [m for m in self.net if isinstance(m, nn.Conv2d)]
 
-    def _glow_shape(self, cin):
-        mods = list(self.net)
-        convs = self.conv_layers()
-        return (len(convs) == 3 and len(mods) == 5 and [cv.kernel_size[0] for cv in convs] == [3, 1, 3]
-                and convs[0].out_channels == convs[1].out_channels == convs[1].in_channels
-                and convs[0].out_channels % 64 == 0 and convs[0].out_channels <= 256
-                and 9 * cin <= 256 and 9 * convs[2].out_channels <= 512 and self.leaky >= 0.0)
-
-    def apply_native_taps(self, x, c0, cin):
-        """The Glow conditioner shape only: returns (y_taps [B, 9 * out, H, W], bias [out]) -- the last 3x3 convolution
-        left as nine stacked 1x1 products for nfb_affine_coupling_image_taps to sum on the fly -- or None."""
-        import torch
-        if not self._glow_shape(cin):
-            return None
-        B, ctot, H, W = x.shape
-        c1, c2, c3 = self.conv_layers()
-        cout, hid = c3.out_channels, c1.out_channels
-        yt = torch.empty(B, 9 * cout, H, W, device=x.device, dtype=torch.float32)
-        with torch.cuda.device(x.device):
-            packed = self._packed_conditioner(c1, c2, c3, cin, hid, cout)
-            L.check(L.lib().nfb_glow_conditioner_packed(L.ptr(x), ctot, c0, cin, L.ptr(packed), L.ptr(c1.bias),
-                                                        L.ptr(c2.bias), L.ptr(yt), B, H, W, hid, cout,
-                                                        float(self.leaky), L.stream_ptr()))
-        return yt, c3.bias
+    def glow_shape(self, cin):
+        """True when the net on `cin` input channels is the Glow conditioner that csrc/nfb_glow_fused.cu runs as one
+        kernel: 3x3, 1x1 and 3x3 convolutions with no ActNorm, a LeakyReLU slope >= 0, and channel counts the library
+        accepts (nfb_glow_conditioner_packed_bytes >= 0).  Fixed for a module and cin, so it is worked out once."""
+        known = self.__dict__.setdefault("_nfb_glow_shape", {})
+        if cin not in known:
+            cv = self.conv_layers()
+            known[cin] = (len(self.net) == 5 and [c.kernel_size[0] for c in cv] == [3, 1, 3]   # 5 modules: no ActNorm
+                          and cv[0].out_channels == cv[1].in_channels == cv[1].out_channels and self.leaky >= 0.0
+                          and L.lib().nfb_glow_conditioner_packed_bytes(cin, cv[0].out_channels, cv[2].out_channels) >= 0)
+        return known[cin]
 
     def apply_native(self, x, c0, cin):
-        """y = net(x[:, c0:c0+cin]) for a contiguous CUDA NCHW tensor x; returns [B, out, H, W]."""
-        import torch
+        """y = net(x[:, c0:c0+cin]) for a contiguous CUDA NCHW tensor x; returns [B, out, H, W].  An ActNorm still
+        waiting for its data-dependent init (flows/normalization.py:19-29) gets it from its conv's raw output."""
         B, ctot, H, W = x.shape
-        from ..utils.nn import ActNorm
-        mods = list(self.net)
-        convs = self.conv_layers()
-        if self._glow_shape(cin):
-            # the Glow conditioner shape: ONE fused tensor-core kernel (csrc/nfb_glow_fused.cu) + the shifted tap sum
-            c1, c2, c3 = convs
-            cout, hid = c3.out_channels, c1.out_channels
-            yt = torch.empty(B, 9 * cout, H, W, device=x.device, dtype=torch.float32)
-            out = torch.empty(B, cout, H, W, device=x.device, dtype=torch.float32)
-            with torch.cuda.device(x.device):
-                packed = self._packed_conditioner(c1, c2, c3, cin, hid, cout)   # once per parameter version
-                L.check(L.lib().nfb_glow_conditioner_packed(L.ptr(x), ctot, c0, cin, L.ptr(packed), L.ptr(c1.bias),
-                                                            L.ptr(c2.bias), L.ptr(yt), B, H, W, hid, cout,
-                                                            float(self.leaky), L.stream_ptr()))
-                L.check(L.lib().nfb_tap_shift_add(L.ptr(yt), L.ptr(c3.bias), L.ptr(out), B, cout, H, W, 3, L.stream_ptr()))
-            return out
-        cur, cur_tot, cur_c0 = x, ctot, c0
-        with torch.cuda.device(x.device):
-            for j, conv in enumerate(mods):
-                if not isinstance(conv, nn.Conv2d):
-                    continue
-                last = conv is mods[-1]
-                an = mods[j + 1].actNorm if j + 1 < len(mods) and isinstance(mods[j + 1], ActNorm) else None
-                w, b = conv.weight, conv.bias
-                y = torch.empty(B, conv.out_channels, H, W, device=x.device, dtype=torch.float32)
-
-                def run(wt, bt, act):
-                    L.check(L.lib().nfb_conv2d(L.ptr(cur), cur_tot, cur_c0, L.ptr(wt), L.ptr(bt), L.ptr(y), B,
-                                               conv.in_channels, H, W, conv.out_channels, conv.kernel_size[0], act,
-                                               L.stream_ptr()))
-                if an is not None:
-                    # ActNorm after the conv = per-channel affine: folded into the conv's weights and bias.  First
-                    # call: raw conv output -> data-dependent init (flows/normalization.py:19-29), then the fold.
-                    if not an._done():
-                        run(w, None, -1.0)
-                        an._data_init(y, "forward")
-                    with torch.no_grad():
-                        e = torch.exp(an.s.detach().reshape(-1))
-                        w = (conv.weight.detach() * e[:, None, None, None]).contiguous()
-                        b = an.t.detach().reshape(-1).contiguous()
-                k = conv.kernel_size[0]
-                if (last and an is None and k > 1 and conv.in_channels >= 128 and k * k * conv.out_channels <= 256
-                        and conv.out_channels <= 64):
-                    # k x k conv with few outputs: k*k stacked 1x1 products on the tensor core + a shifted sum
+        dev = x.device
+        with torch.cuda.device(dev):
+            if self.glow_shape(cin):
+                # ONE fused tensor-core kernel (csrc/nfb_glow_fused.cu) leaves the last 3x3 convolution as nine stacked
+                # 1x1 products; the shifted tap sum adds them up
+                c1, c2, c3 = self.conv_layers()
+                yt = torch.empty(B, 9 * c3.out_channels, H, W, device=dev)
+                out = torch.empty(B, c3.out_channels, H, W, device=dev)
+                L.check(L.lib().nfb_glow_conditioner_packed(L.ptr(x), ctot, c0, cin, L.ptr(self._packed_conditioner(cin)),
+                                                            L.ptr(c1.bias), L.ptr(c2.bias), L.ptr(yt), B, H, W,
+                                                            c1.out_channels, c3.out_channels, float(self.leaky),
+                                                            L.stream_ptr()))
+                L.check(L.lib().nfb_tap_shift_add(L.ptr(yt), L.ptr(c3.bias), L.ptr(out), B, c3.out_channels, H, W, 3,
+                                                  L.stream_ptr()))
+                return out
+            cur, cur_tot, cur_c0 = x, ctot, c0
+            for conv, an, act in self._layers():
+                y = torch.empty(B, conv.out_channels, H, W, device=dev)
+                k, ci, co = conv.kernel_size[0], conv.in_channels, conv.out_channels
+                if an is not None and not an._done():
+                    L.check(L.lib().nfb_conv2d(L.ptr(cur), cur_tot, cur_c0, L.ptr(conv.weight), None, L.ptr(y), B, ci,
+                                               H, W, co, k, -1.0, L.stream_ptr()))
+                    an._data_init(y, "forward")
+                w, b = self._fold(conv, an)
+                if conv is self.net[-1] and k > 1 and ci >= 128 and k * k * co <= 256 and co <= 64:
+                    # last k x k conv with few outputs: k*k stacked 1x1 products on the tensor core + a shifted sum
                     # (csrc/nfb_glow.cu tap_shift_add_kernel) instead of an im2col GEMM with K = k*k*cin
-                    wt = self._tap_weights(conv)
-                    yt = torch.empty(B, k * k * conv.out_channels, H, W, device=x.device, dtype=torch.float32)
-                    L.check(L.lib().nfb_conv2d(L.ptr(cur), cur_tot, cur_c0, L.ptr(wt), None, L.ptr(yt), B,
-                                               conv.in_channels, H, W, k * k * conv.out_channels, 1, -1.0, L.stream_ptr()))
-                    L.check(L.lib().nfb_tap_shift_add(L.ptr(yt), L.ptr(b), L.ptr(y), B, conv.out_channels, H, W, k,
-                                                      L.stream_ptr()))
+                    yt = torch.empty(B, k * k * co, H, W, device=dev)
+                    L.check(L.lib().nfb_conv2d(L.ptr(cur), cur_tot, cur_c0, L.ptr(self._tap_weights(conv)), None,
+                                               L.ptr(yt), B, ci, H, W, k * k * co, 1, -1.0, L.stream_ptr()))
+                    L.check(L.lib().nfb_tap_shift_add(L.ptr(yt), L.ptr(b), L.ptr(y), B, co, H, W, k, L.stream_ptr()))
                 else:
-                    run(w, b, -1.0 if last else float(self.leaky))
-                cur, cur_tot, cur_c0 = y, conv.out_channels, 0
+                    L.check(L.lib().nfb_conv2d(L.ptr(cur), cur_tot, cur_c0, L.ptr(w), L.ptr(b), L.ptr(y), B, ci, H, W,
+                                               co, k, act, L.stream_ptr()))
+                cur, cur_tot, cur_c0 = y, co, 0
         return cur
 
-    def _folded_layers(self, differentiable=False):
-        """[(conv, w, b, act)] per convolution with a following ActNorm folded in (w * exp(s), b = t), as apply_native
-        runs them; act = LeakyReLU slope, or -1.0 for the last layer.  differentiable=True: w / b keep autograd history
-        to the parameters (the gradient chain of the training pass)."""
-        import torch
+    def _layers(self):
+        """[(conv, the ActNorm that follows it or None, act)] per convolution; act = LeakyReLU slope, or -1.0 for the
+        last layer."""
         from ..utils.nn import ActNorm
         mods = list(self.net)
-        out = []
-        for j, conv in enumerate(mods):
-            if not isinstance(conv, nn.Conv2d):
-                continue
-            an = mods[j + 1].actNorm if j + 1 < len(mods) and isinstance(mods[j + 1], ActNorm) else None
-            w, b = conv.weight, conv.bias
-            if an is not None:
-                w = conv.weight * torch.exp(an.s.reshape(-1))[:, None, None, None]
-                b = an.t.reshape(-1)
-            if not differentiable:
-                w, b = w.detach().contiguous(), b.detach().contiguous()
-            out.append((conv, w, b, -1.0 if conv is mods[-1] else float(self.leaky)))
-        return out
+        return [(conv, mods[j + 1].actNorm if j + 1 < len(mods) and isinstance(mods[j + 1], ActNorm) else None,
+                 -1.0 if conv is mods[-1] else float(self.leaky))
+                for j, conv in enumerate(mods) if isinstance(conv, nn.Conv2d)]
+
+    @staticmethod
+    def _fold(conv, an, differentiable=False):
+        """(w, b) of conv with the ActNorm after it folded in (w * exp(s), b = t).  differentiable=True: w / b keep
+        autograd history to the parameters (the gradient chain of the training pass)."""
+        w, b = conv.weight, conv.bias
+        if an is not None:
+            w = conv.weight * torch.exp(an.s.reshape(-1))[:, None, None, None]
+            b = an.t.reshape(-1)
+        if not differentiable:
+            w, b = w.detach().contiguous(), b.detach().contiguous()
+        return w, b
+
+    def _folded_layers(self, differentiable=False):
+        """[(conv, w, b, act)] per convolution, as apply_native runs them (see _layers and _fold)."""
+        return [(conv, *self._fold(conv, an, differentiable), act) for conv, an, act in self._layers()]
 
     def native_activations(self, x, c0, cin):
         """Training-pass recompute of the conditioner on x[:, c0:c0+cin] layer by layer (nfb_conv2d): the list of every
         layer's output (post-activation); the last one is the parameter tensor.  ActNorm must be initialised.  For the
-        Glow shape the forward ran the fused kernel with the tap-form coupling instead: the recomputed activations and
-        parameter tensor are the same sums rounded in a different order (~1e-5 relative), so the adjoint is taken at
-        values within that of the forward's; a ReLU whose input lies that close to 0 may take the other branch."""
-        import torch
+        Glow shape the forward ran the fused kernel and the tap sum instead: the recomputed activations and parameter
+        tensor are the same sums rounded in a different order (~1e-5 relative), so the adjoint is taken at values within
+        that of the forward's; a ReLU whose input lies that close to 0 may take the other branch."""
         B, ctot, H, W = x.shape
         acts, cur, cur_tot, cur_c0 = [], x, ctot, c0
         for conv, w, b, act in self._folded_layers():
@@ -158,7 +131,6 @@ class ConvNet2d(nn.Module):
         """Adjoint of native_activations: g_out = gradient of the last output; the input gradient is ACCUMULATED into
         g_x [B, cin, H, W].  LeakyReLU' comes from the stored post-activation tensors.  Returns {id(parameter): grad};
         folded ActNorm gradients go back to (weight, s, t) by torch autograd over the fold."""
-        import torch
         lib = L.lib()
         B, ctot, H, W = x.shape
         layers = self._folded_layers()
@@ -193,37 +165,28 @@ class ConvNet2d(nn.Module):
             got = torch.autograd.grad(outs, params, gs, allow_unused=True)
         return {id(p): gp for p, gp in zip(params, got)}
 
-    def _packed_conditioner(self, c1, c2, c3, cin, hid, cout):
-        """bf16 hi | lo records of the three convolutions in the fused kernel's layout (csrc/nfb_glow_fused.cu), cached per
-        parameter version (and packed-weight generation): round 2a re-packed them on every call (5.5 % of a Glow pass)."""
-        import torch
-        from .._native import generation
-        ws = (c1.weight, c2.weight, c3.weight)
-        sig = tuple((t.data_ptr(), t._version) for t in ws) + (generation(),)
-        cache = self.__dict__.get("_nfb_packed")
-        if cache is None or cache[0] != sig:
-            nbytes = int(L.lib().nfb_glow_conditioner_packed_bytes(cin, hid, cout))
-            buf = torch.empty(nbytes, dtype=torch.uint8, device=c1.weight.device)
+    def _packed_conditioner(self, cin):
+        """bf16 hi | lo records of the three convolutions in the fused kernel's layout (csrc/nfb_glow_fused.cu), once per
+        parameter version: re-packing them on every call cost 5.5 % of a Glow pass."""
+        c1, c2, c3 = self.conv_layers()
+
+        def pack():
+            hid, cout = c1.out_channels, c3.out_channels
+            buf = torch.empty(int(L.lib().nfb_glow_conditioner_packed_bytes(cin, hid, cout)), dtype=torch.uint8,
+                              device=c1.weight.device)
             L.check(L.lib().nfb_glow_conditioner_pack(L.ptr(c1.weight), L.ptr(c2.weight), L.ptr(self._tap_weights(c3)),
                                                       cin, hid, cout, L.ptr(buf), L.stream_ptr()))
-            cache = (sig, buf)
-            self.__dict__["_nfb_packed"] = cache
-        return cache[1]
+            return buf
+        return cached(self, "_nfb_packed", (c1.weight, c2.weight, c3.weight), (), pack)
 
     def _tap_weights(self, conv):
-        """[cout, cin, k, k] -> [k*k*cout, cin, 1, 1] with row (kh*k + kw)*cout + n = W[n, :, kh, kw]; cached per
-        parameter version (and packed-weight generation)."""
-        import torch
-        from .._native import generation
-        sig = (conv.weight.data_ptr(), conv.weight._version, generation())
-        cache = self.__dict__.get("_nfb_tapw")
-        if cache is None or cache[0] != sig:
+        """[cout, cin, k, k] -> [k*k*cout, cin, 1, 1] with row (kh*k + kw)*cout + n = W[n, :, kh, kw]; once per
+        parameter version."""
+        def permute():
             with torch.no_grad():
                 w = conv.weight.detach()
-                wt = w.permute(2, 3, 0, 1).reshape(-1, w.shape[1], 1, 1).contiguous()
-            cache = (sig, wt)
-            self.__dict__["_nfb_tapw"] = cache
-        return cache[1]
+                return w.permute(2, 3, 0, 1).reshape(-1, w.shape[1], 1, 1).contiguous()
+        return cached(self, "_nfb_tapw", (conv.weight,), (), permute)
 
     def forward(self, x):
         from .._native import require_cuda_f32

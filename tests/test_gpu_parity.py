@@ -328,6 +328,20 @@ def test_glow_sampling_direction_matches_reference():
     zo, ldo = O.glow_block(z0, O._cast(sd, np.float64), "flows.0.0.", {}, "forward")
     np.testing.assert_allclose(z.cpu().numpy(), zo, rtol=1e-4, atol=2e-4)
     np.testing.assert_allclose(ldb.cpu().numpy(), ldo, rtol=1e-4, atol=1e-3)
+    # a Glow-shaped conditioner on samples too large for the tap-form coupling (9 * 2 * 24 * 16 * 16 * 4 B > 200 KB):
+    # the step-by-step path with the fused conditioner, in both directions
+    torch.manual_seed(8)
+    big = nf.flows.GlowBlock(48, 256).cuda()
+    with torch.no_grad():
+        big.flows[0].flows[1].param_map.net[-1].weight.normal_(0, 0.01)
+    z0 = np.random.default_rng(5).normal(size=(4, 48, 16, 16))
+    got = {"inverse": big.inverse(cuda(z0))}   # (initialises the ActNorm from this batch first)
+    got["forward"] = big.forward(cuda(z0))
+    sdb = {k: v.cpu().numpy().astype(np.float64) for k, v in big.state_dict().items()}
+    for direction, (z, ldb) in got.items():
+        zo, ldo = O.glow_block(z0, sdb, "", {}, direction)
+        np.testing.assert_allclose(z.cpu().numpy(), zo, rtol=1e-4, atol=2e-4)
+        np.testing.assert_allclose(ldb.cpu().numpy(), ldo, rtol=1e-4, atol=1e-2)
     # sampling: shapes, finiteness, and log_q consistent with the density of what was drawn
     y = torch.from_numpy(a["y"]).cuda()
     torch.manual_seed(7)
