@@ -92,6 +92,46 @@ int nfb_glu_residual(const float* h_dev, const float* t_dev, const float* c_dev,
 int nfb_rowdot(const float* a_dev, const float* b_dev, int64_t rows, int32_t d, float c, int32_t accumulate,
                float* out_dev, void* stream);
 
+/* ---- training pass of the residual block (`forward_kld(x).backward()` of examples/residual.ipynb) ----
+ * g = Linear_L o Swish_L o ... o Linear_1 o Swish_1 (nets/lipschitz.py LipschitzMLP) pushed forward together with nt
+ * tangents t_0 (the "dual" network: t_l = W_l (sigma_l'(h_{l-1}) * t_{l-1})), then reverse mode over it.  Stacked
+ * tensors hold the primal rows first, then tangent 0, 1, ...: [(1 + nt) rows, width].
+ * Swish: sigma(h) = h sigmoid(b h) / 1.1 with b = softplus(beta). */
+#define NFB_LIPSCHITZ_MLP_MAX_LAYERS 8
+typedef struct {
+    int32_t num_layers;                                 /* Linear layers, 1 .. NFB_LIPSCHITZ_MLP_MAX_LAYERS */
+    int32_t widths[NFB_LIPSCHITZ_MLP_MAX_LAYERS + 1];   /* widths[0] = input features, widths[num_layers] = output */
+    const float* w[NFB_LIPSCHITZ_MLP_MAX_LAYERS];       /* effective weight W~_l [widths[l+1], widths[l]] (compute_weight) */
+    const float* bias[NFB_LIPSCHITZ_MLP_MAX_LAYERS];    /* [widths[l+1]] */
+    float b[NFB_LIPSCHITZ_MLP_MAX_LAYERS];              /* softplus(beta) of the Swish in front of Linear l */
+} nfb_lipschitz_mlp_desc_t;
+/* Bytes of device scratch nfb_lipschitz_mlp_dual_backward needs for `rows` rows and nt tangents (-1: bad descriptor). */
+int64_t nfb_lipschitz_mlp_dual_backward_workspace_bytes(const nfb_lipschitz_mlp_desc_t* desc, int32_t nt, int64_t rows);
+/* Gradients of  sum_r g_seed[r] . g(x_r) + sum_t sum_r t_seeds[t, r] . (J(x_r) tangents0[t, r])  w.r.t. x, every W~_l,
+ * bias_l and b_l, in one call: the dual forward is recomputed from x and tangents0 [nt, rows, widths[0]], then the
+ * adjoint runs layer by layer (dgrad and wgrad GEMMs on the tensor core over the stacked rows, the element-wise adjoint
+ * of the Swish with its second derivative).  g_seed [rows, out] and t_seeds [nt, rows, out] may be NULL (zero).
+ * Outputs, each OVERWRITTEN and each optional: gx [rows, widths[0]]; gW[l] [widths[l+1], widths[l]]; gbias[l];
+ * gb [num_layers] (the b_l gradients, reduced in a fixed order: deterministic).  gW / gbias themselves may be NULL. */
+int nfb_lipschitz_mlp_dual_backward(const nfb_lipschitz_mlp_desc_t* desc, const float* x_dev, const float* tangents0_dev,
+                                    int32_t nt, const float* g_seed_dev, const float* t_seeds_dev, int64_t rows,
+                                    void* workspace_dev, int64_t workspace_bytes, float* gx_dev, float* const* gW_dev,
+                                    float* const* gbias_dev, float* gb_dev, void* stream);
+/* The element-wise pieces of that pass, stand-alone (H, A: stacked [(1 + nt) rows, width]; H without the bias, which
+ * is added to the primal rows; bias may be NULL).  swish_dual: A = [sigma(h); sigma'(h) t_1; ...].
+ * swish_dual_adjoint: from Abar (the cotangent of A) writes hbar = sigma' abar + sigma'' sum_t t_t tabar_t to
+ * out_primal [rows, width] and tbar_t = sigma' tabar_t to out_tangent [nt rows, width] (either may be NULL or alias
+ * Abar), and *g_b_dev = d/db (fixed-order sum; partials_dev: NFB_SWISH_DUAL_PARTIALS doubles of scratch). */
+#define NFB_SWISH_DUAL_PARTIALS 1024
+int nfb_swish_dual(const float* H_dev, const float* bias_dev, float b, int64_t rows, int32_t width, int32_t nt,
+                   float* A_dev, void* stream);
+int nfb_swish_dual_adjoint(const float* H_dev, const float* bias_dev, float b, int64_t rows, int32_t width, int32_t nt,
+                           const float* Abar_dev, float* out_primal_dev, float* out_tangent_dev, double* partials_dev,
+                           float* g_b_dev, void* stream);
+/* Adjoint of nfb_logabsdet_i_plus_j_2x2: seeds [2, batch, 2] = g_ld[r] * (column t of (I + J_r)^-T). */
+int nfb_logabsdet_i_plus_j_2x2_backward(const float* jt_dev, const float* g_ld_dev, int64_t batch, float* seeds_dev,
+                                        void* stream);
+
 /* flows/affine/autoregressive.py:96-128 MaskedAffineAutoregressive, element-wise part: params [rows, features, 2] =
  * (unconstrained_scale, shift) from the MADE conditioner; scale = sigmoid(u + 2) + 1e-3.  inverse = 0: y = scale x + shift,
  * log_det (+)= sum log scale; inverse = 1: y = (x - shift) / scale, log_det (+)= -sum log scale. */

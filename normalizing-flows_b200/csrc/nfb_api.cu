@@ -1384,6 +1384,141 @@ int nfb_gemm_f32(const nfb_gemm_desc_t* d, void* stream) {
     return launch_gemm_tc(a, err_dev, S(stream));
 }
 
+// ---- training pass of the residual block ----
+int nfb_swish_dual(const float* H, const float* bias, float b, int64_t rows, int32_t width, int32_t nt, float* A,
+                   void* stream) {
+    NFB_CHECK(rows == 0 || (H && A), NFB_ERR_ARG, "nfb_swish_dual: null pointer");
+    NFB_CHECK(rows >= 0 && width >= 1 && nt >= 0, NFB_ERR_ARG, "nfb_swish_dual: bad shape");
+    return launch_swish_dual(H, bias, b, rows, width, nt, A, S(stream));
+}
+int nfb_swish_dual_adjoint(const float* H, const float* bias, float b, int64_t rows, int32_t width, int32_t nt,
+                           const float* Abar, float* out_primal, float* out_tangent, double* partials, float* g_b,
+                           void* stream) {
+    NFB_CHECK(partials && (rows == 0 || (H && Abar)), NFB_ERR_ARG, "nfb_swish_dual_adjoint: null pointer");
+    NFB_CHECK(rows >= 0 && width >= 1 && nt >= 0, NFB_ERR_ARG, "nfb_swish_dual_adjoint: bad shape");
+    return launch_swish_dual_adjoint(H, bias, b, rows, width, nt, Abar, out_primal, out_tangent, partials, g_b, S(stream));
+}
+int nfb_logabsdet_i_plus_j_2x2_backward(const float* jt, const float* g_ld, int64_t batch, float* seeds, void* stream) {
+    NFB_CHECK(batch == 0 || (jt && g_ld && seeds), NFB_ERR_ARG, "nfb_logabsdet_i_plus_j_2x2_backward: null pointer");
+    return launch_logdet2_backward(jt, g_ld, batch, seeds, S(stream));
+}
+
+namespace {
+// Scratch of the dual backward, carved from the caller's workspace (every piece 256-byte aligned):
+//   H[l], l < L      stacked input of Swish l (= output of Linear l-1 without bias; H[0] = [x; tangents0])
+//   A[l], l < L      stacked output of Swish l (the A operand of Linear l)      both [(1 + nt) rows, widths[l]]
+//   Y0, Y1           cotangent ping-pong buffers                              [(1 + nt) rows, max width]
+//   partials         per-CTA fp64 partial sums of the b gradient              [NFB_SWISH_DUAL_PARTIALS]
+struct MlpDualWs {
+    float* H[NFB_LIPSCHITZ_MLP_MAX_LAYERS]; float* A[NFB_LIPSCHITZ_MLP_MAX_LAYERS];
+    float* Y[2]; double* partials;
+};
+int64_t mlp_dual_layout(const nfb_lipschitz_mlp_desc_t* d, int nt, long long rows, char* base, MlpDualWs* ws) {
+    if (!d || d->num_layers < 1 || d->num_layers > NFB_LIPSCHITZ_MLP_MAX_LAYERS || nt < 0 || rows < 0) return -1;
+    const long long rows2 = (1 + nt) * rows;
+    size_t off = 0;
+    auto take = [&](size_t bytes) { char* p = base ? base + off : nullptr; off += (bytes + 255) / 256 * 256; return p; };
+    int wmax = 0;
+    for (int l = 0; l <= d->num_layers; ++l) {
+        if (d->widths[l] < 1) return -1;
+        wmax = std::max(wmax, (int)d->widths[l]);
+    }
+    for (int l = 0; l < d->num_layers; ++l) {
+        float* h = reinterpret_cast<float*>(take((size_t)rows2 * d->widths[l] * 4));
+        float* a = reinterpret_cast<float*>(take((size_t)rows2 * d->widths[l] * 4));
+        if (ws) { ws->H[l] = h; ws->A[l] = a; }
+    }
+    for (int i = 0; i < 2; ++i) {
+        float* y = reinterpret_cast<float*>(take((size_t)rows2 * wmax * 4));
+        if (ws) ws->Y[i] = y;
+    }
+    double* p = reinterpret_cast<double*>(take(NFB_SWISH_DUAL_PARTIALS * sizeof(double)));
+    if (ws) ws->partials = p;
+    return (int64_t)off;
+}
+}  // namespace
+
+int64_t nfb_lipschitz_mlp_dual_backward_workspace_bytes(const nfb_lipschitz_mlp_desc_t* d, int32_t nt, int64_t rows) {
+    return mlp_dual_layout(d, nt, rows, nullptr, nullptr);
+}
+
+int nfb_lipschitz_mlp_dual_backward(const nfb_lipschitz_mlp_desc_t* d, const float* x, const float* tangents0, int32_t nt,
+                                    const float* g_seed, const float* t_seeds, int64_t rows, void* workspace,
+                                    int64_t workspace_bytes, float* gx, float* const* gW, float* const* gbias, float* gb,
+                                    void* stream) {
+    NFB_CHECK(d && workspace && (rows == 0 || x), NFB_ERR_ARG, "nfb_lipschitz_mlp_dual_backward: null pointer");
+    NFB_CHECK(nt == 0 || rows == 0 || tangents0, NFB_ERR_ARG, "nfb_lipschitz_mlp_dual_backward: nt > 0 needs tangents0");
+    const int64_t need = mlp_dual_layout(d, nt, rows, nullptr, nullptr);
+    NFB_CHECK(need >= 0, NFB_ERR_ARG, "nfb_lipschitz_mlp_dual_backward: bad descriptor or shape");
+    NFB_CHECK(workspace_bytes >= need, NFB_ERR_ARG, "nfb_lipschitz_mlp_dual_backward: workspace of %lld bytes, needs %lld",
+              (long long)workspace_bytes, (long long)need);
+    const int L = d->num_layers;
+    for (int l = 0; l < L; ++l)
+        NFB_CHECK(d->w[l] && d->bias[l], NFB_ERR_ARG, "nfb_lipschitz_mlp_dual_backward: null weight or bias");
+    MlpDualWs ws{};
+    mlp_dual_layout(d, nt, rows, static_cast<char*>(workspace), &ws);
+    cudaStream_t st = S(stream);
+    const int* w = d->widths;
+    const long long rows2 = (1 + nt) * rows;
+    const int D = w[0], out = w[L];
+    if (rows == 0) {   // empty batch: every gradient is zero
+        for (int l = 0; l < L; ++l) {
+            if (gW && gW[l]) NFB_CUDA(cudaMemsetAsync(gW[l], 0, (size_t)w[l + 1] * w[l] * 4, st));
+            if (gbias && gbias[l]) NFB_CUDA(cudaMemsetAsync(gbias[l], 0, (size_t)w[l + 1] * 4, st));
+        }
+        if (gb) NFB_CUDA(cudaMemsetAsync(gb, 0, (size_t)L * 4, st));
+        return NFB_OK;
+    }
+    int* err_dev = nullptr;
+    NFB_TRY(glow_err_buf(&err_dev));
+    // dual forward (recompute): H[0] = [x; tangents0]; A[l] = swish_dual(H[l]); H[l+1] = A[l] W~_l^T (no bias)
+    NFB_CUDA(cudaMemcpyAsync(ws.H[0], x, (size_t)rows * D * 4, cudaMemcpyDeviceToDevice, st));
+    if (nt) NFB_CUDA(cudaMemcpyAsync(ws.H[0] + (size_t)rows * D, tangents0, (size_t)nt * rows * D * 4,
+                                     cudaMemcpyDeviceToDevice, st));
+    for (int l = 0; l < L; ++l) {
+        NFB_TRY(launch_swish_dual(ws.H[l], l ? d->bias[l - 1] : nullptr, d->b[l], rows, w[l], nt, ws.A[l], st));
+        if (l + 1 == L) break;   // the network's output is not needed by the adjoint
+        GemmTcArgs a{};
+        a.A = ws.A[l]; a.lda = w[l]; a.B = d->w[l]; a.ldb = w[l]; a.C = ws.H[l + 1]; a.ldc = w[l + 1];
+        a.M = rows2; a.N = w[l + 1]; a.K = w[l];
+        NFB_TRY(launch_gemm_tc(a, err_dev, st));
+    }
+    // seeds: Y = [g_seed; t_seeds] (zero where absent)
+    float* Y = ws.Y[0];
+    if (g_seed) NFB_CUDA(cudaMemcpyAsync(Y, g_seed, (size_t)rows * out * 4, cudaMemcpyDeviceToDevice, st));
+    else NFB_CUDA(cudaMemsetAsync(Y, 0, (size_t)rows * out * 4, st));
+    if (nt) {
+        float* ty = Y + (size_t)rows * out;
+        if (t_seeds) NFB_CUDA(cudaMemcpyAsync(ty, t_seeds, (size_t)nt * rows * out * 4, cudaMemcpyDeviceToDevice, st));
+        else NFB_CUDA(cudaMemsetAsync(ty, 0, (size_t)nt * rows * out * 4, st));
+    }
+    // adjoint, Linear l and Swish l from the output back to the input
+    for (int l = L - 1; l >= 0; --l) {
+        const int n_out = w[l + 1], n_in = w[l];
+        if (gW && gW[l]) {   // gW~_l = Y^T A[l], reduced over all (1 + nt) rows stacks
+            GemmTcArgs a{};
+            a.A = Y; a.lda = n_out; a.a_mn = 1; a.B = ws.A[l]; a.ldb = n_in; a.b_mn = 1;
+            a.C = gW[l]; a.ldc = n_in; a.M = n_out; a.N = n_in; a.K = rows2;
+            NFB_TRY(launch_gemm_tc(a, err_dev, st));
+        }
+        if (gbias && gbias[l]) {   // primal rows only
+            NFB_CUDA(cudaMemsetAsync(gbias[l], 0, (size_t)n_out * 4, st));
+            NFB_TRY(launch_colsum(Y, n_out, rows, n_out, gbias[l], st));
+        }
+        float* Abar = ws.Y[(L - l) & 1];   // the other buffer
+        GemmTcArgs a{};   // [abar; tabar] = Y W~_l
+        a.A = Y; a.lda = n_out; a.B = d->w[l]; a.ldb = n_in; a.b_mn = 1; a.C = Abar; a.ldc = n_in;
+        a.M = rows2; a.N = n_in; a.K = n_out;
+        NFB_TRY(launch_gemm_tc(a, err_dev, st));
+        float* outp = l ? Abar : gx;
+        float* outt = l ? Abar + (size_t)rows * n_in : nullptr;
+        NFB_TRY(launch_swish_dual_adjoint(ws.H[l], l ? d->bias[l - 1] : nullptr, d->b[l], rows, n_in, nt, Abar, outp, outt,
+                                          ws.partials, gb ? gb + l : nullptr, st));
+        Y = Abar;
+    }
+    return NFB_OK;
+}
+
 int nfb_flow_create(nfb_flow_t** out, int32_t features) {
     NFB_CHECK(out, NFB_ERR_ARG, "nfb_flow_create: null out");
     NFB_CHECK(features >= 1, NFB_ERR_ARG, "nfb_flow_create: features must be >= 1");

@@ -256,6 +256,10 @@ int launch_logdet2(const float* jt, long long B, float* out, cudaStream_t st);
 int launch_glu_residual(const float* h, const float* t, const float* c, long long n, float* out, cudaStream_t st);
 int launch_rowdot(const float* a, const float* b, long long rows, int d, float c, int accumulate, float* out,
                   cudaStream_t st);
+int launch_swish_dual(const float* H, const float* bias, float b, long long B, int w, int nt, float* A, cudaStream_t st);
+int launch_swish_dual_adjoint(const float* H, const float* bias, float b, long long B, int w, int nt, const float* Abar,
+                              float* out_primal, float* out_tangent, double* partials, float* g_b, cudaStream_t st);
+int launch_logdet2_backward(const float* jt, const float* g_ld, long long B, float* seeds, cudaStream_t st);
 
 // tensor-core fp32 accumulation truncates: relative loss per K=16 MMA step, compensated at pack time (nfb_api.cu)
 constexpr float kAccStepGain = 2.4e-8f;

@@ -234,3 +234,36 @@ class DensityFn(torch.autograd.Function):
         it = iter(gp)
         out = [next(it) if p.requires_grad else None for p in model.parameters()]
         return (None, gx, *out)
+
+
+class LayerInverseFn(torch.autograd.Function):
+    """(z', log_det) = layer.inverse(z) of ONE NativeFlow called on its own (a layer of a stack that also holds non-native
+    layers, e.g. the ActNorms between Residual blocks).  The forward is the layer's kernel (FlowHandle.layer_apply); the
+    backward re-materialises the layer with `layer_inverse` above (interim, like DensityFn's torch path)."""
+
+    @staticmethod
+    def forward(ctx, layer, z, *params):
+        from . import _lib as L
+        out, ld = layer._single().layer_apply(0, L.NFB_INVERSE, z)
+        ctx.layer, ctx.params = layer, params
+        ctx.versions = [p._version for p in params]
+        ctx.save_for_backward(z)
+        return out, ld
+
+    @staticmethod
+    def backward(ctx, g_out, g_ld):
+        (z,) = ctx.saved_tensors
+        if any(p._version != v for p, v in zip(ctx.params, ctx.versions)):
+            raise RuntimeError(f"{type(ctx.layer).__name__} backward: a parameter was modified in place after the forward pass")
+        need_z = ctx.needs_input_grad[1]
+        params = [p for p in ctx.params if p.requires_grad]
+        with torch.enable_grad():
+            zz = z.detach().requires_grad_(need_z)
+            out, ld = layer_inverse(ctx.layer, zz)
+            pairs = [(t, g) for t, g in ((out, g_out), (ld, g_ld)) if g is not None and t.requires_grad]
+            wrt = ([zz] if need_z else []) + params
+            grads = torch.autograd.grad([t for t, _ in pairs], wrt, [g for _, g in pairs], allow_unused=True) \
+                if pairs and wrt else [None] * len(wrt)
+        gz = grads[0] if need_z else None
+        it = iter(grads[1:] if need_z else grads)
+        return (None, gz, *[next(it) if p.requires_grad else None for p in ctx.params])

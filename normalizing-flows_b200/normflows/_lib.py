@@ -76,6 +76,16 @@ class GemmDesc(C.Structure):
                 ("resid", C.c_void_p), ("ldres", C.c_int64)]
 
 
+LIPSCHITZ_MLP_MAX_LAYERS = 8
+SWISH_DUAL_PARTIALS = 1024
+
+
+class LipschitzMlpDesc(C.Structure):
+    _fields_ = [("num_layers", C.c_int32), ("widths", C.c_int32 * (LIPSCHITZ_MLP_MAX_LAYERS + 1)),
+                ("w", C.c_void_p * LIPSCHITZ_MLP_MAX_LAYERS), ("bias", C.c_void_p * LIPSCHITZ_MLP_MAX_LAYERS),
+                ("b", C.c_float * LIPSCHITZ_MLP_MAX_LAYERS)]
+
+
 # every symbol include/nfb200.h declares: (restype, argtypes)
 _VP, _I32, _I64, _F = C.c_void_p, C.c_int32, C.c_int64, C.c_float
 SYMBOLS = {
@@ -91,6 +101,12 @@ SYMBOLS = {
     "nfb_logabsdet_i_plus_j_2x2": (C.c_int, [_VP, _I64, _VP, _VP]),
     "nfb_glu_residual": (C.c_int, [_VP, _VP, _VP, _I64, _VP, _VP]),
     "nfb_rowdot": (C.c_int, [_VP, _VP, _I64, _I32, _F, _I32, _VP, _VP]),
+    "nfb_lipschitz_mlp_dual_backward_workspace_bytes": (_I64, [C.POINTER(LipschitzMlpDesc), _I32, _I64]),
+    "nfb_lipschitz_mlp_dual_backward": (C.c_int, [C.POINTER(LipschitzMlpDesc), _VP, _VP, _I32, _VP, _VP, _I64, _VP, _I64,
+                                                  _VP, C.POINTER(_VP), C.POINTER(_VP), _VP, _VP]),
+    "nfb_swish_dual": (C.c_int, [_VP, _VP, _F, _I64, _I32, _I32, _VP, _VP]),
+    "nfb_swish_dual_adjoint": (C.c_int, [_VP, _VP, _F, _I64, _I32, _I32, _VP, _VP, _VP, _VP, _VP, _VP]),
+    "nfb_logabsdet_i_plus_j_2x2_backward": (C.c_int, [_VP, _VP, _I64, _VP, _VP]),
     "nfb_maf_affine": (C.c_int, [_VP, _VP, _VP, _VP, _I64, _I32, _I32, _I32, _VP]),
     "nfb_logit_transform": (C.c_int, [_VP, _VP, _VP, _I64, _I64, _F, _I32, _I32, _VP]),
     "nfb_gemm_f32": (C.c_int, [C.POINTER(GemmDesc), _VP]),

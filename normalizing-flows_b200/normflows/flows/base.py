@@ -3,6 +3,7 @@ import torch
 from torch import nn
 
 from .. import _lib as L
+from .._image_autograd import wants_grad
 from .._native import FlowHandle
 
 
@@ -35,6 +36,11 @@ class NativeFlow(Flow):
         return self._single().layer_apply(0, L.NFB_FORWARD, z)
 
     def inverse(self, z, context=None):
+        # under autograd (a layer called on its own, e.g. between the blocks of a stack that is not all native) the call
+        # joins the graph; the sampling direction (`forward`) stays value-only
+        if wants_grad(self, z):
+            from .._autograd import LayerInverseFn
+            return LayerInverseFn.apply(self, z, *self.parameters())
         return self._single().layer_apply(0, L.NFB_INVERSE, z)
 
     def _native_tensors(self):
