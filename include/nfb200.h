@@ -72,6 +72,29 @@ int nfb_rqs_spline_tails(const float* x_dev, const float* params_dev, float* y_d
 int nfb_periodic_features(const float* x_dev, float* y_dev, int64_t rows, int32_t dim, const int32_t* slot_dev,
                           const float* weights_dev, const float* scale_dev, const float* bias_dev, void* stream);
 
+/* ---- training pass of the stand-alone splines (density direction, inverse = 0): gradients of
+ *   sum_r,j g_y[r, j] y[r, j] + sum_r g_log_det[r] log_det[r]
+ * w.r.t. x and the parameters, with the forward's semantics in every tails mode (analytic adjoint, nfb_spline_bwd.cuh).
+ * params_row_stride = feats * P (P = 2 num_bins + num_derivatives): one parameter record per element, g_params has the
+ * same layout; params_row_stride = 0: ONE table [feats, P] shared by every row (the unconditional CDF of the coupling
+ * layers), g_params [feats, P] receives the sum over rows.  g_y / g_log_det may be NULL (zero); g_x / g_params are
+ * optional and overwritten.  Circular features: derivative K repeats derivative 0, so both gradients land on parameter
+ * 2K (parameter 3K, in the tails-list layout, gets 0); tails-list inputs outside the interval come out as 0, so their
+ * g_x and parameter gradients are 0; NaN inputs pass through. */
+int nfb_rqs_spline_backward(const float* x_dev, const float* params_dev, int64_t params_row_stride, const float* g_y_dev,
+                            const float* g_log_det_dev, float* g_x_dev, float* g_params_dev, int64_t rows, int32_t feats,
+                            int32_t num_bins, float tail_bound, float wh_scale, void* stream);
+int nfb_rqs_spline_tails_backward(const float* x_dev, const float* params_dev, int64_t params_row_stride,
+                                  const float* g_y_dev, const float* g_log_det_dev, float* g_x_dev, float* g_params_dev,
+                                  int64_t rows, int32_t feats, int32_t num_bins, int32_t num_derivatives,
+                                  const float* tail_bound_dev, const int32_t* circular_dev, float wh_scale, void* stream);
+/* Adjoint of nfb_periodic_features: g_x (optional, overwritten; passes g_y through on non-periodic features),
+ * g_weights [n_periodic, 2] and g_bias [n_periodic] (optional, overwritten with the sums over rows). */
+int nfb_periodic_features_backward(const float* x_dev, const float* g_y_dev, int64_t rows, int32_t dim,
+                                   const int32_t* slot_dev, const float* weights_dev, const float* scale_dev,
+                                   int32_t n_periodic, float* g_x_dev, float* g_weights_dev, float* g_bias_dev,
+                                   void* stream);
+
 /* distributions/base.py:94-103 DiagGaussian.log_prob: log_q[r] (+)= log N(z_r; loc, exp(log_scale)) */
 int nfb_diag_gaussian_log_prob(const float* z_dev, const float* loc_dev, const float* log_scale_dev,
                                float* log_q_dev, int64_t rows, int32_t dim, int32_t accumulate,
@@ -88,6 +111,10 @@ int nfb_logabsdet_i_plus_j_2x2(const float* jt_dev, int64_t batch, float* out_de
 /* nets/resnet.py:48-50, nets/made.py:212-214: out = h + t * sigmoid(c), the GLU gate of a context-conditioned residual
  * block (t = block output, c = context_layer(context), h = block input); element-wise over n values */
 int nfb_glu_residual(const float* h_dev, const float* t_dev, const float* c_dev, int64_t n, float* out_dev, void* stream);
+/* Adjoint of nfb_glu_residual: g_h = g_out, g_t = g_out sigmoid(c), g_c = g_out t sigmoid'(c); each optional, g_t / g_c
+ * may alias g_out. */
+int nfb_glu_residual_backward(const float* g_out_dev, const float* t_dev, const float* c_dev, int64_t n, float* g_h_dev,
+                              float* g_t_dev, float* g_c_dev, void* stream);
 /* out[r] (+)= c * sum_j a[r, j] b[r, j]  (one Hutchinson trace term v^T J^k eps per sample, residual.py:355-366) */
 int nfb_rowdot(const float* a_dev, const float* b_dev, int64_t rows, int32_t d, float c, int32_t accumulate,
                float* out_dev, void* stream);
@@ -296,6 +323,32 @@ typedef struct {
     const float* w_final; const float* b_final; const float* m_final;
 } nfb_resnet_desc_t;
 
+/* A residual conditioner called on its own with an optional context (nets/resnet.py:92-104, nets/made.py:296-304):
+ * ResidualNet concatenates the context to its input ahead of initial_layer (net.in_features = input + context
+ * features), MADE adds context_layer(context) to the initial layer's output (w_context / b_context).  With a context,
+ * every residual block ends in the GLU gate h + t * sigmoid(block_context_layer(context)). */
+typedef struct {
+    nfb_resnet_desc_t net;
+    int32_t context_features;                 /* 0: no context (the pointers below are ignored) */
+    const float* w_context;                   /* MADE context_layer.weight [hidden, context]; NULL: ResidualNet */
+    const float* b_context;
+    const float* const* w_block_context;      /* [num_blocks] blocks.<b>.context_layer.weight [hidden, context] */
+    const float* const* b_block_context;
+} nfb_resnet_ctx_desc_t;
+/* Bytes of device scratch nfb_resnet_backward needs for `rows` rows (-1: bad descriptor). */
+int64_t nfb_resnet_backward_workspace_bytes(const nfb_resnet_ctx_desc_t* desc, int64_t rows);
+/* Gradients of sum g_out . net(x, context) in one call: the activations are recomputed from x / context, then dgrad
+ * and wgrad of every Linear run on the tensor core (the MADE masks multiply the weight gradients in the GEMM epilogue,
+ * the ReLU masks gate the data gradients), with the GLU adjoint of every context-gated block.
+ * x [rows, input features], context [rows, context_features], g_out [rows, out_features].  Outputs, each optional
+ * and OVERWRITTEN: g_x, g_context; g_w / g_b: 2 + 2 num_blocks entries in the order of nfb_resnet_desc_t: initial,
+ * blocks.0.linear_layers.0, ..., final; g_w_context / g_b_context: 1 + num_blocks entries (MADE context_layer, then
+ * each block's context_layer).  The arrays themselves may be NULL. */
+int nfb_resnet_backward(const nfb_resnet_ctx_desc_t* desc, const float* x_dev, const float* context_dev,
+                        const float* g_out_dev, int64_t rows, void* workspace_dev, int64_t workspace_bytes,
+                        float* g_x_dev, float* g_context_dev, float* const* g_w, float* const* g_b,
+                        float* const* g_w_context, float* const* g_b_context, void* stream);
+
 /* flows/neural_spline/wrapper.py:186-244 AutoregressiveRationalQuadraticSpline */
 typedef struct {
     int32_t features, num_bins;
@@ -334,6 +387,13 @@ typedef struct {
     const float* b[6];
     float leaky;
 } nfb_mlp_desc_t;
+
+/* nets/mlp.py MLP called on its own: gradients of sum g_out . mlp(x) (activations recomputed, LeakyReLU slope
+ * desc->leaky >= 0).  g_x, g_w[l], g_b[l] optional and overwritten. */
+int64_t nfb_mlp_backward_workspace_bytes(const nfb_mlp_desc_t* desc, int64_t rows);
+int nfb_mlp_backward(const nfb_mlp_desc_t* desc, const float* x_dev, const float* g_out_dev, int64_t rows,
+                     void* workspace_dev, int64_t workspace_bytes, float* g_x_dev, float* const* g_w,
+                     float* const* g_b, void* stream);
 
 /* flows/affine/coupling.py:174-229 MaskedAffineFlow */
 typedef struct { int32_t features; const float* b; nfb_mlp_desc_t s; nfb_mlp_desc_t t; } nfb_masked_affine_desc_t;

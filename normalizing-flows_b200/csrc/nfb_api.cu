@@ -1519,6 +1519,346 @@ int nfb_lipschitz_mlp_dual_backward(const nfb_lipschitz_mlp_desc_t* d, const flo
     return NFB_OK;
 }
 
+// ---- training pass of the stand-alone layers (splines, conditioners called as modules, periodic features) ----
+static int spline_backward(const char* who, const float* x, const float* params, int64_t stride, const float* gy,
+                           const float* gld, float* gx, float* gp, int64_t rows, int32_t feats, int32_t K, int32_t nd,
+                           const float* tail, const int32_t* circ, float tail0, float wh_scale, void* stream) {
+    NFB_CHECK(rows >= 0 && feats >= 0, NFB_ERR_ARG, "%s: negative size", who);
+    NFB_CHECK(K >= 1 && K <= 32 && (nd == K - 1 || nd == K || nd == K + 1), NFB_ERR_ARG, "%s: bad bins / derivatives",
+              who);
+    const int64_t P = 2 * (int64_t)K + nd;
+    NFB_CHECK(stride == 0 || stride == feats * P, NFB_ERR_ARG,
+              "%s: params_row_stride must be 0 (shared table) or feats * (2 num_bins + num_derivatives)", who);
+    NFB_CHECK(params && (rows == 0 || feats == 0 || x), NFB_ERR_ARG, "%s: null pointer", who);
+    return launch_spline_adjoint(x, params, stride == 0, gy, gld, rows, feats, K, nd, tail, circ, tail0, wh_scale, gp, gx,
+                                 S(stream));
+}
+int nfb_rqs_spline_backward(const float* x, const float* params, int64_t params_row_stride, const float* g_y,
+                            const float* g_log_det, float* g_x, float* g_params, int64_t rows, int32_t feats,
+                            int32_t num_bins, float tail_bound, float wh_scale, void* stream) {
+    return spline_backward("nfb_rqs_spline_backward", x, params, params_row_stride, g_y, g_log_det, g_x, g_params, rows,
+                           feats, num_bins, num_bins - 1, nullptr, nullptr, tail_bound, wh_scale, stream);
+}
+int nfb_rqs_spline_tails_backward(const float* x, const float* params, int64_t params_row_stride, const float* g_y,
+                                  const float* g_log_det, float* g_x, float* g_params, int64_t rows, int32_t feats,
+                                  int32_t num_bins, int32_t num_derivatives, const float* tail_bound,
+                                  const int32_t* circular, float wh_scale, void* stream) {
+    NFB_CHECK(tail_bound && circular, NFB_ERR_ARG, "nfb_rqs_spline_tails_backward: null pointer");
+    NFB_CHECK(num_derivatives != num_bins - 1, NFB_ERR_ARG,
+              "nfb_rqs_spline_tails_backward: %d derivative parameters for %d bins", num_derivatives, num_bins);
+    return spline_backward("nfb_rqs_spline_tails_backward", x, params, params_row_stride, g_y, g_log_det, g_x, g_params,
+                           rows, feats, num_bins, num_derivatives, tail_bound, circular, 0.f, wh_scale, stream);
+}
+int nfb_periodic_features_backward(const float* x, const float* g_y, int64_t rows, int32_t dim, const int32_t* slot,
+                                   const float* weights, const float* scale, int32_t n_periodic, float* g_x,
+                                   float* g_weights, float* g_bias, void* stream) {
+    NFB_CHECK(rows >= 0 && dim >= 0 && n_periodic >= 0, NFB_ERR_ARG, "nfb_periodic_features_backward: negative size");
+    NFB_CHECK(slot && weights && scale && (rows == 0 || dim == 0 || (x && g_y)), NFB_ERR_ARG,
+              "nfb_periodic_features_backward: null pointer");
+    return launch_periodic_features_bwd(x, g_y, rows, dim, slot, weights, scale, n_periodic, g_x, g_weights, g_bias,
+                                        S(stream));
+}
+int nfb_glu_residual_backward(const float* g_out, const float* t, const float* c, int64_t n, float* g_h, float* g_t,
+                              float* g_c, void* stream) {
+    NFB_CHECK(n >= 0 && (n == 0 || (g_out && t && c)), NFB_ERR_ARG, "nfb_glu_residual_backward: null pointer");
+    return launch_glu_residual_bwd(g_out, t, c, n, g_h, g_t, g_c, S(stream));
+}
+
+namespace {
+// Scratch of nfb_resnet_backward (every piece 256-byte aligned).  H = hidden, nb = blocks, C = context features:
+//   in0   [rows, in]  ResidualNet with a context: cat(x, context), the initial layer's input; later its data gradient
+//   weff  masked effective weights W * mask of every Linear (MADE only)
+//   h[b]  [rows, H], b <= nb: input of block b (h[nb] = the final layer's input)
+//   t1[b], t2[b], c[b] [rows, H]: block b's first / second Linear output and its context gate logits (t2, c: context)
+//   ga, gt, gt1 [rows, H]: cotangents;  gc0 [rows, C]: context columns of in0's gradient (ResidualNet with a context)
+struct ResnetWs {
+    float* in0; float* gc0; float* w0e; float* wbe[2 * 64]; float* wfe;
+    float* h[65]; float* t1[64]; float* t2[64]; float* c[64];
+    float* ga; float* gt; float* gt1;
+};
+constexpr int kResnetMaxBlocks = 64;
+int64_t resnet_layout(const nfb_resnet_ctx_desc_t* d, long long rows, char* base, ResnetWs* ws) {
+    if (!d || rows < 0) return -1;
+    const nfb_resnet_desc_t& n = d->net;
+    const int nb = n.num_blocks, H = n.hidden_features, C = d->context_features;
+    if (nb < 0 || nb > kResnetMaxBlocks || H < 1 || n.in_features < 1 || n.out_features < 1 || C < 0) return -1;
+    const bool concat = C > 0 && !d->w_context;
+    if (concat && n.in_features <= C) return -1;
+    const bool masked = n.m_initial != nullptr;
+    size_t off = 0;
+    auto take = [&](size_t floats) { float* p = base ? reinterpret_cast<float*>(base + off) : nullptr;
+                                     off += (floats * 4 + 255) / 256 * 256; return p; };
+    const size_t RH = (size_t)rows * H;
+    float* in0 = concat ? take((size_t)rows * n.in_features) : nullptr;
+    float* gc0 = concat ? take((size_t)rows * C) : nullptr;
+    if (ws) { ws->in0 = in0; ws->gc0 = gc0; }
+    if (masked) {
+        float* p = take((size_t)H * n.in_features);
+        if (ws) ws->w0e = p;
+        for (int i = 0; i < 2 * nb; ++i) { p = take((size_t)H * H); if (ws) ws->wbe[i] = p; }
+        p = take((size_t)n.out_features * H);
+        if (ws) ws->wfe = p;
+    }
+    for (int b = 0; b <= nb; ++b) { float* p = take(RH); if (ws) ws->h[b] = p; }
+    for (int b = 0; b < nb; ++b) {
+        float* p = take(RH); if (ws) ws->t1[b] = p;
+        if (C > 0) { p = take(RH); if (ws) ws->t2[b] = p; p = take(RH); if (ws) ws->c[b] = p; }
+    }
+    float* p = take(RH); if (ws) ws->ga = p;
+    p = take(RH); if (ws) ws->gt = p;
+    p = take(RH); if (ws) ws->gt1 = p;
+    return (int64_t)off;
+}
+
+struct GemmRun {
+    int* err; cudaStream_t st;
+    int operator()(const GemmTcArgs& a) const { return launch_gemm_tc(a, err, st); }
+};
+// Y = act(X) W^T (+ bias) (+ resid) (the forward of one Linear)
+GemmTcArgs fwd_args(const float* X, long long ldx, int relu_x, const float* W, const float* bias, float* Y, long long M,
+                    int N, int K) {
+    GemmTcArgs a{};
+    a.A = X; a.lda = ldx; a.a_relu = relu_x; a.B = W; a.ldb = K; a.C = Y; a.ldc = N; a.M = M; a.N = N; a.K = K; a.bias = bias;
+    return a;
+}
+// gX = gY W  (dgrad)
+GemmTcArgs dgrad_args(const float* gY, const float* W, float* gX, long long M, int n_in, int n_out) {
+    GemmTcArgs a{};
+    a.A = gY; a.lda = n_out; a.B = W; a.ldb = n_in; a.b_mn = 1; a.C = gX; a.ldc = n_in; a.M = M; a.N = n_in; a.K = n_out;
+    return a;
+}
+// dW = gY^T act(X) (* mask), db = colsum(gY)
+int wgrad(const GemmRun& g, const float* gY, int n_out, const float* X, long long ldx, int n_in, int relu_x,
+          const float* mask, long long rows, float* dW, float* db, cudaStream_t st) {
+    if (dW) {
+        GemmTcArgs a{};
+        a.A = gY; a.lda = n_out; a.a_mn = 1; a.B = X; a.ldb = ldx; a.b_mn = 1; a.b_relu = relu_x;
+        a.C = dW; a.ldc = n_in; a.M = n_out; a.N = n_in; a.K = rows; a.mulm = mask; a.ldmask = n_in;
+        NFB_TRY(g(a));
+    }
+    if (db) {
+        NFB_CUDA(cudaMemsetAsync(db, 0, (size_t)n_out * 4, st));
+        NFB_TRY(launch_colsum(gY, n_out, rows, n_out, db, st));
+    }
+    return NFB_OK;
+}
+}  // namespace
+
+int64_t nfb_resnet_backward_workspace_bytes(const nfb_resnet_ctx_desc_t* d, int64_t rows) {
+    return resnet_layout(d, rows, nullptr, nullptr);
+}
+
+int nfb_resnet_backward(const nfb_resnet_ctx_desc_t* d, const float* x, const float* context, const float* g_out,
+                        int64_t rows, void* workspace, int64_t workspace_bytes, float* g_x, float* g_context,
+                        float* const* g_w, float* const* g_b, float* const* g_wc, float* const* g_bc, void* stream) {
+    const int64_t need = resnet_layout(d, rows, nullptr, nullptr);
+    NFB_CHECK(need >= 0, NFB_ERR_ARG, "nfb_resnet_backward: bad descriptor or shape");
+    NFB_CHECK(workspace_bytes >= need && (need == 0 || workspace), NFB_ERR_ARG,
+              "nfb_resnet_backward: workspace of %lld bytes, needs %lld", (long long)workspace_bytes, (long long)need);
+    const nfb_resnet_desc_t& n = d->net;
+    const int nb = n.num_blocks, H = n.hidden_features, C = d->context_features, out = n.out_features;
+    const bool ctx = C > 0, concat = ctx && !d->w_context, masked = n.m_initial != nullptr;
+    const int nin = n.in_features, nx = concat ? nin - C : nin;
+    NFB_CHECK(n.w_initial && n.b_initial && n.w_final && n.b_final && (nb == 0 || (n.w_blocks && n.b_blocks)),
+              NFB_ERR_ARG, "nfb_resnet_backward: null weight or bias");
+    NFB_CHECK(!masked || (n.m_final && (nb == 0 || n.m_blocks)), NFB_ERR_ARG, "nfb_resnet_backward: missing masks");
+    NFB_CHECK(!ctx || ((d->w_context ? d->b_context != nullptr : true) &&
+                       (nb == 0 || (d->w_block_context && d->b_block_context))),
+              NFB_ERR_ARG, "nfb_resnet_backward: null context layer");
+    NFB_CHECK(rows == 0 || (x && g_out && (!ctx || context)), NFB_ERR_ARG, "nfb_resnet_backward: null input");
+    cudaStream_t st = S(stream);
+    auto zero = [&](float* p, size_t numel) { return p ? (int)cudaMemsetAsync(p, 0, numel * 4, st) : 0; };
+    auto wsz = [&](int i) { return (size_t)H * (i == 0 ? nin : H); };  // weights of linear i < 1 + 2 nb
+    if (rows == 0) {   // empty batch: every gradient is zero
+        for (int i = 0; i < 1 + 2 * nb; ++i) {
+            NFB_CUDA((cudaError_t)zero(g_w ? g_w[i] : nullptr, wsz(i)));
+            NFB_CUDA((cudaError_t)zero(g_b ? g_b[i] : nullptr, H));
+        }
+        NFB_CUDA((cudaError_t)zero(g_w ? g_w[1 + 2 * nb] : nullptr, (size_t)out * H));
+        NFB_CUDA((cudaError_t)zero(g_b ? g_b[1 + 2 * nb] : nullptr, out));
+        if (ctx)
+            for (int i = 0; i <= nb; ++i) {
+                NFB_CUDA((cudaError_t)zero(g_wc ? g_wc[i] : nullptr, (size_t)H * C));
+                NFB_CUDA((cudaError_t)zero(g_bc ? g_bc[i] : nullptr, H));
+            }
+        return NFB_OK;
+    }
+    ResnetWs ws{};
+    resnet_layout(d, rows, static_cast<char*>(workspace), &ws);
+    int* err_dev = nullptr;
+    NFB_TRY(glow_err_buf(&err_dev));
+    const GemmRun g{err_dev, st};
+    // effective weights
+    const float* w0 = n.w_initial; const float* wf = n.w_final;
+    const float* wb[2 * kResnetMaxBlocks];
+    for (int i = 0; i < 2 * nb; ++i) wb[i] = n.w_blocks[i];
+    if (masked) {
+        NFB_TRY(launch_mask_mul(n.w_initial, n.m_initial, ws.w0e, (long long)H * nin, st));
+        for (int i = 0; i < 2 * nb; ++i) NFB_TRY(launch_mask_mul(n.w_blocks[i], n.m_blocks[i], ws.wbe[i], (long long)H * H, st));
+        NFB_TRY(launch_mask_mul(n.w_final, n.m_final, ws.wfe, (long long)out * H, st));
+        w0 = ws.w0e; wf = ws.wfe;
+        for (int i = 0; i < 2 * nb; ++i) wb[i] = ws.wbe[i];
+    }
+    auto mask_of = [&](int i) -> const float* {   // linear i: 0 initial, 1 + j block linear j, 1 + 2 nb final
+        if (!masked) return nullptr;
+        return i == 0 ? n.m_initial : (i == 1 + 2 * nb ? n.m_final : n.m_blocks[i - 1]);
+    };
+    // ---- recompute (the same GEMMs as the forward, nets/*.forward through nfb_gemm_f32) ----
+    const float* in = x;
+    long long ld_in = nin;
+    if (concat) {
+        NFB_CUDA(cudaMemcpy2DAsync(ws.in0, (size_t)nin * 4, x, (size_t)nx * 4, (size_t)nx * 4, rows,
+                                   cudaMemcpyDeviceToDevice, st));
+        NFB_CUDA(cudaMemcpy2DAsync(ws.in0 + nx, (size_t)nin * 4, context, (size_t)C * 4, (size_t)C * 4, rows,
+                                   cudaMemcpyDeviceToDevice, st));
+        in = ws.in0;
+    }
+    NFB_TRY(g(fwd_args(in, ld_in, 0, w0, n.b_initial, ws.h[0], rows, H, nin)));
+    if (ctx && !concat) {
+        GemmTcArgs a = fwd_args(context, C, 0, d->w_context, d->b_context, ws.h[0], rows, H, C);
+        a.resid = ws.h[0]; a.ldres = H;
+        NFB_TRY(g(a));
+    }
+    for (int b = 0; b < nb; ++b) {
+        NFB_TRY(g(fwd_args(ws.h[b], H, 1, wb[2 * b], n.b_blocks[2 * b], ws.t1[b], rows, H, H)));
+        if (!ctx) {
+            GemmTcArgs a = fwd_args(ws.t1[b], H, 1, wb[2 * b + 1], n.b_blocks[2 * b + 1], ws.h[b + 1], rows, H, H);
+            a.resid = ws.h[b]; a.ldres = H;
+            NFB_TRY(g(a));
+        } else {
+            NFB_TRY(g(fwd_args(ws.t1[b], H, 1, wb[2 * b + 1], n.b_blocks[2 * b + 1], ws.t2[b], rows, H, H)));
+            NFB_TRY(g(fwd_args(context, C, 0, d->w_block_context[b], d->b_block_context[b], ws.c[b], rows, H, C)));
+            NFB_TRY(launch_glu_residual(ws.h[b], ws.t2[b], ws.c[b], (long long)rows * H, ws.h[b + 1], st));
+        }
+    }
+    // ---- adjoint ----
+    if (g_context) NFB_CUDA(cudaMemsetAsync(g_context, 0, (size_t)rows * C * 4, st));
+    auto ctx_layer = [&](const float* gY, const float* W, int slot) -> int {   // a Linear of the context
+        NFB_TRY(wgrad(g, gY, H, context, C, C, 0, nullptr, rows, g_wc ? g_wc[slot] : nullptr, g_bc ? g_bc[slot] : nullptr,
+                      st));
+        if (g_context) {
+            GemmTcArgs a = dgrad_args(gY, W, g_context, rows, C, H);
+            a.accumulate = 1;
+            NFB_TRY(g(a));
+        }
+        return NFB_OK;
+    };
+    const int fl = 1 + 2 * nb;
+    NFB_TRY(wgrad(g, g_out, out, ws.h[nb], H, H, 0, mask_of(fl), rows, g_w ? g_w[fl] : nullptr, g_b ? g_b[fl] : nullptr,
+                  st));
+    NFB_TRY(g(dgrad_args(g_out, wf, ws.ga, rows, H, out)));
+    for (int b = nb - 1; b >= 0; --b) {
+        const int l1 = 1 + 2 * b, l2 = 2 + 2 * b;
+        const float* gt2 = ws.ga;  // h_{b+1} = h_b + t2 (no context)
+        if (ctx) {                 // h_{b+1} = h_b + t2 * sigmoid(c)
+            NFB_TRY(launch_glu_residual_bwd(ws.ga, ws.t2[b], ws.c[b], (long long)rows * H, nullptr, ws.gt, ws.gt1, st));
+            NFB_TRY(ctx_layer(ws.gt1, d->w_block_context[b], 1 + b));
+            gt2 = ws.gt;
+        }
+        // t2 = W2 relu(t1) + b2
+        NFB_TRY(wgrad(g, gt2, H, ws.t1[b], H, H, 1, mask_of(l2), rows, g_w ? g_w[l2] : nullptr, g_b ? g_b[l2] : nullptr, st));
+        GemmTcArgs a = dgrad_args(gt2, wb[2 * b + 1], ws.gt1, rows, H, H);
+        a.mask = ws.t1[b]; a.ldmask = H;
+        NFB_TRY(g(a));   // g_t1 = (g_t2 W2) * (t1 > 0)
+        // t1 = W1 relu(h_b) + b1
+        NFB_TRY(wgrad(g, ws.gt1, H, ws.h[b], H, H, 1, mask_of(l1), rows, g_w ? g_w[l1] : nullptr, g_b ? g_b[l1] : nullptr,
+                      st));
+        GemmTcArgs c = dgrad_args(ws.gt1, wb[2 * b], ws.ga, rows, H, H);
+        c.mask = ws.h[b]; c.ldmask = H; c.resid = ws.ga; c.ldres = H;
+        NFB_TRY(g(c));   // g_h_b = g_h_{b+1} + (g_t1 W1) * (h_b > 0)     (in place)
+    }
+    NFB_TRY(wgrad(g, ws.ga, H, in, ld_in, nin, 0, mask_of(0), rows, g_w ? g_w[0] : nullptr, g_b ? g_b[0] : nullptr, st));
+    if (ctx && !concat) NFB_TRY(ctx_layer(ws.ga, d->w_context, 0));
+    if (concat) {
+        if (g_x || g_context) {
+            NFB_TRY(g(dgrad_args(ws.ga, w0, ws.in0, rows, nin, H)));   // [g_x | g_context] of cat(x, context)
+            if (g_x)
+                NFB_CUDA(cudaMemcpy2DAsync(g_x, (size_t)nx * 4, ws.in0, (size_t)nin * 4, (size_t)nx * 4, rows,
+                                           cudaMemcpyDeviceToDevice, st));
+            if (g_context) {   // += the context columns (g_context holds the block context layers' share)
+                NFB_CUDA(cudaMemcpy2DAsync(ws.gc0, (size_t)C * 4, ws.in0 + nx, (size_t)nin * 4, (size_t)C * 4, rows,
+                                           cudaMemcpyDeviceToDevice, st));
+                NFB_TRY(launch_axpy(ws.gc0, 1.f, g_context, (long long)rows * C, 1, st));
+            }
+        }
+    } else if (g_x) {
+        NFB_TRY(g(dgrad_args(ws.ga, w0, g_x, rows, nin, H)));
+    }
+    return NFB_OK;
+}
+
+namespace {
+// Scratch of nfb_mlp_backward: A[l] [rows, sizes[l + 1]], l < num_layers - 1 (hidden activations), two cotangent
+// buffers [rows, max width].
+int64_t mlp_layout(const nfb_mlp_desc_t* d, long long rows, char* base, float** A, float** Y) {
+    if (!d || d->num_layers < 1 || d->num_layers > 6 || rows < 0 || d->leaky < 0.f) return -1;
+    size_t off = 0;
+    auto take = [&](size_t floats) { float* p = base ? reinterpret_cast<float*>(base + off) : nullptr;
+                                     off += (floats * 4 + 255) / 256 * 256; return p; };
+    int wmax = 0;
+    for (int l = 0; l <= d->num_layers; ++l) {
+        if (d->sizes[l] < 1) return -1;
+        wmax = std::max(wmax, (int)d->sizes[l]);
+    }
+    for (int l = 0; l + 1 < d->num_layers; ++l) { float* p = take((size_t)rows * d->sizes[l + 1]); if (A) A[l] = p; }
+    for (int i = 0; i < 2; ++i) { float* p = take((size_t)rows * wmax); if (Y) Y[i] = p; }
+    return (int64_t)off;
+}
+}  // namespace
+
+int64_t nfb_mlp_backward_workspace_bytes(const nfb_mlp_desc_t* d, int64_t rows) {
+    return mlp_layout(d, rows, nullptr, nullptr, nullptr);
+}
+
+int nfb_mlp_backward(const nfb_mlp_desc_t* d, const float* x, const float* g_out, int64_t rows, void* workspace,
+                     int64_t workspace_bytes, float* g_x, float* const* g_w, float* const* g_b, void* stream) {
+    const int64_t need = mlp_layout(d, rows, nullptr, nullptr, nullptr);
+    NFB_CHECK(need >= 0, NFB_ERR_ARG, "nfb_mlp_backward: bad descriptor or shape");
+    NFB_CHECK(workspace_bytes >= need && (need == 0 || workspace), NFB_ERR_ARG,
+              "nfb_mlp_backward: workspace of %lld bytes, needs %lld", (long long)workspace_bytes, (long long)need);
+    const int L = d->num_layers;
+    const int* w = d->sizes;
+    for (int l = 0; l < L; ++l) NFB_CHECK(d->w[l] && d->b[l], NFB_ERR_ARG, "nfb_mlp_backward: null weight or bias");
+    NFB_CHECK(rows == 0 || (x && g_out), NFB_ERR_ARG, "nfb_mlp_backward: null input");
+    cudaStream_t st = S(stream);
+    if (rows == 0) {
+        for (int l = 0; l < L; ++l) {
+            if (g_w && g_w[l]) NFB_CUDA(cudaMemsetAsync(g_w[l], 0, (size_t)w[l + 1] * w[l] * 4, st));
+            if (g_b && g_b[l]) NFB_CUDA(cudaMemsetAsync(g_b[l], 0, (size_t)w[l + 1] * 4, st));
+        }
+        return NFB_OK;
+    }
+    float* A[6] = {}; float* Y[2] = {};
+    mlp_layout(d, rows, static_cast<char*>(workspace), A, Y);
+    int* err_dev = nullptr;
+    NFB_TRY(glow_err_buf(&err_dev));
+    const GemmRun g{err_dev, st};
+    const float slope = d->leaky;
+    // recompute: A[l] = leaky(A[l-1] W_l^T + b_l)  (ReLU fused into the GEMM for slope 0)
+    for (int l = 0; l + 1 < L; ++l) {
+        GemmTcArgs a = fwd_args(l ? A[l - 1] : x, w[l], 0, d->w[l], d->b[l], A[l], rows, w[l + 1], w[l]);
+        a.relu_out = slope == 0.f;
+        NFB_TRY(g(a));
+        if (slope != 0.f) NFB_TRY(launch_leaky_gate(A[l], A[l], slope, (long long)rows * w[l + 1], A[l], st));
+    }
+    const float* gY = g_out;
+    for (int l = L - 1; l >= 0; --l) {
+        const float* X = l ? A[l - 1] : x;
+        NFB_TRY(wgrad(g, gY, w[l + 1], X, w[l], w[l], 0, nullptr, rows, g_w ? g_w[l] : nullptr, g_b ? g_b[l] : nullptr, st));
+        if (l == 0) {
+            if (g_x) NFB_TRY(g(dgrad_args(gY, d->w[0], g_x, rows, w[0], w[1])));
+            break;
+        }
+        float* gA = Y[l & 1];
+        GemmTcArgs a = dgrad_args(gY, d->w[l], gA, rows, w[l], w[l + 1]);
+        if (slope == 0.f) { a.mask = A[l - 1]; a.ldmask = w[l]; }
+        NFB_TRY(g(a));
+        if (slope != 0.f) NFB_TRY(launch_leaky_gate(gA, A[l - 1], slope, (long long)rows * w[l], gA, st));
+        gY = gA;
+    }
+    return NFB_OK;
+}
+
 int nfb_flow_create(nfb_flow_t** out, int32_t features) {
     NFB_CHECK(out, NFB_ERR_ARG, "nfb_flow_create: null out");
     NFB_CHECK(features >= 1, NFB_ERR_ARG, "nfb_flow_create: features must be >= 1");

@@ -131,6 +131,198 @@ int launch_spline_bwd_shared(const float* xin, int ldx, const float* table, cons
     return NFB_OK;
 }
 
+// ---- stand-alone splines (nfb_rqs_spline / nfb_rqs_spline_tails, density direction) ----
+// Per-row parameters: one thread per (row, feature) element, 256 consecutive elements per block; the block's
+// 256 x P parameter slab is contiguous: staged through shared memory with coalesced loads (P = 2K + nd), the gradient
+// slab written back the same way.  KT = 8: the templated fast path (K known at compile time); KT = 0: any K <= 32.
+template <int KT>
+__global__ void __launch_bounds__(256) spline_adjoint_rows_kernel(
+    const float* __restrict__ x, const float* __restrict__ params, const float* __restrict__ gy,
+    const float* __restrict__ g_ld, long long rows, int feats, int K, int nd, const float* __restrict__ tail,
+    const int* __restrict__ circ, float tail0, float wh_scale, float* __restrict__ g_params, float* __restrict__ gx) {
+    constexpr int KMAX = KT ? KT : 32;
+    if (KT) K = KT;
+    extern __shared__ float sp[];
+    const int P = 2 * K + nd;
+    const long long e0 = (long long)blockIdx.x * 256;
+    const long long n_el = rows * feats;
+    const int n_valid = (int)(n_el - e0 < 256 ? n_el - e0 : 256);
+    const float* src = params + e0 * P;
+    for (int i = threadIdx.x; i < n_valid * P; i += 256) sp[i] = __ldg(src + i);
+    __syncthreads();
+    const long long e = e0 + threadIdx.x;
+    float gp[3 * KMAX + 1];
+    if (e < n_el) {
+        const long long row = e / feats;
+        const int f = (int)(e - row * feats);
+        float y, lad, g;
+        rqs_adjoint_params<KMAX, float>(K, nd, circ ? circ[f] != 0 : false, x[e], sp + threadIdx.x * P, wh_scale,
+                                        tail ? tail[f] : tail0, gy ? gy[e] : 0.f, g_ld ? g_ld[row] : 0.f, y, lad, g, gp);
+        if (gx) gx[e] = g;
+    }
+    __syncthreads();
+    if (e < n_el)
+        for (int k = 0; k < P; ++k) sp[threadIdx.x * P + k] = gp[k];
+    __syncthreads();
+    if (g_params) {
+        float* dst = g_params + e0 * P;
+        for (int i = threadIdx.x; i < n_valid * P; i += 256) dst[i] = sp[i];
+    }
+}
+
+// One parameter table [feats][P] shared by every row (the unconditional CDF of the coupling layers): grid = (row
+// chunks, feats); each thread walks rows of its chunk for ONE feature and keeps P partial sums, block reduction, one
+// atomic per table entry and block (g_table zeroed by the caller).
+template <int KT>
+__global__ void __launch_bounds__(256) spline_adjoint_shared_kernel(
+    const float* __restrict__ x, const float* __restrict__ table, const float* __restrict__ gy,
+    const float* __restrict__ g_ld, long long rows, long long rows_per_block, int feats, int K, int nd,
+    const float* __restrict__ tail, const int* __restrict__ circ, float tail0, float wh_scale,
+    float* __restrict__ g_table, float* __restrict__ gx) {
+    constexpr int KMAX = KT ? KT : 32;
+    if (KT) K = KT;
+    extern __shared__ float red[];  // [8][P]
+    const int P = 2 * K + nd;
+    const int f = blockIdx.y;
+    float p[3 * KMAX + 1], acc[3 * KMAX + 1], gp[3 * KMAX + 1];
+    for (int k = 0; k < P; ++k) { p[k] = __ldg(table + (long long)f * P + k); acc[k] = 0.f; }
+    const bool c = circ ? circ[f] != 0 : false;
+    const float tb = tail ? tail[f] : tail0;
+    const long long r0 = (long long)blockIdx.x * rows_per_block;
+    const long long r1 = r0 + rows_per_block < rows ? r0 + rows_per_block : rows;
+    for (long long row = r0 + threadIdx.x; row < r1; row += 256) {
+        const long long e = row * feats + f;
+        float y, lad, g;
+        rqs_adjoint_params<KMAX, float>(K, nd, c, x[e], p, wh_scale, tb, gy ? gy[e] : 0.f, g_ld ? g_ld[row] : 0.f, y,
+                                        lad, g, gp);
+        if (gx) gx[e] = g;
+        for (int k = 0; k < P; ++k) acc[k] += gp[k];
+    }
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int k = 0; k < P; ++k) {
+        const float v = warp_sum(acc[k]);
+        if (lane == 0) red[w * P + k] = v;
+    }
+    __syncthreads();
+    if (g_table)
+        for (int k = threadIdx.x; k < P; k += 256) {
+            float s = 0.f;
+            for (int j = 0; j < 8; ++j) s += red[j * P + k];
+            atomicAdd(g_table + (long long)f * P + k, s);
+        }
+}
+
+int launch_spline_adjoint(const float* x, const float* params, int shared, const float* gy, const float* g_ld,
+                          long long rows, int feats, int K, int nd, const float* tail, const int* circ, float tail0,
+                          float wh_scale, float* g_params, float* gx, cudaStream_t st) {
+    NFB_CHECK(K >= 1 && K <= 32, NFB_ERR_ARG, "rqs backward: num_bins %d out of range [1,32]", K);
+    NFB_CHECK(nd == K - 1 || nd == K || nd == K + 1, NFB_ERR_ARG, "rqs backward: %d derivative parameters for %d bins",
+              nd, K);
+    const int P = 2 * K + nd;
+    if (shared && g_params) NFB_CUDA(cudaMemsetAsync(g_params, 0, (size_t)feats * P * 4, st));
+    if (rows == 0 || feats == 0) return NFB_OK;
+    const bool fast = K == 8;
+    if (!shared) {
+        // dynamic shared memory up to the K = 32 tails-list slab (256 x 97 floats), set once per device
+        static PerDevice per_dev;
+        if (per_dev.ensure([] {
+                const int most = 256 * (3 * 32 + 1) * 4;
+                cudaError_t e = cudaFuncSetAttribute(spline_adjoint_rows_kernel<8>,
+                                                     cudaFuncAttributeMaxDynamicSharedMemorySize, most);
+                return e != cudaSuccess ? e : cudaFuncSetAttribute(spline_adjoint_rows_kernel<0>,
+                                                                   cudaFuncAttributeMaxDynamicSharedMemorySize, most);
+            }) < 0)
+            return NFB_ERR_CUDA;
+        const long long n = rows * feats;
+        const size_t smem = (size_t)256 * P * 4;
+        const unsigned grid = (unsigned)((n + 255) / 256);
+        if (fast)
+            spline_adjoint_rows_kernel<8><<<grid, 256, smem, st>>>(x, params, gy, g_ld, rows, feats, K, nd, tail, circ,
+                                                                    tail0, wh_scale, g_params, gx);
+        else
+            spline_adjoint_rows_kernel<0><<<grid, 256, smem, st>>>(x, params, gy, g_ld, rows, feats, K, nd, tail, circ,
+                                                                    tail0, wh_scale, g_params, gx);
+    } else {
+        const long long rpb = 2048;
+        const dim3 grid((unsigned)((rows + rpb - 1) / rpb), (unsigned)feats);
+        const size_t smem = (size_t)8 * P * 4;
+        if (fast)
+            spline_adjoint_shared_kernel<8><<<grid, 256, smem, st>>>(x, params, gy, g_ld, rows, rpb, feats, K, nd, tail,
+                                                                      circ, tail0, wh_scale, g_params, gx);
+        else
+            spline_adjoint_shared_kernel<0><<<grid, 256, smem, st>>>(x, params, gy, g_ld, rows, rpb, feats, K, nd, tail,
+                                                                      circ, tail0, wh_scale, g_params, gx);
+    }
+    NFB_LAUNCH_CHECK();
+    return NFB_OK;
+}
+
+// Adjoint of PeriodicFeaturesElementwise (utils/nn.py:64-130; forward: nfb_kernels.cu periodic_features_kernel).
+// grid = (row chunks, dim): each thread walks rows of its chunk for one column, writes gx and, for a periodic column,
+// keeps the partial sums of d/dw0 = g sin(s x), d/dw1 = g cos(s x), d/db = g; block reduction, three atomics per block
+// (g_w / g_b zeroed by the caller).
+__global__ void __launch_bounds__(256) periodic_features_bwd_kernel(
+    const float* __restrict__ x, const float* __restrict__ gy, long long rows, long long rows_per_block, int dim,
+    const int* __restrict__ slot, const float* __restrict__ w, const float* __restrict__ scale, float* __restrict__ gx,
+    float* __restrict__ g_w, float* __restrict__ g_b) {
+    const int j = blockIdx.y;
+    const int k = slot[j];
+    const long long r0 = (long long)blockIdx.x * rows_per_block;
+    const long long r1 = r0 + rows_per_block < rows ? r0 + rows_per_block : rows;
+    const float s = k >= 0 ? scale[k] : 0.f, w0 = k >= 0 ? w[2 * k] : 0.f, w1 = k >= 0 ? w[2 * k + 1] : 0.f;
+    float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+    for (long long r = r0 + threadIdx.x; r < r1; r += 256) {
+        const long long e = r * dim + j;
+        const float g = gy[e];
+        if (k < 0) {
+            if (gx) gx[e] = g;
+            continue;
+        }
+        float sn, cs;
+        sincosf(s * x[e], &sn, &cs);
+        if (gx) gx[e] = g * s * (w0 * cs - w1 * sn);
+        a0 = fmaf(g, sn, a0); a1 = fmaf(g, cs, a1); a2 += g;
+    }
+    if (k < 0) return;
+    __shared__ float red[3][8];
+    a0 = warp_sum(a0); a1 = warp_sum(a1); a2 = warp_sum(a2);
+    const int wi = threadIdx.x >> 5;
+    if ((threadIdx.x & 31) == 0) { red[0][wi] = a0; red[1][wi] = a1; red[2][wi] = a2; }
+    __syncthreads();
+    if (threadIdx.x < 3) {
+        float t = 0.f;
+        for (int i = 0; i < 8; ++i) t += red[threadIdx.x][i];
+        if (threadIdx.x < 2) { if (g_w) atomicAdd(g_w + 2 * k + threadIdx.x, t); }
+        else if (g_b) atomicAdd(g_b + k, t);
+    }
+}
+int launch_periodic_features_bwd(const float* x, const float* gy, long long rows, int dim, const int* slot,
+                                 const float* w, const float* scale, int n_periodic, float* gx, float* g_w, float* g_b,
+                                 cudaStream_t st) {
+    if (g_w) NFB_CUDA(cudaMemsetAsync(g_w, 0, (size_t)n_periodic * 2 * 4, st));
+    if (g_b) NFB_CUDA(cudaMemsetAsync(g_b, 0, (size_t)n_periodic * 4, st));
+    if (rows == 0 || dim == 0) return NFB_OK;
+    const long long rpb = 4096;
+    periodic_features_bwd_kernel<<<dim3((unsigned)((rows + rpb - 1) / rpb), (unsigned)dim), 256, 0, st>>>(
+        x, gy, rows, rpb, dim, slot, w, scale, gx, g_w, g_b);
+    NFB_LAUNCH_CHECK();
+    return NFB_OK;
+}
+
+// out = gate > 0 ? in : slope * in.  LeakyReLU (gate = in) and its adjoint (in = the output gradient, gate = the
+// activation, whose sign is that of its argument for slope >= 0) of nets/mlp.py.  In place allowed.
+__global__ void leaky_gate_kernel(const float* __restrict__ in, const float* __restrict__ gate, float slope, long long n,
+                                  float* __restrict__ out) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = gate[i] > 0.f ? in[i] : slope * in[i];
+}
+int launch_leaky_gate(const float* in, const float* gate, float slope, long long n, float* out, cudaStream_t st) {
+    if (n == 0) return NFB_OK;
+    leaky_gate_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(in, gate, slope, n, out);
+    NFB_LAUNCH_CHECK();
+    return NFB_OK;
+}
+
 // out[n] += sum_m G[m, n]
 __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ G, long long ld, long long M, int N,
                                                      long long rows_per_block, float* __restrict__ out) {

@@ -247,6 +247,15 @@ int launch_scatter_cols(const float* in, float* out, const int* idx, long long r
 int launch_gather_cols_ld(const float* in, int ld_in, float* out, int n_out, const int* idx, long long rows,
                           cudaStream_t st);
 int launch_axpy(const float* x, float a, float* y, long long n, int accumulate, cudaStream_t st);
+// stand-alone splines (nfb_rqs_spline*): params [rows, feats, 2K + nd] per row, or (shared) one table [feats, 2K + nd]
+// whose gradient is the sum over rows; tail / circ per feature (NULL: tail0 / linear)
+int launch_spline_adjoint(const float* x, const float* params, int shared, const float* gy, const float* g_ld,
+                          long long rows, int feats, int K, int nd, const float* tail, const int* circ, float tail0,
+                          float wh_scale, float* g_params, float* gx, cudaStream_t st);
+int launch_periodic_features_bwd(const float* x, const float* gy, long long rows, int dim, const int* slot,
+                                 const float* w, const float* scale, int n_periodic, float* gx, float* g_w, float* g_b,
+                                 cudaStream_t st);
+int launch_leaky_gate(const float* in, const float* gate, float slope, long long n, float* out, cudaStream_t st);
 int launch_split_table(const float* tab, int n, float* gw, float* gh, float* gd, cudaStream_t st);
 
 // ---- invertible residual block, element-wise pieces (nfb_residual.cu) ----
@@ -254,6 +263,8 @@ int launch_swish(const float* x, float b, long long n, float* a, float* da, cuda
 int launch_mul_rows(const float* S, const float* m, long long n, int nt, float* T, cudaStream_t st);
 int launch_logdet2(const float* jt, long long B, float* out, cudaStream_t st);
 int launch_glu_residual(const float* h, const float* t, const float* c, long long n, float* out, cudaStream_t st);
+int launch_glu_residual_bwd(const float* g, const float* t, const float* c, long long n, float* gh, float* gt, float* gc,
+                            cudaStream_t st);
 int launch_rowdot(const float* a, const float* b, long long rows, int d, float c, int accumulate, float* out,
                   cudaStream_t st);
 int launch_swish_dual(const float* H, const float* bias, float b, long long B, int w, int nt, float* A, cudaStream_t st);

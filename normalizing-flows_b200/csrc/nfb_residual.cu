@@ -76,6 +76,25 @@ int launch_glu_residual(const float* h, const float* t, const float* c, long lon
     return NFB_OK;
 }
 
+// Adjoint of the GLU gate out = h + t sigmoid(c): gh = g (optional copy), gt = g sigmoid(c), gc = g t sigmoid'(c).
+// gt / gc may alias g.
+__global__ void glu_residual_bwd_kernel(const float* __restrict__ g, const float* __restrict__ t,
+                                        const float* __restrict__ c, long long n, float* gh, float* gt, float* gc) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float gi = g[i], sg = 1.f / (1.f + __expf(-c[i]));
+    if (gh) gh[i] = gi;
+    if (gc) gc[i] = gi * t[i] * sg * (1.f - sg);
+    if (gt) gt[i] = gi * sg;
+}
+int launch_glu_residual_bwd(const float* g, const float* t, const float* c, long long n, float* gh, float* gt, float* gc,
+                            cudaStream_t st) {
+    if (n == 0) return NFB_OK;
+    glu_residual_bwd_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(g, t, c, n, gh, gt, gc);
+    NFB_LAUNCH_CHECK();
+    return NFB_OK;
+}
+
 // out[r] = (accumulate ? out[r] : 0) + c * sum_j a[r, j] * b[r, j]   (one warp per row)
 __global__ void __launch_bounds__(256) rowdot_kernel(const float* __restrict__ a, const float* __restrict__ b, long long rows,
                                                      int d, float c, int accumulate, float* __restrict__ out) {

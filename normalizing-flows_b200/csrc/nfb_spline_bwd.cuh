@@ -1,8 +1,7 @@
 // nfb_spline_bwd.cuh -- analytic backward of the monotone rational-quadratic spline element
-// (utils/splines.py:100-219, forward branch :200-219), the arithmetic core of SURVEY 8f-1 ("backward of the
-// fused blocks").  NOT yet wired into a kernel: the function is host/device and templated on the scalar type so
-// that tests/native can check it in double precision against finite differences and against gradients minted
-// from the reference's autograd (tests/test_spline_host.py) before a backward kernel is built around it.
+// (utils/splines.py:100-219, forward branch :200-219; tails :28-57).  Host/device and templated on the scalar type so
+// that tests/native can check it in double precision against finite differences and against gradients minted from the
+// reference's autograd (tests/test_spline_host.py, tests/test_conditional_training.py).  Kernels: nfb_backward.cu.
 //
 // Same formulation as rqs_core (nfb_spline.cuh): logits in the log2 domain, knots on the unit interval
 // (knot j = a * prefix_{j-1} + 1e-3 j, a = (1 - 1e-3 K) / sum), bin by search on the width knots, softplus on the
@@ -25,44 +24,49 @@ template <typename T> __host__ __device__ __forceinline__ T t_exp(T x);
 template <> __host__ __device__ __forceinline__ float t_exp<float>(float x) { return fast_ex2(x * kLog2e); }
 template <> __host__ __device__ __forceinline__ double t_exp<double>(double x) { return exp(x); }
 
-// Forward (y, lad) and backward in one pass (the backward needs every forward intermediate).
-template <int K, typename T>
-__host__ __device__ inline void rqs_fwd_bwd(T x, const T (&lw)[K], const T (&lh)[K], const T (&ud)[K - 1], T tail,
-                                            T gy, T glad, T& y, T& lad, T& gx, T (&glw)[K], T (&glh)[K],
-                                            T (&gud)[K - 1]) {
+// Forward (y, lad) and backward in one pass (the backward needs every forward intermediate), for K <= KMAX bins
+// given at run time (KMAX == K on the templated fast path, where every loop unrolls).  udk[0..K] are the raw
+// derivative logits of all K + 1 knots, boundary knots included; gudk[0..K] receives their gradients.  Outside
+// [-tail, tail] (and for NaN) the element is the identity, or, with `zero_outside` (the tails-list branch of
+// utils/splines.py:48-57, which never copies outside inputs), the constant 0: gx = 0 there.
+template <int KMAX, typename T>
+__host__ __device__ inline void rqs_adjoint(int K, T x, const T* lw, const T* lh, const T* udk, T tail, T gy, T glad,
+                                            bool zero_outside, T& y, T& lad, T& gx, T* glw, T* glh, T* gudk) {
     const T m = (T)1e-3, md = (T)1e-3, cfac = (T)1 - m * (T)K, ln2 = (T)0.6931471805599453;
 #pragma unroll
-    for (int i = 0; i < K; ++i) { glw[i] = (T)0; glh[i] = (T)0; }
-#pragma unroll
-    for (int i = 0; i < K - 1; ++i) gud[i] = (T)0;
-    if (!(x >= -tail && x <= tail)) {  // linear tails (and NaN): identity, lad 0  (:28,:40-41)
-        y = x; lad = (T)0; gx = gy;
+    for (int i = 0; i < KMAX; ++i) if (i < K) { glw[i] = (T)0; glh[i] = (T)0; gudk[i] = (T)0; }
+    gudk[K] = (T)0;
+    if (!(x >= -tail && x <= tail)) {  // outside the interval, and NaN  (:28,:40-41)
+        y = zero_outside ? (T)0 : x; lad = (T)0; gx = zero_outside ? (T)0 : gy;
         return;
     }
     // ---- forward ----
     T mw = lw[0], mh = lh[0];
 #pragma unroll
-    for (int i = 1; i < K; ++i) { mw = lw[i] > mw ? lw[i] : mw; mh = lh[i] > mh ? lh[i] : mh; }
-    T ew[K], eh[K], cw[K], ch[K];
+    for (int i = 1; i < KMAX; ++i) if (i < K) { mw = lw[i] > mw ? lw[i] : mw; mh = lh[i] > mh ? lh[i] : mh; }
+    T ew[KMAX], eh[KMAX], cw[KMAX], ch[KMAX];
     T sw = (T)0, sh = (T)0;
 #pragma unroll
-    for (int i = 0; i < K; ++i) {
-        ew[i] = t_exp2<T>(lw[i] - mw); eh[i] = t_exp2<T>(lh[i] - mh);
-        sw += ew[i]; sh += eh[i];
-        cw[i] = sw; ch[i] = sh;
+    for (int i = 0; i < KMAX; ++i) {
+        if (i < K) {
+            ew[i] = t_exp2<T>(lw[i] - mw); eh[i] = t_exp2<T>(lh[i] - mh);
+            sw += ew[i]; sh += eh[i];
+            cw[i] = sw; ch[i] = sh;
+        }
     }
     const T aw = cfac / sw, ah = cfac / sh;
-    T kw[K + 1], kh[K + 1];
+    T kw[KMAX + 1], kh[KMAX + 1];
     kw[0] = (T)0; kh[0] = (T)0; kw[K] = (T)1; kh[K] = (T)1;
 #pragma unroll
-    for (int i = 0; i < K - 1; ++i) { kw[i + 1] = aw * cw[i] + m * (T)(i + 1); kh[i + 1] = ah * ch[i] + m * (T)(i + 1); }
+    for (int i = 0; i < KMAX - 1; ++i)
+        if (i < K - 1) { kw[i + 1] = aw * cw[i] + m * (T)(i + 1); kh[i + 1] = ah * ch[i] + m * (T)(i + 1); }
     const T two_b = (T)2 * tail;
     const T xu = x / two_b + (T)0.5;
     int b = 0;
 #pragma unroll
-    for (int i = 1; i < K; ++i) b += (xu >= kw[i]) ? 1 : 0;  // knots increase: count = bin index
+    for (int i = 1; i < KMAX; ++i) if (i < K) b += (xu >= kw[i]) ? 1 : 0;  // knots increase: count = bin index
     const T l_w = kw[b], r_w = kw[b + 1], l_h = kh[b], r_h = kh[b + 1];
-    const T u0 = b == 0 ? (T)NFB_BOUNDARY_UD : ud[b - 1], u1 = b == K - 1 ? (T)NFB_BOUNDARY_UD : ud[b];
+    const T u0 = udk[b], u1 = udk[b + 1];
     auto softplus = [](T u) { return u > (T)20 ? u : (u < (T)-30 ? t_exp<T>(u) : t_log<T>((T)1 + t_exp<T>(u))); };
     auto sigmoid = [](T u) { return (T)1 / ((T)1 + t_exp<T>(-u)); };
     const T d0 = md + softplus(u0), d1 = md + softplus(u1);
@@ -106,11 +110,11 @@ __host__ __device__ inline void rqs_fwd_bwd(T x, const T (&lw)[K], const T (&lh)
     const T g_rh = g_h;
     const T g_lh = g_out - g_h;
     gx = g_xu / two_b;
-    if (b > 0) gud[b - 1] += g_d0 * (u0 > (T)20 ? (T)1 : sigmoid(u0));
-    if (b < K - 1) gud[b] += g_d1 * (u1 > (T)20 ? (T)1 : sigmoid(u1));
+    gudk[b] += g_d0 * (u0 > (T)20 ? (T)1 : sigmoid(u0));
+    gudk[b + 1] += g_d1 * (u1 > (T)20 ? (T)1 : sigmoid(u1));
     // ---- knots -> softmax logits.  knot j = cfac * prefix_{j-1} / sum + m j  (1 <= j <= K-1) ----
     //   d knot_j / d e_t = cfac * ([t <= j-1] - prefix_{j-1} / sum) / sum ;  d e_t / d logit_t = ln2 * e_t
-    auto knots_bwd = [&](const T (&e)[K], const T (&c)[K], T sum, T g_left, T g_right, T (&g)[K]) {
+    auto knots_bwd = [&](const T* e, const T* c, T sum, T g_left, T g_right, T* g) {
         const T gk[2] = {b >= 1 ? g_left : (T)0, b + 1 <= K - 1 ? g_right : (T)0};
         const int jj[2] = {b, b + 1};
 #pragma unroll
@@ -119,11 +123,56 @@ __host__ __device__ inline void rqs_fwd_bwd(T x, const T (&lw)[K], const T (&lh)
             const int j = jj[q];
             const T frac = c[j - 1] / sum, base = gk[q] * cfac / sum;
 #pragma unroll
-            for (int t = 0; t < K; ++t) g[t] += base * ((t <= j - 1 ? (T)1 : (T)0) - frac) * ln2 * e[t];
+            for (int t = 0; t < KMAX; ++t)
+                if (t < K) g[t] += base * ((t <= j - 1 ? (T)1 : (T)0) - frac) * ln2 * e[t];
         }
     };
     knots_bwd(ew, cw, sw, g_lw, g_rw, glw);
     knots_bwd(eh, ch, sh, g_lh, g_rh, glh);
+}
+
+// Linear tails, K - 1 interior derivative logits (the fused blocks' layout): boundary knots pinned to the constant.
+template <int K, typename T>
+__host__ __device__ inline void rqs_fwd_bwd(T x, const T (&lw)[K], const T (&lh)[K], const T (&ud)[K - 1], T tail,
+                                            T gy, T glad, T& y, T& lad, T& gx, T (&glw)[K], T (&glh)[K],
+                                            T (&gud)[K - 1]) {
+    T udk[K + 1], gudk[K + 1];
+    udk[0] = (T)NFB_BOUNDARY_UD; udk[K] = (T)NFB_BOUNDARY_UD;
+#pragma unroll
+    for (int i = 0; i < K - 1; ++i) udk[i + 1] = ud[i];
+    rqs_adjoint<K, T>(K, x, lw, lh, udk, tail, gy, glad, false, y, lad, gx, glw, glh, gudk);
+#pragma unroll
+    for (int i = 0; i < K - 1; ++i) gud[i] = gudk[i + 1];
+}
+
+// One element of the stand-alone splines (nfb_rqs_spline / nfb_rqs_spline_tails), on its raw parameter record
+// p[2K + nd] = [widths(K) | heights(K) | derivatives(nd)], with the knot layout of rqs_eval_dyn (nfb_spline.cuh):
+//   nd = K - 1: linear tails, boundary knots pinned to the constant of utils/splines.py:35-38;
+//   nd = K:     tails="circular" (:42-47), knot K repeats knot 0, identity outside;
+//   nd = K + 1: tails list (:48-57), every knot has a parameter; a linear feature (circular = false) pins both ends
+//               (their parameters get no gradient), a circular one copies knot 0 into knot K; outside inputs give 0.
+// A circular feature's derivative 0 is used twice, so both gradients land on parameter 2K; parameter 3K gets 0.
+// wh_scale multiplies the width / height logits.  gp[2K + nd] is overwritten.
+template <int KMAX, typename T>
+__host__ __device__ inline void rqs_adjoint_params(int K, int nd, bool circular, T x, const T* p, T wh_scale, T tail,
+                                                   T gy, T glad, T& y, T& lad, T& gx, T* gp) {
+    const T s2 = wh_scale * (T)1.4426950408889634;
+    T lw[KMAX], lh[KMAX], udk[KMAX + 1], gudk[KMAX + 1];
+#pragma unroll
+    for (int i = 0; i < KMAX; ++i) if (i < K) { lw[i] = p[i] * s2; lh[i] = p[K + i] * s2; }
+    const int dshift = nd == K - 1 ? 1 : 0;
+    const bool learned_ends = nd != K - 1 && circular;
+    udk[0] = learned_ends ? p[2 * K] : (T)NFB_BOUNDARY_UD;
+    udk[K] = udk[0];
+#pragma unroll
+    for (int i = 1; i < KMAX; ++i) if (i < K) udk[i] = p[2 * K + i - dshift];
+    rqs_adjoint<KMAX, T>(K, x, lw, lh, udk, tail, gy, glad, nd == K + 1, y, lad, gx, gp, gp + K, gudk);
+#pragma unroll
+    for (int i = 0; i < KMAX; ++i) if (i < K) { gp[i] *= s2; gp[K + i] *= s2; }
+    for (int i = 0; i < nd; ++i) gp[2 * K + i] = (T)0;
+#pragma unroll
+    for (int i = 1; i < KMAX; ++i) if (i < K) gp[2 * K + i - dshift] = gudk[i];
+    if (learned_ends) gp[2 * K] = gudk[0] + gudk[K];
 }
 
 }  // namespace nfb

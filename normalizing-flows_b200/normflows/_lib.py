@@ -24,6 +24,12 @@ class ResnetDesc(C.Structure):
                 ("w_final", C.c_void_p), ("b_final", C.c_void_p), ("m_final", C.c_void_p)]
 
 
+class ResnetCtxDesc(C.Structure):
+    _fields_ = [("net", ResnetDesc), ("context_features", C.c_int32),
+                ("w_context", C.c_void_p), ("b_context", C.c_void_p),
+                ("w_block_context", C.POINTER(C.c_void_p)), ("b_block_context", C.POINTER(C.c_void_p))]
+
+
 class ArRqsDesc(C.Structure):
     _fields_ = [("features", C.c_int32), ("num_bins", C.c_int32), ("tail_bound", C.c_float),
                 ("net", ResnetDesc)]
@@ -95,6 +101,17 @@ SYMBOLS = {
     "nfb_rqs_spline": (C.c_int, [_VP, _VP, _VP, _VP, _I64, _I32, _I32, _F, _F, _I32, _I32, _VP]),
     "nfb_rqs_spline_tails": (C.c_int, [_VP, _VP, _VP, _VP, _I64, _I32, _I32, _I32, _VP, _VP, _F, _I32, _I32, _VP]),
     "nfb_periodic_features": (C.c_int, [_VP, _VP, _I64, _I32, _VP, _VP, _VP, _VP, _VP]),
+    "nfb_rqs_spline_backward": (C.c_int, [_VP, _VP, _I64, _VP, _VP, _VP, _VP, _I64, _I32, _I32, _F, _F, _VP]),
+    "nfb_rqs_spline_tails_backward": (C.c_int, [_VP, _VP, _I64, _VP, _VP, _VP, _VP, _I64, _I32, _I32, _I32, _VP, _VP, _F,
+                                                _VP]),
+    "nfb_periodic_features_backward": (C.c_int, [_VP, _VP, _I64, _I32, _VP, _VP, _VP, _I32, _VP, _VP, _VP, _VP]),
+    "nfb_glu_residual_backward": (C.c_int, [_VP, _VP, _VP, _I64, _VP, _VP, _VP, _VP]),
+    "nfb_resnet_backward_workspace_bytes": (_I64, [C.POINTER(ResnetCtxDesc), _I64]),
+    "nfb_resnet_backward": (C.c_int, [C.POINTER(ResnetCtxDesc), _VP, _VP, _VP, _I64, _VP, _I64, _VP, _VP,
+                                      C.POINTER(_VP), C.POINTER(_VP), C.POINTER(_VP), C.POINTER(_VP), _VP]),
+    "nfb_mlp_backward_workspace_bytes": (_I64, [C.POINTER(MlpDesc), _I64]),
+    "nfb_mlp_backward": (C.c_int, [C.POINTER(MlpDesc), _VP, _VP, _I64, _VP, _I64, _VP, C.POINTER(_VP), C.POINTER(_VP),
+                                   _VP]),
     "nfb_diag_gaussian_log_prob": (C.c_int, [_VP, _VP, _VP, _VP, _I64, _I32, _I32, _VP]),
     "nfb_swish": (C.c_int, [_VP, _F, _I64, _VP, _VP, _VP]),
     "nfb_mul_rows": (C.c_int, [_VP, _VP, _I64, _I32, _VP, _VP]),

@@ -1,0 +1,213 @@
+"""Gradients of the stand-alone layers: the context-conditioned and circular spline layers, and the conditioner nets
+(ResidualNet, MADE, MLP, PeriodicFeaturesElementwise) called as modules.  Density direction only.
+
+A module that supports this defines
+  `_value(x, context, keep)`  its kernel forward (the module's no-grad path; `keep`, when not None, is a dict in which
+                              it may leave tensors for the backward, e.g. the conditioner output of a spline layer), and
+  `_adjoint(x, context, keep, grads, need_x, need_ctx)` -> (g_x, g_context, {parameter: gradient})
+and `apply_module` routes a call through `ModuleFn` when a gradient is wanted.  The backward is the C ABI's adjoints:
+nfb_rqs_spline(_tails)_backward -> nfb_resnet_backward / nfb_mlp_backward (one call per conditioner) ->
+nfb_periodic_features_backward."""
+import ctypes as C
+
+import torch
+
+from . import _lib as L
+from ._image_autograd import wants_grad
+from ._native import mlp_desc, require_cuda_f32, resnet_desc
+
+
+def _vp(ts):
+    return (C.c_void_p * max(1, len(ts)))(*[t.data_ptr() if t is not None else None for t in ts])
+
+
+def _grad_like(p):
+    return torch.empty_like(p) if p.requires_grad else None
+
+
+def _workspace(nbytes, device):
+    if nbytes < 0:
+        raise RuntimeError("native backward: bad descriptor or shape")
+    return torch.empty(max(1, int(nbytes)), dtype=torch.uint8, device=device)
+
+
+class ModuleFn(torch.autograd.Function):
+    """out = module._value(x, context) with the module's native adjoint as the backward.  Refuses to run the backward if a
+    parameter was modified in place after the forward (the saved activations would no longer match)."""
+
+    @staticmethod
+    def forward(ctx, module, x, context, *params):
+        keep = {}
+        out = module._value(x, context, keep)
+        ctx.module, ctx.keep, ctx.params = module, keep, params
+        ctx.versions = [p._version for p in params]
+        ctx.save_for_backward(x, context)
+        return out
+
+    @staticmethod
+    def backward(ctx, *grads):
+        x, context = ctx.saved_tensors
+        if any(p._version != v for p, v in zip(ctx.params, ctx.versions)):
+            raise RuntimeError(f"{type(ctx.module).__name__} backward: a parameter was modified in place after the "
+                               "forward pass")
+        grads = [g.contiguous() if g is not None else None for g in grads]
+        gx, gctx, gmap = ctx.module._adjoint(x, context, ctx.keep, grads, ctx.needs_input_grad[1],
+                                             ctx.needs_input_grad[2])
+        return (None, gx if ctx.needs_input_grad[1] else None, gctx if ctx.needs_input_grad[2] else None,
+                *[gmap.get(p) if p.requires_grad else None for p in ctx.params])
+
+
+def apply_module(module, x, context=None):
+    x = require_cuda_f32(x)
+    if context is not None:
+        context = require_cuda_f32(context, "context")
+    if wants_grad(module, x, context):
+        return ModuleFn.apply(module, x, context, *module.parameters())
+    return module._value(x, context, None)
+
+
+# ---- element adjoints ------------------------------------------------------------------------------------------
+def spline_backward(x, params, shared, num_bins, gy, g_ld, wh_scale, tail_bound=None, num_derivatives=None,
+                    tails=None, circular=None, want_params=True):
+    """(g_x, g_params) of nfb_rqs_spline (tails=None: scalar tail_bound, linear tails) or nfb_rqs_spline_tails
+    (tails = float32 [feats] bounds, circular = int32 [feats] flags).  shared: params is one [feats, P] table."""
+    rows, feats = x.shape
+    nd = num_bins - 1 if num_derivatives is None else num_derivatives
+    P = 2 * num_bins + nd
+    gx = torch.empty_like(x)
+    gp = torch.empty(params.shape, dtype=torch.float32, device=x.device) if want_params else None
+    stride = 0 if shared else feats * P
+    with torch.cuda.device(x.device):
+        if tails is None:
+            L.check(L.lib().nfb_rqs_spline_backward(L.ptr(x), L.ptr(params), stride, L.ptr(gy), L.ptr(g_ld), L.ptr(gx),
+                                                    L.ptr(gp), rows, feats, num_bins, C.c_float(tail_bound),
+                                                    C.c_float(wh_scale), L.stream_ptr()))
+        else:
+            L.check(L.lib().nfb_rqs_spline_tails_backward(L.ptr(x), L.ptr(params), stride, L.ptr(gy), L.ptr(g_ld),
+                                                          L.ptr(gx), L.ptr(gp), rows, feats, num_bins, nd, L.ptr(tails),
+                                                          L.ptr(circular), C.c_float(wh_scale), L.stream_ptr()))
+    return gx, gp
+
+
+def resnet_backward(net, masked, x, context, g_out, need_x=True, need_ctx=True):
+    """(g_x, g_context | None, {parameter: gradient}) of a ResidualNet / MADE through nfb_resnet_backward."""
+    d = L.ResnetCtxDesc()
+    d.net, keep = resnet_desc(net, masked)
+    blocks = list(net.blocks)
+    nb = len(blocks)
+    lin_w = [net.initial_layer.weight] + [l.weight for b in blocks for l in b.linear_layers] + [net.final_layer.weight]
+    lin_b = [net.initial_layer.bias] + [l.bias for b in blocks for l in b.linear_layers] + [net.final_layer.bias]
+    ctx_w, ctx_b = [], []
+    if context is not None:
+        own = getattr(net, "context_layer", None)   # MADE: context_layer(context) added to the initial layer
+        ctx_w = [own.weight if own is not None else None] + [b.context_layer.weight for b in blocks]
+        ctx_b = [own.bias if own is not None else None] + [b.context_layer.bias for b in blocks]
+        d.context_features = context.shape[1]
+        d.w_context = ctx_w[0].data_ptr() if own is not None else None
+        d.b_context = ctx_b[0].data_ptr() if own is not None else None
+        wbc, bbc = _vp(ctx_w[1:]), _vp(ctx_b[1:])
+        d.w_block_context = C.cast(wbc, C.POINTER(C.c_void_p))
+        d.b_block_context = C.cast(bbc, C.POINTER(C.c_void_p))
+        keep = (keep, wbc, bbc)
+    rows = x.shape[0]
+    gw = [_grad_like(p) for p in lin_w]
+    gb = [_grad_like(p) for p in lin_b]
+    gwc = [_grad_like(p) if p is not None else None for p in ctx_w]
+    gbc = [_grad_like(p) if p is not None else None for p in ctx_b]
+    gx = torch.empty_like(x) if need_x else None
+    gctx = torch.empty_like(context) if context is not None and need_ctx else None
+    lib = L.lib()
+    ws = _workspace(lib.nfb_resnet_backward_workspace_bytes(C.byref(d), rows), x.device)
+    pw, pb, pwc, pbc = _vp(gw), _vp(gb), _vp(gwc), _vp(gbc)
+    with torch.cuda.device(x.device):
+        L.check(lib.nfb_resnet_backward(C.byref(d), L.ptr(x), L.ptr(context), L.ptr(g_out), rows, L.ptr(ws), ws.numel(),
+                                        L.ptr(gx), L.ptr(gctx), C.cast(pw, C.POINTER(C.c_void_p)),
+                                        C.cast(pb, C.POINTER(C.c_void_p)), C.cast(pwc, C.POINTER(C.c_void_p)),
+                                        C.cast(pbc, C.POINTER(C.c_void_p)), L.stream_ptr()))
+    del keep
+    gmap = {p: g for p, g in zip(lin_w + lin_b + ctx_w + ctx_b, gw + gb + gwc + gbc) if g is not None}
+    return gx, gctx, gmap
+
+
+def mlp_backward(mlp, x, g_out, need_x=True):
+    d = mlp_desc(mlp)
+    lins = mlp.linear_layers()
+    gw = [_grad_like(l.weight) for l in lins]
+    gb = [_grad_like(l.bias) for l in lins]
+    gx = torch.empty_like(x) if need_x else None
+    lib = L.lib()
+    ws = _workspace(lib.nfb_mlp_backward_workspace_bytes(C.byref(d), x.shape[0]), x.device)
+    pw, pb = _vp(gw), _vp(gb)
+    with torch.cuda.device(x.device):
+        L.check(lib.nfb_mlp_backward(C.byref(d), L.ptr(x), L.ptr(g_out), x.shape[0], L.ptr(ws), ws.numel(), L.ptr(gx),
+                                     C.cast(pw, C.POINTER(C.c_void_p)), C.cast(pb, C.POINTER(C.c_void_p)),
+                                     L.stream_ptr()))
+    ps = [l.weight for l in lins] + [l.bias for l in lins]
+    return gx, {p: g for p, g in zip(ps, gw + gb) if g is not None}
+
+
+def periodic_backward(pf, x, g_y):
+    slot, w, scale, bias = pf._tables(x.device)
+    gx = torch.empty_like(x)
+    gw = torch.empty_like(pf.weights)
+    gb = torch.empty_like(pf.bias) if pf.apply_bias else None
+    with torch.cuda.device(x.device):
+        L.check(L.lib().nfb_periodic_features_backward(L.ptr(x), L.ptr(g_y), x.shape[0], x.shape[1], L.ptr(slot),
+                                                       L.ptr(w), L.ptr(scale), len(pf.ind), L.ptr(gx), L.ptr(gw),
+                                                       L.ptr(gb), L.stream_ptr()))
+    gmap = {pf.weights: gw}
+    if gb is not None:
+        gmap[pf.bias] = gb
+    return gx, gmap
+
+
+def conditioner_backward(net, masked, x, context, g_out, need_x=True, need_ctx=True):
+    """ResidualNet / MADE with its optional preprocessing module in front: PeriodicFeaturesElementwise through its
+    adjoint kernel, any other module differentiated by torch autograd."""
+    from .nets.resnet import _preprocess
+    from .utils.nn import PeriodicFeaturesElementwise
+    pre = net.preprocessing
+    xin = _preprocess(pre, x) if pre is not None else x
+    need_in = need_x or (pre is not None and any(p.requires_grad for p in pre.parameters()))
+    gx, gctx, gmap = resnet_backward(net, masked, require_cuda_f32(xin), context, g_out, need_in, need_ctx)
+    if gx is None:
+        return gx, gctx, gmap
+    if isinstance(pre, PeriodicFeaturesElementwise):
+        gx, gm = periodic_backward(pre, x, gx)
+        gmap.update(gm)
+    elif pre is not None:
+        params = [p for p in pre.parameters() if p.requires_grad]
+        with torch.enable_grad():
+            xx = x.detach().requires_grad_(True)
+            grads = torch.autograd.grad(pre(xx), [xx] + params, gx, allow_unused=True)
+        gx = grads[0]
+        gmap.update({p: g for p, g in zip(params, grads[1:]) if g is not None})
+    return gx, gctx, gmap
+
+
+class UnitGaussianFn(torch.autograd.Function):
+    """log N(u; 0, I) per row (nfb_diag_gaussian_log_prob with zero tables) and its adjoint
+    (nfb_gaussian_table_log_prob_backward): the density of ConditionalDiagGaussian on the standardised residual."""
+
+    @staticmethod
+    def forward(ctx, u):
+        zeros = torch.zeros(u.shape[1], device=u.device)
+        out = torch.empty(u.shape[0], dtype=torch.float32, device=u.device)
+        if u.shape[0]:
+            with torch.cuda.device(u.device):
+                L.check(L.lib().nfb_diag_gaussian_log_prob(L.ptr(u), L.ptr(zeros), L.ptr(zeros), L.ptr(out), u.shape[0],
+                                                           u.shape[1], 0, L.stream_ptr()))
+        ctx.save_for_backward(u)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        (u,) = ctx.saved_tensors
+        zeros = torch.zeros(u.shape[1], device=u.device)
+        gu = torch.empty_like(u)
+        if u.shape[0]:
+            with torch.cuda.device(u.device):
+                L.check(L.lib().nfb_gaussian_table_log_prob_backward(L.ptr(u), None, L.ptr(zeros), L.ptr(zeros),
+                                                                     L.ptr(g.contiguous()), L.ptr(gu), None, None,
+                                                                     u.shape[0], u.shape[1], 1, 1, L.stream_ptr()))
+        return gu

@@ -126,14 +126,11 @@ class ConditionalDiagGaussian(BaseDistribution):
     def log_prob(self, z, context=None):
         z = require_cuda_f32(z)
         mean, log_scale = self._params(context)
-        # standardise per sample, then the unit-Gaussian density kernel; the log-scale term is a row sum
+        # standardise per sample, then the unit-Gaussian density kernel (differentiable in u, so in z and the encoder
+        # output); the log-scale term is a row sum
+        from .._standalone import UnitGaussianFn
         u = ((z - mean) * torch.exp(-log_scale)).contiguous().reshape(z.shape[0], -1)
-        zeros = torch.zeros(self.d, device=z.device)
-        out = torch.empty(z.shape[0], dtype=torch.float32, device=z.device)
-        if z.shape[0]:
-            with torch.cuda.device(z.device):
-                L.check(L.lib().nfb_diag_gaussian_log_prob(L.ptr(u), L.ptr(zeros), L.ptr(zeros), L.ptr(out), z.shape[0],
-                                                           self.d, 0, L.stream_ptr()))
+        out = UnitGaussianFn.apply(u)
         return out - torch.sum(log_scale.reshape(z.shape[0], -1), dim=1)
 
 

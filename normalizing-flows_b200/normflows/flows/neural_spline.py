@@ -61,16 +61,33 @@ class AutoregressiveRationalQuadraticSpline(NativeFlow):
     # Context-conditioned layer (ConditionalNormalizingFlow, core.py:216-366): the conditioner takes the context through
     # the MADE's context layers + GLU gates, so it runs as stand-alone tensor-core GEMMs (nets.MADE.forward) and the
     # spline as the stand-alone HBM-bound kernel (csrc/nfb_kernels.cu rqs_rows_kernel) instead of the fused block.
+    # The density direction trains through _standalone.ModuleFn (_value / _adjoint below).
     def _conditional(self, z, context, sampling):
         from .._native import require_cuda_f32, rqs_spline
+        from .._standalone import apply_module
+        if not sampling:  # wrapper.inverse -> Autoregressive.forward: one pass (affine/autoregressive.py:24-27)
+            return apply_module(self, z, context)
         z = require_cuda_f32(z)
         net = self.mprqat.autoregressive_net
-        if not sampling:  # wrapper.inverse -> Autoregressive.forward: one pass (affine/autoregressive.py:24-27)
-            return rqs_spline(z, net(z, context), self.num_bins, self.tail_bound, 1.0, False)
         out, ld = torch.zeros_like(z), None  # D passes (:29-38)
         for _ in range(self.features):
-            out, ld = rqs_spline(z, net(out, context), self.num_bins, self.tail_bound, 1.0, True)
+            out, ld = rqs_spline(z, net._value(out, context, None), self.num_bins, self.tail_bound, 1.0, True)
         return out, ld
+
+    def _value(self, z, context, keep):
+        from .._native import rqs_spline
+        params = self.mprqat.autoregressive_net._value(z, context, None)
+        if keep is not None:
+            keep["params"] = params
+        return rqs_spline(z, params, self.num_bins, self.tail_bound, 1.0, False)
+
+    def _adjoint(self, z, context, keep, grads, need_x, need_ctx):
+        from .._standalone import conditioner_backward, spline_backward
+        gz, g_params = spline_backward(z, keep["params"], False, self.num_bins, grads[0], grads[1], 1.0,
+                                       tail_bound=self.tail_bound)
+        g_net, g_ctx, gmap = conditioner_backward(self.mprqat.autoregressive_net, True, z, context, g_params,
+                                                  need_ctx=need_ctx)
+        return gz + g_net, g_ctx, gmap
 
     def forward(self, z, context=None):
         if self.num_context_channels is not None or context is not None:
@@ -149,27 +166,34 @@ class CoupledRationalQuadraticSpline(NativeFlow):
         """Context-conditioned coupling layer outside the fused block (see AutoregressiveRationalQuadraticSpline):
         Coupling.forward / .inverse of neural_spline/coupling.py:71-128 with the unconditional CDF of :221-253."""
         from .._native import require_cuda_f32, rqs_spline
+        from .._standalone import apply_module
+        if not sampling:
+            return apply_module(self, z, context)
         z = require_cuda_f32(z)
         p, k = self.prqct, self.num_bins
-        idf, trf = p.identity_features, p.transform_features
-        u = p.unconditional_transform
-        b = z.shape[0]
-        up = torch.cat([u.unnormalized_widths, u.unnormalized_heights, u.unnormalized_derivatives], dim=1)
-        up = up.reshape(1, -1).expand(b, -1).contiguous()  # _share_across_batch (:217-219)
-        ident, trans = z[:, idf].contiguous(), z[:, trf].contiguous()
+        ident, trans = z[:, p.identity_features].contiguous(), z[:, p.transform_features].contiguous()
         wh = 1.0 / float(np.sqrt(p.transform_net.hidden_features))
-        if not sampling:
-            params = p.transform_net(ident, context)
-            yt, ld = rqs_spline(trans, params, k, self.tail_bound, wh, False)
-            yi, ldi = rqs_spline(ident, up, k, self.tail_bound, 1.0, False)
-        else:
-            yi, ldi = rqs_spline(ident, up, k, self.tail_bound, 1.0, True)
-            params = p.transform_net(yi, context)
-            yt, ld = rqs_spline(trans, params, k, self.tail_bound, wh, True)
-        out = torch.empty_like(z)
-        out[:, idf] = yi
-        out[:, trf] = yt
-        return out, ld + ldi
+        yi, ldi = rqs_spline(ident, _uncond_rows(p.unconditional_transform, z.shape[0]), k, self.tail_bound, 1.0, True)
+        yt, ld = rqs_spline(trans, p.transform_net._value(yi, context, None), k, self.tail_bound, wh, True)
+        return _merge(z, p, yi, yt), ld + ldi
+
+    def _value(self, z, context, keep):
+        from .._native import rqs_spline
+        p, k = self.prqct, self.num_bins
+        ident, trans = z[:, p.identity_features].contiguous(), z[:, p.transform_features].contiguous()
+        wh = 1.0 / float(np.sqrt(p.transform_net.hidden_features))
+        params = p.transform_net._value(ident, context, None)
+        if keep is not None:
+            keep["params"] = params
+        yt, ld = rqs_spline(trans, params, k, self.tail_bound, wh, False)
+        yi, ldi = rqs_spline(ident, _uncond_rows(p.unconditional_transform, z.shape[0]), k, self.tail_bound, 1.0, False)
+        return _merge(z, p, yi, yt), ld + ldi
+
+    def _adjoint(self, z, context, keep, grads, need_x, need_ctx):
+        from .._standalone import spline_backward
+        spline = lambda x, params, shared, wh, gy, gld: spline_backward(x, params, shared, self.num_bins, gy, gld, wh,
+                                                                        tail_bound=self.tail_bound)
+        return _coupling_adjoint(self.prqct, z, context, keep["params"], grads, spline, need_ctx)
 
     def forward(self, z, context=None):
         if self.num_context_channels is not None or context is not None:
@@ -203,6 +227,43 @@ class CoupledRationalQuadraticSpline(NativeFlow):
         del keep
 
 
+def _uncond_rows(u, rows):
+    """The unconditional CDF's table [n_id, P] repeated for every row (_share_across_batch, coupling.py:217-219)."""
+    up = torch.cat([u.unnormalized_widths, u.unnormalized_heights, u.unnormalized_derivatives], dim=1)
+    return up.reshape(1, -1).expand(rows, -1).contiguous()
+
+
+def _merge(z, p, yi, yt):
+    out = torch.empty_like(z)
+    out[:, p.identity_features] = yi
+    out[:, p.transform_features] = yt
+    return out
+
+
+def _coupling_adjoint(p, z, context, params, grads, spline, need_ctx):
+    """Backward of a coupling layer's density pass (Coupling.forward, neural_spline/coupling.py:71-98):
+    transform features = spline adjoint; identity features = unconditional-CDF adjoint + the conditioner's data
+    gradient.  spline(x, params, shared, wh_scale, g_y, g_log_det) -> (g_x, g_params)."""
+    from .._standalone import conditioner_backward
+    idf, trf = p.identity_features, p.transform_features
+    g_out, g_ld = grads
+    ident, trans = z[:, idf].contiguous(), z[:, trf].contiguous()
+    u = p.unconditional_transform
+    k = u.unnormalized_widths.shape[1]
+    table = torch.cat([u.unnormalized_widths, u.unnormalized_heights, u.unnormalized_derivatives], dim=1).contiguous()
+    wh = 1.0 / float(np.sqrt(p.transform_net.hidden_features))
+    g_tr, g_params = spline(trans, params, False, wh, g_out[:, trf].contiguous(), g_ld)
+    g_id, g_table = spline(ident, table, True, 1.0, g_out[:, idf].contiguous(), g_ld)
+    g_net, g_ctx, gmap = conditioner_backward(p.transform_net, False, ident, context, g_params, need_ctx=need_ctx)
+    gz = torch.empty_like(z)
+    gz[:, idf] = g_id + g_net
+    gz[:, trf] = g_tr
+    gmap[u.unnormalized_widths] = g_table[:, :k]
+    gmap[u.unnormalized_heights] = g_table[:, k:2 * k]
+    gmap[u.unnormalized_derivatives] = g_table[:, 2 * k:]
+    return gz, g_ctx, gmap
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # Circular variants (reference: flows/neural_spline/wrapper.py:88-183, 247-311): `tails` is a per-feature list, so every
 # knot has a derivative parameter (3K+1 per feature; utils/splines.py:48-57) and the bound may differ per feature.
@@ -233,8 +294,8 @@ class _CircularCoupledTransform(nn.Module):
             raise ValueError("Mask can't be empty.")
         circ = set(int(i) for i in ind_circ)
         ind_circ_id = [i for i, f in enumerate(self.identity_features.tolist()) if f in circ]
-        if torch.is_tensor(tail_bound):   # wrapper.py:134-138
-            scale_pf = np.pi / tail_bound[self.identity_features][ind_circ_id] if ind_circ_id else 1.0
+        if torch.is_tensor(tail_bound):   # wrapper.py:134-138: indexed by the position among the identity features
+            scale_pf = np.pi / tail_bound[ind_circ_id] if ind_circ_id else 1.0
         else:
             scale_pf = np.pi / tail_bound
         from ..utils.nn import PeriodicFeaturesElementwise
@@ -271,31 +332,48 @@ class CircularCoupledRationalQuadraticSpline(Flow):
                                                self.ind_circ, tail_bound, torch.as_tensor(mask), activation(),
                                                dropout_probability, init_identity, context_features=num_context_channels)
 
+    def _tails(self, p, device):
+        return (_tail_tensors(self._tail_bound, p.identity_features, self.ind_circ, self.features, device),
+                _tail_tensors(self._tail_bound, p.transform_features, self.ind_circ, self.features, device))
+
     def _run(self, z, context, sampling):
         from .._native import require_cuda_f32, rqs_spline_tails
-        z = require_cuda_f32(z)
-        p, k = self.prqct, self.num_bins
-        idf, trf = p.identity_features, p.transform_features
-        tb_id, c_id = _tail_tensors(self._tail_bound, idf, self.ind_circ, self.features, z.device)
-        tb_tr, c_tr = _tail_tensors(self._tail_bound, trf, self.ind_circ, self.features, z.device)
-        u = p.unconditional_transform
-        b = z.shape[0]
-        up = torch.cat([u.unnormalized_widths, u.unnormalized_heights, u.unnormalized_derivatives], dim=1)
-        up = up.detach().reshape(1, -1).expand(b, -1).contiguous()
-        ident, trans = z[:, idf].contiguous(), z[:, trf].contiguous()
-        wh = 1.0 / float(np.sqrt(p.transform_net.hidden_features))
+        from .._standalone import apply_module
         if not sampling:   # Coupling.forward (coupling.py:71-98)
-            params = p.transform_net(ident, context)
-            yt, ld = rqs_spline_tails(trans, params, k, k + 1, tb_tr, c_tr, wh, False)
-            yi, ldi = rqs_spline_tails(ident, up, k, k + 1, tb_id, c_id, 1.0, False)
-        else:              # Coupling.inverse (:100-128)
-            yi, ldi = rqs_spline_tails(ident, up, k, k + 1, tb_id, c_id, 1.0, True)
-            params = p.transform_net(yi, context)
-            yt, ld = rqs_spline_tails(trans, params, k, k + 1, tb_tr, c_tr, wh, True)
-        out = torch.empty_like(z)
-        out[:, idf] = yi
-        out[:, trf] = yt
-        return out, ld + ldi
+            return apply_module(self, z, context)
+        z = require_cuda_f32(z)   # Coupling.inverse (:100-128)
+        p, k = self.prqct, self.num_bins
+        (tb_id, c_id), (tb_tr, c_tr) = self._tails(p, z.device)
+        ident, trans = z[:, p.identity_features].contiguous(), z[:, p.transform_features].contiguous()
+        wh = 1.0 / float(np.sqrt(p.transform_net.hidden_features))
+        yi, ldi = rqs_spline_tails(ident, _uncond_rows(p.unconditional_transform, z.shape[0]), k, k + 1, tb_id, c_id,
+                                   1.0, True)
+        yt, ld = rqs_spline_tails(trans, p.transform_net._value(yi, context, None), k, k + 1, tb_tr, c_tr, wh, True)
+        return _merge(z, p, yi, yt), ld + ldi
+
+    def _value(self, z, context, keep):
+        from .._native import rqs_spline_tails
+        p, k = self.prqct, self.num_bins
+        (tb_id, c_id), (tb_tr, c_tr) = self._tails(p, z.device)
+        ident, trans = z[:, p.identity_features].contiguous(), z[:, p.transform_features].contiguous()
+        wh = 1.0 / float(np.sqrt(p.transform_net.hidden_features))
+        params = p.transform_net._value(ident, context, None)
+        if keep is not None:
+            keep["params"] = params
+        yt, ld = rqs_spline_tails(trans, params, k, k + 1, tb_tr, c_tr, wh, False)
+        yi, ldi = rqs_spline_tails(ident, _uncond_rows(p.unconditional_transform, z.shape[0]), k, k + 1, tb_id, c_id,
+                                   1.0, False)
+        return _merge(z, p, yi, yt), ld + ldi
+
+    def _adjoint(self, z, context, keep, grads, need_x, need_ctx):
+        from .._standalone import spline_backward
+        p, k = self.prqct, self.num_bins
+        (tb_id, c_id), (tb_tr, c_tr) = self._tails(p, z.device)
+
+        def spline(x, params, shared, wh, gy, gld):
+            tb, circ = (tb_id, c_id) if shared else (tb_tr, c_tr)
+            return spline_backward(x, params, shared, k, gy, gld, wh, num_derivatives=k + 1, tails=tb, circular=circ)
+        return _coupling_adjoint(p, z, context, keep["params"], grads, spline, need_ctx)
 
     def forward(self, z, context=None):   # wrapper.py:177-179: forward = prqct.inverse
         return self._run(z, context, True)
@@ -326,15 +404,35 @@ class CircularAutoregressiveRationalQuadraticSpline(Flow):
 
     def _run(self, z, context, sampling):
         from .._native import require_cuda_f32, rqs_spline_tails
+        from .._standalone import apply_module
+        if not sampling:   # one MADE pass (affine/autoregressive.py:24-27)
+            return apply_module(self, z, context)
         z = require_cuda_f32(z)
         k, net = self.num_bins, self.mprqat.autoregressive_net
         tb, circ = _tail_tensors(self._tail_bound, range(self.features), self.ind_circ, self.features, z.device)
-        if not sampling:   # one MADE pass (affine/autoregressive.py:24-27); MADE has no hidden_features: no 1/sqrt(H)
-            return rqs_spline_tails(z, net(z, context), k, k + 1, tb, circ, 1.0, False)
         out, ld = torch.zeros_like(z), None   # D passes (:29-38)
         for _ in range(self.features):
-            out, ld = rqs_spline_tails(z, net(out, context), k, k + 1, tb, circ, 1.0, True)
+            out, ld = rqs_spline_tails(z, net._value(out, context, None), k, k + 1, tb, circ, 1.0, True)
         return out, ld
+
+    def _value(self, z, context, keep):   # MADE has no hidden_features: no 1/sqrt(H)
+        from .._native import rqs_spline_tails
+        k = self.num_bins
+        tb, circ = _tail_tensors(self._tail_bound, range(self.features), self.ind_circ, self.features, z.device)
+        params = self.mprqat.autoregressive_net._value(z, context, None)
+        if keep is not None:
+            keep["params"] = params
+        return rqs_spline_tails(z, params, k, k + 1, tb, circ, 1.0, False)
+
+    def _adjoint(self, z, context, keep, grads, need_x, need_ctx):
+        from .._standalone import conditioner_backward, spline_backward
+        k = self.num_bins
+        tb, circ = _tail_tensors(self._tail_bound, range(self.features), self.ind_circ, self.features, z.device)
+        gz, g_params = spline_backward(z, keep["params"], False, k, grads[0], grads[1], 1.0, num_derivatives=k + 1,
+                                       tails=tb, circular=circ)
+        g_net, g_ctx, gmap = conditioner_backward(self.mprqat.autoregressive_net, True, z, context, g_params,
+                                                  need_ctx=need_ctx)
+        return gz + g_net, g_ctx, gmap
 
     def forward(self, z, context=None):   # wrapper.py:305-307: forward = mprqat.inverse
         return self._run(z, context, True)

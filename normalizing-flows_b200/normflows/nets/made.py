@@ -9,7 +9,7 @@ import torch
 from torch import nn
 from torch.nn import functional as F, init
 
-from .resnet import _check_plain
+from .resnet import _check_plain, _preprocess
 
 
 class MaskedLinear(nn.Linear):
@@ -80,7 +80,15 @@ class MADE(nn.Module):
 
     def forward(self, inputs, context=None):
         """nets/made.py:296-304, stand-alone call: masked weights, pre-activation residual blocks."""
+        from .._standalone import apply_module
+        return apply_module(self, inputs, context)
+
+    def _value(self, inputs, context, keep):
         from .._native import resnet_forward
         if self.preprocessing is not None:
-            inputs = self.preprocessing(inputs)
+            inputs = _preprocess(self.preprocessing, inputs)
         return resnet_forward(self, inputs, masked=True, context=context)
+
+    def _adjoint(self, inputs, context, keep, grads, need_x, need_ctx):
+        from .._standalone import conditioner_backward
+        return conditioner_backward(self, True, inputs, context, grads[0], need_x, need_ctx)

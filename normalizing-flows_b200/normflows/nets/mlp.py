@@ -29,7 +29,12 @@ class MLP(nn.Module):
 
     def forward(self, x):
         """Stand-alone evaluation (nets/mlp.py:57-58): one tensor-core GEMM per Linear (csrc/nfb_gemm_tc.cu).  Inside
-        MaskedAffineFlow / AffineCouplingBlock the net is evaluated by the fused affine kernel instead."""
+        MaskedAffineFlow / AffineCouplingBlock the net is evaluated by the fused affine kernel instead.  Under autograd
+        the backward is one nfb_mlp_backward call."""
+        from .._standalone import apply_module
+        return apply_module(self, x)
+
+    def _value(self, x, context, keep):
         import torch
         from .._native import linear
         lins = self.linear_layers()
@@ -40,3 +45,8 @@ class MLP(nn.Module):
             if not last and self.leaky != 0.0:
                 h = torch.where(h > 0, h, h * self.leaky)
         return h
+
+    def _adjoint(self, x, context, keep, grads, need_x, need_ctx):
+        from .._standalone import mlp_backward
+        gx, gmap = mlp_backward(self, x, grads[0], need_x)
+        return gx, None, gmap

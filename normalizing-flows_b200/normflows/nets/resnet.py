@@ -19,6 +19,11 @@ def _check_plain(activation, dropout_probability, use_batch_norm, context_featur
         raise NotImplementedError("batch-norm in the conditioner is not on the CUDA path")
 
 
+def _preprocess(module, inputs):
+    """Value of the conditioner's preprocessing module (kernel path for PeriodicFeaturesElementwise, else its call)."""
+    return module._value(inputs, None, None) if hasattr(module, "_value") else module(inputs)
+
+
 class ResidualBlock(nn.Module):
     def __init__(self, features, context_features=None, activation=F.relu, dropout_probability=0.0,
                  use_batch_norm=False, zero_initialization=True):
@@ -46,7 +51,15 @@ class ResidualNet(nn.Module):
 
     def forward(self, inputs, context=None):
         """nets/resnet.py:92-104, stand-alone call (inside a flow the net is part of the fused kernel)."""
+        from .._standalone import apply_module
+        return apply_module(self, inputs, context)
+
+    def _value(self, inputs, context, keep):
         from .._native import resnet_forward
         if self.preprocessing is not None:
-            inputs = self.preprocessing(inputs)
+            inputs = _preprocess(self.preprocessing, inputs)
         return resnet_forward(self, inputs, masked=False, context=context)
+
+    def _adjoint(self, inputs, context, keep, grads, need_x, need_ctx):
+        from .._standalone import conditioner_backward
+        return conditioner_backward(self, False, inputs, context, grads[0], need_x, need_ctx)

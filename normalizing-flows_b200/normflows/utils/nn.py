@@ -62,13 +62,26 @@ class PeriodicFeaturesElementwise(nn.Module):
             self.bias = nn.Parameter(torch.zeros(len(self.ind)))
         self.activation = nn.Identity()
 
-    def forward(self, inputs):
-        from .._native import periodic_features, require_cuda_f32
-        x = require_cuda_f32(inputs)
-        dev = x.device
+    def _tables(self, dev):
+        """(slot [ndim] int32, weights, scale [n_periodic], bias | None) on `dev` in the kernels' layout."""
         slot = torch.full((self.ndim,), -1, dtype=torch.int32)
         slot[self.ind.cpu()] = torch.arange(len(self.ind), dtype=torch.int32)
         sc = self.scale if torch.is_tensor(self.scale) else torch.full((len(self.ind),), float(self.scale))
         sc = sc.to(device=dev, dtype=torch.float32).reshape(-1).expand(len(self.ind)).contiguous()
-        return periodic_features(x, slot.to(dev), self.weights.detach().contiguous(), sc,
-                                 self.bias.detach() if self.apply_bias else None)
+        return (slot.to(dev), self.weights.detach().contiguous(), sc,
+                self.bias.detach() if self.apply_bias else None)
+
+    def forward(self, inputs):
+        from .._standalone import apply_module
+        return apply_module(self, inputs)
+
+    def _value(self, inputs, context, keep):
+        from .._native import periodic_features, require_cuda_f32
+        x = require_cuda_f32(inputs)
+        slot, w, sc, bias = self._tables(x.device)
+        return periodic_features(x, slot, w, sc, bias)
+
+    def _adjoint(self, inputs, context, keep, grads, need_x, need_ctx):
+        from .._standalone import periodic_backward
+        gx, gmap = periodic_backward(self, inputs, grads[0])
+        return gx, None, gmap

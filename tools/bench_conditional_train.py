@@ -1,0 +1,139 @@
+"""Time one training step of the stand-alone spline layers: `forward_kld` + `backward()` + Adam.
+    a    examples/conditional_flow.ipynb: ConditionalNormalizingFlow(DiagGaussian(2, trainable=False),
+         4 x [AutoregressiveRationalQuadraticSpline(2, 2, 128, num_context_channels=4), LULinearPermute(2)]),
+         Adam(lr 3e-4, weight decay 1e-5), batch 128 (the notebook's) and 65 536
+    b    the same with CoupledRationalQuadraticSpline
+    circ examples/circular_nsf.ipynb: 20 x CircularAutoregressiveRationalQuadraticSpline(2, 1, 128, [1],
+         tail_bound=[5, pi], permute_mask=True) on DiagGaussian(2) (the notebook's UniformGaussian is not a package class),
+         Adam(lr 1e-4, weight decay 1e-4), batch 1 024
+Prints one JSON line: ms/step (median of CUDA-event-timed steps after warm-up), samples/s, kernel launches per step
+(torch.profiler, one separate step), peak device memory, and the card's name, power limit and SM clock read in the same
+run.  When the unmodified reference is installed under oracle/_ref, the same model, seed and batch are timed through it
+(eager torch, fp32).
+    python tools/bench_conditional_train.py [--steps 20] [--warmup 5] [--no-reference]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+REF_DIR = os.path.join(ROOT, "oracle", "_ref")
+
+
+CASES = [("a", 128), ("a", 65536), ("b", 128), ("b", 65536), ("circ", 1024)]
+NOTEBOOK_LAYERS = 4   # examples/conditional_flow.ipynb: K = 4 (spline + LU) pairs
+
+
+def build(nf, kind):
+    import math
+    import torch
+    torch.manual_seed(0)
+    if kind == "circ":
+        flows = [nf.flows.CircularAutoregressiveRationalQuadraticSpline(2, 1, 128, [1], tail_bound=torch.tensor([5., math.pi]),
+                                                                        permute_mask=True) for _ in range(20)]
+        return nf.NormalizingFlow(nf.distributions.DiagGaussian(2), flows), (1e-4, 1e-4)
+    flows = []
+    for _ in range(NOTEBOOK_LAYERS):
+        if kind == "a":
+            flows.append(nf.flows.AutoregressiveRationalQuadraticSpline(2, 2, 128, num_context_channels=4))
+        else:
+            flows.append(nf.flows.CoupledRationalQuadraticSpline(2, 2, 128, num_context_channels=4))
+        flows.append(nf.flows.LULinearPermute(2))
+    return nf.ConditionalNormalizingFlow(nf.distributions.DiagGaussian(2, trainable=False), flows), (3e-4, 1e-5)
+
+
+def time_arm(arm, kind, batch, steps, warmup):
+    import numpy as np
+    import torch
+    if arm == "reference":
+        sys.path.insert(0, REF_DIR)
+    else:
+        sys.path[:0] = [ROOT, os.path.join(ROOT, "normalizing-flows_b200")]
+    import normflows as nf
+    dev = torch.device("cuda")
+    model, (lr, wd) = build(nf, kind)
+    model = model.to(dev)
+    g = torch.Generator().manual_seed(1)
+    x = (torch.randn(batch, 2, generator=g) * 1.2).to(dev)
+    ctx = torch.cat([torch.randn(batch, 2, generator=g), 0.5 + 0.5 * torch.rand(batch, 2, generator=g)], 1).to(dev)
+    opt = torch.optim.Adam(model.parameters(), lr=lr, weight_decay=wd)
+    np.random.seed(0)
+    torch.manual_seed(0)
+
+    def step():
+        opt.zero_grad(set_to_none=True)
+        loss = model.forward_kld(x) if kind == "circ" else model.forward_kld(x, ctx)
+        loss.backward()
+        opt.step()
+        return loss
+
+    for _ in range(warmup):
+        step()
+    torch.cuda.synchronize()
+    torch.cuda.reset_peak_memory_stats()
+    times = []
+    for _ in range(steps):
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        loss = step()
+        b.record()
+        b.synchronize()
+        times.append(a.elapsed_time(b))
+    if not torch.isfinite(loss):
+        raise RuntimeError("non-finite loss")
+    peak = torch.cuda.max_memory_allocated()
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        step()
+        torch.cuda.synchronize()
+    launches = sum(1 for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
+                   and "memcpy" not in e.name.lower() and "memset" not in e.name.lower())
+    times.sort()
+    ms = times[len(times) // 2]
+    return {"model": kind, "batch": batch, "ms_per_step": round(ms, 3),
+            "ms_min": round(times[0], 3), "ms_max": round(times[-1], 3),
+            "samples_per_s": round(batch / ms * 1e3, 1), "launches_per_step": launches,
+            "peak_mem_gb": round(peak / 2 ** 30, 2), "loss": round(float(loss), 4)}
+
+
+def gpu_info():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm",
+                            "--format=csv,noheader"], capture_output=True, text=True, timeout=30).stdout
+        name, power, sm, sm_max = [s.strip() for s in q.strip().splitlines()[0].split(",")]
+        return {"gpu": name, "power_limit": power, "sm_clock_at_end": sm, "sm_clock_max": sm_max}
+    except Exception:  # noqa: BLE001 -- recorded as unknown, never guessed
+        import torch
+        return {"gpu": torch.cuda.get_device_name(0), "power_limit": "unknown"}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--no-reference", action="store_true")
+    ap.add_argument("--arm", choices=["native", "reference"], help=argparse.SUPPRESS)
+    a = ap.parse_args()
+    if a.arm:   # one arm in its own process (the two packages share the name `normflows`)
+        print(json.dumps([time_arm(a.arm, k, b, a.steps, a.warmup) for k, b in CASES]))
+        return
+    import torch
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_conditional_train: no CUDA device")
+    arms = ["native"] + (["reference"] if not a.no_reference and os.path.isdir(os.path.join(REF_DIR, "normflows"))
+                         else [])
+    res = {}
+    for arm in arms:
+        cmd = [sys.executable, os.path.abspath(__file__), "--arm", arm, "--steps", str(a.steps), "--warmup", str(a.warmup)]
+        r = subprocess.run(cmd, capture_output=True, text=True)
+        if r.returncode:
+            res[arm] = {"error": r.stderr.strip().splitlines()[-1] if r.stderr.strip() else f"exit {r.returncode}"}
+        else:
+            res[arm] = json.loads(r.stdout.strip().splitlines()[-1])
+    print(json.dumps({"metric": "conditional_spline_train_step", **gpu_info(), **res}))
+
+
+if __name__ == "__main__":
+    main()
