@@ -143,10 +143,10 @@ struct FusedPack {
     DevBuf wstream, steps, uncond;
     std::vector<float> bias_h, bias_f;
     std::vector<int> in_idx, tr_idx, id_idx;
-    struct Rec { int row0, nrows, kc; size_t off_hi, off_lo; };
     struct Gemm { DevBuf src_row, src_col, row_scale, recs_dev; const float* W; const float* M; int src_cols, n_pad, k_pad;
-                  int max_rows = 0; std::vector<Rec> recs; };
+                  int max_rows = 0; std::vector<FusedRec> recs; };
     std::vector<int> hperm;  // sorted-by-degree order of the hidden units (identity for unmasked nets)
+    int own[2][2] = {{-1, -1}, {-1, -1}};  // hidden output slices of each consumer warpgroup (FusedLayer::own)
     std::vector<Gemm> gemms;
     // LU + this block as one launch (built when the next layer in list order is an LU)
     bool pair_ok = false;
@@ -326,44 +326,22 @@ int build_fused(nfb_flow* f, Layer& L, cudaStream_t st) {
     // accumulator of the final layer at 24 registers and its staging tile small (nfb_fused_rqs.cu)
     const int fpc = kFusedFeaturesPerChunk;
     const int n_chunks = ((T + fpc - 1) / fpc + 1) & ~1;   // even: a record carries one chunk per consumer warpgroup
-    const int kcs_h = H / 64;
     const int crow = fpc * 24;  // rows (MMA N) per final-layer chunk
     if (n_hidden > 7) return NFB_OK;  // tables inside FusedLayer
 
     // ---- MADE masks: sort hidden units by degree so that every masked matrix is block-triangular, and
-    //      find the all-zero [64 x 64] blocks to drop (nets/made.py:57-76 degree rules) ----
+    //      find the all-zero [64 x 64] blocks to drop (nfb_fused_plan.h) ----
     const bool masked = n.m0 != nullptr;
-    std::vector<int> perm(H);
-    for (int i = 0; i < H; ++i) perm[i] = i;
     std::vector<float> m_init, m_hid, m_fin;
     if (masked) {
         NFB_TRY(download(n.m0, (size_t)H * n.in, m_init));
-        std::vector<int> deg(H, 0);  // row sum of the input mask = number of inputs a unit may see = its degree
-        for (int i = 0; i < H; ++i) for (int j = 0; j < n.in; ++j) deg[i] += m_init[(size_t)i * n.in + j] != 0.f;
-        std::stable_sort(perm.begin(), perm.end(), [&](int x, int y) { return deg[x] < deg[y]; });
         if (n.nb > 0) NFB_TRY(download(n.mb[0], (size_t)H * H, m_hid));  // all hidden masks share the structure
         NFB_TRY(download(n.mf, (size_t)n.out * H, m_fin));
     }
+    const FusedNeeds needs = fused_needs(H, n.in, T, fpc, n_chunks, masked ? m_init.data() : nullptr,
+                                         m_hid.empty() ? nullptr : m_hid.data(), masked ? m_fin.data() : nullptr);
+    const std::vector<int>& perm = needs.perm;
     F.hperm = perm;
-    // does output slice j (rows [64 j, 64 j + 64) in sorted order) of a hidden GEMM have a non-zero in K-chunk kc?
-    auto hidden_needs = [&](int j, int kc) -> bool {
-        if (!masked || m_hid.empty()) return true;
-        for (int i = 64 * j; i < 64 * j + 64; ++i)
-            for (int k = kc * 64; k < kc * 64 + 64; ++k)
-                if (m_hid[(size_t)perm[i] * H + perm[k]] != 0.f) return true;
-        return false;
-    };
-    // does chunk c of the final layer have a non-zero in K-chunk kc?
-    auto final_needs = [&](int c, int kc) -> bool {
-        if (!masked) return true;
-        for (int i = 0; i < crow; ++i) {
-            const int t = fpc * c + i / 24, q = i % 24;
-            if (t >= T || q >= 23) continue;
-            for (int k = kc * 64; k < kc * 64 + 64; ++k)
-                if (m_fin[(size_t)(t * 23 + q) * H + perm[k]] != 0.f) return true;
-        }
-        return false;
-    };
 
     // ---- GEMM source tables (effective matrices are built in sorted hidden order) ----
     F.gemms.clear();
@@ -395,66 +373,17 @@ int build_fused(nfb_flow* f, Layer& L, cudaStream_t st) {
         NFB_TRY(add_gemm(n.wf, n.mf, H, n_chunks * crow, H, fr, perm, fs));
     }
 
-    // ---- step table + record list (same order).  A record carries the same K-chunk of two output slices, one per
-    //      consumer warpgroup of the kernel: hidden GEMMs split their 64-column slices in two halves ([0, half) and
-    //      [half, ns)), the final layer deals its chunks alternately.  K-chunks ascend (the accumulation order is part
-    //      of the validated numerics); K-chunk 0 is always kept, so that every slice has a first record that initialises
-    //      its accumulator; a K-chunk only one of the two slices reaches is skipped by the other warpgroup. ----
-    std::vector<FusedStep> steps;
-    size_t off = 0;
-    // rows [row_a, row_a + nrows) for warpgroup 0 and (row_b >= 0) [row_b, row_b + nrows) for warpgroup 1
-    auto add_pair = [&](FusedPack::Gemm& g, int row_a, int row_b, int nrows, const std::vector<bool>& need_a,
-                        const std::vector<bool>& need_b, bool onto) {
-        const int tot = row_b >= 0 ? 2 * nrows : nrows;
-        std::vector<int> kcs;
-        for (size_t kc = 0; kc < need_a.size(); ++kc)
-            if (kc == 0 || need_a[kc] || (row_b >= 0 && need_b[kc])) kcs.push_back((int)kc);
-        for (size_t i = 0; i < kcs.size(); ++i) {
-            const int kc = kcs[i];
-            FusedStep st{};
-            st.bytes16 = (uint16_t)(tot * 16);
-            st.n8 = (uint8_t)(nrows / 8);
-            st.kc = (uint8_t)kc;
-            st.flags = (uint8_t)(((i == 0 && !onto) ? kStepFirst : 0) | (i + 1 == kcs.size() ? kStepLast : 0) |
-                                 ((kc > 0 && !need_a[kc]) ? kStepSkip0 : 0) |
-                                 ((row_b < 0 || (kc > 0 && !need_b[kc])) ? kStepSkip1 : 0));
-            steps.push_back(st);
-            g.recs.push_back(FusedPack::Rec{row_a, nrows, kc, off, off + (size_t)tot * 128});
-            if (row_b >= 0)
-                g.recs.push_back(FusedPack::Rec{row_b, nrows, kc, off + (size_t)nrows * 128, off + (size_t)(tot + nrows) * 128});
-            off += (size_t)tot * 256;
-        }
-    };
-    const int half = (kcs_h + 1) / 2;
-    for (int ph = 0; ph < n_hidden; ++ph) {
-        const bool accum_onto = (ph > 0 && (ph & 1) == 0);  // second GEMM of a residual block: h += ...
-        const int kcs = (ph == 0) ? 1 : kcs_h;
-        auto need = [&](int j) {
-            std::vector<bool> v(kcs);
-            for (int kc = 0; kc < kcs; ++kc) v[kc] = ph == 0 || hidden_needs(j, kc);
-            return v;
-        };
-        for (int q = 0; q < half; ++q) {
-            const int jb = q + half < kcs_h ? q + half : -1;
-            add_pair(F.gemms[ph], 64 * q, jb >= 0 ? 64 * jb : -1, 64, need(q), jb >= 0 ? need(jb) : need(q), accum_onto);
-        }
-    }
-    for (int c = 0; c < n_chunks; c += 2) {
-        auto need = [&](int cc) {
-            std::vector<bool> v(kcs_h);
-            for (int kc = 0; kc < kcs_h; ++kc) v[kc] = final_needs(cc, kc);
-            return v;
-        };
-        add_pair(F.gemms[n_hidden], c * crow, (c + 1) * crow, crow, need(c), need(c + 1), false);
-    }
-    F.steps_host = steps;
-    F.n_steps = (int)steps.size();
+    // ---- slice ownership, step table and record list (nfb_fused_plan.h) ----
+    FusedPlan plan = plan_fused(needs, n_hidden, crow);
+    for (int g = 0; g <= n_hidden; ++g) F.gemms[g].recs = std::move(plan.recs[g]);
+    std::copy(&plan.own[0][0], &plan.own[0][0] + 4, &F.own[0][0]);
+    F.steps_host = plan.steps;
+    F.n_steps = (int)plan.steps.size();
     F.D = L.D; F.H = H; F.n_hidden = n_hidden; F.T = T; F.F = fpc; F.n_chunks = n_chunks; F.tail = L.tail;
     F.n_id = ar ? 0 : L.n_id;
-    const size_t total = off;
-    F.rqs_bytes = total;
-    NFB_TRY(F.wstream.reserve(total));
-    NFB_TRY(F.steps.upload(steps));
+    F.rqs_bytes = plan.bytes;
+    NFB_TRY(F.wstream.reserve(plan.bytes));
+    NFB_TRY(F.steps.upload(plan.steps));
 
     // ---- index lists ----
     std::vector<int> in_idx(64, -1), tr_idx(T);
@@ -696,6 +625,8 @@ int repack_fused(nfb_flow* f, Layer& L, cudaStream_t st, Layer* Ufold = nullptr)
         Lh.tr_idx[k] = (unsigned char)(k < (int)F.tr_idx.size() ? F.tr_idx[k] : 0);
         Lh.id_idx[k] = (unsigned char)(k < (int)F.id_idx.size() ? F.id_idx[k] : 0);
     }
+    for (int w = 0; w < 2; ++w)
+        for (int q = 0; q < 2; ++q) Lh.own[w][q] = (signed char)F.own[w][q];
     Lh.a_sc[0] = 1.f; Lh.a_inv[0] = 1.f;
     for (int gi = 0; gi < ng; ++gi) {
         Lh.a_sc[1 + gi] = pow2f(F.pa[gi]);
@@ -773,10 +704,13 @@ int repack_lu(nfb_flow* f, Layer& L, cudaStream_t st, bool packed_already = fals
     return NFB_OK;
 }
 
-// the LU map in front of a block: one 64-row record W_hi | W_lo, all four products (the map transforms z itself, ~2^-22)
+// the LU map in front of a block: one 64-row record W_hi | W_lo for warpgroup 0, all four products (the map transforms
+// z itself, ~2^-22)
 FusedStep lu_step() {
     FusedStep s{};
-    s.bytes16 = 64 * 16; s.n8 = 8; s.kc = 0; s.flags = kStepFirst | kStepLast | kStepQuad | kStepSkip1;
+    s.bytes16 = 64 * 16; s.n8 = 8;
+    s.kc = 0; s.flags = kStepFirst | kStepLast | kStepQuad | kStepHalf;
+    s.kc1 = 0; s.flags1 = kStepFirst | kStepLast | kStepQuad | kStepHalf | kStepSkip;
     return s;
 }
 

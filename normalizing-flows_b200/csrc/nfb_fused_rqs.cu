@@ -17,12 +17,14 @@
 //
 // Structure (384 threads, 1 CTA/SM, persistent over (layer, tile) work units of the whole stack):
 //   warp 8     weight producer: 1-D bulk TMA (cp.async.bulk) of pre-swizzled fp16 records from the packed weight stream
-//              (read from L2) into a 3 x 32 KB ring.  A record is one W_hi tile and its W_lo twin for one K-chunk: the
-//              output slices of BOTH consumer warpgroups stacked (rows [0, 8 n8) for warpgroup 0, [8 n8, 16 n8) for 1).
+//              (read from L2) into a 3 x 32 KB ring.  A record is one W_hi tile and its W_lo twin: one half per
+//              consumer warpgroup stacked (rows [0, 8 n8) for warpgroup 0, [8 n8, 16 n8) for 1), each with its own
+//              K-chunk, or a single half at offset 0 (nfb_fused_plan.h).
 //              Its warpgroup gives its registers to the consumers (setmaxnreg); warps 9-11 exit.
 //   warps 0-7  two warpgroups; each issues the wgmma (M = the 64 rows of the tile, K = 16) of its half of every record
-//              and runs its epilogues.  A hidden GEMM's output columns are split between them (warpgroup w: 64-column
-//              slices [w h, w h + h), h = ceil(H / 128)), so the whole output -- and the conditioner's residual stream,
+//              and runs its epilogues.  A hidden GEMM's output columns are split between them (warpgroup w owns up to
+//              ceil(H / 128) 64-column slices, FusedLayer::own, chosen by the packer so that the non-zero blocks of the
+//              MADE masks split evenly), so the whole output -- and the conditioner's residual stream,
 //              64 x H fp32 -- lives in registers (2 x 32 per thread each) and ONE A-operand buffer suffices: both
 //              warpgroups finish the GEMM, then overwrite its input with its output (bias, ReLU, fp16 hi/lo split).  The
 //              second GEMM of each residual block accumulates straight onto the residual stream (h += W2 relu(...));
@@ -115,25 +117,27 @@ template <typename T> __device__ __forceinline__ T uniform(T v) {
 __device__ __forceinline__ float pow2i(int e) { return __uint_as_float((uint32_t)(127 + e) << 23); }
 
 // the products of one record: acc (+)= A[K-chunk] W^T as W_hi A_hi + W_hi A_lo + W_lo A_hi (+ W_lo A_lo), four K=16
-// slabs each, in that order (first: the first product overwrites the accumulator; on = 0: none)
+// slabs each, in that order (first: the first product overwrites the accumulator; on = 0: none; slabs: only the
+// first `slabs` K=16 slabs, the others being all zero)
 template <int NREG, bool QUAD>
 __device__ __forceinline__ void mma_record(float (&acc)[NREG], uint32_t a_hi, uint32_t a_lo, uint32_t w_hi, uint32_t w_lo,
-                                           bool first, uint32_t on) {
+                                           bool first, uint32_t on, uint32_t slabs) {
     const uint64_t ah = wgmma_desc(a_hi), al = wgmma_desc(a_lo), bh = wgmma_desc(w_hi), bl = wgmma_desc(w_lo);
-    auto mma = [&](uint64_t a, uint64_t b, uint32_t sd) {
-        if constexpr (NREG == 32) wgmma_f16_n64(acc, a, b, sd, on);
-        else wgmma_f16_n48(acc, a, b, sd, on);
+    auto mma = [&](uint64_t a, uint64_t b, uint32_t sd, int s) {
+        const uint32_t go = on & (uint32_t)(s < (int)slabs);
+        if constexpr (NREG == 32) wgmma_f16_n64(acc, a, b, sd, go);
+        else wgmma_f16_n48(acc, a, b, sd, go);
     };
     uint32_t sd = first ? 0u : 1u;
 #pragma unroll
-    for (int s = 0; s < 4; ++s) { mma(ah + 2 * s, bh + 2 * s, sd); sd = 1u; }
+    for (int s = 0; s < 4; ++s) { mma(ah + 2 * s, bh + 2 * s, sd, s); sd = 1u; }
 #pragma unroll
-    for (int s = 0; s < 4; ++s) mma(al + 2 * s, bh + 2 * s, 1u);
+    for (int s = 0; s < 4; ++s) mma(al + 2 * s, bh + 2 * s, 1u, s);
 #pragma unroll
-    for (int s = 0; s < 4; ++s) mma(ah + 2 * s, bl + 2 * s, 1u);
+    for (int s = 0; s < 4; ++s) mma(ah + 2 * s, bl + 2 * s, 1u, s);
     if constexpr (QUAD) {
 #pragma unroll
-        for (int s = 0; s < 4; ++s) mma(al + 2 * s, bl + 2 * s, 1u);
+        for (int s = 0; s < 4; ++s) mma(al + 2 * s, bl + 2 * s, 1u, s);
     }
 }
 
@@ -260,7 +264,6 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
     const int rb = ra + 8;
     const int cq = 2 * (lane & 3);                 // first of its two columns in every 8-column group
     const uint32_t aA = sbase;                     // the A operand
-    const uint32_t skip_bit = wg ? kStepSkip1 : kStepSkip0;
     float* stg = reinterpret_cast<float*>(smem + kOffStg + wg * kStgBytes);
     uint32_t slot = 0, wpar = 0;
 
@@ -270,14 +273,16 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
         const long long tile = uniform(unit_q[2 * (ui & 3u) + 1]);
         if (layer < 0) break;
         const FusedLayer& L = p.layers[layer];
-        const int D = L.D, ns = uniform(L.H >> 6), half = (ns + 1) >> 1;
+        const int D = L.D;
+        auto own = [&](int q) { return uniform((int)L.own[wg][q]); };   // this warpgroup's slices (-1: none)
         const int n_steps = uniform(L.n_steps), lu_steps = uniform(L.has_lu ? 1 : 0);
         const int n_hidden = uniform(L.n_hidden), n_pairs = uniform(L.n_chunks >> 1);
         int sidx = 0;
-        // The records of one output slice (until the one flagged last): this warpgroup's half of each goes into acc
-        // (live: the warpgroup has a slice here; a record's skip bit: its half is all zero).  Every record is waited
-        // for and handed back by both warpgroups; a slot is handed back as soon as the products that read it have
-        // completed (an empty wgmma group stands in for a skipped half, so the group count stays uniform).
+        // The records of one output slice (until the one this warpgroup's flags mark last): its half of each goes
+        // into acc, multiplied with its K-chunk (live: the warpgroup has a slice here; its skip bit: the record has no
+        // half for it, or an all-zero one).  Every record is waited for and handed back by both warpgroups; a slot is
+        // handed back as soon as the products that read it have completed (an empty wgmma group stands in for a
+        // skipped half, so the group count stays uniform).
         auto run_slice = [&](auto& acc, bool live, auto quad) {
             int prev = -1;
             for (;;) {
@@ -286,19 +291,20 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
                 st.raw.x = uniform(st.raw.x);
                 st.raw.y = uniform(st.raw.y);
                 sidx = sidx + 1 == n_steps ? lu_steps : sidx + 1;
+                const uint32_t kc = wg ? st.s.kc1 : st.s.kc;
+                const uint32_t fl = wg ? st.s.flags1 : st.s.flags;
                 mbar_wait(bar(kBarWFull + slot), wpar, p.err, 220 + slot);
-                const uint32_t w = sbase + kOffW + slot * kSlotBytes + (uint32_t)wg * st.s.n8 * 1024u;
-                const uint32_t kc = st.s.kc;
+                const uint32_t w = sbase + kOffW + slot * kSlotBytes + ((fl & kStepHalf) ? 0u : (uint32_t)wg * st.s.n8 * 1024u);
                 wgmma_fence();
                 mma_record<sizeof(acc) / sizeof(float), decltype(quad)::value>(
                     acc, aA + kc * kTileA, aA + (4 + kc) * kTileA, w, w + ((uint32_t)st.s.bytes16 << 3),
-                    (st.s.flags & kStepFirst) != 0, (uint32_t)(live && !(st.s.flags & skip_bit)));
+                    (fl & kStepFirst) != 0, (uint32_t)(live && !(fl & kStepSkip)), 4u - ((fl >> kStepSlabShift) & 3u));
                 wgmma_commit();
                 wgmma_wait<1>();   // the previous record's products are complete: hand its slot back
                 mbar_arrive_if(bar(kBarWEmpty + (prev < 0 ? 0 : prev)), prev >= 0 && (et & 127) == 0);
                 prev = (int)slot;
                 if (++slot == kSlots) { slot = 0; wpar ^= 1; }
-                if (st.s.flags & kStepLast) break;
+                if (fl & kStepLast) break;
             }
             wgmma_wait<0>();
             wgmma_hold(acc);
@@ -509,7 +515,8 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
             if (!folded) build_a_net();   // (ends with a barrier: every thread has read its raw identity columns)
             if (!SAMPLE && L.n_id > 0) uncond();
 
-            // ---- hidden layers: warpgroup wg owns the 64-column slices [wg half, wg half + half) of every output ----
+            // ---- hidden layers: warpgroup wg owns the 64-column slices own(0), own(1) of every output (the packer's
+            //      choice, nfb_fused_plan.h); a warpgroup without a slice passes the GEMM's records as one dead slice ----
             float hres[2][32];   // its part of the residual stream h
             for (int ph = 0; ph < n_hidden; ++ph) {
                 const bool t_phase = (ph & 1) != 0;   // first GEMM of a residual block: its own accumulator
@@ -517,10 +524,10 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
                 float tacc[2][32];
 #pragma unroll
                 for (int q = 0; q < 2; ++q) {
-                    if (q < half) {
-                        const bool live = wg * half + q < ns;
-                        if (t_phase) run_slice(tacc[q], live, NoQuad());
-                        else run_slice(hres[q], live, NoQuad());
+                    const int j = own(q);
+                    if (q == 0 || j >= 0) {
+                        if (t_phase) run_slice(tacc[q], j >= 0, NoQuad());
+                        else run_slice(hres[q], j >= 0, NoQuad());
                     }
                 }
                 cons_bar_sync();   // every product of this GEMM has read the A operand: overwrite it with the output
@@ -550,8 +557,8 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
                 };
 #pragma unroll
                 for (int q = 0; q < 2; ++q) {
-                    const int j = wg * half + q;   // output slice = A K-chunk j of the next GEMM
-                    if (q < half && j < ns) {
+                    const int j = own(q);   // output slice = A K-chunk j of the next GEMM
+                    if (j >= 0) {
                         if (t_phase) epilogue(tacc[q], j);
                         else epilogue(hres[q], j);
                     }

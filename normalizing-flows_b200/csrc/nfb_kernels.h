@@ -1,6 +1,7 @@
 // nfb_kernels.h -- internal launch interface between the C-ABI layer (nfb_api.cu) and the kernels.
 #pragma once
 #include "nfb_common.cuh"
+#include "nfb_fused_plan.h"
 
 #include <mutex>
 
@@ -154,22 +155,7 @@ int launch_affine_stack(const void* ops_dev, int n_ops, const float* zin, float*
 // ---- fused neural-spline block (nfb_fused_rqs.cu) ----
 constexpr int kFusedTileRows = 64;          // rows of a work unit (the M of one wgmma)
 constexpr int kFusedFeaturesPerChunk = 2;   // spline features per final-layer record (N = 24 per feature)
-// One weight record of the packed stream: a W_hi tile followed by its W_lo twin, multiplied with K-chunk kc of the A
-// operand.  Each tile stacks the [8 n8 x 64] halves of the two consumer warpgroups of the fused kernel (warpgroup 0's
-// output slice, then warpgroup 1's).  The records of a slice are consecutive; the slices come in the order the kernel
-// consumes them (LU map, hidden GEMMs slice by slice, final-layer chunks).
-enum { kStepFirst = 1,    // first record of its slice: overwrites the accumulator
-       kStepLast = 2,     // last record of its slice: the slice's epilogue follows
-       kStepQuad = 4,     // four products (W_lo A_lo as well): the LU map, which transforms z itself
-       kStepSkip0 = 8,    // warpgroup 0's half is all zero (MADE mask): no products
-       kStepSkip1 = 16 }; // the same for warpgroup 1
-struct __align__(8) FusedStep {
-    uint16_t bytes16;    // record size / 16
-    uint8_t n8;          // rows of each warpgroup's half of a tile / 8 (MMA N / 8)
-    uint8_t kc;          // A-operand K-chunk
-    uint8_t flags;       // kStep*
-    uint8_t pad_[3];
-};
+// (the step table and record layout of the packed weight stream: nfb_fused_plan.h)
 
 // One fused [LULinearPermute +] spline block, packed.  Device-resident (uploaded at pack time): the kernel
 // reads it through a pointer so that ONE persistent launch can walk a whole stack of blocks.
@@ -187,6 +173,7 @@ struct FusedLayer {
     signed char in_idx[64];    // conditioner input column per k (-1 = zero pad)
     unsigned char tr_idx[64];  // transformed feature columns
     unsigned char id_idx[64];  // identity feature columns (coupled layer)
+    signed char own[2][2];     // 64-column output slices of the hidden GEMMs owned by each consumer warpgroup (-1: none)
     // fp16 operand scaling (all powers of two; nfb_api.cu plan_scales): index 0 = LU stage, 1 + g = GEMM g of the
     // conditioner (g = n_hidden: final layer).  A operand = true value * u_row * a_sc; true value = acc * a_inv / u_row.
     float a_sc[10], a_inv[10];
