@@ -349,6 +349,26 @@ int nfb_resnet_backward(const nfb_resnet_ctx_desc_t* desc, const float* x_dev, c
                         float* g_x_dev, float* g_context_dev, float* const* g_w, float* const* g_b,
                         float* const* g_w_context, float* const* g_b_context, void* stream);
 
+/* Bytes of device scratch nfb_maf_inverse_backward needs for `rows` rows (-1: bad descriptor). */
+int64_t nfb_maf_inverse_backward_workspace_bytes(const nfb_resnet_ctx_desc_t* desc, int32_t features, int64_t rows);
+/* Gradients of sum g_y . y + g_log_det . log_det through the density pass of MaskedAffineAutoregressive
+ * (flows/affine/autoregressive.py:26-33,114-128): y solves y = (x - shift) / scale with (u, shift) the interleaved
+ * pairs of p = MADE(y, context) [rows, features, 2], scale = sigmoid(u + 2) + 1e-3, log_det = -sum log scale.
+ * desc is the MADE (masks set, in_features = features, out_features = 2 features, context through w_context).
+ * The MADE's activations are recomputed once at the forward's output y; the cotangent lam of y then follows
+ * lam = g_y + MADE_dgrad_y(pbar(lam)) for features - 1 passes (exact: MADE's Jacobian in y is strictly lower
+ * triangular), each pass one element kernel and one data-gradient-only MADE adjoint, and a last pass forms
+ * g_x = lam / scale and the weight / context gradients of the final pbar.  Equals the gradient of the reference's
+ * unrolled D-pass loop.  x, y [rows, features], context [rows, context_features], g_y [rows, features] and g_log_det
+ * [rows] (either may be NULL: zero).  Outputs as in nfb_resnet_backward, each optional and OVERWRITTEN: g_x, g_context,
+ * g_w / g_b (2 + 2 num_blocks entries: initial, blocks.0.linear_layers.0, ..., final), g_w_context / g_b_context
+ * (1 + num_blocks entries: context_layer, then each block's context_layer).  rows = 0: every gradient is zero. */
+int nfb_maf_inverse_backward(const nfb_resnet_ctx_desc_t* desc, int32_t features, const float* x_dev, const float* y_dev,
+                             const float* context_dev, const float* g_y_dev, const float* g_log_det_dev, int64_t rows,
+                             void* workspace_dev, int64_t workspace_bytes, float* g_x_dev, float* g_context_dev,
+                             float* const* g_w, float* const* g_b, float* const* g_w_context,
+                             float* const* g_b_context, void* stream);
+
 /* flows/neural_spline/wrapper.py:186-244 AutoregressiveRationalQuadraticSpline */
 typedef struct {
     int32_t features, num_bins;

@@ -1578,94 +1578,130 @@ int wgrad(const GemmRun& g, const float* gY, int n_out, const float* X, long lon
 }
 }  // namespace
 
-int64_t nfb_resnet_backward_workspace_bytes(const nfb_resnet_ctx_desc_t* d, int64_t rows) {
-    return resnet_layout(d, rows, nullptr, nullptr);
+namespace {
+// One backward of a ResidualNet / MADE: the effective weights, the recomputed activations (ws) and the initial layer's
+// input, shared by every adjoint run on them (nfb_maf_inverse_backward runs several on one recompute).
+struct ResnetPass {
+    const nfb_resnet_ctx_desc_t* d;
+    long long rows;
+    ResnetWs ws;
+    GemmRun g;
+    const float* w0; const float* wf; const float* wb[2 * kResnetMaxBlocks];
+    const float* in; long long ld_in;   // x, or cat(x, context) in ws.in0
+};
+
+int resnet_validate(const char* who, const nfb_resnet_ctx_desc_t* d, int64_t rows, const float* x, const float* context,
+                    const float* g_out, void* workspace, int64_t workspace_bytes, int64_t need) {
+    NFB_CHECK(need >= 0, NFB_ERR_ARG, "%s: bad descriptor or shape", who);
+    NFB_CHECK(workspace_bytes >= need && (need == 0 || workspace), NFB_ERR_ARG, "%s: workspace of %lld bytes, needs %lld",
+              who, (long long)workspace_bytes, (long long)need);
+    const nfb_resnet_desc_t& n = d->net;
+    const int nb = n.num_blocks;
+    const bool ctx = d->context_features > 0, masked = n.m_initial != nullptr;
+    NFB_CHECK(n.w_initial && n.b_initial && n.w_final && n.b_final && (nb == 0 || (n.w_blocks && n.b_blocks)),
+              NFB_ERR_ARG, "%s: null weight or bias", who);
+    NFB_CHECK(!masked || (n.m_final && (nb == 0 || n.m_blocks)), NFB_ERR_ARG, "%s: missing masks", who);
+    NFB_CHECK(!ctx || ((d->w_context ? d->b_context != nullptr : true) &&
+                       (nb == 0 || (d->w_block_context && d->b_block_context))),
+              NFB_ERR_ARG, "%s: null context layer", who);
+    NFB_CHECK(rows == 0 || (x && g_out && (!ctx || context)), NFB_ERR_ARG, "%s: null input", who);
+    return NFB_OK;
 }
 
-int nfb_resnet_backward(const nfb_resnet_ctx_desc_t* d, const float* x, const float* context, const float* g_out,
-                        int64_t rows, void* workspace, int64_t workspace_bytes, float* g_x, float* g_context,
-                        float* const* g_w, float* const* g_b, float* const* g_wc, float* const* g_bc, void* stream) {
-    const int64_t need = resnet_layout(d, rows, nullptr, nullptr);
-    NFB_CHECK(need >= 0, NFB_ERR_ARG, "nfb_resnet_backward: bad descriptor or shape");
-    NFB_CHECK(workspace_bytes >= need && (need == 0 || workspace), NFB_ERR_ARG,
-              "nfb_resnet_backward: workspace of %lld bytes, needs %lld", (long long)workspace_bytes, (long long)need);
+// empty batch: every parameter gradient is zero
+int resnet_zero_grads(const nfb_resnet_ctx_desc_t* d, float* const* g_w, float* const* g_b, float* const* g_wc,
+                      float* const* g_bc, cudaStream_t st) {
     const nfb_resnet_desc_t& n = d->net;
+    const int nb = n.num_blocks, H = n.hidden_features, C = d->context_features, out = n.out_features, nin = n.in_features;
+    auto zero = [&](float* p, size_t numel) { return p ? (int)cudaMemsetAsync(p, 0, numel * 4, st) : 0; };
+    auto wsz = [&](int i) { return (size_t)H * (i == 0 ? nin : H); };  // weights of linear i < 1 + 2 nb
+    for (int i = 0; i < 1 + 2 * nb; ++i) {
+        NFB_CUDA((cudaError_t)zero(g_w ? g_w[i] : nullptr, wsz(i)));
+        NFB_CUDA((cudaError_t)zero(g_b ? g_b[i] : nullptr, H));
+    }
+    NFB_CUDA((cudaError_t)zero(g_w ? g_w[1 + 2 * nb] : nullptr, (size_t)out * H));
+    NFB_CUDA((cudaError_t)zero(g_b ? g_b[1 + 2 * nb] : nullptr, out));
+    if (C > 0)
+        for (int i = 0; i <= nb; ++i) {
+            NFB_CUDA((cudaError_t)zero(g_wc ? g_wc[i] : nullptr, (size_t)H * C));
+            NFB_CUDA((cudaError_t)zero(g_bc ? g_bc[i] : nullptr, H));
+        }
+    return NFB_OK;
+}
+
+// Effective weights and the activations of the forward at x / context (the same GEMMs as the forward,
+// nets/*.forward through nfb_gemm_f32).  rows > 0.
+int resnet_recompute(ResnetPass& r, const float* x, const float* context, void* workspace, cudaStream_t st) {
+    const nfb_resnet_ctx_desc_t* d = r.d;
+    const nfb_resnet_desc_t& n = d->net;
+    const long long rows = r.rows;
     const int nb = n.num_blocks, H = n.hidden_features, C = d->context_features, out = n.out_features;
     const bool ctx = C > 0, concat = ctx && !d->w_context, masked = n.m_initial != nullptr;
     const int nin = n.in_features, nx = concat ? nin - C : nin;
-    NFB_CHECK(n.w_initial && n.b_initial && n.w_final && n.b_final && (nb == 0 || (n.w_blocks && n.b_blocks)),
-              NFB_ERR_ARG, "nfb_resnet_backward: null weight or bias");
-    NFB_CHECK(!masked || (n.m_final && (nb == 0 || n.m_blocks)), NFB_ERR_ARG, "nfb_resnet_backward: missing masks");
-    NFB_CHECK(!ctx || ((d->w_context ? d->b_context != nullptr : true) &&
-                       (nb == 0 || (d->w_block_context && d->b_block_context))),
-              NFB_ERR_ARG, "nfb_resnet_backward: null context layer");
-    NFB_CHECK(rows == 0 || (x && g_out && (!ctx || context)), NFB_ERR_ARG, "nfb_resnet_backward: null input");
-    cudaStream_t st = S(stream);
-    auto zero = [&](float* p, size_t numel) { return p ? (int)cudaMemsetAsync(p, 0, numel * 4, st) : 0; };
-    auto wsz = [&](int i) { return (size_t)H * (i == 0 ? nin : H); };  // weights of linear i < 1 + 2 nb
-    if (rows == 0) {   // empty batch: every gradient is zero
-        for (int i = 0; i < 1 + 2 * nb; ++i) {
-            NFB_CUDA((cudaError_t)zero(g_w ? g_w[i] : nullptr, wsz(i)));
-            NFB_CUDA((cudaError_t)zero(g_b ? g_b[i] : nullptr, H));
-        }
-        NFB_CUDA((cudaError_t)zero(g_w ? g_w[1 + 2 * nb] : nullptr, (size_t)out * H));
-        NFB_CUDA((cudaError_t)zero(g_b ? g_b[1 + 2 * nb] : nullptr, out));
-        if (ctx)
-            for (int i = 0; i <= nb; ++i) {
-                NFB_CUDA((cudaError_t)zero(g_wc ? g_wc[i] : nullptr, (size_t)H * C));
-                NFB_CUDA((cudaError_t)zero(g_bc ? g_bc[i] : nullptr, H));
-            }
-        return NFB_OK;
-    }
-    ResnetWs ws{};
+    ResnetWs& ws = r.ws;
     resnet_layout(d, rows, static_cast<char*>(workspace), &ws);
     int* err_dev = nullptr;
     NFB_TRY(glow_err_buf(&err_dev));
-    const GemmRun g{err_dev, st};
+    r.g = GemmRun{err_dev, st};
+    const GemmRun& g = r.g;
     // effective weights
-    const float* w0 = n.w_initial; const float* wf = n.w_final;
-    const float* wb[2 * kResnetMaxBlocks];
-    for (int i = 0; i < 2 * nb; ++i) wb[i] = n.w_blocks[i];
+    r.w0 = n.w_initial; r.wf = n.w_final;
+    for (int i = 0; i < 2 * nb; ++i) r.wb[i] = n.w_blocks[i];
     if (masked) {
         NFB_TRY(launch_mask_mul(n.w_initial, n.m_initial, ws.w0e, (long long)H * nin, st));
         for (int i = 0; i < 2 * nb; ++i) NFB_TRY(launch_mask_mul(n.w_blocks[i], n.m_blocks[i], ws.wbe[i], (long long)H * H, st));
         NFB_TRY(launch_mask_mul(n.w_final, n.m_final, ws.wfe, (long long)out * H, st));
-        w0 = ws.w0e; wf = ws.wfe;
-        for (int i = 0; i < 2 * nb; ++i) wb[i] = ws.wbe[i];
+        r.w0 = ws.w0e; r.wf = ws.wfe;
+        for (int i = 0; i < 2 * nb; ++i) r.wb[i] = ws.wbe[i];
     }
-    auto mask_of = [&](int i) -> const float* {   // linear i: 0 initial, 1 + j block linear j, 1 + 2 nb final
-        if (!masked) return nullptr;
-        return i == 0 ? n.m_initial : (i == 1 + 2 * nb ? n.m_final : n.m_blocks[i - 1]);
-    };
-    // ---- recompute (the same GEMMs as the forward, nets/*.forward through nfb_gemm_f32) ----
-    const float* in = x;
-    long long ld_in = nin;
+    r.in = x;
+    r.ld_in = nin;
     if (concat) {
         NFB_CUDA(cudaMemcpy2DAsync(ws.in0, (size_t)nin * 4, x, (size_t)nx * 4, (size_t)nx * 4, rows,
                                    cudaMemcpyDeviceToDevice, st));
         NFB_CUDA(cudaMemcpy2DAsync(ws.in0 + nx, (size_t)nin * 4, context, (size_t)C * 4, (size_t)C * 4, rows,
                                    cudaMemcpyDeviceToDevice, st));
-        in = ws.in0;
+        r.in = ws.in0;
     }
-    NFB_TRY(g(fwd_args(in, ld_in, 0, w0, n.b_initial, ws.h[0], rows, H, nin)));
+    NFB_TRY(g(fwd_args(r.in, r.ld_in, 0, r.w0, n.b_initial, ws.h[0], rows, H, nin)));
     if (ctx && !concat) {
         GemmTcArgs a = fwd_args(context, C, 0, d->w_context, d->b_context, ws.h[0], rows, H, C);
         a.resid = ws.h[0]; a.ldres = H;
         NFB_TRY(g(a));
     }
     for (int b = 0; b < nb; ++b) {
-        NFB_TRY(g(fwd_args(ws.h[b], H, 1, wb[2 * b], n.b_blocks[2 * b], ws.t1[b], rows, H, H)));
+        NFB_TRY(g(fwd_args(ws.h[b], H, 1, r.wb[2 * b], n.b_blocks[2 * b], ws.t1[b], rows, H, H)));
         if (!ctx) {
-            GemmTcArgs a = fwd_args(ws.t1[b], H, 1, wb[2 * b + 1], n.b_blocks[2 * b + 1], ws.h[b + 1], rows, H, H);
+            GemmTcArgs a = fwd_args(ws.t1[b], H, 1, r.wb[2 * b + 1], n.b_blocks[2 * b + 1], ws.h[b + 1], rows, H, H);
             a.resid = ws.h[b]; a.ldres = H;
             NFB_TRY(g(a));
         } else {
-            NFB_TRY(g(fwd_args(ws.t1[b], H, 1, wb[2 * b + 1], n.b_blocks[2 * b + 1], ws.t2[b], rows, H, H)));
+            NFB_TRY(g(fwd_args(ws.t1[b], H, 1, r.wb[2 * b + 1], n.b_blocks[2 * b + 1], ws.t2[b], rows, H, H)));
             NFB_TRY(g(fwd_args(context, C, 0, d->w_block_context[b], d->b_block_context[b], ws.c[b], rows, H, C)));
             NFB_TRY(launch_glu_residual(ws.h[b], ws.t2[b], ws.c[b], (long long)rows * H, ws.h[b + 1], st));
         }
     }
-    // ---- adjoint ----
+    return NFB_OK;
+}
+
+// Adjoint of the recomputed net for the output cotangent g_out.  data_only: the data gradient g_x alone -- no weight
+// gradient, no bias column sum, no context GEMM, no context gradient (g_context and the g_* arrays are ignored).
+int resnet_adjoint(const ResnetPass& r, const float* context, const float* g_out, bool data_only, float* g_x,
+                   float* g_context, float* const* g_w, float* const* g_b, float* const* g_wc, float* const* g_bc,
+                   cudaStream_t st) {
+    if (data_only) { g_context = nullptr; g_w = g_b = g_wc = g_bc = nullptr; }
+    const nfb_resnet_ctx_desc_t* d = r.d;
+    const nfb_resnet_desc_t& n = d->net;
+    const long long rows = r.rows;
+    const int nb = n.num_blocks, H = n.hidden_features, C = d->context_features, out = n.out_features;
+    const bool ctx = C > 0, concat = ctx && !d->w_context, masked = n.m_initial != nullptr;
+    const int nin = n.in_features, nx = concat ? nin - C : nin;
+    const ResnetWs& ws = r.ws;
+    const GemmRun& g = r.g;
+    auto mask_of = [&](int i) -> const float* {   // linear i: 0 initial, 1 + j block linear j, 1 + 2 nb final
+        if (!masked) return nullptr;
+        return i == 0 ? n.m_initial : (i == 1 + 2 * nb ? n.m_final : n.m_blocks[i - 1]);
+    };
     if (g_context) NFB_CUDA(cudaMemsetAsync(g_context, 0, (size_t)rows * C * 4, st));
     auto ctx_layer = [&](const float* gY, const float* W, int slot) -> int {   // a Linear of the context
         NFB_TRY(wgrad(g, gY, H, context, C, C, 0, nullptr, rows, g_wc ? g_wc[slot] : nullptr, g_bc ? g_bc[slot] : nullptr,
@@ -1680,32 +1716,33 @@ int nfb_resnet_backward(const nfb_resnet_ctx_desc_t* d, const float* x, const fl
     const int fl = 1 + 2 * nb;
     NFB_TRY(wgrad(g, g_out, out, ws.h[nb], H, H, 0, mask_of(fl), rows, g_w ? g_w[fl] : nullptr, g_b ? g_b[fl] : nullptr,
                   st));
-    NFB_TRY(g(dgrad_args(g_out, wf, ws.ga, rows, H, out)));
+    NFB_TRY(g(dgrad_args(g_out, r.wf, ws.ga, rows, H, out)));
     for (int b = nb - 1; b >= 0; --b) {
         const int l1 = 1 + 2 * b, l2 = 2 + 2 * b;
         const float* gt2 = ws.ga;  // h_{b+1} = h_b + t2 (no context)
         if (ctx) {                 // h_{b+1} = h_b + t2 * sigmoid(c)
-            NFB_TRY(launch_glu_residual_bwd(ws.ga, ws.t2[b], ws.c[b], (long long)rows * H, nullptr, ws.gt, ws.gt1, st));
-            NFB_TRY(ctx_layer(ws.gt1, d->w_block_context[b], 1 + b));
+            NFB_TRY(launch_glu_residual_bwd(ws.ga, ws.t2[b], ws.c[b], (long long)rows * H, nullptr, ws.gt,
+                                            data_only ? nullptr : ws.gt1, st));
+            if (!data_only) NFB_TRY(ctx_layer(ws.gt1, d->w_block_context[b], 1 + b));
             gt2 = ws.gt;
         }
         // t2 = W2 relu(t1) + b2
         NFB_TRY(wgrad(g, gt2, H, ws.t1[b], H, H, 1, mask_of(l2), rows, g_w ? g_w[l2] : nullptr, g_b ? g_b[l2] : nullptr, st));
-        GemmTcArgs a = dgrad_args(gt2, wb[2 * b + 1], ws.gt1, rows, H, H);
+        GemmTcArgs a = dgrad_args(gt2, r.wb[2 * b + 1], ws.gt1, rows, H, H);
         a.mask = ws.t1[b]; a.ldmask = H;
         NFB_TRY(g(a));   // g_t1 = (g_t2 W2) * (t1 > 0)
         // t1 = W1 relu(h_b) + b1
         NFB_TRY(wgrad(g, ws.gt1, H, ws.h[b], H, H, 1, mask_of(l1), rows, g_w ? g_w[l1] : nullptr, g_b ? g_b[l1] : nullptr,
                       st));
-        GemmTcArgs c = dgrad_args(ws.gt1, wb[2 * b], ws.ga, rows, H, H);
+        GemmTcArgs c = dgrad_args(ws.gt1, r.wb[2 * b], ws.ga, rows, H, H);
         c.mask = ws.h[b]; c.ldmask = H; c.resid = ws.ga; c.ldres = H;
         NFB_TRY(g(c));   // g_h_b = g_h_{b+1} + (g_t1 W1) * (h_b > 0)     (in place)
     }
-    NFB_TRY(wgrad(g, ws.ga, H, in, ld_in, nin, 0, mask_of(0), rows, g_w ? g_w[0] : nullptr, g_b ? g_b[0] : nullptr, st));
-    if (ctx && !concat) NFB_TRY(ctx_layer(ws.ga, d->w_context, 0));
+    NFB_TRY(wgrad(g, ws.ga, H, r.in, r.ld_in, nin, 0, mask_of(0), rows, g_w ? g_w[0] : nullptr, g_b ? g_b[0] : nullptr, st));
+    if (ctx && !concat && !data_only) NFB_TRY(ctx_layer(ws.ga, d->w_context, 0));
     if (concat) {
         if (g_x || g_context) {
-            NFB_TRY(g(dgrad_args(ws.ga, w0, ws.in0, rows, nin, H)));   // [g_x | g_context] of cat(x, context)
+            NFB_TRY(g(dgrad_args(ws.ga, r.w0, ws.in0, rows, nin, H)));   // [g_x | g_context] of cat(x, context)
             if (g_x)
                 NFB_CUDA(cudaMemcpy2DAsync(g_x, (size_t)nx * 4, ws.in0, (size_t)nin * 4, (size_t)nx * 4, rows,
                                            cudaMemcpyDeviceToDevice, st));
@@ -1716,9 +1753,82 @@ int nfb_resnet_backward(const nfb_resnet_ctx_desc_t* d, const float* x, const fl
             }
         }
     } else if (g_x) {
-        NFB_TRY(g(dgrad_args(ws.ga, w0, g_x, rows, nin, H)));
+        NFB_TRY(g(dgrad_args(ws.ga, r.w0, g_x, rows, nin, H)));
     }
     return NFB_OK;
+}
+
+// Scratch of nfb_maf_inverse_backward: the conditioner's (resnet_layout), then
+//   P    [rows, 2 D]  MADE(y, context), the conditioner output at the layer's output
+//   pbar [rows, 2 D]  its cotangent
+//   gin  [rows, D]    MADE data gradient of the latest fixed-point pass
+int64_t maf_layout(const nfb_resnet_ctx_desc_t* d, int32_t features, long long rows, char* base, ResnetWs* ws, float** P,
+                   float** pbar, float** gin) {
+    const int64_t off0 = resnet_layout(d, rows, base, ws);
+    if (off0 < 0 || features < 1) return -1;
+    size_t off = (size_t)off0;
+    auto take = [&](size_t floats) { float* p = base ? reinterpret_cast<float*>(base + off) : nullptr;
+                                     off += (floats * 4 + 255) / 256 * 256; return p; };
+    float* p = take((size_t)rows * 2 * features); if (P) *P = p;
+    p = take((size_t)rows * 2 * features); if (pbar) *pbar = p;
+    p = take((size_t)rows * features); if (gin) *gin = p;
+    return (int64_t)off;
+}
+}  // namespace
+
+int64_t nfb_resnet_backward_workspace_bytes(const nfb_resnet_ctx_desc_t* d, int64_t rows) {
+    return resnet_layout(d, rows, nullptr, nullptr);
+}
+
+int nfb_resnet_backward(const nfb_resnet_ctx_desc_t* d, const float* x, const float* context, const float* g_out,
+                        int64_t rows, void* workspace, int64_t workspace_bytes, float* g_x, float* g_context,
+                        float* const* g_w, float* const* g_b, float* const* g_wc, float* const* g_bc, void* stream) {
+    NFB_TRY(resnet_validate("nfb_resnet_backward", d, rows, x, context, g_out, workspace, workspace_bytes,
+                            resnet_layout(d, rows, nullptr, nullptr)));
+    cudaStream_t st = S(stream);
+    if (rows == 0) return resnet_zero_grads(d, g_w, g_b, g_wc, g_bc, st);
+    ResnetPass r{};
+    r.d = d;
+    r.rows = rows;
+    NFB_TRY(resnet_recompute(r, x, context, workspace, st));
+    return resnet_adjoint(r, context, g_out, false, g_x, g_context, g_w, g_b, g_wc, g_bc, st);
+}
+
+int64_t nfb_maf_inverse_backward_workspace_bytes(const nfb_resnet_ctx_desc_t* d, int32_t features, int64_t rows) {
+    return maf_layout(d, features, rows, nullptr, nullptr, nullptr, nullptr, nullptr);
+}
+
+int nfb_maf_inverse_backward(const nfb_resnet_ctx_desc_t* d, int32_t features, const float* x, const float* y,
+                             const float* context, const float* g_y, const float* g_log_det, int64_t rows,
+                             void* workspace, int64_t workspace_bytes, float* g_x, float* g_context, float* const* g_w,
+                             float* const* g_b, float* const* g_wc, float* const* g_bc, void* stream) {
+    const char* who = "nfb_maf_inverse_backward";
+    NFB_CHECK(d && d->net.m_initial, NFB_ERR_ARG, "%s: the descriptor must be a MADE (mask pointers set)", who);
+    NFB_CHECK(features >= 1 && d->net.in_features == features && d->net.out_features == 2 * features, NFB_ERR_ARG,
+              "%s: a MADE of %d -> %d features does not parameterise %d features", who, d->net.in_features,
+              d->net.out_features, features);
+    NFB_CHECK(d->context_features == 0 || d->w_context, NFB_ERR_ARG, "%s: a MADE takes its context through w_context",
+              who);
+    NFB_TRY(resnet_validate(who, d, rows, y, context, x /* g_y and g_log_det may be NULL: zero */, workspace,
+                            workspace_bytes, maf_layout(d, features, rows, nullptr, nullptr, nullptr, nullptr, nullptr)));
+    cudaStream_t st = S(stream);
+    if (rows == 0) return resnet_zero_grads(d, g_w, g_b, g_wc, g_bc, st);
+    ResnetPass r{};
+    r.d = d;
+    r.rows = rows;
+    float *P = nullptr, *pbar = nullptr, *gin = nullptr;
+    maf_layout(d, features, rows, static_cast<char*>(workspace), nullptr, &P, &pbar, &gin);
+    // one recompute at the layer's output y; its ReLU masks and gate logits serve every pass below
+    NFB_TRY(resnet_recompute(r, y, context, workspace, st));
+    const int H = d->net.hidden_features, nb = d->net.num_blocks;
+    NFB_TRY(r.g(fwd_args(r.ws.h[nb], H, 0, r.wf, d->net.b_final, P, rows, 2 * features, H)));
+    // lam = g_y + MADE_dgrad_x(A(lam)), D - 1 times: exact, as MADE's Jacobian in y is strictly lower triangular
+    for (int it = 0; it + 1 < features; ++it) {
+        NFB_TRY(launch_maf_affine_adjoint(x, P, g_y, g_log_det, it ? gin : nullptr, rows, features, pbar, nullptr, st));
+        NFB_TRY(resnet_adjoint(r, context, pbar, true, gin, nullptr, nullptr, nullptr, nullptr, nullptr, st));
+    }
+    NFB_TRY(launch_maf_affine_adjoint(x, P, g_y, g_log_det, features > 1 ? gin : nullptr, rows, features, pbar, g_x, st));
+    return resnet_adjoint(r, context, pbar, false, nullptr, g_context, g_w, g_b, g_wc, g_bc, st);
 }
 
 namespace {

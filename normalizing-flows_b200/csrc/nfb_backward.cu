@@ -10,6 +10,7 @@
 // All of these are HBM-bound streaming kernels: coalesced through shared-memory staging where the natural access
 // is strided (23 parameters per element), one pass over the data.
 #include "nfb_kernels.h"
+#include "nfb_maf_bwd.cuh"
 #include "nfb_spline_bwd.cuh"
 
 namespace nfb {
@@ -491,6 +492,32 @@ __global__ void split_table_kernel(const float* __restrict__ tab, int n, float* 
 int launch_split_table(const float* tab, int n, float* gw, float* gh, float* gd, cudaStream_t st) {
     if (n == 0) return NFB_OK;
     split_table_kernel<<<(n * kP + 255) / 256, 256, 0, st>>>(tab, n, gw, gh, gd);
+    NFB_LAUNCH_CHECK();
+    return NFB_OK;
+}
+
+// One pass of the MAF density adjoint (nfb_maf_bwd.cuh), one thread per element: lam = g_y + g_in (g_in, the MADE data
+// gradient of the previous pass, NULL on the first), pbar [rows, d, 2] in the MADE output layout, and g_x = lam / scale
+// when g_x is given (the last pass).  g_y / g_ld NULL: zero.
+__global__ void __launch_bounds__(256) maf_affine_adjoint_kernel(const float* __restrict__ x,
+                                                                 const float* __restrict__ params,
+                                                                 const float* __restrict__ gy, const float* __restrict__ gld,
+                                                                 const float* __restrict__ gin, long long n, int d,
+                                                                 float* __restrict__ pbar, float* __restrict__ gx) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float2 p = reinterpret_cast<const float2*>(params)[i];
+    const float lam = (gy ? gy[i] : 0.f) + (gin ? gin[i] : 0.f);
+    float gu, gs, g;
+    maf_affine_adjoint<float>(x[i], p.x, p.y, lam, gld ? gld[i / d] : 0.f, gu, gs, g);
+    reinterpret_cast<float2*>(pbar)[i] = make_float2(gu, gs);
+    if (gx) gx[i] = g;
+}
+int launch_maf_affine_adjoint(const float* x, const float* params, const float* gy, const float* gld, const float* gin,
+                              long long rows, int d, float* pbar, float* gx, cudaStream_t st) {
+    const long long n = rows * d;
+    if (n == 0) return NFB_OK;
+    maf_affine_adjoint_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(x, params, gy, gld, gin, n, d, pbar, gx);
     NFB_LAUNCH_CHECK();
     return NFB_OK;
 }

@@ -244,6 +244,9 @@ int launch_periodic_features_bwd(const float* x, const float* gy, long long rows
                                  cudaStream_t st);
 int launch_leaky_gate(const float* in, const float* gate, float slope, long long n, float* out, cudaStream_t st);
 int launch_split_table(const float* tab, int n, float* gw, float* gh, float* gd, cudaStream_t st);
+// one fixed-point pass of the MAF density adjoint: params [rows, d, 2], pbar [rows, d, 2]; gin, gx optional
+int launch_maf_affine_adjoint(const float* x, const float* params, const float* gy, const float* gld, const float* gin,
+                              long long rows, int d, float* pbar, float* gx, cudaStream_t st);
 
 // ---- invertible residual block, element-wise pieces (nfb_residual.cu) ----
 int launch_swish(const float* x, float b, long long n, float* a, float* da, cudaStream_t st);

@@ -109,6 +109,9 @@ SYMBOLS = {
     "nfb_resnet_backward_workspace_bytes": (_I64, [C.POINTER(ResnetCtxDesc), _I64]),
     "nfb_resnet_backward": (C.c_int, [C.POINTER(ResnetCtxDesc), _VP, _VP, _VP, _I64, _VP, _I64, _VP, _VP,
                                       C.POINTER(_VP), C.POINTER(_VP), C.POINTER(_VP), C.POINTER(_VP), _VP]),
+    "nfb_maf_inverse_backward_workspace_bytes": (_I64, [C.POINTER(ResnetCtxDesc), _I32, _I64]),
+    "nfb_maf_inverse_backward": (C.c_int, [C.POINTER(ResnetCtxDesc), _I32, _VP, _VP, _VP, _VP, _VP, _I64, _VP, _I64, _VP,
+                                           _VP, C.POINTER(_VP), C.POINTER(_VP), C.POINTER(_VP), C.POINTER(_VP), _VP]),
     "nfb_mlp_backward_workspace_bytes": (_I64, [C.POINTER(MlpDesc), _I64]),
     "nfb_mlp_backward": (C.c_int, [C.POINTER(MlpDesc), _VP, _VP, _I64, _VP, _I64, _VP, C.POINTER(_VP), C.POINTER(_VP),
                                    _VP]),

@@ -89,8 +89,10 @@ def spline_backward(x, params, shared, num_bins, gy, g_ld, wh_scale, tail_bound=
     return gx, gp
 
 
-def resnet_backward(net, masked, x, context, g_out, need_x=True, need_ctx=True):
-    """(g_x, g_context | None, {parameter: gradient}) of a ResidualNet / MADE through nfb_resnet_backward."""
+def _resnet_grad_call(net, masked, context):
+    """The nfb_resnet_ctx_desc_t of a ResidualNet / MADE and its parameter-gradient outputs, in the slot order of
+    nfb_resnet_backward / nfb_maf_inverse_backward: (desc, keepalive, gradient arrays (g_w, g_b, g_w_context,
+    g_b_context) as C pointer arrays, {parameter: gradient} of the parameters that require grad)."""
     d = L.ResnetCtxDesc()
     d.net, keep = resnet_desc(net, masked)
     blocks = list(net.blocks)
@@ -109,23 +111,44 @@ def resnet_backward(net, masked, x, context, g_out, need_x=True, need_ctx=True):
         d.w_block_context = C.cast(wbc, C.POINTER(C.c_void_p))
         d.b_block_context = C.cast(bbc, C.POINTER(C.c_void_p))
         keep = (keep, wbc, bbc)
-    rows = x.shape[0]
     gw = [_grad_like(p) for p in lin_w]
     gb = [_grad_like(p) for p in lin_b]
     gwc = [_grad_like(p) if p is not None else None for p in ctx_w]
     gbc = [_grad_like(p) if p is not None else None for p in ctx_b]
+    arrays = [_vp(gw), _vp(gb), _vp(gwc), _vp(gbc)]
+    gmap = {p: g for p, g in zip(lin_w + lin_b + ctx_w + ctx_b, gw + gb + gwc + gbc) if g is not None}
+    return d, (keep, arrays), [C.cast(a, C.POINTER(C.c_void_p)) for a in arrays], gmap
+
+
+def resnet_backward(net, masked, x, context, g_out, need_x=True, need_ctx=True):
+    """(g_x, g_context | None, {parameter: gradient}) of a ResidualNet / MADE through nfb_resnet_backward."""
+    d, keep, arrays, gmap = _resnet_grad_call(net, masked, context)
+    rows = x.shape[0]
     gx = torch.empty_like(x) if need_x else None
     gctx = torch.empty_like(context) if context is not None and need_ctx else None
     lib = L.lib()
     ws = _workspace(lib.nfb_resnet_backward_workspace_bytes(C.byref(d), rows), x.device)
-    pw, pb, pwc, pbc = _vp(gw), _vp(gb), _vp(gwc), _vp(gbc)
     with torch.cuda.device(x.device):
         L.check(lib.nfb_resnet_backward(C.byref(d), L.ptr(x), L.ptr(context), L.ptr(g_out), rows, L.ptr(ws), ws.numel(),
-                                        L.ptr(gx), L.ptr(gctx), C.cast(pw, C.POINTER(C.c_void_p)),
-                                        C.cast(pb, C.POINTER(C.c_void_p)), C.cast(pwc, C.POINTER(C.c_void_p)),
-                                        C.cast(pbc, C.POINTER(C.c_void_p)), L.stream_ptr()))
+                                        L.ptr(gx), L.ptr(gctx), *arrays, L.stream_ptr()))
     del keep
-    gmap = {p: g for p, g in zip(lin_w + lin_b + ctx_w + ctx_b, gw + gb + gwc + gbc) if g is not None}
+    return gx, gctx, gmap
+
+
+def maf_inverse_backward(made, features, x, y, context, g_y, g_ld, need_x=True, need_ctx=True):
+    """(g_x, g_context | None, {parameter: gradient}) of MaskedAffineAutoregressive's density pass y = inverse(x)
+    through nfb_maf_inverse_backward (the fixed-point adjoint of the D-pass loop; made = its autoregressive_net)."""
+    d, keep, arrays, gmap = _resnet_grad_call(made, True, context)
+    rows = x.shape[0]
+    gx = torch.empty_like(x) if need_x else None
+    gctx = torch.empty_like(context) if context is not None and need_ctx else None
+    lib = L.lib()
+    ws = _workspace(lib.nfb_maf_inverse_backward_workspace_bytes(C.byref(d), features, rows), x.device)
+    with torch.cuda.device(x.device):
+        L.check(lib.nfb_maf_inverse_backward(C.byref(d), features, L.ptr(x), L.ptr(y), L.ptr(context), L.ptr(g_y),
+                                             L.ptr(g_ld), rows, L.ptr(ws), ws.numel(), L.ptr(gx), L.ptr(gctx), *arrays,
+                                             L.stream_ptr()))
+    del keep
     return gx, gctx, gmap
 
 

@@ -3,12 +3,14 @@
 Same class names, constructor and module tree (`autoregressive_net` = nets.MADE with output_multiplier 2).  `forward`
 is ONE conditioner pass + an element-wise affine; `inverse` is D sequential passes (:29-38), exactly like the
 reference.  The conditioner runs as tensor-core GEMMs (csrc/nfb_gemm_tc.cu via nets.MADE.forward), the element-wise
-part and its log-det reduction in csrc/nfb_kernels.cu (`maf_affine_kernel`)."""
+part and its log-det reduction in csrc/nfb_kernels.cu (`maf_affine_kernel`).  Under grad, `inverse` goes through
+`MafInverseFn`, whose backward is the fixed-point adjoint of the D-pass loop (nfb_maf_inverse_backward, DESIGN §3.9)."""
 import numpy as np
 import torch
 from torch.nn import functional as F
 
 from .. import _lib as L
+from .._image_autograd import wants_grad
 from .._native import require_cuda_f32
 from ..nets import made as made_module
 from .base import Flow
@@ -55,6 +57,14 @@ class MaskedAffineAutoregressive(Autoregressive):
     def _output_dim_multiplier(self):
         return 2
 
+    def inverse(self, inputs, context=None):
+        """The density direction; differentiable (MafInverseFn) when a gradient is wanted."""
+        if wants_grad(self, inputs, context):
+            x = require_cuda_f32(inputs)
+            ctx = require_cuda_f32(context, "context") if context is not None else None
+            return MafInverseFn.apply(self, x, ctx, *self.parameters())
+        return super().inverse(inputs, context)
+
     def _affine(self, inputs, params, inverse):
         x = require_cuda_f32(inputs)
         if x.dim() != 2 or x.shape[1] != self.features:
@@ -73,3 +83,32 @@ class MaskedAffineAutoregressive(Autoregressive):
 
     def _elementwise_inverse(self, inputs, autoregressive_params):
         return self._affine(inputs, autoregressive_params, True)
+
+
+class MafInverseFn(torch.autograd.Function):
+    """(y, log_det) = MaskedAffineAutoregressive.inverse(x, context): the forward is the layer's D-pass loop under
+    no_grad (the value path, so values are bit-identical with and without grad); the backward is the fixed-point
+    adjoint nfb_maf_inverse_backward, which equals the gradient of the unrolled loop.  Refuses to run the backward if a
+    parameter was modified in place after the forward."""
+
+    @staticmethod
+    def forward(ctx, layer, x, context, *params):
+        y, ld = Autoregressive.inverse(layer, x, context)
+        ctx.layer, ctx.params = layer, params
+        ctx.versions = [p._version for p in params]
+        ctx.save_for_backward(x, y, context)
+        return y, ld
+
+    @staticmethod
+    def backward(ctx, g_y, g_ld):
+        from .._standalone import maf_inverse_backward
+        x, y, context = ctx.saved_tensors
+        layer = ctx.layer
+        if any(p._version != v for p, v in zip(ctx.params, ctx.versions)):
+            raise RuntimeError(f"{type(layer).__name__} backward: a parameter was modified in place after the "
+                               "forward pass")
+        need_x, need_ctx = ctx.needs_input_grad[1], ctx.needs_input_grad[2]
+        gx, gctx, gmap = maf_inverse_backward(layer.autoregressive_net, layer.features, x, y, context,
+                                              g_y.contiguous() if g_y is not None else None,
+                                              g_ld.contiguous() if g_ld is not None else None, need_x, need_ctx)
+        return (None, gx, gctx, *[gmap.get(p) if p.requires_grad else None for p in ctx.params])

@@ -1,4 +1,4 @@
-"""Time one training step of the stand-alone spline layers: `forward_kld` + `backward()` + Adam.
+"""Time one training step of the stand-alone spline and MAF layers: `forward_kld` + `backward()` + Adam.
     a    examples/conditional_flow.ipynb: ConditionalNormalizingFlow(DiagGaussian(2, trainable=False),
          4 x [AutoregressiveRationalQuadraticSpline(2, 2, 128, num_context_channels=4), LULinearPermute(2)]),
          Adam(lr 3e-4, weight decay 1e-5), batch 128 (the notebook's) and 65 536
@@ -6,6 +6,11 @@
     circ examples/circular_nsf.ipynb: 20 x CircularAutoregressiveRationalQuadraticSpline(2, 1, 128, [1],
          tail_bound=[5, pi], permute_mask=True) on DiagGaussian(2) (the notebook's UniformGaussian is not a package class),
          Adam(lr 1e-4, weight decay 1e-4), batch 1 024
+    maf  examples/conditional_flow.ipynb's third model: 4 x [MaskedAffineAutoregressive(2, 128, context_features=4,
+         num_blocks=2), LULinearPermute(2)] on DiagGaussian(2, trainable=False), Adam(lr 1e-3, weight decay 1e-5),
+         batch 128 (the notebook's) and 65 536
+    maf16 4 x [MaskedAffineAutoregressive(16, 256, num_blocks=2), LULinearPermute(16)] on DiagGaussian(16), no context,
+         Adam(lr 1e-3, weight decay 1e-5), batch 65 536: the D - 1 adjoint passes of each MAF layer dominate
 Prints one JSON line: ms/step (median of CUDA-event-timed steps after warm-up), samples/s, kernel launches per step
 (torch.profiler, one separate step), peak device memory, and the card's name, power limit and SM clock read in the same
 run.  When the unmodified reference is installed under oracle/_ref, the same model, seed and batch are timed through it
@@ -22,26 +27,36 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 REF_DIR = os.path.join(ROOT, "oracle", "_ref")
 
 
-CASES = [("a", 128), ("a", 65536), ("b", 128), ("b", 65536), ("circ", 1024)]
+CASES = [("a", 128), ("a", 65536), ("b", 128), ("b", 65536), ("circ", 1024), ("maf", 128), ("maf", 65536),
+         ("maf16", 65536)]
 NOTEBOOK_LAYERS = 4   # examples/conditional_flow.ipynb: K = 4 (spline + LU) pairs
 
 
 def build(nf, kind):
+    """-> (model, (lr, weight decay), input features, whether the model takes a context)"""
     import math
     import torch
     torch.manual_seed(0)
     if kind == "circ":
         flows = [nf.flows.CircularAutoregressiveRationalQuadraticSpline(2, 1, 128, [1], tail_bound=torch.tensor([5., math.pi]),
                                                                         permute_mask=True) for _ in range(20)]
-        return nf.NormalizingFlow(nf.distributions.DiagGaussian(2), flows), (1e-4, 1e-4)
+        return nf.NormalizingFlow(nf.distributions.DiagGaussian(2), flows), (1e-4, 1e-4), 2, False
+    if kind == "maf16":
+        flows = []
+        for _ in range(NOTEBOOK_LAYERS):
+            flows += [nf.flows.MaskedAffineAutoregressive(16, 256, num_blocks=2), nf.flows.LULinearPermute(16)]
+        return nf.NormalizingFlow(nf.distributions.DiagGaussian(16), flows), (1e-3, 1e-5), 16, False
     flows = []
     for _ in range(NOTEBOOK_LAYERS):
         if kind == "a":
             flows.append(nf.flows.AutoregressiveRationalQuadraticSpline(2, 2, 128, num_context_channels=4))
-        else:
+        elif kind == "b":
             flows.append(nf.flows.CoupledRationalQuadraticSpline(2, 2, 128, num_context_channels=4))
+        else:
+            flows.append(nf.flows.MaskedAffineAutoregressive(2, 128, context_features=4, num_blocks=2))
         flows.append(nf.flows.LULinearPermute(2))
-    return nf.ConditionalNormalizingFlow(nf.distributions.DiagGaussian(2, trainable=False), flows), (3e-4, 1e-5)
+    lr = (1e-3, 1e-5) if kind == "maf" else (3e-4, 1e-5)
+    return nf.ConditionalNormalizingFlow(nf.distributions.DiagGaussian(2, trainable=False), flows), lr, 2, True
 
 
 def time_arm(arm, kind, batch, steps, warmup):
@@ -53,18 +68,19 @@ def time_arm(arm, kind, batch, steps, warmup):
         sys.path[:0] = [ROOT, os.path.join(ROOT, "normalizing-flows_b200")]
     import normflows as nf
     dev = torch.device("cuda")
-    model, (lr, wd) = build(nf, kind)
+    model, (lr, wd), dim, conditional = build(nf, kind)
     model = model.to(dev)
     g = torch.Generator().manual_seed(1)
-    x = (torch.randn(batch, 2, generator=g) * 1.2).to(dev)
-    ctx = torch.cat([torch.randn(batch, 2, generator=g), 0.5 + 0.5 * torch.rand(batch, 2, generator=g)], 1).to(dev)
+    x = (torch.randn(batch, dim, generator=g) * 1.2).to(dev)
+    ctx = torch.cat([torch.randn(batch, 2, generator=g), 0.5 + 0.5 * torch.rand(batch, 2, generator=g)], 1).to(dev) \
+        if conditional else None
     opt = torch.optim.Adam(model.parameters(), lr=lr, weight_decay=wd)
     np.random.seed(0)
     torch.manual_seed(0)
 
     def step():
         opt.zero_grad(set_to_none=True)
-        loss = model.forward_kld(x) if kind == "circ" else model.forward_kld(x, ctx)
+        loss = model.forward_kld(x) if ctx is None else model.forward_kld(x, ctx)
         loss.backward()
         opt.step()
         return loss
