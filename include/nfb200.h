@@ -88,6 +88,20 @@ int nfb_rqs_spline_tails_backward(const float* x_dev, const float* params_dev, i
                                   const float* g_y_dev, const float* g_log_det_dev, float* g_x_dev, float* g_params_dev,
                                   int64_t rows, int32_t feats, int32_t num_bins, int32_t num_derivatives,
                                   const float* tail_bound_dev, const int32_t* circular_dev, float wh_scale, void* stream);
+/* ---- training pass of the stand-alone splines in the sampling direction (inverse = 1): gradients of
+ * sum g_x . x + g_log_det . log_det through x = g(z), log_det = -sum log f'(x) (utils/splines.py:172-198), f the forward
+ * spline.  Same arguments, layouts and conventions as the _backward pair above, but z_dev is the input of the inverse
+ * spline and g_x_dev the cotangent of its output; g_z_dev receives the gradient of z.  The bin is the one the inverse
+ * spline selects (search on the height knots at z), also for a z on an interior knot. */
+int nfb_rqs_spline_inverse_backward(const float* z_dev, const float* params_dev, int64_t params_row_stride,
+                                    const float* g_x_dev, const float* g_log_det_dev, float* g_z_dev,
+                                    float* g_params_dev, int64_t rows, int32_t feats, int32_t num_bins, float tail_bound,
+                                    float wh_scale, void* stream);
+int nfb_rqs_spline_tails_inverse_backward(const float* z_dev, const float* params_dev, int64_t params_row_stride,
+                                          const float* g_x_dev, const float* g_log_det_dev, float* g_z_dev,
+                                          float* g_params_dev, int64_t rows, int32_t feats, int32_t num_bins,
+                                          int32_t num_derivatives, const float* tail_bound_dev,
+                                          const int32_t* circular_dev, float wh_scale, void* stream);
 /* Adjoint of nfb_periodic_features: g_x (optional, overwritten; passes g_y through on non-periodic features),
  * g_weights [n_periodic, 2] and g_bias [n_periodic] (optional, overwritten with the sums over rows). */
 int nfb_periodic_features_backward(const float* x_dev, const float* g_y_dev, int64_t rows, int32_t dim,
@@ -368,6 +382,37 @@ int nfb_maf_inverse_backward(const nfb_resnet_ctx_desc_t* desc, int32_t features
                              void* workspace_dev, int64_t workspace_bytes, float* g_x_dev, float* g_context_dev,
                              float* const* g_w, float* const* g_b, float* const* g_w_context,
                              float* const* g_b_context, void* stream);
+
+/* Bytes of device scratch nfb_ar_rqs_sampling_backward needs for `rows` rows (-1: bad descriptor or shape). */
+int64_t nfb_ar_rqs_sampling_backward_workspace_bytes(const nfb_resnet_ctx_desc_t* desc, int32_t features,
+                                                     int32_t num_bins, int32_t num_derivatives, int64_t rows);
+/* Gradients of sum g_x . x + g_log_det . log_det through the sampling direction of an autoregressive spline layer
+ * (AutoregressiveRationalQuadraticSpline / CircularAutoregressiveRationalQuadraticSpline.forward,
+ * flows/affine/autoregressive.py:29-38): x solves x = G(z; MADE(pre(x), context)) with G the inverse spline on the
+ * records [rows, features, 2K + nd] of the MADE output and log_det = -sum log f'(x), computed by the reference with D
+ * sequential passes.  desc is the MADE (masks set, in_features = features, out_features = features (2K + nd), context
+ * through w_context).  The spline: num_bins K, num_derivatives nd = K - 1 with the scalar tail_bound (linear tails;
+ * tail_bound_dev and circular_dev NULL), or nd = K / K + 1 with tail_bound_dev [features] and circular_dev [features]
+ * as in nfb_rqs_spline_tails (tail_bound unused).  pre is PeriodicFeaturesElementwise given by its tables in the layout
+ * of nfb_periodic_features (pf_slot_dev NULL: pre is the identity).
+ * The MADE's activations are recomputed once at pre(x); the cotangent lam of x then follows
+ * lam = g_x + pre'(x) MADE_dgrad(pbar(lam)) for features - 1 data-gradient-only passes (exact: MADE's Jacobian is
+ * strictly lower triangular in its degree order), pbar(lam) the parameter gradient of the inverse-spline adjoint
+ * (nfb_rqs_spline(_tails)_inverse_backward), and one last pass forms g_z and the weight / context / periodic-feature
+ * gradients.  Equals the gradient of the reference's unrolled D-pass loop.  z, x [rows, features] (the layer's input and
+ * output), context [rows, context_features], g_x [rows, features] and g_log_det [rows] (either may be NULL: zero).
+ * Outputs, each optional and OVERWRITTEN: g_z, g_context, g_w / g_b / g_w_context / g_b_context in
+ * nfb_resnet_backward's slot order, g_pf_weights [n_periodic, 2] and g_pf_bias [n_periodic].  rows = 0: every
+ * gradient is zero. */
+int nfb_ar_rqs_sampling_backward(const nfb_resnet_ctx_desc_t* desc, int32_t features, int32_t num_bins,
+                                 int32_t num_derivatives, float tail_bound, const float* tail_bound_dev,
+                                 const int32_t* circular_dev, const int32_t* pf_slot_dev, const float* pf_weights_dev,
+                                 const float* pf_scale_dev, const float* pf_bias_dev, int32_t pf_n_periodic,
+                                 const float* z_dev, const float* x_dev, const float* context_dev, const float* g_x_dev,
+                                 const float* g_log_det_dev, int64_t rows, void* workspace_dev, int64_t workspace_bytes,
+                                 float* g_z_dev, float* g_context_dev, float* const* g_w, float* const* g_b,
+                                 float* const* g_w_context, float* const* g_b_context, float* g_pf_weights_dev,
+                                 float* g_pf_bias_dev, void* stream);
 
 /* flows/neural_spline/wrapper.py:186-244 AutoregressiveRationalQuadraticSpline */
 typedef struct {

@@ -1456,7 +1456,8 @@ int nfb_lipschitz_mlp_dual_backward(const nfb_lipschitz_mlp_desc_t* d, const flo
 // ---- training pass of the stand-alone layers (splines, conditioners called as modules, periodic features) ----
 static int spline_backward(const char* who, const float* x, const float* params, int64_t stride, const float* gy,
                            const float* gld, float* gx, float* gp, int64_t rows, int32_t feats, int32_t K, int32_t nd,
-                           const float* tail, const int32_t* circ, float tail0, float wh_scale, void* stream) {
+                           const float* tail, const int32_t* circ, float tail0, float wh_scale, void* stream,
+                           bool inverse = false) {
     NFB_CHECK(rows >= 0 && feats >= 0, NFB_ERR_ARG, "%s: negative size", who);
     NFB_CHECK(K >= 1 && K <= 32 && (nd == K - 1 || nd == K || nd == K + 1), NFB_ERR_ARG, "%s: bad bins / derivatives",
               who);
@@ -1464,6 +1465,9 @@ static int spline_backward(const char* who, const float* x, const float* params,
     NFB_CHECK(stride == 0 || stride == feats * P, NFB_ERR_ARG,
               "%s: params_row_stride must be 0 (shared table) or feats * (2 num_bins + num_derivatives)", who);
     NFB_CHECK(params && (rows == 0 || feats == 0 || x), NFB_ERR_ARG, "%s: null pointer", who);
+    if (inverse)
+        return launch_spline_inverse_adjoint(x, params, stride == 0, gy, nullptr, gld, rows, feats, K, nd, tail, circ,
+                                             tail0, wh_scale, gp, gx, S(stream));
     return launch_spline_adjoint(x, params, stride == 0, gy, gld, rows, feats, K, nd, tail, circ, tail0, wh_scale, gp, gx,
                                  S(stream));
 }
@@ -1482,6 +1486,24 @@ int nfb_rqs_spline_tails_backward(const float* x, const float* params, int64_t p
               "nfb_rqs_spline_tails_backward: %d derivative parameters for %d bins", num_derivatives, num_bins);
     return spline_backward("nfb_rqs_spline_tails_backward", x, params, params_row_stride, g_y, g_log_det, g_x, g_params,
                            rows, feats, num_bins, num_derivatives, tail_bound, circular, 0.f, wh_scale, stream);
+}
+int nfb_rqs_spline_inverse_backward(const float* z, const float* params, int64_t params_row_stride, const float* g_x,
+                                    const float* g_log_det, float* g_z, float* g_params, int64_t rows, int32_t feats,
+                                    int32_t num_bins, float tail_bound, float wh_scale, void* stream) {
+    return spline_backward("nfb_rqs_spline_inverse_backward", z, params, params_row_stride, g_x, g_log_det, g_z, g_params,
+                           rows, feats, num_bins, num_bins - 1, nullptr, nullptr, tail_bound, wh_scale, stream, true);
+}
+int nfb_rqs_spline_tails_inverse_backward(const float* z, const float* params, int64_t params_row_stride,
+                                          const float* g_x, const float* g_log_det, float* g_z, float* g_params,
+                                          int64_t rows, int32_t feats, int32_t num_bins, int32_t num_derivatives,
+                                          const float* tail_bound, const int32_t* circular, float wh_scale,
+                                          void* stream) {
+    NFB_CHECK(tail_bound && circular, NFB_ERR_ARG, "nfb_rqs_spline_tails_inverse_backward: null pointer");
+    NFB_CHECK(num_derivatives != num_bins - 1, NFB_ERR_ARG,
+              "nfb_rqs_spline_tails_inverse_backward: %d derivative parameters for %d bins", num_derivatives, num_bins);
+    return spline_backward("nfb_rqs_spline_tails_inverse_backward", z, params, params_row_stride, g_x, g_log_det, g_z,
+                           g_params, rows, feats, num_bins, num_derivatives, tail_bound, circular, 0.f, wh_scale, stream,
+                           true);
 }
 int nfb_periodic_features_backward(const float* x, const float* g_y, int64_t rows, int32_t dim, const int32_t* slot,
                                    const float* weights, const float* scale, int32_t n_periodic, float* g_x,
@@ -1829,6 +1851,102 @@ int nfb_maf_inverse_backward(const nfb_resnet_ctx_desc_t* d, int32_t features, c
     }
     NFB_TRY(launch_maf_affine_adjoint(x, P, g_y, g_log_det, features > 1 ? gin : nullptr, rows, features, pbar, g_x, st));
     return resnet_adjoint(r, context, pbar, false, nullptr, g_context, g_w, g_b, g_wc, g_bc, st);
+}
+
+namespace {
+// Scratch of nfb_ar_rqs_sampling_backward: the conditioner's (resnet_layout), then
+//   P    [rows, D, 2K + nd]  MADE(pre(x), context), the spline parameters at the layer's output
+//   pbar [rows, D, 2K + nd]  their cotangent
+//   gin  [rows, D]           data gradient of the latest fixed-point pass (through pre)
+//   gxin [rows, D]           MADE data gradient at pre(x)
+//   xin  [rows, D]           pre(x), the MADE's input (periodic features)
+int64_t ar_rqs_layout(const nfb_resnet_ctx_desc_t* d, int32_t features, int32_t K, int32_t nd, long long rows,
+                      char* base, float** P, float** pbar, float** gin, float** gxin, float** xin) {
+    const int64_t off0 = resnet_layout(d, rows, base, nullptr);
+    if (off0 < 0 || features < 1 || K < 1 || K > 32 || (nd != K - 1 && nd != K && nd != K + 1)) return -1;
+    size_t off = (size_t)off0;
+    auto take = [&](size_t floats) { float* p = base ? reinterpret_cast<float*>(base + off) : nullptr;
+                                     off += (floats * 4 + 255) / 256 * 256; return p; };
+    const size_t np = (size_t)rows * features * (2 * K + nd);
+    float* p = take(np); if (P) *P = p;
+    p = take(np); if (pbar) *pbar = p;
+    p = take((size_t)rows * features); if (gin) *gin = p;
+    p = take((size_t)rows * features); if (gxin) *gxin = p;
+    p = take((size_t)rows * features); if (xin) *xin = p;
+    return (int64_t)off;
+}
+}  // namespace
+
+int64_t nfb_ar_rqs_sampling_backward_workspace_bytes(const nfb_resnet_ctx_desc_t* d, int32_t features, int32_t num_bins,
+                                                     int32_t num_derivatives, int64_t rows) {
+    return ar_rqs_layout(d, features, num_bins, num_derivatives, rows, nullptr, nullptr, nullptr, nullptr, nullptr,
+                         nullptr);
+}
+
+int nfb_ar_rqs_sampling_backward(const nfb_resnet_ctx_desc_t* d, int32_t features, int32_t num_bins,
+                                 int32_t num_derivatives, float tail_bound, const float* tails, const int32_t* circular,
+                                 const int32_t* pf_slot, const float* pf_weights, const float* pf_scale,
+                                 const float* pf_bias, int32_t pf_n_periodic, const float* z, const float* x,
+                                 const float* context, const float* g_x, const float* g_log_det, int64_t rows,
+                                 void* workspace, int64_t workspace_bytes, float* g_z, float* g_context,
+                                 float* const* g_w, float* const* g_b, float* const* g_wc, float* const* g_bc,
+                                 float* g_pf_weights, float* g_pf_bias, void* stream) {
+    const char* who = "nfb_ar_rqs_sampling_backward";
+    const int D = features, K = num_bins, nd = num_derivatives, P = 2 * K + nd;
+    NFB_CHECK(d && d->net.m_initial, NFB_ERR_ARG, "%s: the descriptor must be a MADE (mask pointers set)", who);
+    NFB_CHECK(K >= 1 && K <= 32 && (nd == K - 1 || nd == K || nd == K + 1), NFB_ERR_ARG,
+              "%s: %d derivative parameters for %d bins", who, nd, K);
+    NFB_CHECK(D >= 1 && d->net.in_features == D && d->net.out_features == D * P, NFB_ERR_ARG,
+              "%s: a MADE of %d -> %d features does not parameterise %d features of %d spline parameters", who,
+              d->net.in_features, d->net.out_features, D, P);
+    NFB_CHECK(d->context_features == 0 || d->w_context, NFB_ERR_ARG, "%s: a MADE takes its context through w_context",
+              who);
+    NFB_CHECK(nd == K - 1 ? (!tails && !circular) : (tails && circular), NFB_ERR_ARG,
+              "%s: per-feature tail bounds and circular flags go with num_derivatives = K or K + 1, and only there", who);
+    const bool pf = pf_slot != nullptr;
+    NFB_CHECK(!pf || (pf_weights && pf_scale && pf_n_periodic >= 0), NFB_ERR_ARG, "%s: incomplete periodic tables", who);
+    NFB_TRY(resnet_validate(who, d, rows, x, context, z /* g_x and g_log_det may be NULL: zero */, workspace,
+                            workspace_bytes, nfb_ar_rqs_sampling_backward_workspace_bytes(d, D, K, nd, rows)));
+    cudaStream_t st = S(stream);
+    if (rows == 0) {
+        if (g_pf_weights) NFB_CUDA(cudaMemsetAsync(g_pf_weights, 0, (size_t)pf_n_periodic * 2 * 4, st));
+        if (g_pf_bias) NFB_CUDA(cudaMemsetAsync(g_pf_bias, 0, (size_t)pf_n_periodic * 4, st));
+        return resnet_zero_grads(d, g_w, g_b, g_wc, g_bc, st);
+    }
+    float *Pm = nullptr, *pbar = nullptr, *gin = nullptr, *gxin = nullptr, *xin = nullptr;
+    ar_rqs_layout(d, D, K, nd, rows, static_cast<char*>(workspace), &Pm, &pbar, &gin, &gxin, &xin);
+    // one recompute at pre(x), x the layer's output; its ReLU masks and gate logits serve every pass below
+    const float* in = x;
+    if (pf) {
+        NFB_TRY(launch_periodic_features(x, xin, rows, D, pf_slot, pf_weights, pf_scale, pf_bias, st));
+        in = xin;
+    }
+    ResnetPass r{};
+    r.d = d;
+    r.rows = rows;
+    NFB_TRY(resnet_recompute(r, in, context, workspace, st));
+    const int H = d->net.hidden_features, nb = d->net.num_blocks;
+    NFB_TRY(r.g(fwd_args(r.ws.h[nb], H, 0, r.wf, d->net.b_final, Pm, rows, D * P, H)));
+    auto spline = [&](const float* lam_in, float* gz) {   // pbar (and g_z) for lam = g_x + lam_in
+        return launch_spline_inverse_adjoint(z, Pm, 0, g_x, lam_in, g_log_det, rows, D, K, nd, tails, circular,
+                                             tail_bound, 1.f, pbar, gz, st);
+    };
+    // lam = g_x + pre'(x) MADE_dgrad(pbar(lam)), D - 1 times: exact, as MADE's Jacobian in x is strictly lower
+    // triangular (in the degree order)
+    for (int it = 0; it + 1 < D; ++it) {
+        NFB_TRY(spline(it ? gin : nullptr, nullptr));
+        NFB_TRY(resnet_adjoint(r, context, pbar, true, pf ? gxin : gin, nullptr, nullptr, nullptr, nullptr, nullptr, st));
+        if (pf)
+            NFB_TRY(launch_periodic_features_bwd(x, gxin, rows, D, pf_slot, pf_weights, pf_scale, pf_n_periodic, gin,
+                                                 nullptr, nullptr, st));
+    }
+    NFB_TRY(spline(D > 1 ? gin : nullptr, g_z));
+    const bool pf_grads = pf && (g_pf_weights || g_pf_bias);
+    NFB_TRY(resnet_adjoint(r, context, pbar, false, pf_grads ? gxin : nullptr, g_context, g_w, g_b, g_wc, g_bc, st));
+    if (pf_grads)
+        NFB_TRY(launch_periodic_features_bwd(x, gxin, rows, D, pf_slot, pf_weights, pf_scale, pf_n_periodic, nullptr,
+                                             g_pf_weights, g_pf_bias, st));
+    return NFB_OK;
 }
 
 namespace {

@@ -132,15 +132,28 @@ int launch_spline_bwd_shared(const float* xin, int ldx, const float* table, cons
     return NFB_OK;
 }
 
-// ---- stand-alone splines (nfb_rqs_spline / nfb_rqs_spline_tails, density direction) ----
+// ---- stand-alone splines (nfb_rqs_spline / nfb_rqs_spline_tails): density direction (rqs_adjoint_params) and, with
+// INV, the sampling direction (rqs_inverse_adjoint_params: x is then the spline's input z, gy the cotangent of its
+// output, gx receives g_z).  gin, when given, is added to gy (the fixed-point passes of nfb_ar_rqs_sampling_backward).
 // Per-row parameters: one thread per (row, feature) element, 256 consecutive elements per block; the block's
 // 256 x P parameter slab is contiguous: staged through shared memory with coalesced loads (P = 2K + nd), the gradient
 // slab written back the same way.  KT = 8: the templated fast path (K known at compile time); KT = 0: any K <= 32.
-template <int KT>
-__global__ void __launch_bounds__(256) spline_adjoint_rows_kernel(
+template <int KMAX, bool INV>
+__device__ __forceinline__ void spline_element(int K, int nd, bool circ, float x, const float* p, float wh_scale,
+                                               float tail, float gy, float gld, float& g, float* gp) {
+    float y, lad;
+    if (INV)
+        rqs_inverse_adjoint_params<KMAX, float>(K, nd, circ, x, p, wh_scale, tail, gy, gld, y, lad, g, gp);
+    else
+        rqs_adjoint_params<KMAX, float>(K, nd, circ, x, p, wh_scale, tail, gy, gld, y, lad, g, gp);
+}
+
+template <int KT, bool INV>
+__device__ __forceinline__ void spline_adjoint_rows_body(
     const float* __restrict__ x, const float* __restrict__ params, const float* __restrict__ gy,
-    const float* __restrict__ g_ld, long long rows, int feats, int K, int nd, const float* __restrict__ tail,
-    const int* __restrict__ circ, float tail0, float wh_scale, float* __restrict__ g_params, float* __restrict__ gx) {
+    const float* __restrict__ gin, const float* __restrict__ g_ld, long long rows, int feats, int K, int nd,
+    const float* __restrict__ tail, const int* __restrict__ circ, float tail0, float wh_scale,
+    float* __restrict__ g_params, float* __restrict__ gx) {
     constexpr int KMAX = KT ? KT : 32;
     if (KT) K = KT;
     extern __shared__ float sp[];
@@ -156,9 +169,10 @@ __global__ void __launch_bounds__(256) spline_adjoint_rows_kernel(
     if (e < n_el) {
         const long long row = e / feats;
         const int f = (int)(e - row * feats);
-        float y, lad, g;
-        rqs_adjoint_params<KMAX, float>(K, nd, circ ? circ[f] != 0 : false, x[e], sp + threadIdx.x * P, wh_scale,
-                                        tail ? tail[f] : tail0, gy ? gy[e] : 0.f, g_ld ? g_ld[row] : 0.f, y, lad, g, gp);
+        float g;
+        spline_element<KMAX, INV>(K, nd, circ ? circ[f] != 0 : false, x[e], sp + threadIdx.x * P, wh_scale,
+                                  tail ? tail[f] : tail0, (gy ? gy[e] : 0.f) + (gin ? gin[e] : 0.f),
+                                  g_ld ? g_ld[row] : 0.f, g, gp);
         if (gx) gx[e] = g;
     }
     __syncthreads();
@@ -174,11 +188,11 @@ __global__ void __launch_bounds__(256) spline_adjoint_rows_kernel(
 // One parameter table [feats][P] shared by every row (the unconditional CDF of the coupling layers): grid = (row
 // chunks, feats); each thread walks rows of its chunk for ONE feature and keeps P partial sums, block reduction, one
 // atomic per table entry and block (g_table zeroed by the caller).
-template <int KT>
-__global__ void __launch_bounds__(256) spline_adjoint_shared_kernel(
+template <int KT, bool INV>
+__device__ __forceinline__ void spline_adjoint_shared_body(
     const float* __restrict__ x, const float* __restrict__ table, const float* __restrict__ gy,
-    const float* __restrict__ g_ld, long long rows, long long rows_per_block, int feats, int K, int nd,
-    const float* __restrict__ tail, const int* __restrict__ circ, float tail0, float wh_scale,
+    const float* __restrict__ gin, const float* __restrict__ g_ld, long long rows, long long rows_per_block, int feats,
+    int K, int nd, const float* __restrict__ tail, const int* __restrict__ circ, float tail0, float wh_scale,
     float* __restrict__ g_table, float* __restrict__ gx) {
     constexpr int KMAX = KT ? KT : 32;
     if (KT) K = KT;
@@ -193,9 +207,9 @@ __global__ void __launch_bounds__(256) spline_adjoint_shared_kernel(
     const long long r1 = r0 + rows_per_block < rows ? r0 + rows_per_block : rows;
     for (long long row = r0 + threadIdx.x; row < r1; row += 256) {
         const long long e = row * feats + f;
-        float y, lad, g;
-        rqs_adjoint_params<KMAX, float>(K, nd, c, x[e], p, wh_scale, tb, gy ? gy[e] : 0.f, g_ld ? g_ld[row] : 0.f, y,
-                                        lad, g, gp);
+        float g;
+        spline_element<KMAX, INV>(K, nd, c, x[e], p, wh_scale, tb, (gy ? gy[e] : 0.f) + (gin ? gin[e] : 0.f),
+                                  g_ld ? g_ld[row] : 0.f, g, gp);
         if (gx) gx[e] = g;
         for (int k = 0; k < P; ++k) acc[k] += gp[k];
     }
@@ -213,9 +227,44 @@ __global__ void __launch_bounds__(256) spline_adjoint_shared_kernel(
         }
 }
 
-int launch_spline_adjoint(const float* x, const float* params, int shared, const float* gy, const float* g_ld,
-                          long long rows, int feats, int K, int nd, const float* tail, const int* circ, float tail0,
-                          float wh_scale, float* g_params, float* gx, cudaStream_t st) {
+#define NFB_SPLINE_ROWS_ARGS                                                                                         \
+    const float* __restrict__ x, const float* __restrict__ params, const float* __restrict__ gy,                     \
+        const float* __restrict__ gin, const float* __restrict__ g_ld, long long rows, int feats, int K, int nd,     \
+        const float* __restrict__ tail, const int* __restrict__ circ, float tail0, float wh_scale,                   \
+        float *__restrict__ g_params, float *__restrict__ gx
+#define NFB_SPLINE_SHARED_ARGS                                                                                       \
+    const float* __restrict__ x, const float* __restrict__ table, const float* __restrict__ gy,                      \
+        const float* __restrict__ gin, const float* __restrict__ g_ld, long long rows, long long rows_per_block,     \
+        int feats, int K, int nd, const float* __restrict__ tail, const int* __restrict__ circ, float tail0,         \
+        float wh_scale, float *__restrict__ g_table, float *__restrict__ gx
+template <int KT>
+__global__ void __launch_bounds__(256) spline_adjoint_rows_kernel(NFB_SPLINE_ROWS_ARGS) {
+    spline_adjoint_rows_body<KT, false>(x, params, gy, gin, g_ld, rows, feats, K, nd, tail, circ, tail0, wh_scale,
+                                        g_params, gx);
+}
+template <int KT>
+__global__ void __launch_bounds__(256) spline_inverse_adjoint_rows_kernel(NFB_SPLINE_ROWS_ARGS) {
+    spline_adjoint_rows_body<KT, true>(x, params, gy, gin, g_ld, rows, feats, K, nd, tail, circ, tail0, wh_scale,
+                                       g_params, gx);
+}
+template <int KT>
+__global__ void __launch_bounds__(256) spline_adjoint_shared_kernel(NFB_SPLINE_SHARED_ARGS) {
+    spline_adjoint_shared_body<KT, false>(x, table, gy, gin, g_ld, rows, rows_per_block, feats, K, nd, tail, circ,
+                                          tail0, wh_scale, g_table, gx);
+}
+template <int KT>
+__global__ void __launch_bounds__(256) spline_inverse_adjoint_shared_kernel(NFB_SPLINE_SHARED_ARGS) {
+    spline_adjoint_shared_body<KT, true>(x, table, gy, gin, g_ld, rows, rows_per_block, feats, K, nd, tail, circ,
+                                         tail0, wh_scale, g_table, gx);
+}
+#undef NFB_SPLINE_ROWS_ARGS
+#undef NFB_SPLINE_SHARED_ARGS
+
+namespace {
+template <bool INV>
+int spline_adjoint_launch(const float* x, const float* params, int shared, const float* gy, const float* gin,
+                          const float* g_ld, long long rows, int feats, int K, int nd, const float* tail, const int* circ,
+                          float tail0, float wh_scale, float* g_params, float* gx, cudaStream_t st) {
     NFB_CHECK(K >= 1 && K <= 32, NFB_ERR_ARG, "rqs backward: num_bins %d out of range [1,32]", K);
     NFB_CHECK(nd == K - 1 || nd == K || nd == K + 1, NFB_ERR_ARG, "rqs backward: %d derivative parameters for %d bins",
               nd, K);
@@ -223,39 +272,50 @@ int launch_spline_adjoint(const float* x, const float* params, int shared, const
     if (shared && g_params) NFB_CUDA(cudaMemsetAsync(g_params, 0, (size_t)feats * P * 4, st));
     if (rows == 0 || feats == 0) return NFB_OK;
     const bool fast = K == 8;
+    auto rows8 = INV ? spline_inverse_adjoint_rows_kernel<8> : spline_adjoint_rows_kernel<8>;
+    auto rows0 = INV ? spline_inverse_adjoint_rows_kernel<0> : spline_adjoint_rows_kernel<0>;
+    auto shared8 = INV ? spline_inverse_adjoint_shared_kernel<8> : spline_adjoint_shared_kernel<8>;
+    auto shared0 = INV ? spline_inverse_adjoint_shared_kernel<0> : spline_adjoint_shared_kernel<0>;
     if (!shared) {
         // dynamic shared memory up to the K = 32 tails-list slab (256 x 97 floats), set once per device
         static PerDevice per_dev;
         if (per_dev.ensure([] {
                 const int most = 256 * (3 * 32 + 1) * 4;
-                cudaError_t e = cudaFuncSetAttribute(spline_adjoint_rows_kernel<8>,
-                                                     cudaFuncAttributeMaxDynamicSharedMemorySize, most);
-                return e != cudaSuccess ? e : cudaFuncSetAttribute(spline_adjoint_rows_kernel<0>,
-                                                                   cudaFuncAttributeMaxDynamicSharedMemorySize, most);
+                auto r8 = INV ? spline_inverse_adjoint_rows_kernel<8> : spline_adjoint_rows_kernel<8>;
+                auto r0 = INV ? spline_inverse_adjoint_rows_kernel<0> : spline_adjoint_rows_kernel<0>;
+                cudaError_t e = cudaFuncSetAttribute(r8, cudaFuncAttributeMaxDynamicSharedMemorySize, most);
+                return e != cudaSuccess ? e : cudaFuncSetAttribute(r0, cudaFuncAttributeMaxDynamicSharedMemorySize, most);
             }) < 0)
             return NFB_ERR_CUDA;
         const long long n = rows * feats;
         const size_t smem = (size_t)256 * P * 4;
         const unsigned grid = (unsigned)((n + 255) / 256);
-        if (fast)
-            spline_adjoint_rows_kernel<8><<<grid, 256, smem, st>>>(x, params, gy, g_ld, rows, feats, K, nd, tail, circ,
-                                                                    tail0, wh_scale, g_params, gx);
-        else
-            spline_adjoint_rows_kernel<0><<<grid, 256, smem, st>>>(x, params, gy, g_ld, rows, feats, K, nd, tail, circ,
-                                                                    tail0, wh_scale, g_params, gx);
+        (fast ? rows8 : rows0)<<<grid, 256, smem, st>>>(x, params, gy, gin, g_ld, rows, feats, K, nd, tail, circ, tail0,
+                                                        wh_scale, g_params, gx);
     } else {
         const long long rpb = 2048;
         const dim3 grid((unsigned)((rows + rpb - 1) / rpb), (unsigned)feats);
         const size_t smem = (size_t)8 * P * 4;
-        if (fast)
-            spline_adjoint_shared_kernel<8><<<grid, 256, smem, st>>>(x, params, gy, g_ld, rows, rpb, feats, K, nd, tail,
-                                                                      circ, tail0, wh_scale, g_params, gx);
-        else
-            spline_adjoint_shared_kernel<0><<<grid, 256, smem, st>>>(x, params, gy, g_ld, rows, rpb, feats, K, nd, tail,
-                                                                      circ, tail0, wh_scale, g_params, gx);
+        (fast ? shared8 : shared0)<<<grid, 256, smem, st>>>(x, params, gy, gin, g_ld, rows, rpb, feats, K, nd, tail,
+                                                            circ, tail0, wh_scale, g_params, gx);
     }
     NFB_LAUNCH_CHECK();
     return NFB_OK;
+}
+}  // namespace
+
+int launch_spline_adjoint(const float* x, const float* params, int shared, const float* gy, const float* g_ld,
+                          long long rows, int feats, int K, int nd, const float* tail, const int* circ, float tail0,
+                          float wh_scale, float* g_params, float* gx, cudaStream_t st) {
+    return spline_adjoint_launch<false>(x, params, shared, gy, nullptr, g_ld, rows, feats, K, nd, tail, circ, tail0,
+                                        wh_scale, g_params, gx, st);
+}
+int launch_spline_inverse_adjoint(const float* z, const float* params, int shared, const float* gx, const float* gin,
+                                  const float* g_ld, long long rows, int feats, int K, int nd, const float* tail,
+                                  const int* circ, float tail0, float wh_scale, float* g_params, float* gz,
+                                  cudaStream_t st) {
+    return spline_adjoint_launch<true>(z, params, shared, gx, gin, g_ld, rows, feats, K, nd, tail, circ, tail0, wh_scale,
+                                       g_params, gz, st);
 }
 
 // Adjoint of PeriodicFeaturesElementwise (utils/nn.py:64-130; forward: nfb_kernels.cu periodic_features_kernel).

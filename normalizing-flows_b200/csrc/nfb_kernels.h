@@ -239,6 +239,11 @@ int launch_axpy(const float* x, float a, float* y, long long n, int accumulate, 
 int launch_spline_adjoint(const float* x, const float* params, int shared, const float* gy, const float* g_ld,
                           long long rows, int feats, int K, int nd, const float* tail, const int* circ, float tail0,
                           float wh_scale, float* g_params, float* gx, cudaStream_t st);
+// the inverse spline's adjoint (rqs_inverse_adjoint_params): z in, gx (+ gin, optional) the cotangent of its output
+int launch_spline_inverse_adjoint(const float* z, const float* params, int shared, const float* gx, const float* gin,
+                                  const float* g_ld, long long rows, int feats, int K, int nd, const float* tail,
+                                  const int* circ, float tail0, float wh_scale, float* g_params, float* gz,
+                                  cudaStream_t st);
 int launch_periodic_features_bwd(const float* x, const float* gy, long long rows, int dim, const int* slot,
                                  const float* w, const float* scale, int n_periodic, float* gx, float* g_w, float* g_b,
                                  cudaStream_t st);

@@ -112,6 +112,14 @@ SYMBOLS = {
     "nfb_maf_inverse_backward_workspace_bytes": (_I64, [C.POINTER(ResnetCtxDesc), _I32, _I64]),
     "nfb_maf_inverse_backward": (C.c_int, [C.POINTER(ResnetCtxDesc), _I32, _VP, _VP, _VP, _VP, _VP, _I64, _VP, _I64, _VP,
                                            _VP, C.POINTER(_VP), C.POINTER(_VP), C.POINTER(_VP), C.POINTER(_VP), _VP]),
+    "nfb_rqs_spline_inverse_backward": (C.c_int, [_VP, _VP, _I64, _VP, _VP, _VP, _VP, _I64, _I32, _I32, _F, _F, _VP]),
+    "nfb_rqs_spline_tails_inverse_backward": (C.c_int, [_VP, _VP, _I64, _VP, _VP, _VP, _VP, _I64, _I32, _I32, _I32, _VP,
+                                                        _VP, _F, _VP]),
+    "nfb_ar_rqs_sampling_backward_workspace_bytes": (_I64, [C.POINTER(ResnetCtxDesc), _I32, _I32, _I32, _I64]),
+    "nfb_ar_rqs_sampling_backward": (C.c_int, [C.POINTER(ResnetCtxDesc), _I32, _I32, _I32, _F, _VP, _VP, _VP, _VP, _VP,
+                                               _VP, _I32, _VP, _VP, _VP, _VP, _VP, _I64, _VP, _I64, _VP, _VP,
+                                               C.POINTER(_VP), C.POINTER(_VP), C.POINTER(_VP), C.POINTER(_VP), _VP, _VP,
+                                               _VP]),
     "nfb_mlp_backward_workspace_bytes": (_I64, [C.POINTER(MlpDesc), _I64]),
     "nfb_mlp_backward": (C.c_int, [C.POINTER(MlpDesc), _VP, _VP, _I64, _VP, _I64, _VP, C.POINTER(_VP), C.POINTER(_VP),
                                    _VP]),

@@ -7,7 +7,12 @@ A module that supports this defines
   `_adjoint(x, context, keep, grads, need_x, need_ctx)` -> (g_x, g_context, {parameter: gradient})
 and `apply_module` routes a call through `ModuleFn` when a gradient is wanted.  The backward is the C ABI's adjoints:
 nfb_rqs_spline(_tails)_backward -> nfb_resnet_backward / nfb_mlp_backward (one call per conditioner) ->
-nfb_periodic_features_backward."""
+nfb_periodic_features_backward.
+
+The sampling direction (`forward` of the autoregressive and coupling spline layers, which reverse_kld differentiates)
+goes the same way through `SamplingFn`: a module defines `_sampling_value(z, context, keep)` (its unchanged sampling
+code) and `_sampling_adjoint(z, x, context, keep, g_x, g_ld, need_z, need_ctx)`, built on the inverse-spline adjoints
+nfb_rqs_spline(_tails)_inverse_backward and the fixed-point adjoint nfb_ar_rqs_sampling_backward."""
 import ctypes as C
 
 import torch
@@ -66,6 +71,43 @@ def apply_module(module, x, context=None):
     return module._value(x, context, None)
 
 
+class SamplingFn(torch.autograd.Function):
+    """(x, log_det) = module._sampling_value(z, context): the layer's sampling code under no_grad, so values are
+    bit-identical with and without grad; the backward is the module's `_sampling_adjoint`.  Refuses to run the backward
+    if a parameter was modified in place after the forward."""
+
+    @staticmethod
+    def forward(ctx, module, z, context, *params):
+        keep = {}
+        x, ld = module._sampling_value(z, context, keep)
+        ctx.module, ctx.keep, ctx.params = module, keep, params
+        ctx.versions = [p._version for p in params]
+        ctx.save_for_backward(z, x, context)
+        return x, ld
+
+    @staticmethod
+    def backward(ctx, g_x, g_ld):
+        z, x, context = ctx.saved_tensors
+        if any(p._version != v for p, v in zip(ctx.params, ctx.versions)):
+            raise RuntimeError(f"{type(ctx.module).__name__} backward: a parameter was modified in place after the "
+                               "forward pass")
+        need_z, need_ctx = ctx.needs_input_grad[1], ctx.needs_input_grad[2]
+        gz, gctx, gmap = ctx.module._sampling_adjoint(z, x, context, ctx.keep,
+                                                      g_x.contiguous() if g_x is not None else None,
+                                                      g_ld.contiguous() if g_ld is not None else None, need_z, need_ctx)
+        return (None, gz if need_z else None, gctx if need_ctx else None,
+                *[gmap.get(p) if p.requires_grad else None for p in ctx.params])
+
+
+def apply_sampling(module, z, context=None):
+    z = require_cuda_f32(z)
+    if context is not None:
+        context = require_cuda_f32(context, "context")
+    if wants_grad(module, z, context):
+        return SamplingFn.apply(module, z, context, *module.parameters())
+    return module._sampling_value(z, context, None)
+
+
 # ---- element adjoints ------------------------------------------------------------------------------------------
 def spline_backward(x, params, shared, num_bins, gy, g_ld, wh_scale, tail_bound=None, num_derivatives=None,
                     tails=None, circular=None, want_params=True):
@@ -87,6 +129,29 @@ def spline_backward(x, params, shared, num_bins, gy, g_ld, wh_scale, tail_bound=
                                                           L.ptr(gx), L.ptr(gp), rows, feats, num_bins, nd, L.ptr(tails),
                                                           L.ptr(circular), C.c_float(wh_scale), L.stream_ptr()))
     return gx, gp
+
+
+def spline_inverse_backward(z, params, shared, num_bins, gx, g_ld, wh_scale, tail_bound=None, num_derivatives=None,
+                            tails=None, circular=None, need_z=True):
+    """(g_z | None, g_params) of the inverse spline x = g(z) (nfb_rqs_spline(_tails) with inverse = 1) through
+    nfb_rqs_spline(_tails)_inverse_backward; arguments as in spline_backward, gx the cotangent of x."""
+    rows, feats = z.shape
+    gz = torch.empty_like(z) if need_z else None
+    gp = torch.empty(params.shape, dtype=torch.float32, device=z.device)
+    stride = 0 if shared else feats * (2 * num_bins + (num_bins - 1 if num_derivatives is None else num_derivatives))
+    if rows == 0:
+        return gz, gp.zero_()
+    with torch.cuda.device(z.device):
+        if tails is None:
+            L.check(L.lib().nfb_rqs_spline_inverse_backward(L.ptr(z), L.ptr(params), stride, L.ptr(gx), L.ptr(g_ld),
+                                                            L.ptr(gz), L.ptr(gp), rows, feats, num_bins,
+                                                            C.c_float(tail_bound), C.c_float(wh_scale), L.stream_ptr()))
+        else:
+            L.check(L.lib().nfb_rqs_spline_tails_inverse_backward(L.ptr(z), L.ptr(params), stride, L.ptr(gx),
+                                                                  L.ptr(g_ld), L.ptr(gz), L.ptr(gp), rows, feats,
+                                                                  num_bins, num_derivatives, L.ptr(tails),
+                                                                  L.ptr(circular), C.c_float(wh_scale), L.stream_ptr()))
+    return gz, gp
 
 
 def _resnet_grad_call(net, masked, context):
@@ -150,6 +215,43 @@ def maf_inverse_backward(made, features, x, y, context, g_y, g_ld, need_x=True, 
                                              L.stream_ptr()))
     del keep
     return gx, gctx, gmap
+
+
+def ar_rqs_sampling_backward(made, features, num_bins, num_derivatives, tail_bound, tails, circular, z, x, context,
+                             g_x, g_ld, need_z=True, need_ctx=True):
+    """(g_z | None, g_context | None, {parameter: gradient}) of an autoregressive spline layer's sampling direction
+    x = forward(z, context) through nfb_ar_rqs_sampling_backward (the fixed-point adjoint of the D-pass loop; made = its
+    autoregressive_net, whose PeriodicFeaturesElementwise preprocessing, if any, is differentiated in the same call).
+    tails / circular None: linear tails with the scalar tail_bound."""
+    from .utils.nn import PeriodicFeaturesElementwise
+    d, keep, arrays, gmap = _resnet_grad_call(made, True, context)
+    rows = z.shape[0]
+    pre = made.preprocessing
+    if pre is not None and not isinstance(pre, PeriodicFeaturesElementwise):
+        raise NotImplementedError("the sampling backward of an autoregressive spline takes PeriodicFeaturesElementwise "
+                                  "as its only preprocessing")
+    slot = w = scale = bias = g_pw = g_pb = None
+    n_periodic = 0
+    if pre is not None:
+        slot, w, scale, bias = pre._tables(z.device)
+        n_periodic = len(pre.ind)
+        g_pw = _grad_like(pre.weights)
+        g_pb = _grad_like(pre.bias) if pre.apply_bias else None
+        gmap.update({p: g for p, g in ((pre.weights, g_pw), (getattr(pre, "bias", None), g_pb)) if g is not None})
+    gz = torch.empty_like(z) if need_z else None
+    gctx = torch.empty_like(context) if context is not None and need_ctx else None
+    lib = L.lib()
+    ws = _workspace(lib.nfb_ar_rqs_sampling_backward_workspace_bytes(C.byref(d), features, num_bins, num_derivatives,
+                                                                     rows), z.device)
+    with torch.cuda.device(z.device):
+        L.check(lib.nfb_ar_rqs_sampling_backward(C.byref(d), features, num_bins, num_derivatives,
+                                                 C.c_float(tail_bound if tails is None else 0.0), L.ptr(tails),
+                                                 L.ptr(circular), L.ptr(slot), L.ptr(w), L.ptr(scale), L.ptr(bias),
+                                                 n_periodic, L.ptr(z), L.ptr(x), L.ptr(context), L.ptr(g_x), L.ptr(g_ld),
+                                                 rows, L.ptr(ws), ws.numel(), L.ptr(gz), L.ptr(gctx), *arrays, L.ptr(g_pw),
+                                                 L.ptr(g_pb), L.stream_ptr()))
+    del keep
+    return gz, gctx, gmap
 
 
 def mlp_backward(mlp, x, g_out, need_x=True):

@@ -12,7 +12,7 @@ from torch import nn
 from . import _lib as L
 from ._image_autograd import wants_grad
 from ._native import FlowHandle
-from .distributions.base import DiagGaussian
+from .distributions.base import ConditionalDiagGaussian, DiagGaussian, UniformGaussian
 from .flows.base import NativeFlow
 
 
@@ -124,32 +124,53 @@ class NormalizingFlow(nn.Module):
         x, log_det = self.forward_and_log_det(z)
         return x, log_q - log_det
 
-    def _no_sampling_grad(self, what):
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
-            raise NotImplementedError(
-                f"{what}: gradients through the sampling direction are not on the CUDA path yet "
-                "(evaluate under torch.no_grad(); forward_kld / log_prob are differentiable)")
+    def _takes_layer_loop(self):
+        return self._stack() is None
+
+    def _no_sampling_grad(self, what, context=None):
+        """Gradients through the sampling direction exist when the stack runs layer by layer, every layer's sampling
+        direction is differentiable (the stand-alone spline layers, `_sampling_differentiable`) and the base's draw is
+        reparameterised (UniformGaussian, DiagGaussian, ConditionalDiagGaussian).  Otherwise, under grad, raise."""
+        if not (torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())):
+            return
+        if (isinstance(self.q0, (UniformGaussian, DiagGaussian, ConditionalDiagGaussian)) and self._takes_layer_loop()
+                and all(hasattr(f, "_sampling_differentiable") and f._sampling_differentiable(context)
+                        for f in self.flows)):
+            return
+        raise NotImplementedError(
+            f"{what}: gradients through the sampling direction are not on the CUDA path yet "
+            "(evaluate under torch.no_grad(); forward_kld / log_prob are differentiable)")
+
+    def _log_q_no_param_grad(self, z, **context):
+        """log q(z) by the density pass with the parameters' requires_grad switched off and back on, as the reference
+        does (core.py:121-129, 149-157, 356-364): under grad, z's gradient flows, the parameters' does not."""
+        from .utils import set_requires_grad
+        set_requires_grad(self, False)
+        log_q = self.log_prob(z, **context)
+        set_requires_grad(self, True)
+        return log_q
 
     def reverse_kld(self, num_samples=1, beta=1.0, score_fn=True):
         """core.py:104-131.  z ~ q0 pushed through every layer's `.forward` (one persistent launch for coupling
         stacks), log_q = log q0(z0) - sum log_det; `score_fn=False` re-evaluates log_q by the density pass of the
-        drawn samples (the reference does the same with parameter gradients switched off)."""
+        drawn samples with parameter gradients switched off, like the reference.  Differentiable for the stacks
+        _no_sampling_grad admits (the stand-alone spline layers on a reparameterised base)."""
         self._no_sampling_grad("reverse_kld")
         z, log_q = self.sample(num_samples)
         if not score_fn:
-            log_q = self.log_prob(z)
+            log_q = self._log_q_no_param_grad(z)
         log_p = self.p.log_prob(z)
         return torch.mean(log_q) - beta * torch.mean(log_p)
 
     def reverse_alpha_div(self, num_samples=1, alpha=1, dreg=False):
-        """core.py:133-165 (value; see reverse_kld for the gradient caveat)."""
+        """core.py:133-165 (differentiable for the stacks reverse_kld is)."""
         import numpy as np
         self._no_sampling_grad("reverse_alpha_div")
         z, log_q = self.sample(num_samples)
         log_p = self.p.log_prob(z)
         if dreg:
             w_const = torch.exp(log_p - log_q).detach()
-            log_q = self.log_prob(z)
+            log_q = self._log_q_no_param_grad(z)
             w = torch.exp(log_p - log_q)
             w_alpha = w_const ** alpha
             w_alpha = w_alpha / torch.mean(w_alpha)
@@ -222,11 +243,15 @@ class ConditionalNormalizingFlow(NormalizingFlow):
     def forward_kld(self, x, context=None):
         return -torch.mean(self.log_prob(x, context=context))
 
+    def _takes_layer_loop(self):
+        return True   # every call above walks the layers
+
     def reverse_kld(self, num_samples=1, context=None, beta=1.0, score_fn=True):
-        self._no_sampling_grad("reverse_kld")
+        """core.py:337-366; differentiable when every layer's sampling direction is (see NormalizingFlow)."""
+        self._no_sampling_grad("reverse_kld", context)
         z, log_q = self.sample(num_samples, context=context)
         if not score_fn:
-            log_q = self.log_prob(z, context=context)
+            log_q = self._log_q_no_param_grad(z, context=context)
         log_p = self.p.log_prob(z, context=context)
         return torch.mean(log_q) - beta * torch.mean(log_p)
 

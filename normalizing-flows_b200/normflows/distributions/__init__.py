@@ -1,2 +1,3 @@
-from .base import BaseDistribution, DiagGaussian, ClassCondDiagGaussian, ConditionalDiagGaussian, GlowBase
-from .target import TwoMoons
+from .base import (BaseDistribution, DiagGaussian, ClassCondDiagGaussian, ConditionalDiagGaussian, GlowBase,
+                   UniformGaussian)
+from .target import Target, TwoMoons

@@ -61,6 +61,50 @@ class DiagGaussian(BaseDistribution):
         return gaussian_table_log_prob(z, self.loc.reshape(self.d, 1), ls.reshape(self.d, 1), None, 1)
 
 
+class UniformGaussian(BaseDistribution):
+    """Uniform on the features `ind` (width scale[ind], centred at 0), Gaussian with standard deviation scale on the
+    others (reference: distributions/base.py:198-270); the base of examples/paper_example_nsf.ipynb.  Same buffers
+    (`ind`, `ind_`, `inv_perm`, `scale`).  Sampling is torch RNG, reparameterised like DiagGaussian.forward; the density is
+    the diagonal-Gaussian kernel on the Gaussian columns plus the uniform part's constant.  Like the reference it does
+    not check the uniform support."""
+
+    def __init__(self, ndim, ind, scale=None):
+        super().__init__()
+        self.ndim = ndim
+        if isinstance(ind, int):
+            ind = [ind]
+        if torch.is_tensor(ind):
+            self.register_buffer("ind", ind.long())
+        else:
+            self.register_buffer("ind", torch.tensor(ind, dtype=torch.long))
+        uniform = set(self.ind.tolist())
+        self.register_buffer("ind_", torch.tensor([i for i in range(ndim) if i not in uniform], dtype=torch.long))
+        perm_ = torch.cat((self.ind, self.ind_))
+        inv_perm_ = torch.zeros_like(perm_)
+        inv_perm_[perm_] = torch.arange(ndim)
+        self.register_buffer("inv_perm", inv_perm_)
+        self.register_buffer("scale", torch.ones(ndim) if scale is None else scale)
+
+    def forward(self, num_samples=1, context=None):
+        z = self.sample(num_samples)
+        return z, self.log_prob(z)
+
+    def sample(self, num_samples=1, context=None):
+        eps_u = torch.rand((num_samples, len(self.ind)), dtype=self.scale.dtype, device=self.scale.device) - 0.5
+        eps_g = torch.randn((num_samples, len(self.ind_)), dtype=self.scale.dtype, device=self.scale.device)
+        z = torch.cat((eps_u, eps_g), -1)
+        return self.scale * z[..., self.inv_perm]
+
+    def log_prob(self, z, context=None):
+        z = require_cuda_f32(z)
+        const = -torch.sum(torch.log(self.scale[self.ind]))
+        if len(self.ind_) == 0:
+            return const.expand(z.shape[0]).to(torch.float32)
+        zg = z[:, self.ind_].contiguous()
+        ls = torch.log(self.scale[self.ind_]).float().reshape(-1, 1)
+        return gaussian_table_log_prob(zg, torch.zeros_like(ls), ls, None, 1) + const
+
+
 class ClassCondDiagGaussian(BaseDistribution):
     """Class-conditional diagonal Gaussian (reference: distributions/base.py:281-344); `log_prob(z, y)` with
     integer labels runs in csrc/nfb_glow.cu."""

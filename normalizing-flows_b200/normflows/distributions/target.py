@@ -1,8 +1,37 @@
-"""Synthetic 2-D target used to generate benchmark/test inputs (reference:
-normflows/distributions/target.py:99-129 TwoMoons; rejection sampler :34-73)."""
+"""Targets (reference: normflows/distributions/target.py): the Target base class that user targets subclass
+(:8-73), and the synthetic 2-D TwoMoons used to generate benchmark/test inputs (:99-129)."""
 import numpy as np
 import torch
 from torch import nn
+
+
+class Target(nn.Module):
+    """Base class of sample target distributions (reference: distributions/target.py:8-73): `prop_scale` / `prop_shift`
+    buffers of the uniform proposal, rejection sampling against exp(log_prob - max_log_prob).  A subclass sets
+    `n_dims` and `max_log_prob` and implements `log_prob` (e.g. examples/paper_example_nsf.ipynb's GaussianVonMises)."""
+
+    def __init__(self, prop_scale=torch.tensor(6.0), prop_shift=torch.tensor(-3.0)):
+        super().__init__()
+        self.register_buffer("prop_scale", prop_scale)
+        self.register_buffer("prop_shift", prop_shift)
+
+    def log_prob(self, z):
+        raise NotImplementedError("The log probability is not implemented yet.")
+
+    def rejection_sampling(self, num_steps=1):
+        eps = torch.rand((num_steps, self.n_dims), dtype=self.prop_scale.dtype, device=self.prop_scale.device)
+        z_ = self.prop_scale * eps + self.prop_shift
+        prob = torch.rand(num_steps, dtype=self.prop_scale.dtype, device=self.prop_scale.device)
+        prob_ = torch.exp(self.log_prob(z_) - self.max_log_prob)
+        return z_[prob_ > prob, :]
+
+    def sample(self, num_samples=1):
+        z = torch.zeros((0, self.n_dims), dtype=self.prop_scale.dtype, device=self.prop_scale.device)
+        while len(z) < num_samples:
+            z_ = self.rejection_sampling(num_samples)
+            ind = np.min([len(z_), num_samples - len(z)])
+            z = torch.cat([z, z_[:ind, :]], 0)
+        return z
 
 
 class TwoMoons(nn.Module):

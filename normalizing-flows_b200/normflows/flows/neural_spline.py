@@ -6,7 +6,8 @@ Module trees mirror the reference so `state_dict()` keys match:
   CoupledRationalQuadraticSpline.prqct.{identity_features,transform_features,transform_net,
                                         unconditional_transform.unnormalized_*}
 NOTE the wrappers swap directions (wrapper.py:79-85,238-244): `inverse()` is the density direction
-(one conditioner pass), `forward()` is sampling (D passes for the autoregressive layer)."""
+(one conditioner pass), `forward()` is sampling (D passes for the autoregressive layer).  The stand-alone layers (the
+context-conditioned and circular ones) are differentiable in both directions (_standalone.ModuleFn / SamplingFn)."""
 import ctypes as C
 
 import numpy as np
@@ -61,18 +62,30 @@ class AutoregressiveRationalQuadraticSpline(NativeFlow):
     # Context-conditioned layer (ConditionalNormalizingFlow, core.py:216-366): the conditioner takes the context through
     # the MADE's context layers + GLU gates, so it runs as stand-alone tensor-core GEMMs (nets.MADE.forward) and the
     # spline as the stand-alone HBM-bound kernel (csrc/nfb_kernels.cu rqs_rows_kernel) instead of the fused block.
-    # The density direction trains through _standalone.ModuleFn (_value / _adjoint below).
+    # The density direction trains through _standalone.ModuleFn (_value / _adjoint below), the sampling direction
+    # through _standalone.SamplingFn (_sampling_value / _sampling_adjoint: the fixed-point adjoint of the D-pass loop).
     def _conditional(self, z, context, sampling):
-        from .._native import require_cuda_f32, rqs_spline
-        from .._standalone import apply_module
+        from .._standalone import apply_module, apply_sampling
         if not sampling:  # wrapper.inverse -> Autoregressive.forward: one pass (affine/autoregressive.py:24-27)
             return apply_module(self, z, context)
-        z = require_cuda_f32(z)
+        return apply_sampling(self, z, context)
+
+    def _sampling_value(self, z, context, keep):
+        from .._native import rqs_spline
         net = self.mprqat.autoregressive_net
         out, ld = torch.zeros_like(z), None  # D passes (:29-38)
         for _ in range(self.features):
             out, ld = rqs_spline(z, net._value(out, context, None), self.num_bins, self.tail_bound, 1.0, True)
         return out, ld
+
+    def _sampling_adjoint(self, z, x, context, keep, g_x, g_ld, need_z, need_ctx):
+        from .._standalone import ar_rqs_sampling_backward
+        return ar_rqs_sampling_backward(self.mprqat.autoregressive_net, self.features, self.num_bins, self.num_bins - 1,
+                                        self.tail_bound, None, None, z, x, context, g_x, g_ld, need_z, need_ctx)
+
+    def _sampling_differentiable(self, context=None):
+        """The stand-alone (context) path is differentiable in the sampling direction; the fused path is not."""
+        return self.num_context_channels is not None or context is not None
 
     def _value(self, z, context, keep):
         from .._native import rqs_spline
@@ -165,17 +178,31 @@ class CoupledRationalQuadraticSpline(NativeFlow):
     def _conditional(self, z, context, sampling):
         """Context-conditioned coupling layer outside the fused block (see AutoregressiveRationalQuadraticSpline):
         Coupling.forward / .inverse of neural_spline/coupling.py:71-128 with the unconditional CDF of :221-253."""
-        from .._native import require_cuda_f32, rqs_spline
-        from .._standalone import apply_module
+        from .._standalone import apply_module, apply_sampling
         if not sampling:
             return apply_module(self, z, context)
-        z = require_cuda_f32(z)
+        return apply_sampling(self, z, context)
+
+    def _sampling_value(self, z, context, keep):
+        from .._native import rqs_spline
         p, k = self.prqct, self.num_bins
         ident, trans = z[:, p.identity_features].contiguous(), z[:, p.transform_features].contiguous()
         wh = 1.0 / float(np.sqrt(p.transform_net.hidden_features))
         yi, ldi = rqs_spline(ident, _uncond_rows(p.unconditional_transform, z.shape[0]), k, self.tail_bound, 1.0, True)
-        yt, ld = rqs_spline(trans, p.transform_net._value(yi, context, None), k, self.tail_bound, wh, True)
+        params = p.transform_net._value(yi, context, None)
+        if keep is not None:
+            keep["params"], keep["yi"] = params, yi
+        yt, ld = rqs_spline(trans, params, k, self.tail_bound, wh, True)
         return _merge(z, p, yi, yt), ld + ldi
+
+    def _sampling_adjoint(self, z, x, context, keep, g_x, g_ld, need_z, need_ctx):
+        from .._standalone import spline_inverse_backward
+        spline = lambda zz, params, shared, wh, gx, gld: spline_inverse_backward(
+            zz, params, shared, self.num_bins, gx, gld, wh, tail_bound=self.tail_bound, need_z=need_z)
+        return _coupling_sampling_adjoint(self.prqct, z, context, keep, g_x, g_ld, spline, need_z, need_ctx)
+
+    def _sampling_differentiable(self, context=None):
+        return self.num_context_channels is not None or context is not None
 
     def _value(self, z, context, keep):
         from .._native import rqs_spline
@@ -264,6 +291,35 @@ def _coupling_adjoint(p, z, context, params, grads, spline, need_ctx):
     return gz, g_ctx, gmap
 
 
+def _coupling_sampling_adjoint(p, z, context, keep, g_out, g_ld, spline, need_z, need_ctx):
+    """Backward of a coupling layer's sampling pass (Coupling.inverse, neural_spline/coupling.py:100-128): the inverse
+    unconditional CDF gives yi on the identity features, the conditioner reads yi, the inverse spline maps the transform
+    features.  Transform features: inverse-spline adjoint; then the conditioner's backward at yi (periodic features
+    included); identity features: the unconditional CDF's inverse adjoint on g_yi = g_out[idf] + the conditioner's data
+    gradient.  spline(z, params, shared, wh_scale, g_x, g_log_det) -> (g_z | None, g_params)."""
+    from .._standalone import conditioner_backward
+    idf, trf = p.identity_features, p.transform_features
+    if g_out is None:
+        g_out = torch.zeros_like(z)
+    ident, trans = z[:, idf].contiguous(), z[:, trf].contiguous()
+    u = p.unconditional_transform
+    k = u.unnormalized_widths.shape[1]
+    table = torch.cat([u.unnormalized_widths, u.unnormalized_heights, u.unnormalized_derivatives], dim=1).contiguous()
+    wh = 1.0 / float(np.sqrt(p.transform_net.hidden_features))
+    g_tr, g_params = spline(trans, keep["params"], False, wh, g_out[:, trf].contiguous(), g_ld)
+    g_net, g_ctx, gmap = conditioner_backward(p.transform_net, False, keep["yi"], context, g_params, need_ctx=need_ctx)
+    g_id, g_table = spline(ident, table, True, 1.0, (g_out[:, idf] + g_net).contiguous(), g_ld)
+    gz = None
+    if need_z:
+        gz = torch.empty_like(z)
+        gz[:, idf] = g_id
+        gz[:, trf] = g_tr
+    gmap[u.unnormalized_widths] = g_table[:, :k]
+    gmap[u.unnormalized_heights] = g_table[:, k:2 * k]
+    gmap[u.unnormalized_derivatives] = g_table[:, 2 * k:]
+    return gz, g_ctx, gmap
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # Circular variants (reference: flows/neural_spline/wrapper.py:88-183, 247-311): `tails` is a per-feature list, so every
 # knot has a derivative parameter (3K+1 per feature; utils/splines.py:48-57) and the bound may differ per feature.
@@ -337,19 +393,38 @@ class CircularCoupledRationalQuadraticSpline(Flow):
                 _tail_tensors(self._tail_bound, p.transform_features, self.ind_circ, self.features, device))
 
     def _run(self, z, context, sampling):
-        from .._native import require_cuda_f32, rqs_spline_tails
-        from .._standalone import apply_module
+        from .._standalone import apply_module, apply_sampling
         if not sampling:   # Coupling.forward (coupling.py:71-98)
             return apply_module(self, z, context)
-        z = require_cuda_f32(z)   # Coupling.inverse (:100-128)
+        return apply_sampling(self, z, context)   # Coupling.inverse (:100-128)
+
+    def _sampling_value(self, z, context, keep):
+        from .._native import rqs_spline_tails
         p, k = self.prqct, self.num_bins
         (tb_id, c_id), (tb_tr, c_tr) = self._tails(p, z.device)
         ident, trans = z[:, p.identity_features].contiguous(), z[:, p.transform_features].contiguous()
         wh = 1.0 / float(np.sqrt(p.transform_net.hidden_features))
         yi, ldi = rqs_spline_tails(ident, _uncond_rows(p.unconditional_transform, z.shape[0]), k, k + 1, tb_id, c_id,
                                    1.0, True)
-        yt, ld = rqs_spline_tails(trans, p.transform_net._value(yi, context, None), k, k + 1, tb_tr, c_tr, wh, True)
+        params = p.transform_net._value(yi, context, None)
+        if keep is not None:
+            keep["params"], keep["yi"] = params, yi
+        yt, ld = rqs_spline_tails(trans, params, k, k + 1, tb_tr, c_tr, wh, True)
         return _merge(z, p, yi, yt), ld + ldi
+
+    def _sampling_adjoint(self, z, x, context, keep, g_x, g_ld, need_z, need_ctx):
+        from .._standalone import spline_inverse_backward
+        p, k = self.prqct, self.num_bins
+        (tb_id, c_id), (tb_tr, c_tr) = self._tails(p, z.device)
+
+        def spline(zz, params, shared, wh, gx, gld):
+            tb, circ = (tb_id, c_id) if shared else (tb_tr, c_tr)
+            return spline_inverse_backward(zz, params, shared, k, gx, gld, wh, num_derivatives=k + 1, tails=tb,
+                                           circular=circ, need_z=need_z)
+        return _coupling_sampling_adjoint(p, z, context, keep, g_x, g_ld, spline, need_z, need_ctx)
+
+    def _sampling_differentiable(self, context=None):
+        return True
 
     def _value(self, z, context, keep):
         from .._native import rqs_spline_tails
@@ -403,17 +478,29 @@ class CircularAutoregressiveRationalQuadraticSpline(Flow):
             self.mprqat.register_buffer("tail_bound", tail_bound)    # neural_spline/autoregressive.py:82-83
 
     def _run(self, z, context, sampling):
-        from .._native import require_cuda_f32, rqs_spline_tails
-        from .._standalone import apply_module
+        from .._standalone import apply_module, apply_sampling
         if not sampling:   # one MADE pass (affine/autoregressive.py:24-27)
             return apply_module(self, z, context)
-        z = require_cuda_f32(z)
+        return apply_sampling(self, z, context)
+
+    def _sampling_value(self, z, context, keep):
+        from .._native import rqs_spline_tails
         k, net = self.num_bins, self.mprqat.autoregressive_net
         tb, circ = _tail_tensors(self._tail_bound, range(self.features), self.ind_circ, self.features, z.device)
         out, ld = torch.zeros_like(z), None   # D passes (:29-38)
         for _ in range(self.features):
             out, ld = rqs_spline_tails(z, net._value(out, context, None), k, k + 1, tb, circ, 1.0, True)
         return out, ld
+
+    def _sampling_adjoint(self, z, x, context, keep, g_x, g_ld, need_z, need_ctx):
+        from .._standalone import ar_rqs_sampling_backward
+        k = self.num_bins
+        tb, circ = _tail_tensors(self._tail_bound, range(self.features), self.ind_circ, self.features, z.device)
+        return ar_rqs_sampling_backward(self.mprqat.autoregressive_net, self.features, k, k + 1, 0.0, tb, circ, z, x,
+                                        context, g_x, g_ld, need_z, need_ctx)
+
+    def _sampling_differentiable(self, context=None):
+        return True
 
     def _value(self, z, context, keep):   # MADE has no hidden_features: no 1/sqrt(H)
         from .._native import rqs_spline_tails

@@ -4,18 +4,22 @@
          Adam(lr 3e-4, weight decay 1e-5), batch 128 (the notebook's) and 65 536
     b    the same with CoupledRationalQuadraticSpline
     circ examples/circular_nsf.ipynb: 20 x CircularAutoregressiveRationalQuadraticSpline(2, 1, 128, [1],
-         tail_bound=[5, pi], permute_mask=True) on DiagGaussian(2) (the notebook's UniformGaussian is not a package class),
+         tail_bound=[5, pi], permute_mask=True) on DiagGaussian(2) (the notebook trains it on UniformGaussian),
          Adam(lr 1e-4, weight decay 1e-4), batch 1 024
     maf  examples/conditional_flow.ipynb's third model: 4 x [MaskedAffineAutoregressive(2, 128, context_features=4,
          num_blocks=2), LULinearPermute(2)] on DiagGaussian(2, trainable=False), Adam(lr 1e-3, weight decay 1e-5),
          batch 128 (the notebook's) and 65 536
     maf16 4 x [MaskedAffineAutoregressive(16, 256, num_blocks=2), LULinearPermute(16)] on DiagGaussian(16), no context,
          Adam(lr 1e-3, weight decay 1e-5), batch 65 536: the D - 1 adjoint passes of each MAF layer dominate
+    paper examples/paper_example_nsf.ipynb: 12 x CircularAutoregressiveRationalQuadraticSpline(2, 1, 512, [1],
+         num_bins=10, tail_bound=[5, pi], permute_mask=True) on UniformGaussian(2, [1], [1, 2 pi]) with the GaussianVonMises
+         target; the step is `reverse_kld(2**14)` + `backward()` + Adam(lr 5e-4), the notebook's (reverse KL: gradients
+         through the sampling direction)
 Prints one JSON line: ms/step (median of CUDA-event-timed steps after warm-up), samples/s, kernel launches per step
 (torch.profiler, one separate step), peak device memory, and the card's name, power limit and SM clock read in the same
 run.  When the unmodified reference is installed under oracle/_ref, the same model, seed and batch are timed through it
 (eager torch, fp32).
-    python tools/bench_conditional_train.py [--steps 20] [--warmup 5] [--no-reference]
+    python tools/bench_conditional_train.py [--steps 20] [--warmup 5] [--no-reference] [--cases paper,maf]
 """
 import argparse
 import json
@@ -28,7 +32,7 @@ REF_DIR = os.path.join(ROOT, "oracle", "_ref")
 
 
 CASES = [("a", 128), ("a", 65536), ("b", 128), ("b", 65536), ("circ", 1024), ("maf", 128), ("maf", 65536),
-         ("maf16", 65536)]
+         ("maf16", 65536), ("paper", 16384)]
 NOTEBOOK_LAYERS = 4   # examples/conditional_flow.ipynb: K = 4 (spline + LU) pairs
 
 
@@ -37,6 +41,21 @@ def build(nf, kind):
     import math
     import torch
     torch.manual_seed(0)
+    if kind == "paper":
+        class GaussianVonMises(nf.distributions.Target):   # the notebook's target
+            def __init__(self):
+                super().__init__(prop_scale=torch.tensor(2 * math.pi), prop_shift=torch.tensor(-math.pi))
+                self.n_dims = 2
+                self.max_log_prob = -1.99
+                self.log_const = -1.5 * math.log(2 * math.pi) - math.log(1.2660658777520082)   # np.i0(1)
+
+            def log_prob(self, x):
+                return -0.5 * x[:, 0] ** 2 + torch.cos(x[:, 1] - 3 * x[:, 0]) + self.log_const
+        base = nf.distributions.UniformGaussian(2, [1], torch.tensor([1., 2 * math.pi]))
+        flows = [nf.flows.CircularAutoregressiveRationalQuadraticSpline(2, 1, 512, [1], num_bins=10,
+                                                                        tail_bound=torch.tensor([5., math.pi]),
+                                                                        permute_mask=True) for _ in range(12)]
+        return nf.NormalizingFlow(base, flows, GaussianVonMises()), (5e-4, 0.0), 2, False
     if kind == "circ":
         flows = [nf.flows.CircularAutoregressiveRationalQuadraticSpline(2, 1, 128, [1], tail_bound=torch.tensor([5., math.pi]),
                                                                         permute_mask=True) for _ in range(20)]
@@ -80,7 +99,10 @@ def time_arm(arm, kind, batch, steps, warmup):
 
     def step():
         opt.zero_grad(set_to_none=True)
-        loss = model.forward_kld(x) if ctx is None else model.forward_kld(x, ctx)
+        if kind == "paper":
+            loss = model.reverse_kld(batch)
+        else:
+            loss = model.forward_kld(x) if ctx is None else model.forward_kld(x, ctx)
         loss.backward()
         opt.step()
         return loss
@@ -130,10 +152,12 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--no-reference", action="store_true")
+    ap.add_argument("--cases", help="comma-separated model names (default: all)")
     ap.add_argument("--arm", choices=["native", "reference"], help=argparse.SUPPRESS)
     a = ap.parse_args()
     if a.arm:   # one arm in its own process (the two packages share the name `normflows`)
-        print(json.dumps([time_arm(a.arm, k, b, a.steps, a.warmup) for k, b in CASES]))
+        want = set(a.cases.split(",")) if a.cases else None
+        print(json.dumps([time_arm(a.arm, k, b, a.steps, a.warmup) for k, b in CASES if want is None or k in want]))
         return
     import torch
     if not torch.cuda.is_available():
@@ -143,6 +167,8 @@ def main():
     res = {}
     for arm in arms:
         cmd = [sys.executable, os.path.abspath(__file__), "--arm", arm, "--steps", str(a.steps), "--warmup", str(a.warmup)]
+        if a.cases:
+            cmd += ["--cases", a.cases]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode:
             res[arm] = {"error": r.stderr.strip().splitlines()[-1] if r.stderr.strip() else f"exit {r.returncode}"}
