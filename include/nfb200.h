@@ -526,14 +526,31 @@ int nfb_flow_forward_kld(nfb_flow_t* f, const float* x_dev, int64_t rows, float*
  *   spline block : weight, bias of initial_layer; of blocks[i].linear_layers[0], [1] ...; of final_layer; then (coupled
  *                  only) unconditional_transform.unnormalized_widths, _heights, _derivatives
  *   LULinearPermute : lower_entries, upper_entries, unconstrained_upper_diag, bias
+ *   MaskedAffineFlow : net.<i>.weight, .bias of every Linear of s, then of t (an absent net has none)
+ *   AffineConstFlow / ActNorm : s, t       AffineCouplingBlock : param_map's Linears       Permute : none
  *   base (last two slots) : loc, log_scale
  * `grad_slots[i]` is a device buffer of nfb_flow_grad_slot_numel(f, i) floats that is OVERWRITTEN, or NULL to skip.
- * nfb_flow_num_grad_slots returns -1 when the flow holds a layer kind without a native backward. */
+ * nfb_flow_num_grad_slots returns -1 when the flow holds a layer kind without a native backward.  The affine family's
+ * slots serve nfb_flow_sampling_backward only: nfb_flow_log_prob_backward rejects affine groups (NFB_ERR_UNSUPPORTED). */
 int nfb_flow_num_grad_slots(const nfb_flow_t* f);
 int64_t nfb_flow_grad_slot_numel(const nfb_flow_t* f, int32_t slot);
 int nfb_flow_log_prob_backward(nfb_flow_t* f, const float* x_dev, const float* g_logq_dev, int64_t rows,
                                float* log_q_dev /* optional out */, float* gx_dev /* optional out */,
                                float* const* grad_slots, void* stream);
+
+/* ---- sampling-direction backward of an all-affine stack (reverse_kld / reverse_alpha_div of examples/real_nvp.ipynb)
+ * Gradients of sum_r <g_x[r], x_r> + g_ld[r] log_det_r, with (x, log_det) = nfb_flow_transform(f, NFB_FORWARD, z),
+ * w.r.t. z and every parameter, for stacks of MaskedAffineFlow, AffineConstFlow / ActNorm, AffineCouplingBlock and
+ * Permute only (any other layer: NFB_ERR_UNSUPPORTED).  z is the input that nfb_flow_transform was given.  The call
+ * recomputes the stack from z (the forward kernel's own arithmetic), walks the ops in reverse in one kernel, then reduces
+ * every Linear's weight and bias gradient in a fixed order (no atomics: two calls give identical bits).  Rows run in
+ * chunks, so the workspace (nfb_flow_sampling_backward_workspace_bytes, -1 for an unsupported stack) stays below a fixed
+ * bound; the number of launches does not depend on the number of layers.
+ * g_x / g_ld may be NULL (zero cotangent); g_z and individual slots may be NULL (not wanted).  grad_slots holds the
+ * layers' slots in nfb_flow_grad_slot_numel order (a base's two slots, if any, are not read); rows = 0 writes zeros. */
+int64_t nfb_flow_sampling_backward_workspace_bytes(const nfb_flow_t* f, int64_t rows);
+int nfb_flow_sampling_backward(nfb_flow_t* f, const float* z, const float* g_x, const float* g_ld, int64_t rows,
+                               void* ws, int64_t ws_bytes, float* g_z, float* const* grad_slots, void* stream);
 
 /* ---- host-buffer entry points (what a non-CUDA caller binds; copies are inside) ---- */
 int nfb_flow_log_prob_host(nfb_flow_t* f, const float* x_host, float* log_q_host, int64_t rows);

@@ -199,7 +199,16 @@ struct Layer {
 };
 
 enum GroupKind { G_FUSED_PAIR, G_FUSED, G_AFFINE, G_SINGLE };
-struct Group { GroupKind kind; int first, last; DevBuf ops; };
+struct Group {
+    GroupKind kind; int first, last; DevBuf ops;
+    // affine group, sampling-direction backward: workspace plan (units per row), per-op unit table and the weight
+    // reduction's items (output pointers filled per call)
+    bool bwd_planned = false;
+    int units = 0;
+    long long n_elem = 0;
+    DevBuf bops;
+    std::vector<AffRedItem> items;
+};
 
 }  // namespace
 
@@ -235,7 +244,14 @@ struct nfb_flow {
     DevBuf tr_store, tr_h, tr_P, tr_gP, tr_ga, tr_gb, tr_xp, tr_gxp, tr_zp, tr_gzp, tr_in, tr_gin, tr_g0, tr_g1, tr_small,
         tr_glq, tr_t0, tr_t1, tr_wpack;
     const int* cur_in_ready = nullptr;
+    // affine sampling backward: the reduction items with this call's gradient pointers, staged through pinned memory
+    AffRedItem* afb_host = nullptr;
+    size_t afb_cap = 0;
+    cudaEvent_t afb_ev = nullptr;
+    DevBuf afb_items;
     ~nfb_flow() {
+        if (afb_ev) cudaEventDestroy(afb_ev);
+        if (afb_host) cudaFreeHost(afb_host);
         if (copy_stream) cudaStreamDestroy(copy_stream);
         if (ev_reset) cudaEventDestroy(ev_reset);
         if (ev_copied) cudaEventDestroy(ev_copied);
@@ -971,6 +987,7 @@ bool is_affine_kind(const Layer& L) {
 int copy_mlp(const nfb_mlp_desc_t& d, AffMlp& m, float* slope) {
     NFB_CHECK(d.num_layers >= 0 && d.num_layers <= kAffMaxLayers, NFB_ERR_UNSUPPORTED, "MLP: %d layers > %d", d.num_layers, kAffMaxLayers);
     m.n_layers = d.num_layers;
+    if (d.num_layers == 0) return NFB_OK;   // absent net (MaskedAffineFlow with s or t = None)
     for (int i = 0; i <= d.num_layers; ++i) {
         NFB_CHECK(d.sizes[i] >= 1 && d.sizes[i] <= kAffMaxW, NFB_ERR_UNSUPPORTED, "MLP: layer width %d > %d", d.sizes[i], kAffMaxW);
         m.sizes[i] = d.sizes[i];
@@ -2098,7 +2115,8 @@ int nfb_flow_add_masked_affine(nfb_flow_t* f, const nfb_masked_affine_desc_t* d)
     NFB_CHECK(d->b, NFB_ERR_ARG, "MaskedAffineFlow: null mask");
     L->op.type = kOpMasked; L->op.p0 = d->b; L->op.slope = 0.f;
     NFB_TRY(copy_mlp(d->s, L->op.s, &L->op.slope));
-    NFB_TRY(copy_mlp(d->t, L->op.t, &L->op.slope));
+    L->op.slope_t = 0.f;
+    NFB_TRY(copy_mlp(d->t, L->op.t, &L->op.slope_t));
     if (d->s.num_layers) NFB_CHECK(d->s.sizes[0] == f->D && d->s.sizes[d->s.num_layers] == f->D, NFB_ERR_ARG, "s-net must map D -> D");
     if (d->t.num_layers) NFB_CHECK(d->t.sizes[0] == f->D && d->t.sizes[d->t.num_layers] == f->D, NFB_ERR_ARG, "t-net must map D -> D");
     f->layers.push_back(std::move(L));
@@ -2556,11 +2574,24 @@ int grad_slots_of(const Layer& L) {
     case L_AR_RQS: return 4 + 4 * L.net.nb;
     case L_COUPLED_RQS: return 4 + 4 * L.net.nb + 3;
     case L_LU: return 4;
+    // affine family, in each layer's parameter registration order: MaskedAffineFlow s then t (weight, bias per Linear),
+    // AffineConstFlow s, t, AffineCouplingBlock param_map, Permute none
+    case L_MASKED_AFFINE: return 2 * (L.op.s.n_layers + L.op.t.n_layers);
+    case L_AFFINE_CONST: return 2;
+    case L_AFFINE_COUPLING: return 2 * L.op.s.n_layers;
+    case L_PERMUTE: return 0;
     default: return -1;
     }
 }
 long long grad_slot_numel(const Layer& L, int s) {
     const NetDesc& n = L.net;
+    if (L.kind == L_AFFINE_CONST) return L.D;
+    if (L.kind == L_MASKED_AFFINE || L.kind == L_AFFINE_COUPLING) {
+        const bool t_net = L.kind == L_MASKED_AFFINE && s >= 2 * L.op.s.n_layers;
+        const AffMlp& m = t_net ? L.op.t : L.op.s;
+        const int k = t_net ? s - 2 * L.op.s.n_layers : s, l = k / 2;
+        return (k & 1) ? m.sizes[l + 1] : (long long)m.sizes[l + 1] * m.sizes[l];
+    }
     if (L.kind == L_LU) {
         const long long d = L.D;
         return s == 0 ? d * (d - 1) / 2 : s == 1 ? d * (d - 1) / 2 : d;
@@ -2794,6 +2825,8 @@ int nfb_flow_log_prob_backward(nfb_flow_t* f, const float* x, const float* g_log
     NFB_CHECK(x && g_logq && grad_slots, NFB_ERR_ARG, "null pointer");
     const int n_slots = nfb_flow_num_grad_slots(f);
     NFB_CHECK(n_slots >= 0, NFB_ERR_UNSUPPORTED, "native backward covers spline blocks + LULinearPermute + DiagGaussian");
+    for (auto& grp : f->groups)   // (the affine family has slots for its sampling-direction backward only)
+        NFB_CHECK(grp.kind != G_AFFINE, NFB_ERR_UNSUPPORTED, "native backward: affine-family group");
     if (rows == 0) return NFB_OK;
     cudaStream_t st = S(stream);
     const int D = f->D;
@@ -2876,6 +2909,139 @@ int nfb_flow_log_prob_backward(nfb_flow_t* f, const float* x, const float* g_log
         }
     }
     if (gx_out) NFB_CUDA(cudaMemcpyAsync(gx_out, g, ZS * 4, cudaMemcpyDeviceToDevice, st));
+    return NFB_OK;
+}
+
+}  // extern "C"
+
+// ==========================================================================================
+// sampling-direction backward of an all-affine stack (affine_stack_kernel with direction = 1)
+// ==========================================================================================
+namespace {
+
+constexpr long long kAffBwdWsCap = 256ll << 20;   // workspace bound: rows are processed in chunks below it
+
+// units per row of the workspace, each op's unit table and the weight reduction's items, in grad-slot order
+int plan_affine_bwd(nfb_flow* f, Group& g) {
+    if (g.bwd_planned) return NFB_OK;
+    std::vector<AffBwdOp> bops;
+    g.items.clear();
+    int u = 0;
+    long long e = 0;
+    auto add_net = [&](const AffMlp& m, AffBwdOp& bo, int n) {
+        for (int l = 0; l < m.n_layers; ++l) {
+            bo.u_act[n][l] = u; u += m.sizes[l];
+            bo.u_del[n][l] = u; u += m.sizes[l + 1];
+            g.items.push_back(AffRedItem{bo.u_act[n][l], bo.u_del[n][l], m.sizes[l], m.sizes[l + 1], e, nullptr, nullptr});
+            e += (long long)m.sizes[l + 1] * (m.sizes[l] + 1);
+        }
+    };
+    for (int k = g.first; k <= g.last; ++k) {
+        const Layer& L = *f->layers[k];
+        AffBwdOp bo{};
+        bo.u_z = u; u += f->D;
+        if (L.kind == L_MASKED_AFFINE) {
+            add_net(L.op.s, bo, 0);
+            add_net(L.op.t, bo, 1);
+        } else if (L.kind == L_AFFINE_COUPLING) {
+            add_net(L.op.s, bo, 0);
+        } else if (L.kind == L_AFFINE_CONST) {
+            for (int n = 0; n < 2; ++n) {
+                bo.u_del[n][0] = u; u += f->D;
+                g.items.push_back(AffRedItem{-1, bo.u_del[n][0], 0, f->D, e, nullptr, nullptr});
+                e += f->D;
+            }
+        }
+        bops.push_back(bo);
+    }
+    NFB_TRY(g.bops.upload(bops));
+    g.units = u;
+    g.n_elem = e;
+    g.bwd_planned = true;
+    return NFB_OK;
+}
+
+long long affine_bwd_chunk_rows(const Group& g, long long rows) {
+    const long long per_row = 4ll * g.units + (4 * g.n_elem + kAffSegRows - 1) / kAffSegRows + 1;
+    long long R = std::max(1ll, kAffBwdWsCap / per_row);
+    if (R > kAffSegRows) R -= R % kAffSegRows;
+    return std::max(1ll, std::min(R, rows));
+}
+
+size_t affine_bwd_ws_bytes(const Group& g, long long R) {
+    const size_t data = ((size_t)g.units * R * 4 + 255) & ~(size_t)255;
+    return data + (size_t)((R + kAffSegRows - 1) / kAffSegRows) * g.n_elem * 4;
+}
+
+int affine_only_group(nfb_flow* f, Group** out) {
+    NFB_CHECK(f && f->finalized, NFB_ERR_STATE, "flow not finalized");
+    NFB_CHECK(f->groups.size() == 1 && f->groups[0].kind == G_AFFINE, NFB_ERR_UNSUPPORTED,
+              "sampling backward: the stack must be affine-family layers only");
+    *out = &f->groups[0];
+    return plan_affine_bwd(f, **out);
+}
+
+}  // namespace
+
+extern "C" {
+
+int64_t nfb_flow_sampling_backward_workspace_bytes(const nfb_flow_t* fc, int64_t rows) {
+    nfb_flow* f = const_cast<nfb_flow*>(fc);
+    Group* g = nullptr;
+    if (rows < 0 || affine_only_group(f, &g) != NFB_OK) return -1;
+    return (int64_t)affine_bwd_ws_bytes(*g, affine_bwd_chunk_rows(*g, rows));
+}
+
+int nfb_flow_sampling_backward(nfb_flow_t* f, const float* z, const float* g_x, const float* g_ld, int64_t rows,
+                               void* ws, int64_t ws_bytes, float* g_z, float* const* grad_slots, void* stream) {
+    Group* gp = nullptr;
+    NFB_TRY(affine_only_group(f, &gp));
+    Group& g = *gp;
+    NFB_CHECK(rows >= 0, NFB_ERR_ARG, "rows < 0");
+    NFB_CHECK(rows == 0 || z, NFB_ERR_ARG, "null z");
+    const long long R = affine_bwd_chunk_rows(g, rows);
+    NFB_CHECK(ws && ws_bytes >= (int64_t)affine_bwd_ws_bytes(g, R), NFB_ERR_ARG,
+              "sampling backward: workspace of %lld bytes, %lld needed", (long long)ws_bytes,
+              (long long)affine_bwd_ws_bytes(g, R));
+    cudaStream_t st = S(stream);
+    f->launches = 0;
+    const int n_items = (int)g.items.size();
+    if (n_items) {
+        // this call's output pointers, in slot order (a Linear takes two slots, a column sum one)
+        if (!f->afb_ev) NFB_CUDA(cudaEventCreateWithFlags(&f->afb_ev, cudaEventDisableTiming));
+        else NFB_CUDA(cudaEventSynchronize(f->afb_ev));   // the previous call's staging copy has been read
+        if (f->afb_cap < (size_t)n_items) {
+            if (f->afb_host) cudaFreeHost(f->afb_host);
+            f->afb_host = nullptr; f->afb_cap = 0;
+            NFB_CUDA(cudaMallocHost(reinterpret_cast<void**>(&f->afb_host), n_items * sizeof(AffRedItem)));
+            f->afb_cap = n_items;
+        }
+        int s = 0;
+        for (int i = 0; i < n_items; ++i) {
+            AffRedItem it = g.items[i];
+            if (it.n_in > 0) { it.dw = grad_slots ? grad_slots[s] : nullptr; it.db = grad_slots ? grad_slots[s + 1] : nullptr; s += 2; }
+            else { it.db = grad_slots ? grad_slots[s] : nullptr; s += 1; }
+            f->afb_host[i] = it;
+        }
+        NFB_TRY(f->afb_items.reserve(n_items * sizeof(AffRedItem)));
+        NFB_CUDA(cudaMemcpyAsync(f->afb_items.p, f->afb_host, n_items * sizeof(AffRedItem), cudaMemcpyHostToDevice, st));
+        NFB_CUDA(cudaEventRecord(f->afb_ev, st));
+    }
+    const int D = f->D, n_ops = g.last - g.first + 1;
+    float* W = static_cast<float*>(ws);
+    float* partial = reinterpret_cast<float*>(static_cast<char*>(ws) + (((size_t)g.units * R * 4 + 255) & ~(size_t)255));
+    if (rows == 0) {   // zero parameter gradients
+        NFB_TRY(launch_affine_bwd_reduce(f->afb_items.p, n_items, g.n_elem, W, 0, partial, 0, st));
+        f->launches += g.n_elem ? 1 : 0;
+        return NFB_OK;
+    }
+    for (long long r0 = 0; r0 < rows; r0 += R) {
+        const long long n = std::min(R, (long long)rows - r0);
+        NFB_TRY(launch_affine_bwd_rows(g.ops.p, g.bops.p, n_ops, z + r0 * D, g_x ? g_x + r0 * D : nullptr,
+                                       g_ld ? g_ld + r0 : nullptr, g_z ? g_z + r0 * D : nullptr, W, n, D, st));
+        NFB_TRY(launch_affine_bwd_reduce(f->afb_items.p, n_items, g.n_elem, W, n, partial, r0 > 0, st));
+        f->launches += 1 + (g.n_elem ? 2 : 0);
+    }
     return NFB_OK;
 }
 

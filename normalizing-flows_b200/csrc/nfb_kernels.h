@@ -138,8 +138,8 @@ enum { kOpMasked = 0, kOpConst = 1, kOpCoupling = 2, kOpPermute = 3 };
 struct AffineOp {
     int type;
     int flags;      // coupling: bit0 scale, bits1-2 scale_map (0 exp,1 sigmoid,2 sigmoid_inv), bit3 channel_inv
-    float slope;    // LeakyReLU slope of the MLPs
-    int pad_;
+    float slope;    // LeakyReLU slope of the MLPs (masked: of the s-net)
+    float slope_t;  // masked: LeakyReLU slope of the t-net
     AffMlp s;       // masked: s-net ; coupling: param_map
     AffMlp t;       // masked: t-net
     const float* p0;  // masked: b[D] ; const: s[D]
@@ -151,6 +151,25 @@ struct AffineOp {
 size_t affine_op_size();
 int launch_affine_stack(const void* ops_dev, int n_ops, const float* zin, float* zout, float* logq,
                         long long rows, int d, int accumulate, int direction, cudaStream_t st);
+
+// sampling-direction backward of the affine stack.  The workspace of a chunk of R rows is a list of "units", each R
+// floats (one value per row): unit u of row r lives at ws[u * R + r].
+struct AffBwdOp {
+    int u_z;                       // D units: the op's input row
+    int u_act[2][kAffMaxLayers];   // net n (0 = s / param_map, 1 = t), Linear l: n_in units of its input activations
+    int u_del[2][kAffMaxLayers];   // ... n_out units: pre-activations, overwritten by the output cotangents
+};                                 // (const op: u_del[0][0] / u_del[1][0] hold the per-row g_s / g_t contributions)
+struct AffRedItem {                // one Linear's (dW, db) or, with n_in = 0, one column sum
+    int u_act, u_del, n_in, n_out;
+    long long e_off;               // first element in the flat element list: n_out * n_in weights, then n_out biases
+    float* dw;
+    float* db;
+};
+constexpr int kAffSegRows = 1024;  // rows per partial sum of the weight reduction
+int launch_affine_bwd_rows(const void* ops_dev, const void* bops_dev, int n_ops, const float* zin, const float* gx,
+                           const float* gld, float* gz, float* ws, long long R, int d, cudaStream_t st);
+int launch_affine_bwd_reduce(const void* items_dev, int n_items, long long n_elem, const float* ws, long long R,
+                             float* partial, int accumulate, cudaStream_t st);
 
 // ---- fused neural-spline block (nfb_fused_rqs.cu) ----
 constexpr int kFusedTileRows = 64;          // rows of a work unit (the M of one wgmma)

@@ -108,6 +108,72 @@ def apply_sampling(module, z, context=None):
     return module._sampling_value(z, context, None)
 
 
+def affine_slot_tensors(layers):
+    """The tensors behind the gradient slots of an affine-family stack (include/nfb200.h nfb_flow_grad_slot_numel):
+    each layer's parameters in registration order; an AffineConstFlow s / t registered as a buffer keeps its slot."""
+    from .flows import affine, mixing
+    out = []
+    for layer in layers:
+        if isinstance(layer, affine.MaskedAffineFlow):
+            for net in (layer.s, layer.t):
+                if net is not None:
+                    out += [p for lin in net.linear_layers() for p in (lin.weight, lin.bias)]
+        elif isinstance(layer, affine.AffineConstFlow):
+            out += [layer.s, layer.t]
+        elif isinstance(layer, affine.AffineCouplingBlock):
+            out += [p for lin in layer.flows[1].param_map.linear_layers() for p in (lin.weight, lin.bias)]
+        elif not isinstance(layer, mixing.Permute):
+            raise NotImplementedError(f"{type(layer).__name__} is not in the affine family")
+    return out
+
+
+class AffineSamplingFn(torch.autograd.Function):
+    """(x, log_det) = handle.transform(NFB_FORWARD, z) of an all-affine stack (MaskedAffineFlow, AffineConstFlow /
+    ActNorm, AffineCouplingBlock, Permute): the unchanged one-launch forward, so values are bit-identical with and
+    without grad.  The backward is one nfb_flow_sampling_backward call (recompute + reverse walk, then a fixed-order
+    weight reduction).  Refuses to run the backward if a parameter was modified in place after the forward."""
+
+    @staticmethod
+    def forward(ctx, handle, layers, z, *params):
+        x, ld = handle.transform(L.NFB_FORWARD, z)
+        ctx.handle, ctx.layers, ctx.params = handle, layers, params
+        ctx.versions = [p._version for p in params]
+        ctx.save_for_backward(require_cuda_f32(z))
+        return x, ld
+
+    @staticmethod
+    def backward(ctx, g_x, g_ld):
+        (z,) = ctx.saved_tensors
+        if any(p._version != v for p, v in zip(ctx.params, ctx.versions)):
+            names = "+".join(sorted({type(l).__name__ for l in ctx.layers}))
+            raise RuntimeError(f"{names} backward: a parameter was modified in place after the forward pass")
+        slots = affine_slot_tensors(ctx.layers)
+        bufs = [torch.empty_like(p) if isinstance(p, torch.nn.Parameter) and p.requires_grad else None for p in slots]
+        need_z = ctx.needs_input_grad[2]
+        gz = torch.empty_like(z) if need_z else None
+        g_x = g_x.to(torch.float32).contiguous() if g_x is not None else None
+        g_ld = g_ld.to(torch.float32).contiguous() if g_ld is not None else None
+        lib = L.lib()
+        h = ctx.handle.ensure(z.shape[1], z.device)
+        if lib.nfb_flow_num_grad_slots(h) < len(slots):
+            raise RuntimeError("affine sampling backward: gradient slot mismatch")
+        ws = _workspace(lib.nfb_flow_sampling_backward_workspace_bytes(h, z.shape[0]), z.device)
+        arr = _vp(bufs)
+        with torch.cuda.device(z.device):
+            L.check(lib.nfb_flow_sampling_backward(h, L.ptr(z), L.ptr(g_x), L.ptr(g_ld), z.shape[0], L.ptr(ws),
+                                                   ws.numel(), L.ptr(gz), C.cast(arr, C.POINTER(C.c_void_p)),
+                                                   L.stream_ptr()))
+        gmap = {}   # a parameter behind several slots (a net or layer used twice) gets the sum, as autograd would give
+        for p, b in zip(slots, bufs):
+            if b is not None:
+                gmap[id(p)] = gmap[id(p)] + b if id(p) in gmap else b
+        return (None, None, gz, *[gmap.get(id(p)) if p.requires_grad else None for p in ctx.params])
+
+
+def affine_sampling(handle, layers, z, params):
+    return AffineSamplingFn.apply(handle, list(layers), z, *params)
+
+
 # ---- element adjoints ------------------------------------------------------------------------------------------
 def spline_backward(x, params, shared, num_bins, gy, g_ld, wh_scale, tail_bound=None, num_derivatives=None,
                     tails=None, circular=None, want_params=True):

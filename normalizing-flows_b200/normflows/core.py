@@ -79,6 +79,9 @@ class NormalizingFlow(nn.Module):
         h = self._stack()
         self._run_pending_inits(z, inverse=False)
         if h is not None and z.dim() == 2:
+            if self._all_affine() and wants_grad(self.flows, z):   # one launch forward, one native backward
+                from ._standalone import affine_sampling
+                return affine_sampling(h, self.flows, z, list(self.flows.parameters()))
             return h.transform(L.NFB_FORWARD, z)
         log_det = torch.zeros(len(z), device=z.device)
         for flow in self.flows:
@@ -127,13 +130,20 @@ class NormalizingFlow(nn.Module):
     def _takes_layer_loop(self):
         return self._stack() is None
 
+    def _all_affine(self):
+        """Every layer is in the affine family (MaskedAffineFlow, AffineConstFlow / ActNorm, AffineCouplingBlock,
+        Permute): the all-native stack's sampling direction has a native backward (nfb_flow_sampling_backward)."""
+        return len(self.flows) > 0 and all(getattr(f, "_affine_family", False) for f in self.flows)
+
     def _no_sampling_grad(self, what, context=None):
-        """Gradients through the sampling direction exist when the stack runs layer by layer, every layer's sampling
-        direction is differentiable (the stand-alone spline layers, `_sampling_differentiable`) and the base's draw is
-        reparameterised (UniformGaussian, DiagGaussian, ConditionalDiagGaussian).  Otherwise, under grad, raise."""
+        """Gradients through the sampling direction exist when every layer's sampling direction is differentiable (the
+        stand-alone spline layers and the affine family, `_sampling_differentiable`), the stack runs layer by layer or is
+        all affine-family, and the base's draw is reparameterised (UniformGaussian, DiagGaussian,
+        ConditionalDiagGaussian).  Otherwise, under grad, raise."""
         if not (torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())):
             return
-        if (isinstance(self.q0, (UniformGaussian, DiagGaussian, ConditionalDiagGaussian)) and self._takes_layer_loop()
+        if (isinstance(self.q0, (UniformGaussian, DiagGaussian, ConditionalDiagGaussian))
+                and (self._takes_layer_loop() or self._all_affine())
                 and all(hasattr(f, "_sampling_differentiable") and f._sampling_differentiable(context)
                         for f in self.flows)):
             return
@@ -154,7 +164,7 @@ class NormalizingFlow(nn.Module):
         """core.py:104-131.  z ~ q0 pushed through every layer's `.forward` (one persistent launch for coupling
         stacks), log_q = log q0(z0) - sum log_det; `score_fn=False` re-evaluates log_q by the density pass of the
         drawn samples with parameter gradients switched off, like the reference.  Differentiable for the stacks
-        _no_sampling_grad admits (the stand-alone spline layers on a reparameterised base)."""
+        _no_sampling_grad admits (the stand-alone spline layers or the affine family on a reparameterised base)."""
         self._no_sampling_grad("reverse_kld")
         z, log_q = self.sample(num_samples)
         if not score_fn:

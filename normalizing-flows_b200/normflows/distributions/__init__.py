@@ -1,3 +1,4 @@
 from .base import (BaseDistribution, DiagGaussian, ClassCondDiagGaussian, ConditionalDiagGaussian, GlowBase,
                    UniformGaussian)
-from .target import Target, TwoMoons
+from .prior import TwoModes
+from .target import Target, TwoIndependent, TwoMoons

@@ -1,5 +1,5 @@
 """Targets (reference: normflows/distributions/target.py): the Target base class that user targets subclass
-(:8-73), and the synthetic 2-D TwoMoons used to generate benchmark/test inputs (:99-129)."""
+(:8-73), and the synthetic 2-D TwoMoons used to generate benchmark/test inputs (:99-129), and TwoIndependent (:76-96)."""
 import numpy as np
 import torch
 from torch import nn
@@ -32,6 +32,25 @@ class Target(nn.Module):
             ind = np.min([len(z_), num_samples - len(z)])
             z = torch.cat([z, z_[:ind, :]], 0)
         return z
+
+
+class TwoIndependent(Target):
+    """Two independent targets of equal size side by side (reference: distributions/target.py:76-96), the augmented
+    target of examples/augmented_flow.ipynb: log p(z) = log p1(z1) + log p2(z2) with z1, z2 = z.chunk(2, dim=1).  Both
+    targets are sub-modules (`target1`, `target2`), so a DiagGaussian target's loc / log_scale are parameters of a model
+    that holds this as `p`, and its state_dict keys are the reference's."""
+
+    def __init__(self, target1, target2):
+        super().__init__()
+        self.target1 = target1
+        self.target2 = target2
+
+    def log_prob(self, z):
+        z1, z2 = z.chunk(2, dim=1)
+        return self.target1.log_prob(z1) + self.target2.log_prob(z2)
+
+    def sample(self, num_samples=1):
+        return torch.cat([self.target1.sample(num_samples), self.target2.sample(num_samples)], 1)
 
 
 class TwoMoons(nn.Module):

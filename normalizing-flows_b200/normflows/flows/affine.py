@@ -13,6 +13,8 @@ from .base import Flow, NativeFlow
 
 
 class AffineConstFlow(NativeFlow):
+    _affine_family = True
+
     def __init__(self, shape, scale=True, shift=True):
         super().__init__()
         if isinstance(shape, int):
@@ -111,6 +113,8 @@ class ActNorm(AffineConstFlow):
 
 
 class MaskedAffineFlow(NativeFlow):
+    _affine_family = True
+
     def __init__(self, b, t=None, s=None):
         super().__init__()
         self.register_buffer("b", b.view(1, *b.size()).float())
@@ -164,6 +168,8 @@ _MAPS = {"exp": 0, "sigmoid": 1, "sigmoid_inv": 2}   # scale-map enum of the cou
 
 
 class AffineCouplingBlock(NativeFlow):
+    _affine_family = True
+
     def __init__(self, param_map, scale=True, scale_map="exp", split_mode="channel"):
         super().__init__()
         if scale_map not in _MAPS:

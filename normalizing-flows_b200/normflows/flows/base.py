@@ -23,6 +23,7 @@ class NativeFlow(Flow):
     (append this layer's descriptor to an nfb_flow)."""
 
     use_tensor_cores = True  # class-wide switch; False forces the plain-fp32 kernels (A/B parity)
+    _affine_family = False   # True: the sampling direction has a native backward (nfb_flow_sampling_backward)
 
     def _single(self):
         h = self.__dict__.get("_nfb_single")
@@ -33,11 +34,17 @@ class NativeFlow(Flow):
 
     def forward(self, z, context=None):
         # (layers without context parameters ignore the context, like the reference's `context=None` signatures)
+        if self._affine_family and wants_grad(self, z):
+            from .._standalone import affine_sampling
+            return affine_sampling(self._single(), [self], z, list(self.parameters()))
         return self._single().layer_apply(0, L.NFB_FORWARD, z)
+
+    def _sampling_differentiable(self, context=None):
+        return self._affine_family
 
     def inverse(self, z, context=None):
         # under autograd (a layer called on its own, e.g. between the blocks of a stack that is not all native) the call
-        # joins the graph; the sampling direction (`forward`) stays value-only
+        # joins the graph; the sampling direction (`forward`) does too for the affine family
         if wants_grad(self, z):
             from .._autograd import LayerInverseFn
             return LayerInverseFn.apply(self, z, *self.parameters())

@@ -62,6 +62,8 @@ class LULinearPermute(NativeFlow):
 
 
 class Permute(NativeFlow):
+    _affine_family = True
+
     def __init__(self, num_channels, mode="shuffle"):
         super().__init__()
         if mode not in ("shuffle", "swap"):

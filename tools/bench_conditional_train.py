@@ -15,6 +15,11 @@
          num_bins=10, tail_bound=[5, pi], permute_mask=True) on UniformGaussian(2, [1], [1, 2 pi]) with the GaussianVonMises
          target; the step is `reverse_kld(2**14)` + `backward()` + Adam(lr 5e-4), the notebook's (reverse KL: gradients
          through the sampling direction)
+    realnvp examples/real_nvp.ipynb: 64 x [MaskedAffineFlow(MLP([2, 4, 2]) s and t), ActNorm(2)] on DiagGaussian(2), the
+         TwoModes(2, 0.1) target, `reverse_kld(batch)` + `backward()` + Adam(lr 1e-4, weight decay 1e-6), batch 20 (the
+         notebook's) and 4 096
+    augmented examples/augmented_flow.ipynb: 32 x [MaskedAffineFlow(MLP([4, 16, 4]) s and t), ActNorm(4)] on
+         DiagGaussian(4), target TwoIndependent(TwoMoons(), DiagGaussian(2)), the same step at batch 20
 Prints one JSON line: ms/step (median of CUDA-event-timed steps after warm-up), samples/s, kernel launches per step
 (torch.profiler, one separate step), peak device memory, and the card's name, power limit and SM clock read in the same
 run.  When the unmodified reference is installed under oracle/_ref, the same model, seed and batch are timed through it
@@ -32,7 +37,7 @@ REF_DIR = os.path.join(ROOT, "oracle", "_ref")
 
 
 CASES = [("a", 128), ("a", 65536), ("b", 128), ("b", 65536), ("circ", 1024), ("maf", 128), ("maf", 65536),
-         ("maf16", 65536), ("paper", 16384)]
+         ("maf16", 65536), ("paper", 16384), ("realnvp", 20), ("realnvp", 4096), ("augmented", 20)]
 NOTEBOOK_LAYERS = 4   # examples/conditional_flow.ipynb: K = 4 (spline + LU) pairs
 
 
@@ -56,6 +61,17 @@ def build(nf, kind):
                                                                         tail_bound=torch.tensor([5., math.pi]),
                                                                         permute_mask=True) for _ in range(12)]
         return nf.NormalizingFlow(base, flows, GaussianVonMises()), (5e-4, 0.0), 2, False
+    if kind in ("realnvp", "augmented"):
+        d, hid, K = (2, 2, 64) if kind == "realnvp" else (4, 4, 32)
+        b = torch.Tensor([1 if i % 2 == 0 else 0 for i in range(d)]) if d == 2 else torch.Tensor([1, 1, 0, 0])
+        flows = []
+        for i in range(K):
+            s = nf.nets.MLP([d, hid * d, d], init_zeros=True)
+            t = nf.nets.MLP([d, hid * d, d], init_zeros=True)
+            flows += [nf.flows.MaskedAffineFlow(b if i % 2 == 0 else 1 - b, t, s), nf.flows.ActNorm(d)]
+        target = nf.distributions.TwoModes(2, 0.1) if d == 2 else \
+            nf.distributions.TwoIndependent(nf.distributions.TwoMoons(), nf.distributions.DiagGaussian(2))
+        return nf.NormalizingFlow(nf.distributions.DiagGaussian(d), flows, target), (1e-4, 1e-6), d, False
     if kind == "circ":
         flows = [nf.flows.CircularAutoregressiveRationalQuadraticSpline(2, 1, 128, [1], tail_bound=torch.tensor([5., math.pi]),
                                                                         permute_mask=True) for _ in range(20)]
@@ -93,13 +109,15 @@ def time_arm(arm, kind, batch, steps, warmup):
     x = (torch.randn(batch, dim, generator=g) * 1.2).to(dev)
     ctx = torch.cat([torch.randn(batch, 2, generator=g), 0.5 + 0.5 * torch.rand(batch, 2, generator=g)], 1).to(dev) \
         if conditional else None
+    if kind in ("realnvp", "augmented"):
+        model.sample(num_samples=2 ** 7)   # the notebooks' ActNorm initialisation
     opt = torch.optim.Adam(model.parameters(), lr=lr, weight_decay=wd)
     np.random.seed(0)
     torch.manual_seed(0)
 
     def step():
         opt.zero_grad(set_to_none=True)
-        if kind == "paper":
+        if kind in ("paper", "realnvp", "augmented"):
             loss = model.reverse_kld(batch)
         else:
             loss = model.forward_kld(x) if ctx is None else model.forward_kld(x, ctx)
