@@ -82,6 +82,17 @@ struct DevBuf {
     }
 };
 
+// Bump allocator over a caller's workspace, every piece 256-byte aligned; with base == nullptr it only sizes it.
+struct Carver {
+    char* base = nullptr;
+    size_t off = 0;
+    template <typename T> T* take(size_t count) {
+        T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
+        off += (count * sizeof(T) + 255) / 256 * 256;
+        return p;
+    }
+};
+
 // A batch of small device->host reads through ONE pinned staging buffer and ONE stream synchronisation (every blocking
 // cudaMemcpy of a few hundred bytes costs ~15 us of host time and a device sync; the packer used to issue ~25 per layer
 // pair and optimizer step).  add() queues a copy, run() waits once, get() hands the floats out.
@@ -241,8 +252,8 @@ struct nfb_flow {
     int* h_seq = nullptr;            // pinned: h_seq[c] = rows resident after chunk c
     DevBuf in_ready;                 // device int: rows of the current host batch that have landed
     // training pass workspaces (nfb_flow_backward)
-    DevBuf tr_store, tr_h, tr_P, tr_gP, tr_ga, tr_gb, tr_xp, tr_gxp, tr_zp, tr_gzp, tr_in, tr_gin, tr_g0, tr_g1, tr_small,
-        tr_glq, tr_t0, tr_t1, tr_wpack;
+    DevBuf tr_store, tr_net, tr_P, tr_gP, tr_xp, tr_gxp, tr_zp, tr_gzp, tr_in, tr_gin, tr_g0, tr_g1, tr_small, tr_glq,
+        tr_t0, tr_t1, tr_wpack;
     const int* cur_in_ready = nullptr;
     // affine sampling backward: the reduction items with this call's gradient pointers, staged through pinned memory
     AffRedItem* afb_host = nullptr;
@@ -1355,7 +1366,7 @@ int nfb_logabsdet_i_plus_j_2x2_backward(const float* jt, const float* g_ld, int6
 }
 
 namespace {
-// Scratch of the dual backward, carved from the caller's workspace (every piece 256-byte aligned):
+// Scratch of the dual backward, carved from the caller's workspace:
 //   H[l], l < L      stacked input of Swish l (= output of Linear l-1 without bias; H[0] = [x; tangents0])
 //   A[l], l < L      stacked output of Swish l (the A operand of Linear l)      both [(1 + nt) rows, widths[l]]
 //   Y0, Y1           cotangent ping-pong buffers                              [(1 + nt) rows, max width]
@@ -1367,25 +1378,24 @@ struct MlpDualWs {
 int64_t mlp_dual_layout(const nfb_lipschitz_mlp_desc_t* d, int nt, long long rows, char* base, MlpDualWs* ws) {
     if (!d || d->num_layers < 1 || d->num_layers > NFB_LIPSCHITZ_MLP_MAX_LAYERS || nt < 0 || rows < 0) return -1;
     const long long rows2 = (1 + nt) * rows;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { char* p = base ? base + off : nullptr; off += (bytes + 255) / 256 * 256; return p; };
+    Carver c{base};
     int wmax = 0;
     for (int l = 0; l <= d->num_layers; ++l) {
         if (d->widths[l] < 1) return -1;
         wmax = std::max(wmax, (int)d->widths[l]);
     }
     for (int l = 0; l < d->num_layers; ++l) {
-        float* h = reinterpret_cast<float*>(take((size_t)rows2 * d->widths[l] * 4));
-        float* a = reinterpret_cast<float*>(take((size_t)rows2 * d->widths[l] * 4));
+        float* h = c.take<float>((size_t)rows2 * d->widths[l]);
+        float* a = c.take<float>((size_t)rows2 * d->widths[l]);
         if (ws) { ws->H[l] = h; ws->A[l] = a; }
     }
     for (int i = 0; i < 2; ++i) {
-        float* y = reinterpret_cast<float*>(take((size_t)rows2 * wmax * 4));
+        float* y = c.take<float>((size_t)rows2 * wmax);
         if (ws) ws->Y[i] = y;
     }
-    double* p = reinterpret_cast<double*>(take(NFB_SWISH_DUAL_PARTIALS * sizeof(double)));
+    double* p = c.take<double>(NFB_SWISH_DUAL_PARTIALS);
     if (ws) ws->partials = p;
-    return (int64_t)off;
+    return (int64_t)c.off;
 }
 }  // namespace
 
@@ -1538,54 +1548,63 @@ int nfb_glu_residual_backward(const float* g_out, const float* t, const float* c
 }
 
 namespace {
-// Scratch of nfb_resnet_backward (every piece 256-byte aligned).  H = hidden, nb = blocks, C = context features:
+// Scratch of the ResidualNet / MADE backward.  H = hidden, nb = blocks, C = context features:
 //   in0   [rows, in]  ResidualNet with a context: cat(x, context), the initial layer's input; later its data gradient
-//   weff  masked effective weights W * mask of every Linear (MADE only)
+//   weff  masked effective weights W * mask of every Linear (MADE whose caller brings no effective weights)
 //   h[b]  [rows, H], b <= nb: input of block b (h[nb] = the final layer's input)
 //   t1[b], t2[b], c[b] [rows, H]: block b's first / second Linear output and its context gate logits (t2, c: context)
-//   ga, gt, gt1 [rows, H]: cotangents;  gc0 [rows, C]: context columns of in0's gradient (ResidualNet with a context)
+//   ga, gt, gt1 [rows, H]: cotangents (gt: context);  gc0 [rows, C]: context columns of in0's gradient (ResidualNet
+//   with a context)
 struct ResnetWs {
-    float* in0; float* gc0; float* w0e; float* wbe[2 * 64]; float* wfe;
-    float* h[65]; float* t1[64]; float* t2[64]; float* c[64];
+    float* in0; float* gc0; float* w0e; float* wfe;
+    std::vector<float*> wbe, h, t1, t2, c;
     float* ga; float* gt; float* gt1;
 };
-constexpr int kResnetMaxBlocks = 64;
-int64_t resnet_layout(const nfb_resnet_ctx_desc_t* d, long long rows, char* base, ResnetWs* ws) {
+int64_t resnet_layout(const nfb_resnet_ctx_desc_t* d, long long rows, Carver& c, ResnetWs& ws, bool weff = true) {
     if (!d || rows < 0) return -1;
     const nfb_resnet_desc_t& n = d->net;
     const int nb = n.num_blocks, H = n.hidden_features, C = d->context_features;
-    if (nb < 0 || nb > kResnetMaxBlocks || H < 1 || n.in_features < 1 || n.out_features < 1 || C < 0) return -1;
+    if (nb < 0 || H < 1 || n.in_features < 1 || n.out_features < 1 || C < 0) return -1;
     const bool concat = C > 0 && !d->w_context;
     if (concat && n.in_features <= C) return -1;
-    const bool masked = n.m_initial != nullptr;
-    size_t off = 0;
-    auto take = [&](size_t floats) { float* p = base ? reinterpret_cast<float*>(base + off) : nullptr;
-                                     off += (floats * 4 + 255) / 256 * 256; return p; };
     const size_t RH = (size_t)rows * H;
-    float* in0 = concat ? take((size_t)rows * n.in_features) : nullptr;
-    float* gc0 = concat ? take((size_t)rows * C) : nullptr;
-    if (ws) { ws->in0 = in0; ws->gc0 = gc0; }
-    if (masked) {
-        float* p = take((size_t)H * n.in_features);
-        if (ws) ws->w0e = p;
-        for (int i = 0; i < 2 * nb; ++i) { p = take((size_t)H * H); if (ws) ws->wbe[i] = p; }
-        p = take((size_t)n.out_features * H);
-        if (ws) ws->wfe = p;
+    ws = ResnetWs{};
+    ws.in0 = concat ? c.take<float>((size_t)rows * n.in_features) : nullptr;
+    ws.gc0 = concat ? c.take<float>((size_t)rows * C) : nullptr;
+    if (weff && n.m_initial) {
+        ws.w0e = c.take<float>((size_t)H * n.in_features);
+        for (int i = 0; i < 2 * nb; ++i) ws.wbe.push_back(c.take<float>((size_t)H * H));
+        ws.wfe = c.take<float>((size_t)n.out_features * H);
     }
-    for (int b = 0; b <= nb; ++b) { float* p = take(RH); if (ws) ws->h[b] = p; }
+    for (int b = 0; b <= nb; ++b) ws.h.push_back(c.take<float>(RH));
     for (int b = 0; b < nb; ++b) {
-        float* p = take(RH); if (ws) ws->t1[b] = p;
-        if (C > 0) { p = take(RH); if (ws) ws->t2[b] = p; p = take(RH); if (ws) ws->c[b] = p; }
+        ws.t1.push_back(c.take<float>(RH));
+        if (C > 0) { ws.t2.push_back(c.take<float>(RH)); ws.c.push_back(c.take<float>(RH)); }
     }
-    float* p = take(RH); if (ws) ws->ga = p;
-    p = take(RH); if (ws) ws->gt = p;
-    p = take(RH); if (ws) ws->gt1 = p;
-    return (int64_t)off;
+    ws.ga = c.take<float>(RH);
+    if (C > 0) ws.gt = c.take<float>(RH);
+    ws.gt1 = c.take<float>(RH);
+    return (int64_t)c.off;
 }
 
+// Launches the tensor-core GEMMs of a backward.  Optional: wpack, a buffer into which a GEMM whose B is a weight
+// (reused by every 128-row tile of the batch) splits B to bf16 hi | lo records once (launch_gemm_pack_b), so that
+// the GEMM streams them by TMA instead of converting them per tile; launches, a counter of the kernels and memsets
+// issued.
 struct GemmRun {
     int* err; cudaStream_t st;
-    int operator()(const GemmTcArgs& a) const { return launch_gemm_tc(a, err, st); }
+    DevBuf* wpack = nullptr;
+    long long* launches = nullptr;
+    void count(int k) const { if (launches) *launches += k; }
+    int operator()(const GemmTcArgs& a) const { count(1); return launch_gemm_tc(a, err, st); }
+    int w(GemmTcArgs a) const {   // B is a weight
+        if (!wpack) return (*this)(a);
+        NFB_TRY(wpack->reserve(gemm_tc_packed_b_bytes(a.N, a.K, a.b_mn)));
+        NFB_TRY(launch_gemm_pack_b(a.B, a.ldb, a.b_mn, a.N, a.K, wpack->as<uint8_t>(), st));
+        a.b_packed = wpack->as<uint8_t>();
+        count(2);
+        return launch_gemm_tc(a, err, st);
+    }
 };
 // Y = act(X) W^T (+ bias) (+ resid) (the forward of one Linear)
 GemmTcArgs fwd_args(const float* X, long long ldx, int relu_x, const float* W, const float* bias, float* Y, long long M,
@@ -1602,7 +1621,7 @@ GemmTcArgs dgrad_args(const float* gY, const float* W, float* gX, long long M, i
 }
 // dW = gY^T act(X) (* mask), db = colsum(gY)
 int wgrad(const GemmRun& g, const float* gY, int n_out, const float* X, long long ldx, int n_in, int relu_x,
-          const float* mask, long long rows, float* dW, float* db, cudaStream_t st) {
+          const float* mask, long long rows, float* dW, float* db) {
     if (dW) {
         GemmTcArgs a{};
         a.A = gY; a.lda = n_out; a.a_mn = 1; a.B = X; a.ldb = ldx; a.b_mn = 1; a.b_relu = relu_x;
@@ -1610,23 +1629,33 @@ int wgrad(const GemmRun& g, const float* gY, int n_out, const float* X, long lon
         NFB_TRY(g(a));
     }
     if (db) {
-        NFB_CUDA(cudaMemsetAsync(db, 0, (size_t)n_out * 4, st));
-        NFB_TRY(launch_colsum(gY, n_out, rows, n_out, db, st));
+        NFB_CUDA(cudaMemsetAsync(db, 0, (size_t)n_out * 4, g.st));
+        NFB_TRY(launch_colsum(gY, n_out, rows, n_out, db, g.st));
+        g.count(2);
     }
     return NFB_OK;
 }
 }  // namespace
 
 namespace {
-// One backward of a ResidualNet / MADE: the effective weights, the recomputed activations (ws) and the initial layer's
-// input, shared by every adjoint run on them (nfb_maf_inverse_backward runs several on one recompute).
+// One backward of a ResidualNet / MADE: the effective weights, the recomputed activations (ws, laid out by the caller)
+// and the initial layer's input, shared by every adjoint run on them (nfb_maf_inverse_backward runs several on one
+// recompute).  A caller that keeps its own effective weights sets w0 / wb / wf before resnet_recompute.
 struct ResnetPass {
     const nfb_resnet_ctx_desc_t* d;
     long long rows;
-    ResnetWs ws;
     GemmRun g;
-    const float* w0; const float* wf; const float* wb[2 * kResnetMaxBlocks];
+    ResnetWs ws;
+    const float* w0; const float* wf; std::vector<const float*> wb;
     const float* in; long long ld_in;   // x, or cat(x, context) in ws.in0
+};
+
+// Gradient pointers of Linear i at p[i * stride]; p == nullptr: none wanted.
+struct Slots {
+    float* const* p = nullptr;
+    int stride = 1;
+    Slots(float* const* p_ = nullptr, int stride_ = 1) : p(p_), stride(stride_) {}
+    float* operator[](int i) const { return p ? p[(size_t)i * stride] : nullptr; }
 };
 
 int resnet_validate(const char* who, const nfb_resnet_ctx_desc_t* d, int64_t rows, const float* x, const float* context,
@@ -1648,50 +1677,48 @@ int resnet_validate(const char* who, const nfb_resnet_ctx_desc_t* d, int64_t row
 }
 
 // empty batch: every parameter gradient is zero
-int resnet_zero_grads(const nfb_resnet_ctx_desc_t* d, float* const* g_w, float* const* g_b, float* const* g_wc,
-                      float* const* g_bc, cudaStream_t st) {
+int resnet_zero_grads(const nfb_resnet_ctx_desc_t* d, Slots g_w, Slots g_b, Slots g_wc, Slots g_bc, cudaStream_t st) {
     const nfb_resnet_desc_t& n = d->net;
     const int nb = n.num_blocks, H = n.hidden_features, C = d->context_features, out = n.out_features, nin = n.in_features;
     auto zero = [&](float* p, size_t numel) { return p ? (int)cudaMemsetAsync(p, 0, numel * 4, st) : 0; };
     auto wsz = [&](int i) { return (size_t)H * (i == 0 ? nin : H); };  // weights of linear i < 1 + 2 nb
     for (int i = 0; i < 1 + 2 * nb; ++i) {
-        NFB_CUDA((cudaError_t)zero(g_w ? g_w[i] : nullptr, wsz(i)));
-        NFB_CUDA((cudaError_t)zero(g_b ? g_b[i] : nullptr, H));
+        NFB_CUDA((cudaError_t)zero(g_w[i], wsz(i)));
+        NFB_CUDA((cudaError_t)zero(g_b[i], H));
     }
-    NFB_CUDA((cudaError_t)zero(g_w ? g_w[1 + 2 * nb] : nullptr, (size_t)out * H));
-    NFB_CUDA((cudaError_t)zero(g_b ? g_b[1 + 2 * nb] : nullptr, out));
+    NFB_CUDA((cudaError_t)zero(g_w[1 + 2 * nb], (size_t)out * H));
+    NFB_CUDA((cudaError_t)zero(g_b[1 + 2 * nb], out));
     if (C > 0)
         for (int i = 0; i <= nb; ++i) {
-            NFB_CUDA((cudaError_t)zero(g_wc ? g_wc[i] : nullptr, (size_t)H * C));
-            NFB_CUDA((cudaError_t)zero(g_bc ? g_bc[i] : nullptr, H));
+            NFB_CUDA((cudaError_t)zero(g_wc[i], (size_t)H * C));
+            NFB_CUDA((cudaError_t)zero(g_bc[i], H));
         }
     return NFB_OK;
 }
 
-// Effective weights and the activations of the forward at x / context (the same GEMMs as the forward,
-// nets/*.forward through nfb_gemm_f32).  rows > 0.
-int resnet_recompute(ResnetPass& r, const float* x, const float* context, void* workspace, cudaStream_t st) {
+// Effective weights (unless the caller set them) and the activations of the forward at x / context (the same GEMMs
+// as the forward, nets/*.forward through nfb_gemm_f32).  rows > 0.
+int resnet_recompute(ResnetPass& r, const float* x, const float* context) {
     const nfb_resnet_ctx_desc_t* d = r.d;
     const nfb_resnet_desc_t& n = d->net;
     const long long rows = r.rows;
     const int nb = n.num_blocks, H = n.hidden_features, C = d->context_features, out = n.out_features;
     const bool ctx = C > 0, concat = ctx && !d->w_context, masked = n.m_initial != nullptr;
     const int nin = n.in_features, nx = concat ? nin - C : nin;
-    ResnetWs& ws = r.ws;
-    resnet_layout(d, rows, static_cast<char*>(workspace), &ws);
-    int* err_dev = nullptr;
-    NFB_TRY(glow_err_buf(&err_dev));
-    r.g = GemmRun{err_dev, st};
+    const ResnetWs& ws = r.ws;
     const GemmRun& g = r.g;
-    // effective weights
-    r.w0 = n.w_initial; r.wf = n.w_final;
-    for (int i = 0; i < 2 * nb; ++i) r.wb[i] = n.w_blocks[i];
-    if (masked) {
-        NFB_TRY(launch_mask_mul(n.w_initial, n.m_initial, ws.w0e, (long long)H * nin, st));
-        for (int i = 0; i < 2 * nb; ++i) NFB_TRY(launch_mask_mul(n.w_blocks[i], n.m_blocks[i], ws.wbe[i], (long long)H * H, st));
-        NFB_TRY(launch_mask_mul(n.w_final, n.m_final, ws.wfe, (long long)out * H, st));
-        r.w0 = ws.w0e; r.wf = ws.wfe;
-        for (int i = 0; i < 2 * nb; ++i) r.wb[i] = ws.wbe[i];
+    cudaStream_t st = g.st;
+    if (!r.w0) {
+        r.w0 = n.w_initial; r.wf = n.w_final;
+        r.wb.assign(n.w_blocks, n.w_blocks + 2 * nb);
+        if (masked) {
+            NFB_TRY(launch_mask_mul(n.w_initial, n.m_initial, ws.w0e, (long long)H * nin, st));
+            for (int i = 0; i < 2 * nb; ++i)
+                NFB_TRY(launch_mask_mul(n.w_blocks[i], n.m_blocks[i], ws.wbe[i], (long long)H * H, st));
+            NFB_TRY(launch_mask_mul(n.w_final, n.m_final, ws.wfe, (long long)out * H, st));
+            r.w0 = ws.w0e; r.wf = ws.wfe;
+            r.wb.assign(ws.wbe.begin(), ws.wbe.end());
+        }
     }
     r.in = x;
     r.ld_in = nin;
@@ -1702,21 +1729,21 @@ int resnet_recompute(ResnetPass& r, const float* x, const float* context, void* 
                                    cudaMemcpyDeviceToDevice, st));
         r.in = ws.in0;
     }
-    NFB_TRY(g(fwd_args(r.in, r.ld_in, 0, r.w0, n.b_initial, ws.h[0], rows, H, nin)));
+    NFB_TRY(g.w(fwd_args(r.in, r.ld_in, 0, r.w0, n.b_initial, ws.h[0], rows, H, nin)));
     if (ctx && !concat) {
         GemmTcArgs a = fwd_args(context, C, 0, d->w_context, d->b_context, ws.h[0], rows, H, C);
         a.resid = ws.h[0]; a.ldres = H;
-        NFB_TRY(g(a));
+        NFB_TRY(g.w(a));
     }
     for (int b = 0; b < nb; ++b) {
-        NFB_TRY(g(fwd_args(ws.h[b], H, 1, r.wb[2 * b], n.b_blocks[2 * b], ws.t1[b], rows, H, H)));
+        NFB_TRY(g.w(fwd_args(ws.h[b], H, 1, r.wb[2 * b], n.b_blocks[2 * b], ws.t1[b], rows, H, H)));
         if (!ctx) {
             GemmTcArgs a = fwd_args(ws.t1[b], H, 1, r.wb[2 * b + 1], n.b_blocks[2 * b + 1], ws.h[b + 1], rows, H, H);
             a.resid = ws.h[b]; a.ldres = H;
-            NFB_TRY(g(a));
+            NFB_TRY(g.w(a));
         } else {
-            NFB_TRY(g(fwd_args(ws.t1[b], H, 1, r.wb[2 * b + 1], n.b_blocks[2 * b + 1], ws.t2[b], rows, H, H)));
-            NFB_TRY(g(fwd_args(context, C, 0, d->w_block_context[b], d->b_block_context[b], ws.c[b], rows, H, C)));
+            NFB_TRY(g.w(fwd_args(ws.t1[b], H, 1, r.wb[2 * b + 1], n.b_blocks[2 * b + 1], ws.t2[b], rows, H, H)));
+            NFB_TRY(g.w(fwd_args(context, C, 0, d->w_block_context[b], d->b_block_context[b], ws.c[b], rows, H, C)));
             NFB_TRY(launch_glu_residual(ws.h[b], ws.t2[b], ws.c[b], (long long)rows * H, ws.h[b + 1], st));
         }
     }
@@ -1725,10 +1752,10 @@ int resnet_recompute(ResnetPass& r, const float* x, const float* context, void* 
 
 // Adjoint of the recomputed net for the output cotangent g_out.  data_only: the data gradient g_x alone -- no weight
 // gradient, no bias column sum, no context GEMM, no context gradient (g_context and the g_* arrays are ignored).
+// g_x_add (no concatenated context): g_x += the data gradient, through the GEMM's resid epilogue.
 int resnet_adjoint(const ResnetPass& r, const float* context, const float* g_out, bool data_only, float* g_x,
-                   float* g_context, float* const* g_w, float* const* g_b, float* const* g_wc, float* const* g_bc,
-                   cudaStream_t st) {
-    if (data_only) { g_context = nullptr; g_w = g_b = g_wc = g_bc = nullptr; }
+                   float* g_context, Slots g_w, Slots g_b, Slots g_wc, Slots g_bc, bool g_x_add = false) {
+    if (data_only) { g_context = nullptr; g_w = g_b = g_wc = g_bc = Slots(); }
     const nfb_resnet_ctx_desc_t* d = r.d;
     const nfb_resnet_desc_t& n = d->net;
     const long long rows = r.rows;
@@ -1737,25 +1764,24 @@ int resnet_adjoint(const ResnetPass& r, const float* context, const float* g_out
     const int nin = n.in_features, nx = concat ? nin - C : nin;
     const ResnetWs& ws = r.ws;
     const GemmRun& g = r.g;
+    cudaStream_t st = g.st;
     auto mask_of = [&](int i) -> const float* {   // linear i: 0 initial, 1 + j block linear j, 1 + 2 nb final
         if (!masked) return nullptr;
         return i == 0 ? n.m_initial : (i == 1 + 2 * nb ? n.m_final : n.m_blocks[i - 1]);
     };
     if (g_context) NFB_CUDA(cudaMemsetAsync(g_context, 0, (size_t)rows * C * 4, st));
     auto ctx_layer = [&](const float* gY, const float* W, int slot) -> int {   // a Linear of the context
-        NFB_TRY(wgrad(g, gY, H, context, C, C, 0, nullptr, rows, g_wc ? g_wc[slot] : nullptr, g_bc ? g_bc[slot] : nullptr,
-                      st));
+        NFB_TRY(wgrad(g, gY, H, context, C, C, 0, nullptr, rows, g_wc[slot], g_bc[slot]));
         if (g_context) {
             GemmTcArgs a = dgrad_args(gY, W, g_context, rows, C, H);
             a.accumulate = 1;
-            NFB_TRY(g(a));
+            NFB_TRY(g.w(a));
         }
         return NFB_OK;
     };
     const int fl = 1 + 2 * nb;
-    NFB_TRY(wgrad(g, g_out, out, ws.h[nb], H, H, 0, mask_of(fl), rows, g_w ? g_w[fl] : nullptr, g_b ? g_b[fl] : nullptr,
-                  st));
-    NFB_TRY(g(dgrad_args(g_out, r.wf, ws.ga, rows, H, out)));
+    NFB_TRY(wgrad(g, g_out, out, ws.h[nb], H, H, 0, mask_of(fl), rows, g_w[fl], g_b[fl]));
+    NFB_TRY(g.w(dgrad_args(g_out, r.wf, ws.ga, rows, H, out)));
     for (int b = nb - 1; b >= 0; --b) {
         const int l1 = 1 + 2 * b, l2 = 2 + 2 * b;
         const float* gt2 = ws.ga;  // h_{b+1} = h_b + t2 (no context)
@@ -1766,22 +1792,21 @@ int resnet_adjoint(const ResnetPass& r, const float* context, const float* g_out
             gt2 = ws.gt;
         }
         // t2 = W2 relu(t1) + b2
-        NFB_TRY(wgrad(g, gt2, H, ws.t1[b], H, H, 1, mask_of(l2), rows, g_w ? g_w[l2] : nullptr, g_b ? g_b[l2] : nullptr, st));
+        NFB_TRY(wgrad(g, gt2, H, ws.t1[b], H, H, 1, mask_of(l2), rows, g_w[l2], g_b[l2]));
         GemmTcArgs a = dgrad_args(gt2, r.wb[2 * b + 1], ws.gt1, rows, H, H);
         a.mask = ws.t1[b]; a.ldmask = H;
-        NFB_TRY(g(a));   // g_t1 = (g_t2 W2) * (t1 > 0)
+        NFB_TRY(g.w(a));   // g_t1 = (g_t2 W2) * (t1 > 0)
         // t1 = W1 relu(h_b) + b1
-        NFB_TRY(wgrad(g, ws.gt1, H, ws.h[b], H, H, 1, mask_of(l1), rows, g_w ? g_w[l1] : nullptr, g_b ? g_b[l1] : nullptr,
-                      st));
+        NFB_TRY(wgrad(g, ws.gt1, H, ws.h[b], H, H, 1, mask_of(l1), rows, g_w[l1], g_b[l1]));
         GemmTcArgs c = dgrad_args(ws.gt1, r.wb[2 * b], ws.ga, rows, H, H);
         c.mask = ws.h[b]; c.ldmask = H; c.resid = ws.ga; c.ldres = H;
-        NFB_TRY(g(c));   // g_h_b = g_h_{b+1} + (g_t1 W1) * (h_b > 0)     (in place)
+        NFB_TRY(g.w(c));   // g_h_b = g_h_{b+1} + (g_t1 W1) * (h_b > 0)     (in place)
     }
-    NFB_TRY(wgrad(g, ws.ga, H, r.in, r.ld_in, nin, 0, mask_of(0), rows, g_w ? g_w[0] : nullptr, g_b ? g_b[0] : nullptr, st));
+    NFB_TRY(wgrad(g, ws.ga, H, r.in, r.ld_in, nin, 0, mask_of(0), rows, g_w[0], g_b[0]));
     if (ctx && !concat && !data_only) NFB_TRY(ctx_layer(ws.ga, d->w_context, 0));
     if (concat) {
         if (g_x || g_context) {
-            NFB_TRY(g(dgrad_args(ws.ga, r.w0, ws.in0, rows, nin, H)));   // [g_x | g_context] of cat(x, context)
+            NFB_TRY(g.w(dgrad_args(ws.ga, r.w0, ws.in0, rows, nin, H)));   // [g_x | g_context] of cat(x, context)
             if (g_x)
                 NFB_CUDA(cudaMemcpy2DAsync(g_x, (size_t)nx * 4, ws.in0, (size_t)nin * 4, (size_t)nx * 4, rows,
                                            cudaMemcpyDeviceToDevice, st));
@@ -1792,7 +1817,9 @@ int resnet_adjoint(const ResnetPass& r, const float* context, const float* g_out
             }
         }
     } else if (g_x) {
-        NFB_TRY(g(dgrad_args(ws.ga, r.w0, g_x, rows, nin, H)));
+        GemmTcArgs a = dgrad_args(ws.ga, r.w0, g_x, rows, nin, H);
+        if (g_x_add) { a.resid = g_x; a.ldres = nin; }
+        NFB_TRY(g.w(a));
     }
     return NFB_OK;
 }
@@ -1801,40 +1828,41 @@ int resnet_adjoint(const ResnetPass& r, const float* context, const float* g_out
 //   P    [rows, 2 D]  MADE(y, context), the conditioner output at the layer's output
 //   pbar [rows, 2 D]  its cotangent
 //   gin  [rows, D]    MADE data gradient of the latest fixed-point pass
-int64_t maf_layout(const nfb_resnet_ctx_desc_t* d, int32_t features, long long rows, char* base, ResnetWs* ws, float** P,
+int64_t maf_layout(const nfb_resnet_ctx_desc_t* d, int32_t features, long long rows, char* base, ResnetWs& ws, float** P,
                    float** pbar, float** gin) {
-    const int64_t off0 = resnet_layout(d, rows, base, ws);
-    if (off0 < 0 || features < 1) return -1;
-    size_t off = (size_t)off0;
-    auto take = [&](size_t floats) { float* p = base ? reinterpret_cast<float*>(base + off) : nullptr;
-                                     off += (floats * 4 + 255) / 256 * 256; return p; };
-    float* p = take((size_t)rows * 2 * features); if (P) *P = p;
-    p = take((size_t)rows * 2 * features); if (pbar) *pbar = p;
-    p = take((size_t)rows * features); if (gin) *gin = p;
-    return (int64_t)off;
+    Carver c{base};
+    if (resnet_layout(d, rows, c, ws) < 0 || features < 1) return -1;
+    float* p = c.take<float>((size_t)rows * 2 * features); if (P) *P = p;
+    p = c.take<float>((size_t)rows * 2 * features); if (pbar) *pbar = p;
+    p = c.take<float>((size_t)rows * features); if (gin) *gin = p;
+    return (int64_t)c.off;
 }
 }  // namespace
 
 int64_t nfb_resnet_backward_workspace_bytes(const nfb_resnet_ctx_desc_t* d, int64_t rows) {
-    return resnet_layout(d, rows, nullptr, nullptr);
+    Carver c;
+    ResnetWs ws;
+    return resnet_layout(d, rows, c, ws);
 }
 
 int nfb_resnet_backward(const nfb_resnet_ctx_desc_t* d, const float* x, const float* context, const float* g_out,
                         int64_t rows, void* workspace, int64_t workspace_bytes, float* g_x, float* g_context,
                         float* const* g_w, float* const* g_b, float* const* g_wc, float* const* g_bc, void* stream) {
     NFB_TRY(resnet_validate("nfb_resnet_backward", d, rows, x, context, g_out, workspace, workspace_bytes,
-                            resnet_layout(d, rows, nullptr, nullptr)));
+                            nfb_resnet_backward_workspace_bytes(d, rows)));
     cudaStream_t st = S(stream);
     if (rows == 0) return resnet_zero_grads(d, g_w, g_b, g_wc, g_bc, st);
-    ResnetPass r{};
-    r.d = d;
-    r.rows = rows;
-    NFB_TRY(resnet_recompute(r, x, context, workspace, st));
-    return resnet_adjoint(r, context, g_out, false, g_x, g_context, g_w, g_b, g_wc, g_bc, st);
+    ResnetPass r{d, rows, {nullptr, st}};
+    NFB_TRY(glow_err_buf(&r.g.err));
+    Carver c{static_cast<char*>(workspace)};
+    resnet_layout(d, rows, c, r.ws);
+    NFB_TRY(resnet_recompute(r, x, context));
+    return resnet_adjoint(r, context, g_out, false, g_x, g_context, g_w, g_b, g_wc, g_bc);
 }
 
 int64_t nfb_maf_inverse_backward_workspace_bytes(const nfb_resnet_ctx_desc_t* d, int32_t features, int64_t rows) {
-    return maf_layout(d, features, rows, nullptr, nullptr, nullptr, nullptr, nullptr);
+    ResnetWs ws;
+    return maf_layout(d, features, rows, nullptr, ws, nullptr, nullptr, nullptr);
 }
 
 int nfb_maf_inverse_backward(const nfb_resnet_ctx_desc_t* d, int32_t features, const float* x, const float* y,
@@ -1849,25 +1877,24 @@ int nfb_maf_inverse_backward(const nfb_resnet_ctx_desc_t* d, int32_t features, c
     NFB_CHECK(d->context_features == 0 || d->w_context, NFB_ERR_ARG, "%s: a MADE takes its context through w_context",
               who);
     NFB_TRY(resnet_validate(who, d, rows, y, context, x /* g_y and g_log_det may be NULL: zero */, workspace,
-                            workspace_bytes, maf_layout(d, features, rows, nullptr, nullptr, nullptr, nullptr, nullptr)));
+                            workspace_bytes, nfb_maf_inverse_backward_workspace_bytes(d, features, rows)));
     cudaStream_t st = S(stream);
     if (rows == 0) return resnet_zero_grads(d, g_w, g_b, g_wc, g_bc, st);
-    ResnetPass r{};
-    r.d = d;
-    r.rows = rows;
+    ResnetPass r{d, rows, {nullptr, st}};
+    NFB_TRY(glow_err_buf(&r.g.err));
     float *P = nullptr, *pbar = nullptr, *gin = nullptr;
-    maf_layout(d, features, rows, static_cast<char*>(workspace), nullptr, &P, &pbar, &gin);
+    maf_layout(d, features, rows, static_cast<char*>(workspace), r.ws, &P, &pbar, &gin);
     // one recompute at the layer's output y; its ReLU masks and gate logits serve every pass below
-    NFB_TRY(resnet_recompute(r, y, context, workspace, st));
+    NFB_TRY(resnet_recompute(r, y, context));
     const int H = d->net.hidden_features, nb = d->net.num_blocks;
-    NFB_TRY(r.g(fwd_args(r.ws.h[nb], H, 0, r.wf, d->net.b_final, P, rows, 2 * features, H)));
+    NFB_TRY(r.g.w(fwd_args(r.ws.h[nb], H, 0, r.wf, d->net.b_final, P, rows, 2 * features, H)));
     // lam = g_y + MADE_dgrad_x(A(lam)), D - 1 times: exact, as MADE's Jacobian in y is strictly lower triangular
     for (int it = 0; it + 1 < features; ++it) {
         NFB_TRY(launch_maf_affine_adjoint(x, P, g_y, g_log_det, it ? gin : nullptr, rows, features, pbar, nullptr, st));
-        NFB_TRY(resnet_adjoint(r, context, pbar, true, gin, nullptr, nullptr, nullptr, nullptr, nullptr, st));
+        NFB_TRY(resnet_adjoint(r, context, pbar, true, gin, nullptr, {}, {}, {}, {}));
     }
     NFB_TRY(launch_maf_affine_adjoint(x, P, g_y, g_log_det, features > 1 ? gin : nullptr, rows, features, pbar, g_x, st));
-    return resnet_adjoint(r, context, pbar, false, nullptr, g_context, g_w, g_b, g_wc, g_bc, st);
+    return resnet_adjoint(r, context, pbar, false, nullptr, g_context, g_w, g_b, g_wc, g_bc);
 }
 
 namespace {
@@ -1878,25 +1905,24 @@ namespace {
 //   gxin [rows, D]           MADE data gradient at pre(x)
 //   xin  [rows, D]           pre(x), the MADE's input (periodic features)
 int64_t ar_rqs_layout(const nfb_resnet_ctx_desc_t* d, int32_t features, int32_t K, int32_t nd, long long rows,
-                      char* base, float** P, float** pbar, float** gin, float** gxin, float** xin) {
-    const int64_t off0 = resnet_layout(d, rows, base, nullptr);
-    if (off0 < 0 || features < 1 || K < 1 || K > 32 || (nd != K - 1 && nd != K && nd != K + 1)) return -1;
-    size_t off = (size_t)off0;
-    auto take = [&](size_t floats) { float* p = base ? reinterpret_cast<float*>(base + off) : nullptr;
-                                     off += (floats * 4 + 255) / 256 * 256; return p; };
+                      char* base, ResnetWs& ws, float** P, float** pbar, float** gin, float** gxin, float** xin) {
+    Carver c{base};
+    if (resnet_layout(d, rows, c, ws) < 0 || features < 1 || K < 1 || K > 32 || (nd != K - 1 && nd != K && nd != K + 1))
+        return -1;
     const size_t np = (size_t)rows * features * (2 * K + nd);
-    float* p = take(np); if (P) *P = p;
-    p = take(np); if (pbar) *pbar = p;
-    p = take((size_t)rows * features); if (gin) *gin = p;
-    p = take((size_t)rows * features); if (gxin) *gxin = p;
-    p = take((size_t)rows * features); if (xin) *xin = p;
-    return (int64_t)off;
+    float* p = c.take<float>(np); if (P) *P = p;
+    p = c.take<float>(np); if (pbar) *pbar = p;
+    p = c.take<float>((size_t)rows * features); if (gin) *gin = p;
+    p = c.take<float>((size_t)rows * features); if (gxin) *gxin = p;
+    p = c.take<float>((size_t)rows * features); if (xin) *xin = p;
+    return (int64_t)c.off;
 }
 }  // namespace
 
 int64_t nfb_ar_rqs_sampling_backward_workspace_bytes(const nfb_resnet_ctx_desc_t* d, int32_t features, int32_t num_bins,
                                                      int32_t num_derivatives, int64_t rows) {
-    return ar_rqs_layout(d, features, num_bins, num_derivatives, rows, nullptr, nullptr, nullptr, nullptr, nullptr,
+    ResnetWs ws;
+    return ar_rqs_layout(d, features, num_bins, num_derivatives, rows, nullptr, ws, nullptr, nullptr, nullptr, nullptr,
                          nullptr);
 }
 
@@ -1930,20 +1956,19 @@ int nfb_ar_rqs_sampling_backward(const nfb_resnet_ctx_desc_t* d, int32_t feature
         if (g_pf_bias) NFB_CUDA(cudaMemsetAsync(g_pf_bias, 0, (size_t)pf_n_periodic * 4, st));
         return resnet_zero_grads(d, g_w, g_b, g_wc, g_bc, st);
     }
+    ResnetPass r{d, rows, {nullptr, st}};
+    NFB_TRY(glow_err_buf(&r.g.err));
     float *Pm = nullptr, *pbar = nullptr, *gin = nullptr, *gxin = nullptr, *xin = nullptr;
-    ar_rqs_layout(d, D, K, nd, rows, static_cast<char*>(workspace), &Pm, &pbar, &gin, &gxin, &xin);
+    ar_rqs_layout(d, D, K, nd, rows, static_cast<char*>(workspace), r.ws, &Pm, &pbar, &gin, &gxin, &xin);
     // one recompute at pre(x), x the layer's output; its ReLU masks and gate logits serve every pass below
     const float* in = x;
     if (pf) {
         NFB_TRY(launch_periodic_features(x, xin, rows, D, pf_slot, pf_weights, pf_scale, pf_bias, st));
         in = xin;
     }
-    ResnetPass r{};
-    r.d = d;
-    r.rows = rows;
-    NFB_TRY(resnet_recompute(r, in, context, workspace, st));
+    NFB_TRY(resnet_recompute(r, in, context));
     const int H = d->net.hidden_features, nb = d->net.num_blocks;
-    NFB_TRY(r.g(fwd_args(r.ws.h[nb], H, 0, r.wf, d->net.b_final, Pm, rows, D * P, H)));
+    NFB_TRY(r.g.w(fwd_args(r.ws.h[nb], H, 0, r.wf, d->net.b_final, Pm, rows, D * P, H)));
     auto spline = [&](const float* lam_in, float* gz) {   // pbar (and g_z) for lam = g_x + lam_in
         return launch_spline_inverse_adjoint(z, Pm, 0, g_x, lam_in, g_log_det, rows, D, K, nd, tails, circular,
                                              tail_bound, 1.f, pbar, gz, st);
@@ -1952,14 +1977,14 @@ int nfb_ar_rqs_sampling_backward(const nfb_resnet_ctx_desc_t* d, int32_t feature
     // triangular (in the degree order)
     for (int it = 0; it + 1 < D; ++it) {
         NFB_TRY(spline(it ? gin : nullptr, nullptr));
-        NFB_TRY(resnet_adjoint(r, context, pbar, true, pf ? gxin : gin, nullptr, nullptr, nullptr, nullptr, nullptr, st));
+        NFB_TRY(resnet_adjoint(r, context, pbar, true, pf ? gxin : gin, nullptr, {}, {}, {}, {}));
         if (pf)
             NFB_TRY(launch_periodic_features_bwd(x, gxin, rows, D, pf_slot, pf_weights, pf_scale, pf_n_periodic, gin,
                                                  nullptr, nullptr, st));
     }
     NFB_TRY(spline(D > 1 ? gin : nullptr, g_z));
     const bool pf_grads = pf && (g_pf_weights || g_pf_bias);
-    NFB_TRY(resnet_adjoint(r, context, pbar, false, pf_grads ? gxin : nullptr, g_context, g_w, g_b, g_wc, g_bc, st));
+    NFB_TRY(resnet_adjoint(r, context, pbar, false, pf_grads ? gxin : nullptr, g_context, g_w, g_b, g_wc, g_bc));
     if (pf_grads)
         NFB_TRY(launch_periodic_features_bwd(x, gxin, rows, D, pf_slot, pf_weights, pf_scale, pf_n_periodic, nullptr,
                                              g_pf_weights, g_pf_bias, st));
@@ -1971,17 +1996,18 @@ namespace {
 // buffers [rows, max width].
 int64_t mlp_layout(const nfb_mlp_desc_t* d, long long rows, char* base, float** A, float** Y) {
     if (!d || d->num_layers < 1 || d->num_layers > 6 || rows < 0 || d->leaky < 0.f) return -1;
-    size_t off = 0;
-    auto take = [&](size_t floats) { float* p = base ? reinterpret_cast<float*>(base + off) : nullptr;
-                                     off += (floats * 4 + 255) / 256 * 256; return p; };
+    Carver c{base};
     int wmax = 0;
     for (int l = 0; l <= d->num_layers; ++l) {
         if (d->sizes[l] < 1) return -1;
         wmax = std::max(wmax, (int)d->sizes[l]);
     }
-    for (int l = 0; l + 1 < d->num_layers; ++l) { float* p = take((size_t)rows * d->sizes[l + 1]); if (A) A[l] = p; }
-    for (int i = 0; i < 2; ++i) { float* p = take((size_t)rows * wmax); if (Y) Y[i] = p; }
-    return (int64_t)off;
+    for (int l = 0; l + 1 < d->num_layers; ++l) {
+        float* p = c.take<float>((size_t)rows * d->sizes[l + 1]);
+        if (A) A[l] = p;
+    }
+    for (int i = 0; i < 2; ++i) { float* p = c.take<float>((size_t)rows * wmax); if (Y) Y[i] = p; }
+    return (int64_t)c.off;
 }
 }  // namespace
 
@@ -2023,7 +2049,7 @@ int nfb_mlp_backward(const nfb_mlp_desc_t* d, const float* x, const float* g_out
     const float* gY = g_out;
     for (int l = L - 1; l >= 0; --l) {
         const float* X = l ? A[l - 1] : x;
-        NFB_TRY(wgrad(g, gY, w[l + 1], X, w[l], w[l], 0, nullptr, rows, g_w ? g_w[l] : nullptr, g_b ? g_b[l] : nullptr, st));
+        NFB_TRY(wgrad(g, gY, w[l + 1], X, w[l], w[l], 0, nullptr, rows, g_w ? g_w[l] : nullptr, g_b ? g_b[l] : nullptr));
         if (l == 0) {
             if (g_x) NFB_TRY(g(dgrad_args(gY, d->w[0], g_x, rows, w[0], w[1])));
             break;
@@ -2607,98 +2633,39 @@ long long grad_slot_numel(const Layer& L, int s) {
     return (long long)L.n_id * (u == 2 ? L.K - 1 : L.K);
 }
 
-struct Gemm {
-    nfb_flow* f; cudaStream_t st;
-    int run(GemmTcArgs a) { f->launches++; return launch_gemm_tc(a, f->err.as<int>(), st); }
-    // B is a WEIGHT matrix (reused by every 128-row tile of the batch): split it to bf16 hi | lo records once
-    // (launch_gemm_pack_b) and let the GEMM stream them by TMA instead of converting them per tile.
-    int run_w(GemmTcArgs a) {
-        const size_t bytes = gemm_tc_packed_b_bytes(a.N, a.K, a.b_mn);
-        NFB_TRY(f->tr_wpack.reserve(bytes));
-        NFB_TRY(launch_gemm_pack_b(a.B, a.ldb, a.b_mn, a.N, a.K, f->tr_wpack.as<uint8_t>(), st));
-        a.b_packed = f->tr_wpack.as<uint8_t>();
-        f->launches += 2;
-        return launch_gemm_tc(a, f->err.as<int>(), st);
-    }
-};
-
-// conditioner forward (recompute) into h[0..n_hidden-1] ([rows x H] each) and P ([rows x out])
-int net_recompute(nfb_flow* f, const NetDesc& n, const NetPack& p, const float* in, int ld_in, long long rows, float* hbuf,
-                  float* P, cudaStream_t st) {
-    Gemm g{f, st};
-    const long long HS = rows * n.H;
-    GemmTcArgs a{};
-    a.A = in; a.lda = ld_in; a.B = p.w0; a.ldb = n.in; a.C = hbuf; a.ldc = n.H; a.M = rows; a.N = n.H; a.K = n.in; a.bias = n.b0;
-    NFB_TRY(g.run_w(a));
-    for (int b = 0; b < n.nb; ++b) {
-        float* hprev = hbuf + (size_t)(2 * b) * HS;
-        float* t = hbuf + (size_t)(2 * b + 1) * HS;
-        float* hnext = hbuf + (size_t)(2 * b + 2) * HS;
-        GemmTcArgs t1{};
-        t1.A = hprev; t1.lda = n.H; t1.a_relu = 1; t1.B = p.wb[2 * b]; t1.ldb = n.H; t1.C = t; t1.ldc = n.H;
-        t1.M = rows; t1.N = n.H; t1.K = n.H; t1.bias = n.bb[2 * b];
-        NFB_TRY(g.run_w(t1));
-        GemmTcArgs t2{};
-        t2.A = t; t2.lda = n.H; t2.a_relu = 1; t2.B = p.wb[2 * b + 1]; t2.ldb = n.H; t2.C = hnext; t2.ldc = n.H;
-        t2.M = rows; t2.N = n.H; t2.K = n.H; t2.bias = n.bb[2 * b + 1]; t2.resid = hprev; t2.ldres = n.H;
-        NFB_TRY(g.run_w(t2));
-    }
-    GemmTcArgs fl{};
-    fl.A = hbuf + (size_t)(2 * n.nb) * HS; fl.lda = n.H; fl.B = p.wf; fl.ldb = n.H; fl.C = P; fl.ldc = n.out;
-    fl.M = rows; fl.N = n.out; fl.K = n.H; fl.bias = n.bf;
-    return g.run_w(fl);
-}
-
-// one Linear's parameter gradients: dW = gY^T act(X) (* mask), db = colsum(gY)
-int linear_wgrad(nfb_flow* f, const float* gY, int n_out, const float* X, int ldx, int n_in, int x_relu, const float* mask,
-                 long long rows, float* dW, float* db, cudaStream_t st) {
-    if (dW) {
-        Gemm g{f, st};
-        GemmTcArgs a{};
-        a.A = gY; a.lda = n_out; a.a_mn = 1; a.B = X; a.ldb = ldx; a.b_mn = 1; a.b_relu = x_relu;
-        a.C = dW; a.ldc = n_in; a.M = n_out; a.N = n_in; a.K = rows; a.mulm = mask; a.ldmask = n_in;
-        NFB_TRY(g.run(a));
-    }
-    if (db) {
-        NFB_CUDA(cudaMemsetAsync(db, 0, (size_t)n_out * 4, st));
-        NFB_TRY(launch_colsum(gY, n_out, rows, n_out, db, st));
-        f->launches += 2;
-    }
-    return NFB_OK;
-}
-
 // backward of one spline layer: xp = the layer's input [rows x D], gy = gradient w.r.t. its output; writes the
 // gradient w.r.t. its input into gxp ([rows x D]) and the parameter gradients into `slots`.
 int rqs_layer_backward(nfb_flow* f, Layer& L, const float* xp, const float* gy, const float* glq, long long rows,
                        float* gxp, float* const* slots, cudaStream_t st) {
     const NetDesc& n = L.net;
-    const NetPack& p = L.pack;
     const int D = L.D, H = n.H, T = L.n_tr, P = 3 * L.K - 1;
     const bool coupled = L.kind == L_COUPLED_RQS;
-    const int n_hidden = 1 + 2 * n.nb;
-    const long long HS = rows * H;
     NFB_CHECK(L.K == 8, NFB_ERR_UNSUPPORTED, "native backward: num_bins %d != 8", L.K);
-    NFB_TRY(f->tr_h.reserve((size_t)n_hidden * HS * 4));
+    // the conditioner's backward (no context) on the forward's effective weights (L.pack), each weight operand split
+    // to bf16 records before its GEMM
+    nfb_resnet_ctx_desc_t d{};
+    d.net = {n.in, n.H, n.out, n.nb, n.w0, n.b0, n.m0, n.wb.data(), n.bb.data(), n.mb.data(), n.wf, n.bf, n.mf};
+    ResnetPass r{&d, rows, {f->err.as<int>(), st, &f->tr_wpack, &f->launches}};
+    r.w0 = L.pack.w0; r.wf = L.pack.wf; r.wb = L.pack.wb;
+    Carver c;
+    resnet_layout(&d, rows, c, r.ws, false);
+    NFB_TRY(f->tr_net.reserve(c.off));
+    c = Carver{f->tr_net.as<char>()};
+    resnet_layout(&d, rows, c, r.ws, false);
     NFB_TRY(f->tr_P.reserve((size_t)rows * n.out * 4));
     NFB_TRY(f->tr_gP.reserve((size_t)rows * n.out * 4));
-    NFB_TRY(f->tr_ga.reserve((size_t)HS * 4));
-    NFB_TRY(f->tr_gb.reserve((size_t)HS * 4));
-    float* hb = f->tr_h.as<float>();
     float* Pm = f->tr_P.as<float>();
     float* gP = f->tr_gP.as<float>();
-    float* ga = f->tr_ga.as<float>();
-    float* gb = f->tr_gb.as<float>();
     // conditioner input: all columns (autoregressive) or the gathered identity columns (coupling)
     const float* in = xp;
-    int ld_in = D;
     if (coupled) {
         NFB_TRY(f->tr_in.reserve((size_t)rows * L.n_id * 4));
         NFB_TRY(f->tr_gin.reserve((size_t)rows * L.n_id * 4));
         NFB_TRY(launch_gather_cols_ld(xp, D, f->tr_in.as<float>(), L.n_id, L.id_idx.as<int>(), rows, st));
         in = f->tr_in.as<float>();
-        ld_in = L.n_id;
     }
-    NFB_TRY(net_recompute(f, n, p, in, ld_in, rows, hb, Pm, st));
+    NFB_TRY(resnet_recompute(r, in, nullptr));
+    NFB_TRY(r.g.w(fwd_args(r.ws.h[n.nb], H, 0, r.wf, n.bf, Pm, rows, n.out, H)));
     // spline element backward -> gP, gxp (transformed columns)
     NFB_TRY(launch_spline_bwd_rows(xp, D, Pm, gy, glq, coupled ? L.tr_idx.as<int>() : nullptr, rows, T, L.K, L.tail,
                                    L.wh_scale, gP, gxp, st));
@@ -2713,47 +2680,15 @@ int rqs_layer_backward(nfb_flow* f, Layer& L, const float* xp, const float* gy, 
         NFB_TRY(launch_split_table(gtab, L.n_id, slots[2 * nlin], slots[2 * nlin + 1], slots[2 * nlin + 2], st));
         f->launches += 3;
     }
-    Gemm g{f, st};
-    // final layer
-    float* hlast = hb + (size_t)(2 * n.nb) * HS;
-    NFB_TRY(linear_wgrad(f, gP, n.out, hlast, H, H, 0, n.mf, rows, slots[2 * (nlin - 1)], slots[2 * (nlin - 1) + 1], st));
-    {
-        GemmTcArgs a{};
-        a.A = gP; a.lda = n.out; a.B = p.wf; a.ldb = H; a.b_mn = 1; a.C = ga; a.ldc = H; a.M = rows; a.N = H; a.K = n.out;
-        NFB_TRY(g.run_w(a));  // g_h(last)
-    }
-    for (int b = n.nb - 1; b >= 0; --b) {
-        float* hprev = hb + (size_t)(2 * b) * HS;
-        float* t = hb + (size_t)(2 * b + 1) * HS;
-        const int l1 = 1 + 2 * b, l2 = 2 + 2 * b;  // linear indices of the block's two layers
-        // h_next = h_prev + W2 relu(t) + b2
-        NFB_TRY(linear_wgrad(f, ga, H, t, H, H, 1, n.mb[2 * b + 1], rows, slots[2 * l2], slots[2 * l2 + 1], st));
-        GemmTcArgs a{};
-        a.A = ga; a.lda = H; a.B = p.wb[2 * b + 1]; a.ldb = H; a.b_mn = 1; a.C = gb; a.ldc = H; a.M = rows; a.N = H; a.K = H;
-        a.mask = t; a.ldmask = H;
-        NFB_TRY(g.run_w(a));  // g_t = (g_h W2) * (t > 0)
-        // t = W1 relu(h_prev) + b1
-        NFB_TRY(linear_wgrad(f, gb, H, hprev, H, H, 1, n.mb[2 * b], rows, slots[2 * l1], slots[2 * l1 + 1], st));
-        GemmTcArgs c{};
-        c.A = gb; c.lda = H; c.B = p.wb[2 * b]; c.ldb = H; c.b_mn = 1; c.C = ga; c.ldc = H; c.M = rows; c.N = H; c.K = H;
-        c.mask = hprev; c.ldmask = H; c.resid = ga; c.ldres = H;
-        NFB_TRY(g.run_w(c));  // g_h_prev = g_h + (g_t W1) * (h_prev > 0)     (in place)
-    }
-    // initial layer
-    NFB_TRY(linear_wgrad(f, ga, H, in, ld_in, n.in, 0, n.m0, rows, slots[0], slots[1], st));
-    if (!coupled) {
-        GemmTcArgs a{};
-        a.A = ga; a.lda = H; a.B = p.w0; a.ldb = n.in; a.b_mn = 1; a.C = gxp; a.ldc = D; a.M = rows; a.N = D; a.K = H;
-        a.resid = gxp; a.ldres = D;
-        NFB_TRY(g.run_w(a));  // + conditioner path (in place)
-    } else {
-        GemmTcArgs a{};
-        a.A = ga; a.lda = H; a.B = p.w0; a.ldb = n.in; a.b_mn = 1; a.C = f->tr_gin.as<float>(); a.ldc = L.n_id;
-        a.M = rows; a.N = L.n_id; a.K = H;
-        NFB_TRY(g.run(a));
-        NFB_TRY(launch_scatter_cols(f->tr_gin.as<float>(), gxp, L.id_idx.as<int>(), rows, L.n_id, D, 1, st));
-        f->launches++;
-    }
+    // the slots interleave each Linear's weight and bias gradients: w0, b0, w_blocks..., wf, bf
+    const Slots g_w(slots, 2), g_b(slots + 1, 2);
+    if (!coupled)   // gxp += the conditioner's data gradient (in place)
+        return resnet_adjoint(r, nullptr, gP, false, gxp, nullptr, g_w, g_b, {}, {}, true);
+    NFB_TRY(resnet_adjoint(r, nullptr, gP, false, nullptr, nullptr, g_w, g_b, {}, {}));
+    // the identity columns' data gradient (W0 read unpacked), scatter-added into gxp
+    NFB_TRY(r.g(dgrad_args(r.ws.ga, r.w0, f->tr_gin.as<float>(), rows, L.n_id, H)));
+    NFB_TRY(launch_scatter_cols(f->tr_gin.as<float>(), gxp, L.id_idx.as<int>(), rows, L.n_id, D, 1, st));
+    f->launches++;
     return NFB_OK;
 }
 
@@ -2768,13 +2703,13 @@ int lu_layer_backward(nfb_flow* f, Layer& L, const float* zin, const float* gxp,
     float* zp = f->tr_zp.as<float>();
     float* gzp = f->tr_gzp.as<float>();
     float* dW = f->tr_small.as<float>() + 64 * 23 + 64;
-    Gemm g{f, st};
+    const GemmRun g{f->err.as<int>(), st, nullptr, &f->launches};
     NFB_TRY(launch_gather_cols(zin, zp, L.lu_perm.as<int>(), rows, D, 1, st));
     f->launches++;
     if (slots[0] || slots[1] || slots[2]) {
         GemmTcArgs a{};
         a.A = gxp; a.lda = D; a.a_mn = 1; a.B = zp; a.ldb = D; a.b_mn = 1; a.C = dW; a.ldc = D; a.M = D; a.N = D; a.K = rows;
-        NFB_TRY(g.run(a));
+        NFB_TRY(g(a));
         NFB_TRY(launch_lu_param_bwd(dW, L.lu.lower_entries, L.lu.upper_entries, L.lu.unconstrained_upper_diag, L.lu.eps, D,
                                     glq_sum, slots[0], slots[1], slots[2], st));
         f->launches++;
@@ -2786,7 +2721,7 @@ int lu_layer_backward(nfb_flow* f, Layer& L, const float* zin, const float* gxp,
     }
     GemmTcArgs a{};
     a.A = gxp; a.lda = D; a.B = L.lu_Wd.as<float>(); a.ldb = D; a.b_mn = 1; a.C = gzp; a.ldc = D; a.M = rows; a.N = D; a.K = D;
-    NFB_TRY(g.run(a));
+    NFB_TRY(g(a));
     NFB_TRY(launch_scatter_cols(gzp, gz, L.lu_perm.as<int>(), rows, D, D, 0, st));
     f->launches++;
     return NFB_OK;
