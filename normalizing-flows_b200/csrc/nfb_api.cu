@@ -2127,8 +2127,9 @@ int nfb_flow_add_coupled_rqs(nfb_flow_t* f, const nfb_coupled_rqs_desc_t* d) {
 
 int nfb_flow_add_lu_linear_permute(nfb_flow_t* f, const nfb_lu_desc_t* d) {
     NFB_NEW_LAYER(L_LU);
-    NFB_CHECK(d->permutation && d->lower_entries && d->upper_entries && d->unconstrained_upper_diag && d->bias,
-              NFB_ERR_ARG, "LULinearPermute: null pointer");
+    // (one feature: no off-diagonal entries, so the two empty tensors may have no storage)
+    NFB_CHECK(d->permutation && (f->D == 1 || (d->lower_entries && d->upper_entries)) && d->unconstrained_upper_diag &&
+              d->bias, NFB_ERR_ARG, "LULinearPermute: null pointer");
     NFB_CHECK(f->D <= 64, NFB_ERR_UNSUPPORTED, "LULinearPermute: features %d > 64", f->D);
     L->lu = *d;
     f->layers.push_back(std::move(L));

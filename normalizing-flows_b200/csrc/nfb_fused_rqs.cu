@@ -394,12 +394,13 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
             }
         }
         cons_bar_sync();
-        // Row unit u = 2^-e, e = clamp(floor(log2 max|x_row|) + 1, 0, 40): |x| u < 1 for every input of the row, so every
-        // fp16 operand of this unit stays inside the static bounds the packer derived (nfb_api.cu plan_scales) whatever
-        // the magnitude of the data; u = 1 for ordinary rows (|x| < 1 .. 2).
+        // Row unit u = 2^-e, e = clamp(floor(log2 max|x_row|) + 1, 0, 126): |x| u < 1 for every input below 2^126, and < 4
+        // up to the largest finite float.  Every fp16 operand of this unit stays inside the static bounds the packer
+        // derived (nfb_api.cu plan_scales), which sit at least 4x (2 binades) below the fp16 maximum, whatever the magnitude
+        // of the data; u = 1 for ordinary rows (|x| < 1 .. 2).  (126: 2^-e and 2^e are both normal floats.)
         auto set_row_exp = [&](float zmax) {
             int e = (int)((__float_as_uint(zmax) >> 23) & 0xffu) - 126;
-            rowexp[r] = max(0, min(40, e));
+            rowexp[r] = max(0, min(126, e));
         };
         if (rq == 0) {
             float zmax = 0.f;
@@ -409,14 +410,14 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
             set_row_exp(zmax);
         }
         cons_bar_sync();
-        auto ru = [&](int row) { return pow2i(-rowexp[row]); };
-        auto ruinv = [&](int row) { return pow2i(rowexp[row]); };
+        auto ru = [&](float s, int row) { return s * pow2i(-rowexp[row]); };      // s u_row
+        auto ruinv = [&](float s, int row) { return s * pow2i(rowexp[row]); };    // s / u_row
         auto get_x = [&](int c) -> float { return xs[xs_index(r, c)]; };
         auto put_y = [&](int c, float y) { xs[xs_index(r, c)] = y; };
         // A[:, 0:64] (K-chunk 0): fp16 hi/lo split of value(row, k) * u_row * sc; thread = (row, quarter of k)
         const int ar = et >> 2, aq = et & 3;
         auto store_a = [&](auto value, float sc_base) {
-            const float sc = sc_base * ru(ar);
+            const float sc = ru(sc_base, ar);
             float v[16];
 #pragma unroll
             for (int j = 0; j < 16; ++j) v[j] = value(aq * 16 + j) * sc;
@@ -442,7 +443,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
             run_slice(acc, wg == 0, std::integral_constant<bool, true>());   // (no half for warpgroup 1)
             if (wg == 0) {
                 // x' = acc + b (this thread: rows ra / rb, two columns of every 8-column group)
-                const float ia = L.a_inv[0] * ruinv(ra), ib = L.a_inv[0] * ruinv(rb);
+                const float ia = ruinv(L.a_inv[0], ra), ib = ruinv(L.a_inv[0], rb);
 #pragma unroll
                 for (int i = 0; i < 32; ++i) {
                     const int c = 8 * (i >> 2) + cq + (i & 1);
@@ -531,8 +532,8 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
                     }
                 }
                 cons_bar_sync();   // every product of this GEMM has read the A operand: overwrite it with the output
-                const float inv_a = L.a_inv[1 + ph] * ruinv(ra), inv_b = L.a_inv[1 + ph] * ruinv(rb);
-                const float sc_a = L.a_sc[2 + ph] * ru(ra), sc_b = L.a_sc[2 + ph] * ru(rb);
+                const float inv_a = ruinv(L.a_inv[1 + ph], ra), inv_b = ruinv(L.a_inv[1 + ph], rb);
+                const float sc_a = ru(L.a_sc[2 + ph], ra), sc_b = ru(L.a_sc[2 + ph], rb);
                 // output slice j: bias, ReLU, scale to the next GEMM's units, fp16 hi/lo -> A K-chunk j
                 auto epilogue = [&](const float (&acc)[32], int j) {
                     const float* bias = L.bias_h + ph * 256 + 64 * j;
@@ -569,7 +570,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
 
             // ---- final layer: record c = chunks 2c (warpgroup 0) and 2c + 1 (warpgroup 1), kFusedFeaturesPerChunk
             //      features (x 24 columns) each -> staging -> one spline per thread ----
-            const float inv_f = L.a_inv[1 + n_hidden] * ruinv(r);
+            const float inv_f = ruinv(L.a_inv[1 + n_hidden], r);
             const int f = (et >> 6) & 1;   // feature of the warpgroup's chunk this thread evaluates (for row r)
             for (int ci = 0; ci < n_pairs; ++ci) {
                 float acc[kFusedFeaturesPerChunk * 12];

@@ -73,6 +73,18 @@ __host__ __device__ __forceinline__ float softplus_f(float u) {
     return u > 20.f ? u : sp;
 }
 
+// Root in [0, 1] of a theta^2 + b theta + c = 0 for the inverse spline (:172-198).  The reference's form 2c / (-b - sqrt(disc))
+// is free of cancellation for b >= 0 (and is kept there bit for bit); for b < 0 its denominator cancels.  That happens
+// where the bin is nearly flat at one end and steep at the other (large derivative parameters).  There the fp32 root can
+// land outside [0, 1], so den = delta + s theta (1 - theta) goes negative and the log-det becomes NaN.  The same root as
+// (-b + sqrt(disc)) / 2a has no cancellation for b < 0 (a >= |b| > 0 whenever that root lies in [0, 1]).  The clamp
+// keeps the last ulps inside the bin.
+__host__ __device__ __forceinline__ float rqs_inverse_root(float a, float b, float c) {
+    const float sq = sqrtf(fmaxf(b * b - 4.f * a * c, 0.f));
+    const float theta = b >= 0.f ? (2.f * c) / (-b - sq) : (sq - b) / (2.f * a);
+    return fminf(fmaxf(theta, 0.f), 1.f);
+}
+
 // The unnormalised boundary derivative, as the reference computes it in fp32 (:36).
 #define NFB_BOUNDARY_UD 0.5397424f /* float32(log(exp(1 - 1e-3) - 1)) = 0.5397424172... */
 
@@ -165,8 +177,7 @@ __host__ __device__ __forceinline__ void rqs_core(float x, const float (&lw)[K],
         const float a = t * s + in_h * (delta - d0);
         const float b = in_h * d0 - t * s;
         const float c = -delta * t;
-        const float disc = fmaxf(b * b - 4.f * a * c, 0.f);
-        theta = (2.f * c) / (-b - sqrtf(disc));
+        theta = rqs_inverse_root(a, b, c);
         outu = theta * in_w + l_w;
         tomt = theta * (1.f - theta);
         den = delta + s * tomt;
@@ -259,8 +270,7 @@ __host__ __device__ __forceinline__ void rqs_eval_dyn(int K, float x, P p, float
         const float a = t * s + in_h * (delta - d0);
         const float b = in_h * d0 - t * s;
         const float c = -delta * t;
-        const float disc = fmaxf(b * b - 4.f * a * c, 0.f);
-        theta = (2.f * c) / (-b - sqrtf(disc));
+        theta = rqs_inverse_root(a, b, c);
         out = theta * in_w + in_cw;
         tomt = theta * (1.f - theta);
         den = delta + s * tomt;
