@@ -28,10 +28,13 @@
 //              64 x H fp32 -- lives in registers (2 x 32 per thread each) and ONE A-operand buffer suffices: both
 //              warpgroups finish the GEMM, then overwrite its input with its output (bias, ReLU, fp16 hi/lo split).  The
 //              second GEMM of each residual block accumulates straight onto the residual stream (h += W2 relu(...));
-//              the biases are pre-summed by the packer.  The final layer is computed two features (N = 48) per
-//              warpgroup at a time and staged through shared memory, so that each thread evaluates one (row, feature)
-//              spline; the two warpgroups drift apart by up to the ring depth, so one's splines overlap the other's
-//              products.
+//              the biases are pre-summed by the packer.
+//              In the final layer the warpgroups take different roles: warpgroup 0 multiplies both halves of every
+//              record (two features, N = 48, per half; two accumulators in flight) and stores each pair of chunks to
+//              two staging tiles in shared memory; warpgroup 1 copies its (row, feature) parameters out of the tiles,
+//              hands them back at once and evaluates two splines per thread.  The hand-off is a pair of named barriers
+//              ("full" / "free", one side arrives, the other waits), so the products of one pair of chunks run under the
+//              splines of the pair before.
 // Shared memory: A operand 64 KB (hi|lo x K=256), weight ring 96 KB, x/y tile 16 KB (XOR-swizzled, conflict-free
 // column access), final-layer staging 2 x 13 KB.
 #include <type_traits>
@@ -84,8 +87,16 @@ __device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) {
 __device__ __forceinline__ void cons_bar_sync() {  // both consumer warpgroups
     asm volatile("bar.sync 1, %0;" ::"n"(kCons) : "memory");
 }
-__device__ __forceinline__ void wg_bar_sync(int wg) {  // one consumer warpgroup
-    asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+// Final-layer hand-off between the product warpgroup and the spline warpgroup (producer / consumer form of the named
+// barriers: one side arrives, the other waits; both count kCons).  The arriving side fences first: bar.arrive by
+// itself does not order its thread's earlier shared-memory accesses.
+constexpr int kBarStgFull = 2, kBarStgFree = 3;
+template <int ID> __device__ __forceinline__ void stg_bar_arrive() {
+    __threadfence_block();
+    asm volatile("bar.arrive %0, %1;" ::"n"(ID), "n"(kCons) : "memory");
+}
+template <int ID> __device__ __forceinline__ void stg_bar_wait() {
+    asm volatile("bar.sync %0, %1;" ::"n"(ID), "n"(kCons) : "memory");
 }
 // mbarrier arrive by one thread of the warpgroup, as a predicated instruction: a branch around it would make ptxas
 // serialise the warpgroup's wgmma
@@ -119,27 +130,86 @@ __device__ __forceinline__ float pow2i(int e) { return __uint_as_float((uint32_t
 // the products of one record: acc (+)= A[K-chunk] W^T as W_hi A_hi + W_hi A_lo + W_lo A_hi (+ W_lo A_lo), four K=16
 // slabs each, in that order (first: the first product overwrites the accumulator; on = 0: none; slabs: only the
 // first `slabs` K=16 slabs, the others being all zero)
-template <int NREG, bool QUAD>
-__device__ __forceinline__ void mma_record(float (&acc)[NREG], uint32_t a_hi, uint32_t a_lo, uint32_t w_hi, uint32_t w_lo,
-                                           bool first, uint32_t on, uint32_t slabs) {
-    const uint64_t ah = wgmma_desc(a_hi), al = wgmma_desc(a_lo), bh = wgmma_desc(w_hi), bl = wgmma_desc(w_lo);
-    auto mma = [&](uint64_t a, uint64_t b, uint32_t sd, int s) {
-        const uint32_t go = on & (uint32_t)(s < (int)slabs);
-        if constexpr (NREG == 32) wgmma_f16_n64(acc, a, b, sd, go);
-        else wgmma_f16_n48(acc, a, b, sd, go);
+// With a second accumulator (acc1, its own operands x1): the two halves of a final-layer record, slab by slab in turn,
+// so that two independent chains are in flight; each accumulator sees its products in the same order as alone.
+struct MmaOps { uint32_t a_hi, a_lo, w_hi, w_lo; bool first; uint32_t on, slabs; };
+template <int NREG, bool QUAD, typename ACC1>
+__device__ __forceinline__ void mma_record(float (&acc)[NREG], const MmaOps& x, ACC1& acc1, const MmaOps& x1) {
+    constexpr bool kPair = !std::is_same<ACC1, const std::nullptr_t>::value;
+    auto mma = [](auto& d, uint64_t a, uint64_t b, uint32_t sd, uint32_t go) {
+        if constexpr (NREG == 32) wgmma_f16_n64(d, a, b, sd, go);
+        else wgmma_f16_n48(d, a, b, sd, go);
     };
-    uint32_t sd = first ? 0u : 1u;
+    const uint64_t ah = wgmma_desc(x.a_hi), al = wgmma_desc(x.a_lo), bh = wgmma_desc(x.w_hi), bl = wgmma_desc(x.w_lo);
+    const uint64_t ah1 = wgmma_desc(x1.a_hi), al1 = wgmma_desc(x1.a_lo), bh1 = wgmma_desc(x1.w_hi), bl1 = wgmma_desc(x1.w_lo);
+    auto pass = [&](uint64_t a, uint64_t b, uint64_t a1, uint64_t b1, bool opens) {
 #pragma unroll
-    for (int s = 0; s < 4; ++s) { mma(ah + 2 * s, bh + 2 * s, sd, s); sd = 1u; }
-#pragma unroll
-    for (int s = 0; s < 4; ++s) mma(al + 2 * s, bh + 2 * s, 1u, s);
-#pragma unroll
-    for (int s = 0; s < 4; ++s) mma(ah + 2 * s, bl + 2 * s, 1u, s);
-    if constexpr (QUAD) {
-#pragma unroll
-        for (int s = 0; s < 4; ++s) mma(al + 2 * s, bl + 2 * s, 1u, s);
-    }
+        for (int s = 0; s < 4; ++s) {
+            mma(acc, a + 2 * s, b + 2 * s, opens && s == 0 && x.first ? 0u : 1u, x.on & (uint32_t)(s < (int)x.slabs));
+            if constexpr (kPair)
+                mma(acc1, a1 + 2 * s, b1 + 2 * s, opens && s == 0 && x1.first ? 0u : 1u, x1.on & (uint32_t)(s < (int)x1.slabs));
+        }
+    };
+    pass(ah, bh, ah1, bh1, true);
+    pass(al, bh, al1, bh1, false);
+    pass(ah, bl, ah1, bl1, false);
+    if constexpr (QUAD) pass(al, bl, al1, bl1, false);
 }
+template <int NREG, bool QUAD>
+__device__ __forceinline__ void mma_record(float (&acc)[NREG], const MmaOps& x) {
+    const std::nullptr_t none = nullptr;
+    mma_record<NREG, QUAD>(acc, x, none, x);
+}
+
+// Phase clocks (make CLOCKS=1, a separate library; tools/fused_phase_clocks.py): every thread of a role adds the SM
+// cycles between two consecutive stamps to the phase the second stamp names, and thread 0 of each consumer warpgroup and
+// lane 0 of the producer warp add their sums to g_phase_clocks when the CTA runs out of units.  Without the macro a
+// stamp is nothing and the product kernel is unchanged.
+enum { kClkClaim,       // unit queue, layer-to-layer flag, rows of a host batch in flight
+       kClkLoad,        // z tile -> shared memory, row units, A operand of the first GEMM (and its barriers)
+       kClkLu,          // LU stage: ring wait, products, epilogue
+       kClkHidRing,     // hidden GEMMs: wait for the record (full barrier)
+       kClkHidMma,      // hidden GEMMs: wgmma issue -> complete (wait_group), slot hand-back
+       kClkHidEpi,      // hidden GEMMs: epilogues and the barriers around them; unconditional splines
+       kClkFinRing,     // final layer: wait for the record
+       kClkFinMma,      // final layer: wgmma issue -> complete, slot hand-back
+       kClkFinStage,    // final layer: accumulators <-> staging tiles, hand-off waits
+       kClkFinSpline,   // final layer: spline evaluation
+       kClkStore,       // log-det reduction, tile store, publish
+       kClkProdEmpty,   // producer: wait for an empty slot
+       kClkProdOther,   // producer: everything else (claim, step table, issue)
+       kClkUnits,       // (a count, not cycles) units this role worked on
+       kClkCount };
+template <int P> using ClkPhase = std::integral_constant<int, P>;
+#ifdef NFB_PHASE_CLOCKS
+__device__ unsigned long long g_phase_clocks[3][kClkCount];   // [consumer warpgroup 0, 1, producer][phase]
+struct PhaseClock {   // 32-bit sums: one launch is far below 2^32 cycles
+    uint32_t last, sum[kClkCount];
+    __device__ PhaseClock() {
+        last = (uint32_t)clock64();
+#pragma unroll
+        for (int i = 0; i < kClkCount; ++i) sum[i] = 0;
+    }
+    template <int P> __device__ __forceinline__ void stamp() {
+        const uint32_t t = (uint32_t)clock64();
+        sum[P] += t - last;
+        last = t;
+    }
+    __device__ void flush(int role) const {
+#pragma unroll
+        for (int i = 0; i < kClkCount; ++i) atomicAdd(&g_phase_clocks[role][i], (unsigned long long)sum[i]);
+    }
+};
+#define NFB_CLK_BEGIN() PhaseClock clk
+#define NFB_CLK(P) clk.template stamp<P>()
+#define NFB_CLK_UNIT() (++clk.sum[kClkUnits])
+#define NFB_CLK_END(role, pred) do { if (pred) clk.flush(role); } while (0)
+#else
+#define NFB_CLK_BEGIN() ((void)0)
+#define NFB_CLK(P) ((void)0)
+#define NFB_CLK_UNIT() ((void)0)
+#define NFB_CLK_END(role, pred) ((void)0)
+#endif
 
 // SAMPLE = false: density direction (Flow.inverse of every layer: x -> z, core.py:70-85).
 // SAMPLE = true : sampling direction of coupling-layer stacks (Flow.forward: z -> x, core.py:40-55): the unit is
@@ -204,6 +274,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
         // whole warp walks the table (warp-uniform control flow); one elected lane issues the copy
         uint32_t slot = 0, par = 0;
         int wcur = 0;
+        NFB_CLK_BEGIN();
         for (uint32_t ui = 0;; ++ui) {
             long long u;
             if (p.ticket) {
@@ -224,6 +295,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
             }
             __syncwarp();
             if (!more) break;
+            NFB_CLK_UNIT();
             const FusedLayer& L = p.layers[ulayer];
             const FusedStep* steps = L.steps;  // global (L2-resident)
             const int n_steps = L.n_steps;
@@ -240,7 +312,9 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
                 uint32_t offn = off + bytes;
                 if (sn == n_steps) { sn = lu_steps; offn = lu_bytes; }
                 const uint32_t nbytes = i + 1 < total ? (uint32_t)__ldg(&steps[sn].bytes16) << 4 : 0u;
+                NFB_CLK(kClkProdOther);
                 mbar_wait(bar(kBarWEmpty + slot), par ^ 1, p.err, 100 + slot);
+                NFB_CLK(kClkProdEmpty);
                 if (elect_one_sync()) {
                     mbar_expect_tx(bar(kBarWFull + slot), bytes);
                     bulk_g2s(sbase + kOffW + slot * kSlotBytes, L.wstream + off, bytes, bar(kBarWFull + slot));
@@ -252,6 +326,8 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
                 if (++slot == kSlots) { slot = 0; par ^= 1; }
             }
         }
+        NFB_CLK(kClkProdOther);
+        NFB_CLK_END(2, lane == 0);
         return;
     }
 
@@ -264,26 +340,32 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
     const int rb = ra + 8;
     const int cq = 2 * (lane & 3);                 // first of its two columns in every 8-column group
     const uint32_t aA = sbase;                     // the A operand
-    float* stg = reinterpret_cast<float*>(smem + kOffStg + wg * kStgBytes);
+    float* stg0 = reinterpret_cast<float*>(smem + kOffStg);   // staging tile of a pair's even chunk; the odd one follows
     uint32_t slot = 0, wpar = 0;
+    NFB_CLK_BEGIN();
 
     for (uint32_t ui = 0;; ++ui) {
         mbar_wait(bar(kBarUnit + (ui & 3u)), (ui >> 2) & 1u, p.err, 600 + (int)(ui & 3u));
         const int layer = uniform(unit_q[2 * (ui & 3u)]);
         const long long tile = uniform(unit_q[2 * (ui & 3u) + 1]);
         if (layer < 0) break;
+        NFB_CLK_UNIT();
         const FusedLayer& L = p.layers[layer];
         const int D = L.D;
         auto own = [&](int q) { return uniform((int)L.own[wg][q]); };   // this warpgroup's slices (-1: none)
         const int n_steps = uniform(L.n_steps), lu_steps = uniform(L.has_lu ? 1 : 0);
         const int n_hidden = uniform(L.n_hidden), n_pairs = uniform(L.n_chunks >> 1);
         int sidx = 0;
-        // The records of one output slice (until the one this warpgroup's flags mark last): its half of each goes
-        // into acc, multiplied with its K-chunk (live: the warpgroup has a slice here; its skip bit: the record has no
-        // half for it, or an all-zero one).  Every record is waited for and handed back by both warpgroups; a slot is
-        // handed back as soon as the products that read it have completed (an empty wgmma group stands in for a
-        // skipped half, so the group count stays uniform).
-        auto run_slice = [&](auto& acc, bool live, auto quad) {
+        // A run of consecutive records, until the one whose products `issue` reports as the last of its accumulator(s).
+        // Every record is waited for, and its slot handed back as soon as the products that read it have completed
+        // (an empty wgmma group stands in for skipped products, so the group count stays uniform).  A slot's empty
+        // barrier expects one arrival per consumer warpgroup: `arrivals` is 1 where both warpgroups walk the records
+        // (LU stage, hidden GEMMs) and 2 where one walks them for both (final layer).
+        auto run_records = [&](auto issue, auto arrivals, auto clk_ring, auto clk_mma) {
+            auto hand_back = [&](int s, bool pred) {
+#pragma unroll
+                for (int i = 0; i < decltype(arrivals)::value; ++i) mbar_arrive_if(bar(kBarWEmpty + s), pred && (et & 127) == 0);
+            };
             int prev = -1;
             for (;;) {
                 union { uint2 raw; FusedStep s; } st;
@@ -291,24 +373,38 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
                 st.raw.x = uniform(st.raw.x);
                 st.raw.y = uniform(st.raw.y);
                 sidx = sidx + 1 == n_steps ? lu_steps : sidx + 1;
-                const uint32_t kc = wg ? st.s.kc1 : st.s.kc;
-                const uint32_t fl = wg ? st.s.flags1 : st.s.flags;
+                NFB_CLK(decltype(clk_mma)::value);
                 mbar_wait(bar(kBarWFull + slot), wpar, p.err, 220 + slot);
-                const uint32_t w = sbase + kOffW + slot * kSlotBytes + ((fl & kStepHalf) ? 0u : (uint32_t)wg * st.s.n8 * 1024u);
+                NFB_CLK(decltype(clk_ring)::value);
                 wgmma_fence();
-                mma_record<sizeof(acc) / sizeof(float), decltype(quad)::value>(
-                    acc, aA + kc * kTileA, aA + (4 + kc) * kTileA, w, w + ((uint32_t)st.s.bytes16 << 3),
-                    (fl & kStepFirst) != 0, (uint32_t)(live && !(fl & kStepSkip)), 4u - ((fl >> kStepSlabShift) & 3u));
+                const bool last = issue(st.s);
                 wgmma_commit();
                 wgmma_wait<1>();   // the previous record's products are complete: hand its slot back
-                mbar_arrive_if(bar(kBarWEmpty + (prev < 0 ? 0 : prev)), prev >= 0 && (et & 127) == 0);
+                hand_back(prev < 0 ? 0 : prev, prev >= 0);
                 prev = (int)slot;
                 if (++slot == kSlots) { slot = 0; wpar ^= 1; }
-                if (fl & kStepLast) break;
+                if (last) break;
             }
             wgmma_wait<0>();
+            hand_back(prev, true);
+            NFB_CLK(decltype(clk_mma)::value);
+        };
+        // operands of half h of the record in the current slot (live = 0: no products; the skip bit: the record has no
+        // half h, or an all-zero one)
+        auto half_ops = [&](const FusedStep& s, int h, bool live) {
+            const uint32_t kc = h ? s.kc1 : s.kc, fl = h ? s.flags1 : s.flags;
+            const uint32_t w = sbase + kOffW + slot * kSlotBytes + ((fl & kStepHalf) ? 0u : (uint32_t)h * s.n8 * 1024u);
+            return MmaOps{aA + kc * kTileA, aA + (4 + kc) * kTileA, w, w + ((uint32_t)s.bytes16 << 3), (fl & kStepFirst) != 0,
+                          (uint32_t)(live && !(fl & kStepSkip)), 4u - ((fl >> kStepSlabShift) & 3u)};
+        };
+        // The records of one output slice of this warpgroup (until the one its flags mark last): its half of each goes
+        // into acc, multiplied with its K-chunk (live: the warpgroup has a slice here).
+        auto run_slice = [&](auto& acc, bool live, auto quad, auto clk_ring, auto clk_mma) {
+            run_records([&](const FusedStep& s) {
+                mma_record<sizeof(acc) / sizeof(float), decltype(quad)::value>(acc, half_ops(s, wg, live));
+                return ((wg ? s.flags1 : s.flags) & kStepLast) != 0;
+            }, std::integral_constant<int, 1>(), clk_ring, clk_mma);
             wgmma_hold(acc);
-            mbar_arrive_if(bar(kBarWEmpty + prev), (et & 127) == 0);
         };
         using NoQuad = std::integral_constant<bool, false>;
 
@@ -359,8 +455,9 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
             }
         }
         // this row's running log_q (only this tile's units touch it): fetched now, used at the end of the unit
+        NFB_CLK(kClkClaim);
         float lq_old = 0.f;
-        if (rq == 0 && row_live && (layer > 0 || p.accumulate)) lq_old = __ldcg(p.logq + grow);
+        if (rq == 2 && row_live && (layer > 0 || p.accumulate)) lq_old = __ldcg(p.logq + grow);
         // ---- load z tile -> xs (coalesced global, swizzled shared) ----
         if (D == 64) {
             float4 v[kRows * 16 / kCons];
@@ -433,14 +530,15 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
                 return c >= 0 ? xs[xs_index(ar, c)] : 0.f;
             }, L.a_sc[1]);
         };
-        float ladsum = 0.f;
+        float ladsum = 0.f, lad_even = 0.f;   // (lad_even: warpgroup 1 in the final layer, see there)
         // fold_lu (density direction): the packer multiplied the first conditioner matrix into the LU map, so the first
         // hidden GEMM reads the SAME A operand as the LU stage (the split of z)
         const bool folded = uniform(!SAMPLE && L.has_lu && L.fold_lu);
         if (lu_steps) {
             store_a([&](int k) { return k < D ? xs[xs_index(ar, k)] : 0.f; }, L.a_sc[0]);
             float acc[32];
-            run_slice(acc, wg == 0, std::integral_constant<bool, true>());   // (no half for warpgroup 1)
+            NFB_CLK(kClkLoad);
+            run_slice(acc, wg == 0, std::integral_constant<bool, true>(), ClkPhase<kClkLu>(), ClkPhase<kClkLu>());   // (no half for warpgroup 1)
             if (wg == 0) {
                 // x' = acc + b (this thread: rows ra / rb, two columns of every 8-column group)
                 const float ia = ruinv(L.a_inv[0], ra), ib = ruinv(L.a_inv[0], rb);
@@ -452,6 +550,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
                 }
             }
             cons_bar_sync();   // x' of the whole tile is visible to both warpgroups
+            NFB_CLK(kClkLu);
         }
         auto store_tile = [&]() {  // xs -> global, coalesced
             if (D == 64) {
@@ -515,20 +614,26 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
             }
             if (!folded) build_a_net();   // (ends with a barrier: every thread has read its raw identity columns)
             if (!SAMPLE && L.n_id > 0) uncond();
+            NFB_CLK(kClkLoad);
 
+            // the final layer's splines all run on warpgroup 1: warpgroup 0's sums so far go with them
+            if (wg == 0) ldsum[rq * kRows + r] = ladsum;
             // ---- hidden layers: warpgroup wg owns the 64-column slices own(0), own(1) of every output (the packer's
             //      choice, nfb_fused_plan.h); a warpgroup without a slice passes the GEMM's records as one dead slice ----
-            float hres[2][32];   // its part of the residual stream h
+            // (Both are written first by a wgmma whose scale-d operand is a run-time flag, so to the compiler they would be
+            // read before they are written and stay live across the whole pass, final layer included: 128 registers
+            // the splines and the final layer's accumulators need.  The zeros end that; no product reads them.)
+            float hres[2][32] = {};   // its part of the residual stream h
             for (int ph = 0; ph < n_hidden; ++ph) {
                 const bool t_phase = (ph & 1) != 0;   // first GEMM of a residual block: its own accumulator
                 const bool relu = ph + 1 < n_hidden;
-                float tacc[2][32];
+                float tacc[2][32] = {};
 #pragma unroll
                 for (int q = 0; q < 2; ++q) {
                     const int j = own(q);
                     if (q == 0 || j >= 0) {
-                        if (t_phase) run_slice(tacc[q], j >= 0, NoQuad());
-                        else run_slice(hres[q], j >= 0, NoQuad());
+                        if (t_phase) run_slice(tacc[q], j >= 0, NoQuad(), ClkPhase<kClkHidRing>(), ClkPhase<kClkHidMma>());
+                        else run_slice(hres[q], j >= 0, NoQuad(), ClkPhase<kClkHidRing>(), ClkPhase<kClkHidMma>());
                     }
                 }
                 cons_bar_sync();   // every product of this GEMM has read the A operand: overwrite it with the output
@@ -566,55 +671,100 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
                 }
                 fence_proxy_async_smem();
                 cons_bar_sync();   // the next GEMM's A operand is complete
+                NFB_CLK(kClkHidEpi);
             }
 
-            // ---- final layer: record c = chunks 2c (warpgroup 0) and 2c + 1 (warpgroup 1), kFusedFeaturesPerChunk
-            //      features (x 24 columns) each -> staging -> one spline per thread ----
-            const float inv_f = ruinv(L.a_inv[1 + n_hidden], r);
-            const int f = (et >> 6) & 1;   // feature of the warpgroup's chunk this thread evaluates (for row r)
-            for (int ci = 0; ci < n_pairs; ++ci) {
-                float acc[kFusedFeaturesPerChunk * 12];
-                run_slice(acc, true, NoQuad());
+            // ---- final layer: record c = chunks 2c and 2c + 1, kFusedFeaturesPerChunk features (x 24 columns) each.
+            //      Warpgroup 0 multiplies both halves of every record and stores the two accumulators to the staging
+            //      tiles; warpgroup 1 takes them from there and evaluates the splines, two per thread and pair.  Neither
+            //      waits for the other except through the tiles ("full" / "free"), so the products of pair c + 1 run
+            //      under the splines of pair c. ----
+            if (wg == 0) {
+                for (int ci = 0; ci < n_pairs; ++ci) {
+                    float acc0[kFusedFeaturesPerChunk * 12] = {}, acc1[kFusedFeaturesPerChunk * 12] = {};   // (as hres: not live before)
+                    run_records([&](const FusedStep& s) {
+                        mma_record<kFusedFeaturesPerChunk * 12, false>(acc0, half_ops(s, 0, true), acc1, half_ops(s, 1, true));
+                        return (s.flags & kStepLast) != 0;   // (the pair's last record is the same for both halves)
+                    }, std::integral_constant<int, 2>(), ClkPhase<kClkFinRing>(), ClkPhase<kClkFinMma>());
+                    wgmma_hold(acc0);
+                    wgmma_hold(acc1);
+                    // (no slot is held here: the producer can deliver the next pair's records while this waits)
+                    if (ci > 0) stg_bar_wait<kBarStgFree>();   // the previous pair's parameters have been taken
 #pragma unroll
-                for (int i = 0; i < kFusedFeaturesPerChunk * 12; i += 2) {
-                    const int c = 8 * (i >> 2) + cq;
-                    *reinterpret_cast<float2*>(stg + ((i & 2) ? rb : ra) * kStgLd + c) = make_float2(acc[i], acc[i + 1]);
-                }
-                wg_bar_sync(wg);
-                const int t = (2 * ci + wg) * L.F + f;
-                if (t < L.T) {
-                    // the packer folded log2(e) (and the layer's 1/sqrt(H)) into the w/h columns and biases
-                    const float4* sp = reinterpret_cast<const float4*>(stg + r * kStgLd + 24 * f);
-                    const float4* bp = reinterpret_cast<const float4*>(L.bias_f + t * 24);
-                    float pv[24];
-#pragma unroll
-                    for (int q = 0; q < 6; ++q) {
-                        const float4 s4 = sp[q], b4 = __ldg(bp + q);
-                        pv[4 * q] = fmaf(s4.x, inv_f, b4.x);
-                        pv[4 * q + 1] = fmaf(s4.y, inv_f, b4.y);
-                        pv[4 * q + 2] = fmaf(s4.z, inv_f, b4.z);
-                        pv[4 * q + 3] = fmaf(s4.w, inv_f, b4.w);
+                    for (int i = 0; i < kFusedFeaturesPerChunk * 12; i += 2) {
+                        float* dst = stg0 + ((i & 2) ? rb : ra) * kStgLd + 8 * (i >> 2) + cq;
+                        *reinterpret_cast<float2*>(dst) = make_float2(acc0[i], acc0[i + 1]);
+                        *reinterpret_cast<float2*>(dst + kRows * kStgLd) = make_float2(acc1[i], acc1[i + 1]);
                     }
-                    float lw[8], lh[8], dd[8];
-#pragma unroll
-                    for (int q = 0; q < 8; ++q) { lw[q] = pv[q]; lh[q] = pv[8 + q]; dd[q] = pv[16 + q]; }
-                    const int col = L.tr_idx[t];
-                    float y, l;
-                    float xin = get_x(col);
-                    if (arsamp) xin = row_live ? __ldcg(zdst + grow * D + col) : 0.f;
-                    rqs_core<8, SAMPLE>(xin, lw, lh, [&dd](int k) { return dd[k]; }, L.tail, y, l);
-                    put_y(col, y);
-                    ladsum += l;
+                    stg_bar_arrive<kBarStgFull>();
+                    NFB_CLK(kClkFinStage);
                 }
-                wg_bar_sync(wg);   // the staging tile is free again
+            } else {
+                // It does not walk the final layer's records (the last of the step table): its cursors move past them
+                // as run_records moves warpgroup 0's.
+                if (n_pairs > 0) {
+                    const uint32_t adv = slot + (uint32_t)(n_steps - sidx);
+                    slot = adv % kSlots;
+                    wpar ^= (adv / kSlots) & 1u;
+                    sidx = lu_steps;
+                }
+                // Row r's log-det partial sums keep their membership and order: lad_even continues the sum of the
+                // warpgroup-0 thread of (row, f) over the even chunks, ladsum this thread's own over the odd chunks.
+                const float inv_f = ruinv(L.a_inv[1 + n_hidden], r);
+                const int f = (et >> 6) & 1;   // feature of each chunk this thread evaluates (for row r)
+                lad_even = ldsum[f * kRows + r];
+                for (int ci = 0; ci < n_pairs; ++ci) {
+                    stg_bar_wait<kBarStgFull>();
+                    // One spline after the other, as a loop: two evaluations in one block need more registers than
+                    // a thread has, and spills go through the little L1 the shared memory leaves.  The tiles are
+                    // handed back when the second spline's parameters are in registers.
+#pragma unroll 1
+                    for (int h = 0; h < 2; ++h) {
+                        const int t = (2 * ci + h) * L.F + f;
+                        // the packer folded log2(e) (and the layer's 1/sqrt(H)) into the w/h columns and biases
+                        const float4* sp = reinterpret_cast<const float4*>(stg0 + (h * kRows + r) * kStgLd + 24 * f);
+                        const float4* bp = reinterpret_cast<const float4*>(L.bias_f + t * 24);
+                        float pv[24];
+#pragma unroll
+                        for (int q = 0; q < 6; ++q) {
+                            const float4 s4 = sp[q], b4 = __ldg(bp + q);
+                            pv[4 * q] = fmaf(s4.x, inv_f, b4.x);
+                            pv[4 * q + 1] = fmaf(s4.y, inv_f, b4.y);
+                            pv[4 * q + 2] = fmaf(s4.z, inv_f, b4.z);
+                            pv[4 * q + 3] = fmaf(s4.w, inv_f, b4.w);
+                        }
+                        if (h == 1 && ci + 1 < n_pairs) stg_bar_arrive<kBarStgFree>();   // (the last pair's tiles have no next writer)
+                        NFB_CLK(kClkFinStage);
+                        if (t < L.T) {
+                            float lw[8], lh[8], dd[8];
+#pragma unroll
+                            for (int q = 0; q < 8; ++q) { lw[q] = pv[q]; lh[q] = pv[8 + q]; dd[q] = pv[16 + q]; }
+                            const int col = L.tr_idx[t];
+                            float y, l;
+                            float xin = get_x(col);
+                            if (arsamp) xin = row_live ? __ldcg(zdst + grow * D + col) : 0.f;
+                            rqs_core<8, SAMPLE>(xin, lw, lh, [&dd](int k) { return dd[k]; }, L.tail, y, l);
+                            put_y(col, y);
+                            if (h) ladsum += l;
+                            else lad_even += l;
+                        }
+                        NFB_CLK(kClkFinSpline);
+                    }
+                }
             }
             cons_bar_sync();   // (AR sampling: every output of this pass is in xs before the next pass reads it)
         }  // passes
-        // ---- log-det reduction over the four threads of each row, then store ----
-        if (rq > 0) ldsum[(rq - 1) * kRows + r] = ladsum;
+        // ---- log-det reduction over the four partial sums of each row (warpgroup 1 holds them: threads f = 0 the sums
+        //      that began in quarters 0 and 2 of the threads, threads f = 1 those of quarters 1 and 3; added in quarter
+        //      order), then store ----
+        NFB_CLK(kClkFinStage);
+        if (rq == 3) {
+            ldsum[r] = lad_even;
+            ldsum[kRows + r] = ladsum;
+        }
         cons_bar_sync();
-        if (rq == 0 && row_live) {
-            const float tot = ladsum + ldsum[r] + ldsum[kRows + r] + ldsum[2 * kRows + r] +
+        if (rq == 2 && row_live) {
+            const float tot = lad_even + ldsum[r] + ladsum + ldsum[kRows + r] +
                               (L.lu_logdet ? __ldg(L.lu_logdet) : 0.f);
             __stcg(p.logq + grow, tot + lq_old);
         }
@@ -628,7 +778,9 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
             __threadfence();
             asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p.progress + tile), "r"(layer + 1) : "memory");
         }
+        NFB_CLK(kClkStore);
     }
+    NFB_CLK_END(wg, (et & 127) == 0);
 }
 
 int launch_fused_rqs(const FusedParams& p, int sm_count, int sample, cudaStream_t st) {
@@ -653,6 +805,19 @@ int launch_fused_rqs(const FusedParams& p, int sm_count, int sample, cudaStream_
     NFB_LAUNCH_CHECK();
     return NFB_OK;
 }
+
+#ifdef NFB_PHASE_CLOCKS
+// out[3][kClkCount]: the sums of every fused launch on the current device since the last reset (synchronises the device)
+extern "C" __attribute__((visibility("default"))) int nfb_phase_clocks_read(unsigned long long* out, int reset) {
+    NFB_CUDA(cudaDeviceSynchronize());
+    if (out) NFB_CUDA(cudaMemcpyFromSymbol(out, g_phase_clocks, sizeof(g_phase_clocks)));
+    if (reset) {
+        const unsigned long long zero[3][kClkCount] = {};
+        NFB_CUDA(cudaMemcpyToSymbol(g_phase_clocks, zero, sizeof(zero)));
+    }
+    return NFB_OK;
+}
+#endif
 
 // -----------------------------------------------------------------------------------------
 // packing: fp32 effective matrix [n_pad x k_pad] -> stream of swizzled bf16 split records
