@@ -478,6 +478,18 @@ typedef struct { int32_t features; const float* s; const float* t; } nfb_affine_
 /* flows/mixing.py:9-54 Permute: forward z[:, perm], inverse z[:, inv_perm] (host int32 arrays) */
 typedef struct { int32_t features; const int32_t* perm; const int32_t* inv_perm; } nfb_permute_desc_t;
 
+/* flows/planar.py Planar: x = z + u_hat h(w.z + b), u_hat = u + (log(1 + exp(w.u)) - 1 - w.u) w / |w|^2.  u, w [features],
+ * b [1]; act NFB_PLANAR_TANH or NFB_PLANAR_LEAKY_RELU (negative slope `slope`); features <= 64.  Only the leaky-ReLU
+ * layer has a density direction (NFB_INVERSE on a group holding any other planar / radial layer: NFB_ERR_UNSUPPORTED). */
+#define NFB_PLANAR_TANH 0
+#define NFB_PLANAR_LEAKY_RELU 1
+typedef struct { int32_t features; const float* u; const float* w; const float* b; int32_t act; float slope; } nfb_planar_desc_t;
+
+/* flows/radial.py Radial: x = z + h (z - z0), h = beta_hat / (|alpha| + |z - z0|), beta_hat = log(1 + exp(beta)) - |alpha|.
+ * beta, alpha [1], z0 [features]; features <= 64; sampling direction only.  Consecutive planar / radial layers run as one
+ * launch that forms every layer's constants on the device (a parameter update needs no repack). */
+typedef struct { int32_t features; const float* beta; const float* alpha; const float* z0; } nfb_radial_desc_t;
+
 /* ---- flow object: an ordered list of layers + base density, packed for the device ---- */
 int nfb_flow_create(nfb_flow_t** out, int32_t features);
 int nfb_flow_destroy(nfb_flow_t* f);
@@ -488,6 +500,8 @@ int nfb_flow_add_masked_affine(nfb_flow_t* f, const nfb_masked_affine_desc_t* d)
 int nfb_flow_add_affine_coupling(nfb_flow_t* f, const nfb_affine_coupling_desc_t* d);
 int nfb_flow_add_affine_const(nfb_flow_t* f, const nfb_affine_const_desc_t* d);
 int nfb_flow_add_permute(nfb_flow_t* f, const nfb_permute_desc_t* d);
+int nfb_flow_add_planar(nfb_flow_t* f, const nfb_planar_desc_t* d);
+int nfb_flow_add_radial(nfb_flow_t* f, const nfb_radial_desc_t* d);
 /* q0 = DiagGaussian(features): loc/log_scale [features] (distributions/base.py:71-76) */
 int nfb_flow_set_base_diag_gaussian(nfb_flow_t* f, const float* loc_dev, const float* log_scale_dev);
 /* pack parameters; `use_tensor_cores`=0 forces the plain-fp32 kernels for every layer (A/B parity) */
@@ -528,20 +542,25 @@ int nfb_flow_forward_kld(nfb_flow_t* f, const float* x_dev, int64_t rows, float*
  *   LULinearPermute : lower_entries, upper_entries, unconstrained_upper_diag, bias
  *   MaskedAffineFlow : net.<i>.weight, .bias of every Linear of s, then of t (an absent net has none)
  *   AffineConstFlow / ActNorm : s, t       AffineCouplingBlock : param_map's Linears       Permute : none
+ *   Planar : u, w, b       Radial : beta, alpha, z_0
  *   base (last two slots) : loc, log_scale
  * `grad_slots[i]` is a device buffer of nfb_flow_grad_slot_numel(f, i) floats that is OVERWRITTEN, or NULL to skip.
- * nfb_flow_num_grad_slots returns -1 when the flow holds a layer kind without a native backward.  The affine family's
- * slots serve nfb_flow_sampling_backward only: nfb_flow_log_prob_backward rejects affine groups (NFB_ERR_UNSUPPORTED). */
+ * nfb_flow_num_grad_slots returns -1 when the flow holds a layer kind without a native backward.  The affine and planar
+ * families' slots serve nfb_flow_sampling_backward only: nfb_flow_log_prob_backward rejects their groups
+ * (NFB_ERR_UNSUPPORTED). */
 int nfb_flow_num_grad_slots(const nfb_flow_t* f);
 int64_t nfb_flow_grad_slot_numel(const nfb_flow_t* f, int32_t slot);
 int nfb_flow_log_prob_backward(nfb_flow_t* f, const float* x_dev, const float* g_logq_dev, int64_t rows,
                                float* log_q_dev /* optional out */, float* gx_dev /* optional out */,
                                float* const* grad_slots, void* stream);
 
-/* ---- sampling-direction backward of an all-affine stack (reverse_kld / reverse_alpha_div of examples/real_nvp.ipynb)
- * Gradients of sum_r <g_x[r], x_r> + g_ld[r] log_det_r, with (x, log_det) = nfb_flow_transform(f, NFB_FORWARD, z),
- * w.r.t. z and every parameter, for stacks of MaskedAffineFlow, AffineConstFlow / ActNorm, AffineCouplingBlock and
- * Permute only (any other layer: NFB_ERR_UNSUPPORTED).  z is the input that nfb_flow_transform was given.  The call
+/* ---- sampling-direction backward of an all-affine or all-planar/radial stack (reverse_kld / reverse_alpha_div of
+ * examples/real_nvp.ipynb, planar.ipynb) -- gradients of sum_r <g_x[r], x_r> + g_ld[r] log_det_r, with (x, log_det) =
+ * nfb_flow_transform(f, NFB_FORWARD, z), w.r.t. z and every parameter, for stacks of MaskedAffineFlow, AffineConstFlow /
+ * ActNorm, AffineCouplingBlock and Permute only, or of Planar and Radial only (any other stack, mixes of the two
+ * families included: NFB_ERR_UNSUPPORTED).  z is the input that nfb_flow_transform was given.  A planar / radial stack
+ * reduces each layer's row terms the same way, then takes the sums through u_hat(u, w), softplus(beta) and |alpha| in
+ * one more launch (3 launches per chunk of rows + 1).  The affine call
  * recomputes the stack from z (the forward kernel's own arithmetic), walks the ops in reverse in one kernel, then reduces
  * every Linear's weight and bias gradient in a fixed order (no atomics: two calls give identical bits).  Rows run in
  * chunks, so the workspace (nfb_flow_sampling_backward_workspace_bytes, -1 for an unsupported stack) stays below a fixed

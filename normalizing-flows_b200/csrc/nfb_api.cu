@@ -20,6 +20,7 @@
 
 #include "../../include/nfb200.h"
 #include "nfb_kernels.h"
+#include "nfb_planar_bwd.cuh"
 
 static thread_local std::string g_err;
 static constexpr float kLog2eHost = 1.4426950408889634f;
@@ -130,7 +131,8 @@ int download(const T* dev, size_t n, std::vector<T>& out) {
 
 #define NFB_TRY(expr) do { int rc__ = (expr); if (rc__) return rc__; } while (0)
 
-enum LayerKind { L_AR_RQS, L_COUPLED_RQS, L_LU, L_MASKED_AFFINE, L_AFFINE_COUPLING, L_AFFINE_CONST, L_PERMUTE };
+enum LayerKind { L_AR_RQS, L_COUPLED_RQS, L_LU, L_MASKED_AFFINE, L_AFFINE_COUPLING, L_AFFINE_CONST, L_PERMUTE, L_PLANAR,
+                 L_RADIAL };
 
 struct NetDesc {  // deep copy of nfb_resnet_desc_t
     int in = 0, H = 0, out = 0, nb = 0;
@@ -207,9 +209,11 @@ struct Layer {
     AffineOp op{};
     std::vector<int> perm_fwd, perm_inv;
     DevBuf perm_fwd_dev, perm_inv_dev;
+    // planar / radial
+    PlanarOp pop{};
 };
 
-enum GroupKind { G_FUSED_PAIR, G_FUSED, G_AFFINE, G_SINGLE };
+enum GroupKind { G_FUSED_PAIR, G_FUSED, G_AFFINE, G_PLANAR, G_SINGLE };
 struct Group {
     GroupKind kind; int first, last; DevBuf ops;
     // affine group, sampling-direction backward: workspace plan (units per row), per-op unit table and the weight
@@ -219,6 +223,10 @@ struct Group {
     long long n_elem = 0;
     DevBuf bops;
     std::vector<AffRedItem> items;
+    // planar group: the layers' descriptors (with their workspace plan), the reduction's items (outputs relative to the
+    // sums, rebased per call), workspace units per row, and whether every layer has a density direction
+    std::vector<PlanarOp> pops;
+    bool invertible = true;
 };
 
 }  // namespace
@@ -260,7 +268,14 @@ struct nfb_flow {
     size_t afb_cap = 0;
     cudaEvent_t afb_ev = nullptr;
     DevBuf afb_items;
+    // planar sampling backward: reduction items and per-layer gradient outputs of this call, staged the same way
+    char* plb_host = nullptr;
+    size_t plb_cap = 0;
+    cudaEvent_t plb_ev = nullptr;
+    DevBuf plb_dev;
     ~nfb_flow() {
+        if (plb_ev) cudaEventDestroy(plb_ev);
+        if (plb_host) cudaFreeHost(plb_host);
         if (afb_ev) cudaEventDestroy(afb_ev);
         if (afb_host) cudaFreeHost(afb_host);
         if (copy_stream) cudaStreamDestroy(copy_stream);
@@ -995,6 +1010,8 @@ bool is_affine_kind(const Layer& L) {
            L.kind == L_PERMUTE;
 }
 
+bool is_planar_kind(const Layer& L) { return L.kind == L_PLANAR || L.kind == L_RADIAL; }
+
 int copy_mlp(const nfb_mlp_desc_t& d, AffMlp& m, float* slope) {
     NFB_CHECK(d.num_layers >= 0 && d.num_layers <= kAffMaxLayers, NFB_ERR_UNSUPPORTED, "MLP: %d layers > %d", d.num_layers, kAffMaxLayers);
     m.n_layers = d.num_layers;
@@ -1036,6 +1053,11 @@ int run_group(nfb_flow* f, Group& g, int direction, const float* zin, float* zou
         break;
     case G_AFFINE:
         NFB_TRY(launch_affine_stack(g.ops.p, g.last - g.first + 1, zin, zout, logdet, rows, f->D, 1, direction, st));
+        f->launches++;
+        return NFB_OK;
+    case G_PLANAR:
+        NFB_CHECK(direction == NFB_FORWARD || g.invertible, NFB_ERR_UNSUPPORTED, "This flow has no algebraic inverse.");
+        NFB_TRY(launch_planar_stack(g.ops.p, g.last - g.first + 1, zin, zout, logdet, rows, f->D, 1, direction, st));
         f->launches++;
         return NFB_OK;
     case G_SINGLE:
@@ -2192,6 +2214,29 @@ int nfb_flow_add_permute(nfb_flow_t* f, const nfb_permute_desc_t* d) {
     return NFB_OK;
 }
 
+int nfb_flow_add_planar(nfb_flow_t* f, const nfb_planar_desc_t* d) {
+    NFB_NEW_LAYER(L_PLANAR);
+    NFB_CHECK(f->D <= kPlanarMaxD, NFB_ERR_UNSUPPORTED, "Planar: features %d > %d", f->D, kPlanarMaxD);
+    NFB_CHECK(d->u && d->w && d->b, NFB_ERR_ARG, "Planar: null parameter");
+    NFB_CHECK(d->act == NFB_PLANAR_TANH || d->act == NFB_PLANAR_LEAKY_RELU, NFB_ERR_UNSUPPORTED,
+              "Nonlinearity is not implemented.");
+    L->pop.type = d->act == NFB_PLANAR_TANH ? kPlanarTanh : kPlanarLeaky;
+    L->pop.slope = d->slope;
+    L->pop.a = d->u; L->pop.w = d->w; L->pop.b = d->b;
+    f->layers.push_back(std::move(L));
+    return NFB_OK;
+}
+
+int nfb_flow_add_radial(nfb_flow_t* f, const nfb_radial_desc_t* d) {
+    NFB_NEW_LAYER(L_RADIAL);
+    NFB_CHECK(f->D <= kPlanarMaxD, NFB_ERR_UNSUPPORTED, "Radial: features %d > %d", f->D, kPlanarMaxD);
+    NFB_CHECK(d->beta && d->alpha && d->z0, NFB_ERR_ARG, "Radial: null parameter");
+    L->pop.type = kRadial;
+    L->pop.a = d->z0; L->pop.b = d->beta; L->pop.alpha = d->alpha;
+    f->layers.push_back(std::move(L));
+    return NFB_OK;
+}
+
 int nfb_flow_set_base_diag_gaussian(nfb_flow_t* f, const float* loc, const float* log_scale) {
     NFB_CHECK(f && loc && log_scale, NFB_ERR_ARG, "null argument");
     f->base_loc = loc; f->base_log_scale = log_scale;
@@ -2361,6 +2406,35 @@ int nfb_flow_finalize(nfb_flow_t* f, int32_t use_tensor_cores, void* stream) {
             NFB_TRY(g.ops.upload(ops));
             f->groups.push_back(std::move(g));
             i = j + 1;
+        } else if (is_planar_kind(L)) {
+            // one launch for the run: every layer's constants are formed on the device, so a parameter update needs no
+            // repack.  Workspace plan of the sampling backward: planar 2D + 3 units / sums per layer, radial D + 2
+            int j = i;
+            while (j + 1 < n && is_planar_kind(*f->layers[j + 1])) ++j;
+            Group g; g.kind = G_PLANAR; g.first = i; g.last = j;
+            const int D = f->D;
+            int u = 0;
+            long long e = 0;
+            for (int k = i; k <= j; ++k) {
+                PlanarOp op = f->layers[k]->pop;
+                const int w = op.type == kRadial ? D + 2 : 2 * D + 3;
+                op.u_off = u; op.s_off = (int)e;
+                if (op.type == kRadial) {   // column sums of g_dz, the beta_hat and the alpha_hat terms
+                    g.items.push_back(AffRedItem{-1, u, 0, D + 2, e, nullptr, nullptr});
+                } else {                    // sum c z and sum c; sum h g (and sum h, unused); sum e
+                    g.items.push_back(AffRedItem{u, u + 2 * D, D, 1, e, nullptr, nullptr});
+                    g.items.push_back(AffRedItem{u + D, u + 2 * D + 1, D, 1, e + D + 1, nullptr, nullptr});
+                    g.items.push_back(AffRedItem{-1, u + 2 * D + 2, 0, 1, e + 2 * D + 2, nullptr, nullptr});
+                }
+                g.invertible = g.invertible && op.type == kPlanarLeaky;
+                g.pops.push_back(op);
+                u += w; e += w;
+            }
+            g.units = u;
+            g.n_elem = e;
+            NFB_TRY(g.ops.upload(g.pops));
+            f->groups.push_back(std::move(g));
+            i = j + 1;
         } else {
             Group g; g.kind = G_SINGLE; g.first = g.last = i;
             f->groups.push_back(std::move(g));
@@ -2420,7 +2494,17 @@ int nfb_flow_layer_apply(nfb_flow_t* f, int32_t index, int32_t direction, const 
     }
     if (log_det && !accumulate) NFB_TRY(launch_fill(log_det, rows, 0.f, st));
     int rc;
-    if (is_affine_kind(L)) {
+    if (is_planar_kind(L)) {
+        // the group holding the layer has its descriptor in place: launch that one entry
+        const Group* gp = nullptr;
+        for (auto& g : f->groups)
+            if (g.kind == G_PLANAR && index >= g.first && index <= g.last) gp = &g;
+        NFB_CHECK(gp, NFB_ERR_STATE, "planar layer outside a planar group");
+        NFB_CHECK(direction == NFB_FORWARD || L.pop.type == kPlanarLeaky, NFB_ERR_UNSUPPORTED,
+                  "This flow has no algebraic inverse.");
+        rc = launch_planar_stack(static_cast<const PlanarOp*>(gp->ops.p) + (index - gp->first), 1, z_in, out, log_det,
+                                 rows, f->D, 1, direction, st);
+    } else if (is_affine_kind(L)) {
         DevBuf ops;
         std::vector<AffineOp> v{L.op};
         NFB_TRY(ops.upload(v));
@@ -2449,6 +2533,13 @@ int nfb_flow_transform(nfb_flow_t* f, int32_t direction, const float* z_in, floa
     if (rows == 0) return NFB_OK;
     NFB_TRY(ensure_ws(f, rows));
     float* ld = log_det ? log_det : f->logq.as<float>();
+    if (f->groups.size() == 1 && f->groups[0].kind == G_PLANAR && z_in != z_out) {   // one launch, log-det written
+        Group& g = f->groups[0];
+        NFB_CHECK(direction == NFB_FORWARD || g.invertible, NFB_ERR_UNSUPPORTED, "This flow has no algebraic inverse.");
+        NFB_TRY(launch_planar_stack(g.ops.p, g.last - g.first + 1, z_in, z_out, ld, rows, f->D, 0, direction, st));
+        f->launches++;
+        return NFB_OK;
+    }
     NFB_TRY(launch_fill(ld, rows, 0.f, st));
     f->launches++;
     if (direction == NFB_INVERSE && f->stack_n > 0)
@@ -2607,12 +2698,17 @@ int grad_slots_of(const Layer& L) {
     case L_AFFINE_CONST: return 2;
     case L_AFFINE_COUPLING: return 2 * L.op.s.n_layers;
     case L_PERMUTE: return 0;
+    // planar: u, w, b; radial: beta, alpha, z_0 (registration order)
+    case L_PLANAR: return 3;
+    case L_RADIAL: return 3;
     default: return -1;
     }
 }
 long long grad_slot_numel(const Layer& L, int s) {
     const NetDesc& n = L.net;
     if (L.kind == L_AFFINE_CONST) return L.D;
+    if (L.kind == L_PLANAR) return s == 2 ? 1 : L.D;
+    if (L.kind == L_RADIAL) return s == 2 ? L.D : 1;
     if (L.kind == L_MASKED_AFFINE || L.kind == L_AFFINE_COUPLING) {
         const bool t_net = L.kind == L_MASKED_AFFINE && s >= 2 * L.op.s.n_layers;
         const AffMlp& m = t_net ? L.op.t : L.op.s;
@@ -2761,8 +2857,9 @@ int nfb_flow_log_prob_backward(nfb_flow_t* f, const float* x, const float* g_log
     NFB_CHECK(x && g_logq && grad_slots, NFB_ERR_ARG, "null pointer");
     const int n_slots = nfb_flow_num_grad_slots(f);
     NFB_CHECK(n_slots >= 0, NFB_ERR_UNSUPPORTED, "native backward covers spline blocks + LULinearPermute + DiagGaussian");
-    for (auto& grp : f->groups)   // (the affine family has slots for its sampling-direction backward only)
-        NFB_CHECK(grp.kind != G_AFFINE, NFB_ERR_UNSUPPORTED, "native backward: affine-family group");
+    for (auto& grp : f->groups)   // (the affine and planar families have slots for their sampling-direction backward only)
+        NFB_CHECK(grp.kind != G_AFFINE && grp.kind != G_PLANAR, NFB_ERR_UNSUPPORTED,
+                  "native backward: affine- or planar-family group");
     if (rows == 0) return NFB_OK;
     cudaStream_t st = S(stream);
     const int D = f->D;
@@ -2909,10 +3006,88 @@ size_t affine_bwd_ws_bytes(const Group& g, long long R) {
     return data + (size_t)((R + kAffSegRows - 1) / kAffSegRows) * g.n_elem * 4;
 }
 
+// planar group: the same chunking, plus the reduced sums (n_elem floats) after the segment partials
+long long planar_bwd_chunk_rows(const Group& g, long long rows) {
+    const long long per_row = 4ll * g.units + (4 * g.n_elem + kAffSegRows - 1) / kAffSegRows + 1;
+    long long R = std::max(1ll, (kAffBwdWsCap - 4 * g.n_elem) / per_row);
+    if (R > kAffSegRows) R -= R % kAffSegRows;
+    return std::max(1ll, std::min(R, rows));
+}
+
+size_t planar_bwd_partial_off(const Group& g, long long R) { return ((size_t)g.units * R * 4 + 255) & ~(size_t)255; }
+
+size_t planar_bwd_sums_off(const Group& g, long long R) {
+    return (planar_bwd_partial_off(g, R) + (size_t)((R + kAffSegRows - 1) / kAffSegRows) * g.n_elem * 4 + 255) &
+           ~(size_t)255;
+}
+
+size_t planar_bwd_ws_bytes(const Group& g, long long R) { return planar_bwd_sums_off(g, R) + (size_t)g.n_elem * 4; }
+
+Group* planar_only_group(nfb_flow* f) {
+    return (f && f->finalized && f->groups.size() == 1 && f->groups[0].kind == G_PLANAR) ? &f->groups[0] : nullptr;
+}
+
+// sampling backward of a stack that is one planar / radial group: per chunk of rows the row kernel and the fixed-order
+// reduction (2 launches) into the sums, then one launch through the parameter maps into the slots
+int planar_sampling_backward(nfb_flow* f, Group& g, const float* z, const float* g_x, const float* g_ld, int64_t rows,
+                             void* ws, int64_t ws_bytes, float* g_z, float* const* grad_slots, cudaStream_t st) {
+    NFB_CHECK(rows >= 0, NFB_ERR_ARG, "rows < 0");
+    NFB_CHECK(rows == 0 || z, NFB_ERR_ARG, "null z");
+    const long long R = planar_bwd_chunk_rows(g, rows);
+    NFB_CHECK(ws && ws_bytes >= (int64_t)planar_bwd_ws_bytes(g, R), NFB_ERR_ARG,
+              "sampling backward: workspace of %lld bytes, %lld needed", (long long)ws_bytes,
+              (long long)planar_bwd_ws_bytes(g, R));
+    f->launches = 0;
+    const int n_items = (int)g.items.size(), n_ops = (int)g.pops.size();
+    float* W = static_cast<float*>(ws);
+    float* partial = reinterpret_cast<float*>(static_cast<char*>(ws) + planar_bwd_partial_off(g, R));
+    float* sums = reinterpret_cast<float*>(static_cast<char*>(ws) + planar_bwd_sums_off(g, R));
+    // this call's reduction outputs (into the sums) and gradient slots (three per layer), staged through pinned memory
+    const size_t items_bytes = n_items * sizeof(AffRedItem), bytes = items_bytes + n_ops * sizeof(PlanarGradOut);
+    if (!f->plb_ev) NFB_CUDA(cudaEventCreateWithFlags(&f->plb_ev, cudaEventDisableTiming));
+    else NFB_CUDA(cudaEventSynchronize(f->plb_ev));   // the previous call's staging copy has been read
+    if (f->plb_cap < bytes) {
+        if (f->plb_host) cudaFreeHost(f->plb_host);
+        f->plb_host = nullptr; f->plb_cap = 0;
+        NFB_CUDA(cudaMallocHost(reinterpret_cast<void**>(&f->plb_host), bytes));
+        f->plb_cap = bytes;
+    }
+    AffRedItem* items = reinterpret_cast<AffRedItem*>(f->plb_host);
+    for (int i = 0; i < n_items; ++i) {
+        AffRedItem it = g.items[i];
+        if (it.n_in > 0) it.dw = sums + it.e_off;
+        it.db = sums + it.e_off + (long long)it.n_out * it.n_in;
+        items[i] = it;
+    }
+    PlanarGradOut* outs = reinterpret_cast<PlanarGradOut*>(f->plb_host + items_bytes);
+    for (int k = 0; k < n_ops; ++k)
+        for (int s = 0; s < 3; ++s) outs[k].g[s] = grad_slots ? grad_slots[3 * k + s] : nullptr;
+    NFB_TRY(f->plb_dev.reserve(bytes));
+    NFB_CUDA(cudaMemcpyAsync(f->plb_dev.p, f->plb_host, bytes, cudaMemcpyHostToDevice, st));
+    NFB_CUDA(cudaEventRecord(f->plb_ev, st));
+    const void* items_dev = f->plb_dev.p;
+    const void* outs_dev = static_cast<char*>(f->plb_dev.p) + items_bytes;
+    const int D = f->D;
+    if (rows == 0) {   // zero sums
+        NFB_TRY(launch_affine_bwd_reduce(items_dev, n_items, g.n_elem, W, 0, partial, 0, st));
+        f->launches++;
+    }
+    for (long long r0 = 0; r0 < rows; r0 += R) {
+        const long long n = std::min(R, (long long)rows - r0);
+        NFB_TRY(launch_planar_bwd_rows(g.ops.p, n_ops, z + r0 * D, g_x ? g_x + r0 * D : nullptr, g_ld ? g_ld + r0 : nullptr,
+                                       g_z ? g_z + r0 * D : nullptr, W, n, D, st));
+        NFB_TRY(launch_affine_bwd_reduce(items_dev, n_items, g.n_elem, W, n, partial, r0 > 0, st));
+        f->launches += 3;
+    }
+    NFB_TRY(launch_planar_bwd_chain(g.ops.p, outs_dev, n_ops, sums, D, st));
+    f->launches++;
+    return NFB_OK;
+}
+
 int affine_only_group(nfb_flow* f, Group** out) {
     NFB_CHECK(f && f->finalized, NFB_ERR_STATE, "flow not finalized");
     NFB_CHECK(f->groups.size() == 1 && f->groups[0].kind == G_AFFINE, NFB_ERR_UNSUPPORTED,
-              "sampling backward: the stack must be affine-family layers only");
+              "sampling backward: the stack must be affine-family layers only, or planar / radial layers only");
     *out = &f->groups[0];
     return plan_affine_bwd(f, **out);
 }
@@ -2923,13 +3098,16 @@ extern "C" {
 
 int64_t nfb_flow_sampling_backward_workspace_bytes(const nfb_flow_t* fc, int64_t rows) {
     nfb_flow* f = const_cast<nfb_flow*>(fc);
-    Group* g = nullptr;
+    Group* g = planar_only_group(f);
+    if (g) return rows < 0 ? -1 : (int64_t)planar_bwd_ws_bytes(*g, planar_bwd_chunk_rows(*g, rows));
     if (rows < 0 || affine_only_group(f, &g) != NFB_OK) return -1;
     return (int64_t)affine_bwd_ws_bytes(*g, affine_bwd_chunk_rows(*g, rows));
 }
 
 int nfb_flow_sampling_backward(nfb_flow_t* f, const float* z, const float* g_x, const float* g_ld, int64_t rows,
                                void* ws, int64_t ws_bytes, float* g_z, float* const* grad_slots, void* stream) {
+    if (Group* pg = planar_only_group(f))
+        return planar_sampling_backward(f, *pg, z, g_x, g_ld, rows, ws, ws_bytes, g_z, grad_slots, S(stream));
     Group* gp = nullptr;
     NFB_TRY(affine_only_group(f, &gp));
     Group& g = *gp;

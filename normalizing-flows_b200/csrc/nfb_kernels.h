@@ -171,6 +171,26 @@ int launch_affine_bwd_rows(const void* ops_dev, const void* bops_dev, int n_ops,
 int launch_affine_bwd_reduce(const void* items_dev, int n_items, long long n_elem, const float* ws, long long R,
                              float* partial, int accumulate, cudaStream_t st);
 
+// ---- planar / radial stack (nfb_planar.cu) ----
+constexpr int kPlanarMaxD = 64;
+struct PlanarOp {
+    int type;            // kPlanarTanh, kPlanarLeaky, kRadial (nfb_planar_bwd.cuh)
+    float slope;         // leaky planar: negative slope
+    const float* a;      // planar: u[D] ; radial: z_0[D]
+    const float* w;      // planar: w[D]
+    const float* b;      // planar: b[1] ; radial: beta[1]
+    const float* alpha;  // radial: alpha[1]
+    int u_off;           // sampling backward: first workspace unit of the layer (planar 2D + 3 units, radial D + 2)
+    int s_off;           // sampling backward: first of the layer's reduced sums (planar 2D + 3, radial D + 2)
+};
+struct PlanarGradOut { float* g[3]; };   // planar: g_u, g_w, g_b ; radial: g_beta, g_alpha, g_z0 (each may be null)
+int launch_planar_stack(const void* ops_dev, int n_ops, const float* zin, float* zout, float* logq, long long rows,
+                        int d, int accumulate, int direction, cudaStream_t st);
+int launch_planar_bwd_rows(const void* ops_dev, int n_ops, const float* zin, const float* gx, const float* gld,
+                           float* gz, float* ws, long long R, int d, cudaStream_t st);
+int launch_planar_bwd_chain(const void* ops_dev, const void* outs_dev, int n_ops, const float* sums, int d,
+                            cudaStream_t st);
+
 // ---- fused neural-spline block (nfb_fused_rqs.cu) ----
 constexpr int kFusedTileRows = 64;          // rows of a work unit (the M of one wgmma)
 constexpr int kFusedFeaturesPerChunk = 2;   // spline features per final-layer record (N = 24 per feature)

@@ -64,7 +64,7 @@ def _resnet(net, x, masked):
 
 def layer_inverse(layer, z):
     """(z', log_det[B]) of `layer.inverse(z)` in differentiable torch ops."""
-    from .flows import neural_spline as ns, mixing, affine
+    from .flows import neural_spline as ns, mixing, affine, planar
     b = z.shape[0]
     if isinstance(layer, ns.AutoregressiveRationalQuadraticSpline):
         k = layer.num_bins
@@ -124,6 +124,17 @@ def layer_inverse(layer, z):
     if isinstance(layer, affine.AffineConstFlow):  # includes ActNorm (after init)
         s, t = layer.s.reshape(1, -1), layer.t.reshape(1, -1)
         return (z - t) * torch.exp(-s), -torch.sum(s) * z.new_ones(b)
+    if isinstance(layer, planar.Planar):   # leaky-ReLU layers only (flows/planar.py:66-81)
+        if layer._no_inverse:
+            raise NotImplementedError("This flow has no algebraic inverse.")
+        w, u = layer.w.reshape(1, -1), layer.u.reshape(1, -1)
+        lin = torch.sum(w * z, 1) + layer.b
+        a = (lin < 0) * (layer.h.negative_slope - 1.0) + 1.0
+        inner = torch.sum(w * u)
+        u = u + (torch.log(1 + torch.exp(inner)) - 1 - inner) * w / torch.sum(w ** 2)
+        u = a.reshape(-1, 1) * u
+        inner_ = torch.sum(w * u, 1)
+        return z - u * (lin / (1 + inner_)).reshape(-1, 1), -torch.log(torch.abs(1 + inner_))
     if isinstance(layer, mixing.Permute):
         _, inv = layer._index_lists()
         return z[:, torch.tensor(inv, device=z.device)], z.new_zeros(b)

@@ -10,6 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("NFB200_LIB") or os.path.join(os.path.dirname(_HERE), "libnfb200.so")
 
 NFB_INVERSE, NFB_FORWARD = 0, 1
+NFB_PLANAR_TANH, NFB_PLANAR_LEAKY_RELU = 0, 1   # nfb_planar_desc_t.act
 _FP = C.POINTER(C.c_float)
 _I64P = C.POINTER(C.c_int64)
 _I32P = C.POINTER(C.c_int32)
@@ -70,6 +71,15 @@ class AffineConstDesc(C.Structure):
 
 class PermuteDesc(C.Structure):
     _fields_ = [("features", C.c_int32), ("perm", _I32P), ("inv_perm", _I32P)]
+
+
+class PlanarDesc(C.Structure):
+    _fields_ = [("features", C.c_int32), ("u", C.c_void_p), ("w", C.c_void_p), ("b", C.c_void_p), ("act", C.c_int32),
+                ("slope", C.c_float)]
+
+
+class RadialDesc(C.Structure):
+    _fields_ = [("features", C.c_int32), ("beta", C.c_void_p), ("alpha", C.c_void_p), ("z0", C.c_void_p)]
 
 
 class GemmDesc(C.Structure):
@@ -169,6 +179,8 @@ SYMBOLS = {
     "nfb_flow_add_affine_coupling": (C.c_int, [_VP, C.POINTER(AffineCouplingDesc)]),
     "nfb_flow_add_affine_const": (C.c_int, [_VP, C.POINTER(AffineConstDesc)]),
     "nfb_flow_add_permute": (C.c_int, [_VP, C.POINTER(PermuteDesc)]),
+    "nfb_flow_add_planar": (C.c_int, [_VP, C.POINTER(PlanarDesc)]),
+    "nfb_flow_add_radial": (C.c_int, [_VP, C.POINTER(RadialDesc)]),
     "nfb_flow_set_base_diag_gaussian": (C.c_int, [_VP, _VP, _VP]),
     "nfb_flow_finalize": (C.c_int, [_VP, _I32, _VP]),
     "nfb_flow_repack": (C.c_int, [_VP, _VP]),

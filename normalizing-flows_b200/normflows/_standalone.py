@@ -108,13 +108,18 @@ def apply_sampling(module, z, context=None):
     return module._sampling_value(z, context, None)
 
 
-def affine_slot_tensors(layers):
-    """The tensors behind the gradient slots of an affine-family stack (include/nfb200.h nfb_flow_grad_slot_numel):
-    each layer's parameters in registration order; an AffineConstFlow s / t registered as a buffer keeps its slot."""
-    from .flows import affine, mixing
+def sampling_slot_tensors(layers):
+    """The tensors behind the gradient slots of an affine-family or planar-family stack (include/nfb200.h
+    nfb_flow_grad_slot_numel): each layer's parameters in registration order; an AffineConstFlow s / t registered as a
+    buffer keeps its slot."""
+    from .flows import affine, mixing, planar, radial
     out = []
     for layer in layers:
-        if isinstance(layer, affine.MaskedAffineFlow):
+        if isinstance(layer, planar.Planar):
+            out += [layer.u, layer.w, layer.b]
+        elif isinstance(layer, radial.Radial):
+            out += [layer.beta, layer.alpha, layer.z_0]
+        elif isinstance(layer, affine.MaskedAffineFlow):
             for net in (layer.s, layer.t):
                 if net is not None:
                     out += [p for lin in net.linear_layers() for p in (lin.weight, lin.bias)]
@@ -123,15 +128,19 @@ def affine_slot_tensors(layers):
         elif isinstance(layer, affine.AffineCouplingBlock):
             out += [p for lin in layer.flows[1].param_map.linear_layers() for p in (lin.weight, lin.bias)]
         elif not isinstance(layer, mixing.Permute):
-            raise NotImplementedError(f"{type(layer).__name__} is not in the affine family")
+            raise NotImplementedError(f"{type(layer).__name__} is in neither the affine nor the planar family")
     return out
 
 
-class AffineSamplingFn(torch.autograd.Function):
+affine_slot_tensors = sampling_slot_tensors   # (the name callers of the affine-only version use)
+
+
+class StackSamplingFn(torch.autograd.Function):
     """(x, log_det) = handle.transform(NFB_FORWARD, z) of an all-affine stack (MaskedAffineFlow, AffineConstFlow /
-    ActNorm, AffineCouplingBlock, Permute): the unchanged one-launch forward, so values are bit-identical with and
-    without grad.  The backward is one nfb_flow_sampling_backward call (recompute + reverse walk, then a fixed-order
-    weight reduction).  Refuses to run the backward if a parameter was modified in place after the forward."""
+    ActNorm, AffineCouplingBlock, Permute) or an all-planar one (Planar, Radial): the unchanged one-launch forward, so
+    values are bit-identical with and without grad.  The backward is one nfb_flow_sampling_backward call (recompute +
+    reverse walk, then a fixed-order reduction of the parameter terms).  Refuses to run the backward if a parameter was
+    modified in place after the forward."""
 
     @staticmethod
     def forward(ctx, handle, layers, z, *params):
@@ -147,7 +156,7 @@ class AffineSamplingFn(torch.autograd.Function):
         if any(p._version != v for p, v in zip(ctx.params, ctx.versions)):
             names = "+".join(sorted({type(l).__name__ for l in ctx.layers}))
             raise RuntimeError(f"{names} backward: a parameter was modified in place after the forward pass")
-        slots = affine_slot_tensors(ctx.layers)
+        slots = sampling_slot_tensors(ctx.layers)
         bufs = [torch.empty_like(p) if isinstance(p, torch.nn.Parameter) and p.requires_grad else None for p in slots]
         need_z = ctx.needs_input_grad[2]
         gz = torch.empty_like(z) if need_z else None
@@ -156,7 +165,7 @@ class AffineSamplingFn(torch.autograd.Function):
         lib = L.lib()
         h = ctx.handle.ensure(z.shape[1], z.device)
         if lib.nfb_flow_num_grad_slots(h) < len(slots):
-            raise RuntimeError("affine sampling backward: gradient slot mismatch")
+            raise RuntimeError("sampling backward: gradient slot mismatch")
         ws = _workspace(lib.nfb_flow_sampling_backward_workspace_bytes(h, z.shape[0]), z.device)
         arr = _vp(bufs)
         with torch.cuda.device(z.device):
@@ -170,8 +179,8 @@ class AffineSamplingFn(torch.autograd.Function):
         return (None, None, gz, *[gmap.get(id(p)) if p.requires_grad else None for p in ctx.params])
 
 
-def affine_sampling(handle, layers, z, params):
-    return AffineSamplingFn.apply(handle, list(layers), z, *params)
+def stack_sampling(handle, layers, z, params):
+    return StackSamplingFn.apply(handle, list(layers), z, *params)
 
 
 # ---- element adjoints ------------------------------------------------------------------------------------------

@@ -79,9 +79,9 @@ class NormalizingFlow(nn.Module):
         h = self._stack()
         self._run_pending_inits(z, inverse=False)
         if h is not None and z.dim() == 2:
-            if self._all_affine() and wants_grad(self.flows, z):   # one launch forward, one native backward
-                from ._standalone import affine_sampling
-                return affine_sampling(h, self.flows, z, list(self.flows.parameters()))
+            if self._one_sampling_family() and wants_grad(self.flows, z):   # one launch forward, one native backward
+                from ._standalone import stack_sampling
+                return stack_sampling(h, self.flows, z, list(self.flows.parameters()))
             return h.transform(L.NFB_FORWARD, z)
         log_det = torch.zeros(len(z), device=z.device)
         for flow in self.flows:
@@ -93,7 +93,14 @@ class NormalizingFlow(nn.Module):
         z, _ = self.inverse_and_log_det(x)
         return z
 
+    def _require_inverse(self):
+        """Planar (tanh) and Radial layers have no density direction: raise, like the reference, before any launch."""
+        for f in self.flows:
+            if getattr(f, "_no_inverse", False):
+                raise NotImplementedError("This flow has no algebraic inverse.")
+
     def inverse_and_log_det(self, x):
+        self._require_inverse()
         h = self._stack()
         self._run_pending_inits(x, inverse=True)
         if h is not None and x.dim() == 2:
@@ -105,6 +112,7 @@ class NormalizingFlow(nn.Module):
         return x, log_det
 
     def log_prob(self, x):
+        self._require_inverse()
         h = self._stack()
         self._run_pending_inits(x, inverse=True)
         if h is not None and h.base is not None and x.dim() == 2:
@@ -116,6 +124,7 @@ class NormalizingFlow(nn.Module):
         return log_q + self.q0.log_prob(z)
 
     def forward_kld(self, x):
+        self._require_inverse()
         h = self._stack()
         self._run_pending_inits(x, inverse=True)
         if h is not None and h.base is not None and x.dim() == 2 and not wants_grad(self, x):
@@ -130,20 +139,22 @@ class NormalizingFlow(nn.Module):
     def _takes_layer_loop(self):
         return self._stack() is None
 
-    def _all_affine(self):
+    def _one_sampling_family(self):
         """Every layer is in the affine family (MaskedAffineFlow, AffineConstFlow / ActNorm, AffineCouplingBlock,
-        Permute): the all-native stack's sampling direction has a native backward (nfb_flow_sampling_backward)."""
-        return len(self.flows) > 0 and all(getattr(f, "_affine_family", False) for f in self.flows)
+        Permute), or every layer in the planar family (Planar, Radial): the all-native stack's sampling direction has a
+        native backward (nfb_flow_sampling_backward).  Mixes of the two families do not."""
+        fams = {f._sampling_family() if isinstance(f, NativeFlow) else None for f in self.flows}
+        return len(fams) == 1 and None not in fams
 
     def _no_sampling_grad(self, what, context=None):
         """Gradients through the sampling direction exist when every layer's sampling direction is differentiable (the
-        stand-alone spline layers and the affine family, `_sampling_differentiable`), the stack runs layer by layer or is
-        all affine-family, and the base's draw is reparameterised (UniformGaussian, DiagGaussian,
+        stand-alone spline layers and the affine and planar families, `_sampling_differentiable`), the stack runs layer
+        by layer or is all of one family, and the base's draw is reparameterised (UniformGaussian, DiagGaussian,
         ConditionalDiagGaussian).  Otherwise, under grad, raise."""
         if not (torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())):
             return
         if (isinstance(self.q0, (UniformGaussian, DiagGaussian, ConditionalDiagGaussian))
-                and (self._takes_layer_loop() or self._all_affine())
+                and (self._takes_layer_loop() or self._one_sampling_family())
                 and all(hasattr(f, "_sampling_differentiable") and f._sampling_differentiable(context)
                         for f in self.flows)):
             return
@@ -164,7 +175,8 @@ class NormalizingFlow(nn.Module):
         """core.py:104-131.  z ~ q0 pushed through every layer's `.forward` (one persistent launch for coupling
         stacks), log_q = log q0(z0) - sum log_det; `score_fn=False` re-evaluates log_q by the density pass of the
         drawn samples with parameter gradients switched off, like the reference.  Differentiable for the stacks
-        _no_sampling_grad admits (the stand-alone spline layers or the affine family on a reparameterised base)."""
+        _no_sampling_grad admits (the stand-alone spline layers, the affine or the planar family on a reparameterised
+        base)."""
         self._no_sampling_grad("reverse_kld")
         z, log_q = self.sample(num_samples)
         if not score_fn:

@@ -7,3 +7,5 @@ from .affine import (AffineConstFlow, ActNorm, MaskedAffineFlow, AffineCouplingB
                      Split, Merge)
 from .glow import GlowBlock, Invertible1x1Conv, Squeeze, ImageMerge
 from .residual import Residual, iResBlock
+from .planar import Planar
+from .radial import Radial

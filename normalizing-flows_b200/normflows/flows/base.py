@@ -10,6 +10,8 @@ from .._native import FlowHandle
 class Flow(nn.Module):
     """Generic flow layer: `forward(z) -> (z', log_det[B])`, `inverse(z) -> (z', log_det[B])`."""
 
+    _no_inverse = False   # True: `inverse` raises (Planar with tanh, Radial), and so does a density pass through it
+
     def forward(self, z):
         raise NotImplementedError("Forward pass has not been implemented.")
 
@@ -23,7 +25,9 @@ class NativeFlow(Flow):
     (append this layer's descriptor to an nfb_flow)."""
 
     use_tensor_cores = True  # class-wide switch; False forces the plain-fp32 kernels (A/B parity)
-    _affine_family = False   # True: the sampling direction has a native backward (nfb_flow_sampling_backward)
+    # the sampling direction has a native backward (nfb_flow_sampling_backward) for stacks of one family
+    _affine_family = False
+    _planar_family = False
 
     def _single(self):
         h = self.__dict__.get("_nfb_single")
@@ -34,17 +38,20 @@ class NativeFlow(Flow):
 
     def forward(self, z, context=None):
         # (layers without context parameters ignore the context, like the reference's `context=None` signatures)
-        if self._affine_family and wants_grad(self, z):
-            from .._standalone import affine_sampling
-            return affine_sampling(self._single(), [self], z, list(self.parameters()))
+        if self._sampling_family() and wants_grad(self, z):
+            from .._standalone import stack_sampling
+            return stack_sampling(self._single(), [self], z, list(self.parameters()))
         return self._single().layer_apply(0, L.NFB_FORWARD, z)
 
+    def _sampling_family(self):
+        return "affine" if self._affine_family else "planar" if self._planar_family else None
+
     def _sampling_differentiable(self, context=None):
-        return self._affine_family
+        return self._sampling_family() is not None
 
     def inverse(self, z, context=None):
         # under autograd (a layer called on its own, e.g. between the blocks of a stack that is not all native) the call
-        # joins the graph; the sampling direction (`forward`) does too for the affine family
+        # joins the graph; the sampling direction (`forward`) does too for the affine and planar families
         if wants_grad(self, z):
             from .._autograd import LayerInverseFn
             return LayerInverseFn.apply(self, z, *self.parameters())
