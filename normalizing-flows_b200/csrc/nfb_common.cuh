@@ -154,12 +154,15 @@ template <int R> __device__ __forceinline__ void wgmma_hold(float (&d)[R]) {
     for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 // D (+)= A * B^T, A [64 x 16] and B [N x 16] both K-major (TA / TB = 1: MN-major); scale_d = 0 overwrites D;
-// on = 0: no operation (a predicate, which must be the same for the whole warpgroup, instead of a branch: ptxas
-// serialises the wgmma of a warpgroup when one sits in a branch it cannot prove warp-uniform)
-__device__ __forceinline__ void wgmma_f16_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t scale_d, uint32_t on = 1) {
+// bf16 forms, on = 0: no operation (a predicate, which must be the same for the whole warpgroup, instead of a branch:
+// ptxas serialises the wgmma of a warpgroup when one sits in a branch it cannot prove warp-uniform).
+// The f16 forms (the fused spline kernel's) have no `on`: ptxas lowers a predicated wgmma to a branch around it, so each
+// one lands in a basic block of its own with a warpgroup.arrive in front.  Their caller issues a record's products as
+// one unpredicated chain and skips a whole chain with one warp-uniform branch around it.
+__device__ __forceinline__ void wgmma_f16_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t scale_d) {
     asm volatile(
-        "{\n\t.reg .pred p, q;\n\tsetp.ne.b32 p, %34, 0;\n\tsetp.ne.b32 q, %35, 0;\n\t"
-        "@q wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
         "{"
         "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
         "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31"
@@ -168,20 +171,24 @@ __device__ __forceinline__ void wgmma_f16_n64(float (&d)[32], uint64_t a, uint64
           "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
           "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
           "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-        : "l"(a), "l"(b), "r"(scale_d), "r"(on));
+        : "l"(a), "l"(b), "r"(scale_d));
 }
-__device__ __forceinline__ void wgmma_f16_n48(float (&d)[24], uint64_t a, uint64_t b, uint32_t scale_d, uint32_t on = 1) {
+__device__ __forceinline__ void wgmma_f16_n96(float (&d)[48], uint64_t a, uint64_t b, uint32_t scale_d) {
     asm volatile(
-        "{\n\t.reg .pred p, q;\n\tsetp.ne.b32 p, %26, 0;\n\tsetp.ne.b32 q, %27, 0;\n\t"
-        "@q wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 "
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 "
         "{"
         "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-        "%16,%17,%18,%19,%20,%21,%22,%23"
-        "}, %24, %25, p, 1, 1, 0, 0;\n\t}"
+        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+        "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47"
+        "}, %48, %49, p, 1, 1, 0, 0;\n\t}"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
           "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
-          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
-        : "l"(a), "l"(b), "r"(scale_d), "r"(on));
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+        : "l"(a), "l"(b), "r"(scale_d));
 }
 template <int TA = 0, int TB = 0>
 __device__ __forceinline__ void wgmma_bf16_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t scale_d, uint32_t on = 1) {

@@ -30,7 +30,7 @@
 //              second GEMM of each residual block accumulates straight onto the residual stream (h += W2 relu(...));
 //              the biases are pre-summed by the packer.
 //              In the final layer the warpgroups take different roles: warpgroup 0 multiplies both halves of every
-//              record (two features, N = 48, per half; two accumulators in flight) and stores each pair of chunks to
+//              record (two features, N = 48, per half; both halves as one N = 96 product) and stores each pair of chunks to
 //              two staging tiles in shared memory; warpgroup 1 copies its (row, feature) parameters out of the tiles,
 //              hands them back at once and evaluates two splines per thread.  The hand-off is a pair of named barriers
 //              ("full" / "free", one side arrives, the other waits), so the products of one pair of chunks run under the
@@ -127,38 +127,29 @@ template <typename T> __device__ __forceinline__ T uniform(T v) {
 // 2^e as a float, e in [-126, 127]
 __device__ __forceinline__ float pow2i(int e) { return __uint_as_float((uint32_t)(127 + e) << 23); }
 
-// the products of one record: acc (+)= A[K-chunk] W^T as W_hi A_hi + W_hi A_lo + W_lo A_hi (+ W_lo A_lo), four K=16
-// slabs each, in that order (first: the first product overwrites the accumulator; on = 0: none; slabs: only the
-// first `slabs` K=16 slabs, the others being all zero)
-// With a second accumulator (acc1, its own operands x1): the two halves of a final-layer record, slab by slab in turn,
-// so that two independent chains are in flight; each accumulator sees its products in the same order as alone.
+// the products of one record: acc (+)= A[K-chunk] W^T as W_hi A_hi + W_hi A_lo + W_lo A_hi (+ W_lo A_lo), the first
+// SLABS K = 16 slabs each, in that order (first: the first product overwrites the accumulator; the slabs after SLABS are
+// all zero).  One straight chain: no wgmma of it has a predicate of its own, so ptxas issues them back to back behind
+// one warpgroup.arrive.  Whether a record has products at all is decided by one uniform branch around the chain.
+// N = 64 (32 registers): a hidden GEMM's slice; N = 96 (48): both halves of a final-layer record at once, half 0 in
+// registers 0..23 and half 1 in 24..47 (rows [0, 48) and [48, 96) of the record's tiles).
 struct MmaOps { uint32_t a_hi, a_lo, w_hi, w_lo; bool first; uint32_t on, slabs; };
-template <int NREG, bool QUAD, typename ACC1>
-__device__ __forceinline__ void mma_record(float (&acc)[NREG], const MmaOps& x, ACC1& acc1, const MmaOps& x1) {
-    constexpr bool kPair = !std::is_same<ACC1, const std::nullptr_t>::value;
-    auto mma = [](auto& d, uint64_t a, uint64_t b, uint32_t sd, uint32_t go) {
-        if constexpr (NREG == 32) wgmma_f16_n64(d, a, b, sd, go);
-        else wgmma_f16_n48(d, a, b, sd, go);
-    };
+template <int SLABS, bool QUAD, int NREG>
+__device__ __forceinline__ void mma_record(float (&acc)[NREG], const MmaOps& x) {
+    static_assert(NREG == 32 || NREG == 48, "N = 64 or 96");
     const uint64_t ah = wgmma_desc(x.a_hi), al = wgmma_desc(x.a_lo), bh = wgmma_desc(x.w_hi), bl = wgmma_desc(x.w_lo);
-    const uint64_t ah1 = wgmma_desc(x1.a_hi), al1 = wgmma_desc(x1.a_lo), bh1 = wgmma_desc(x1.w_hi), bl1 = wgmma_desc(x1.w_lo);
-    auto pass = [&](uint64_t a, uint64_t b, uint64_t a1, uint64_t b1, bool opens) {
+    auto pass = [&](uint64_t a, uint64_t b, bool opens) {
 #pragma unroll
-        for (int s = 0; s < 4; ++s) {
-            mma(acc, a + 2 * s, b + 2 * s, opens && s == 0 && x.first ? 0u : 1u, x.on & (uint32_t)(s < (int)x.slabs));
-            if constexpr (kPair)
-                mma(acc1, a1 + 2 * s, b1 + 2 * s, opens && s == 0 && x1.first ? 0u : 1u, x1.on & (uint32_t)(s < (int)x1.slabs));
+        for (int s = 0; s < SLABS; ++s) {
+            const uint32_t sd = opens && s == 0 && x.first ? 0u : 1u;
+            if constexpr (NREG == 32) wgmma_f16_n64(acc, a + 2 * s, b + 2 * s, sd);
+            else wgmma_f16_n96(acc, a + 2 * s, b + 2 * s, sd);
         }
     };
-    pass(ah, bh, ah1, bh1, true);
-    pass(al, bh, al1, bh1, false);
-    pass(ah, bl, ah1, bl1, false);
-    if constexpr (QUAD) pass(al, bl, al1, bl1, false);
-}
-template <int NREG, bool QUAD>
-__device__ __forceinline__ void mma_record(float (&acc)[NREG], const MmaOps& x) {
-    const std::nullptr_t none = nullptr;
-    mma_record<NREG, QUAD>(acc, x, none, x);
+    pass(ah, bh, true);
+    pass(al, bh, false);
+    pass(ah, bl, false);
+    if constexpr (QUAD) pass(al, bl, false);
 }
 
 // Phase clocks (make CLOCKS=1, a separate library; tools/fused_phase_clocks.py): every thread of a role adds the SM
@@ -398,10 +389,12 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
                           (uint32_t)(live && !(fl & kStepSkip)), 4u - ((fl >> kStepSlabShift) & 3u)};
         };
         // The records of one output slice of this warpgroup (until the one its flags mark last): its half of each goes
-        // into acc, multiplied with its K-chunk (live: the warpgroup has a slice here).
+        // into acc, multiplied with its K-chunk (live: the warpgroup has a slice here).  (The packer sets slab bits on
+        // final-layer records only: the LU map and the hidden GEMMs always multiply all four slabs.)
         auto run_slice = [&](auto& acc, bool live, auto quad, auto clk_ring, auto clk_mma) {
             run_records([&](const FusedStep& s) {
-                mma_record<sizeof(acc) / sizeof(float), decltype(quad)::value>(acc, half_ops(s, wg, live));
+                const MmaOps x = half_ops(s, wg, live);
+                if (x.on) mma_record<4, decltype(quad)::value>(acc, x);
                 return ((wg ? s.flags1 : s.flags) & kStepLast) != 0;
             }, std::integral_constant<int, 1>(), clk_ring, clk_mma);
             wgmma_hold(acc);
@@ -680,21 +673,33 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
             //      waits for the other except through the tiles ("full" / "free"), so the products of pair c + 1 run
             //      under the splines of pair c. ----
             if (wg == 0) {
+                static_assert(kFusedFeaturesPerChunk == 2, "a final-layer record is one N = 96 product");
                 for (int ci = 0; ci < n_pairs; ++ci) {
-                    float acc0[kFusedFeaturesPerChunk * 12] = {}, acc1[kFusedFeaturesPerChunk * 12] = {};   // (as hres: not live before)
+                    float acc[48] = {};   // (as hres: not live before) half 0 in 0..23, half 1 in 24..47
                     run_records([&](const FusedStep& s) {
-                        mma_record<kFusedFeaturesPerChunk * 12, false>(acc0, half_ops(s, 0, true), acc1, half_ops(s, 1, true));
+                        // Both halves share the K-chunk and the first / last flags; one N = 96 product covers them, over
+                        // the larger of their slab counts.  A half the record skips, and the slabs past a half's own
+                        // count, are multiplied too: their weights are the masked-out zeros the packer wrote, which add
+                        // an exact zero to every accumulator.  (A record always has a live half: the packer keeps only
+                        // K-chunk 0 and the K-chunks one of the two chunks reaches.)
+                        const MmaOps x = half_ops(s, 0, true), x1 = half_ops(s, 1, true);
+                        const uint32_t n = max(x.on ? x.slabs : 0u, x1.on ? x1.slabs : 0u);
+                        switch (n) {
+                            case 1: mma_record<1, false>(acc, x); break;
+                            case 2: mma_record<2, false>(acc, x); break;
+                            case 3: mma_record<3, false>(acc, x); break;
+                            default: mma_record<4, false>(acc, x); break;
+                        }
                         return (s.flags & kStepLast) != 0;   // (the pair's last record is the same for both halves)
                     }, std::integral_constant<int, 2>(), ClkPhase<kClkFinRing>(), ClkPhase<kClkFinMma>());
-                    wgmma_hold(acc0);
-                    wgmma_hold(acc1);
+                    wgmma_hold(acc);
                     // (no slot is held here: the producer can deliver the next pair's records while this waits)
                     if (ci > 0) stg_bar_wait<kBarStgFree>();   // the previous pair's parameters have been taken
 #pragma unroll
-                    for (int i = 0; i < kFusedFeaturesPerChunk * 12; i += 2) {
+                    for (int i = 0; i < 24; i += 2) {
                         float* dst = stg0 + ((i & 2) ? rb : ra) * kStgLd + 8 * (i >> 2) + cq;
-                        *reinterpret_cast<float2*>(dst) = make_float2(acc0[i], acc0[i + 1]);
-                        *reinterpret_cast<float2*>(dst + kRows * kStgLd) = make_float2(acc1[i], acc1[i + 1]);
+                        *reinterpret_cast<float2*>(dst) = make_float2(acc[i], acc[i + 1]);
+                        *reinterpret_cast<float2*>(dst + kRows * kStgLd) = make_float2(acc[24 + i], acc[25 + i]);
                     }
                     stg_bar_arrive<kBarStgFull>();
                     NFB_CLK(kClkFinStage);
