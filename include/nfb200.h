@@ -545,9 +545,11 @@ int nfb_flow_forward_kld(nfb_flow_t* f, const float* x_dev, int64_t rows, float*
  *   Planar : u, w, b       Radial : beta, alpha, z_0
  *   base (last two slots) : loc, log_scale
  * `grad_slots[i]` is a device buffer of nfb_flow_grad_slot_numel(f, i) floats that is OVERWRITTEN, or NULL to skip.
- * nfb_flow_num_grad_slots returns -1 when the flow holds a layer kind without a native backward.  The affine and planar
- * families' slots serve nfb_flow_sampling_backward only: nfb_flow_log_prob_backward rejects their groups
- * (NFB_ERR_UNSUPPORTED). */
+ * nfb_flow_num_grad_slots returns -1 when the flow holds a layer kind without a native backward.  Groups of affine-family
+ * layers may sit anywhere in the stack: each runs the same recompute + adjoint walk + fixed-order reduction as
+ * nfb_flow_density_backward, with g_logq as its log-det cotangent, in an internal workspace chunked under the same bound.
+ * The planar family's slots serve nfb_flow_sampling_backward only: nfb_flow_log_prob_backward rejects its groups
+ * (NFB_ERR_UNSUPPORTED).  rows = 0 writes zeros into the slots. */
 int nfb_flow_num_grad_slots(const nfb_flow_t* f);
 int64_t nfb_flow_grad_slot_numel(const nfb_flow_t* f, int32_t slot);
 int nfb_flow_log_prob_backward(nfb_flow_t* f, const float* x_dev, const float* g_logq_dev, int64_t rows,
@@ -570,6 +572,19 @@ int nfb_flow_log_prob_backward(nfb_flow_t* f, const float* x_dev, const float* g
 int64_t nfb_flow_sampling_backward_workspace_bytes(const nfb_flow_t* f, int64_t rows);
 int nfb_flow_sampling_backward(nfb_flow_t* f, const float* z, const float* g_x, const float* g_ld, int64_t rows,
                                void* ws, int64_t ws_bytes, float* g_z, float* const* grad_slots, void* stream);
+
+/* ---- density-direction backward of an all-affine stack (forward_kld / log_prob of examples/real_nvp_colab.ipynb, a
+ * stand-alone ActNorm between Residual blocks) -- gradients of sum_r <g_z[r], z_r> + g_ld[r] log_det_r, with
+ * (z, log_det) = nfb_flow_transform(f, NFB_INVERSE, x), w.r.t. x and every parameter, for stacks of MaskedAffineFlow,
+ * AffineConstFlow / ActNorm, AffineCouplingBlock and Permute only (any other stack, Planar / Radial included:
+ * NFB_ERR_UNSUPPORTED).  x is the input that nfb_flow_transform was given.  One kernel recomputes the stack from x
+ * taking the ops last-to-first, then walks them first-to-last; the weight reduction, the row chunking, the workspace
+ * bound and the launch count are those of nfb_flow_sampling_backward.  g_z / g_ld may be NULL (zero cotangent); g_x and
+ * individual slots may be NULL (not wanted); grad_slots is in nfb_flow_grad_slot_numel order (a base's two slots, if
+ * any, are not read); rows = 0 writes zeros. */
+int64_t nfb_flow_density_backward_workspace_bytes(const nfb_flow_t* f, int64_t rows);
+int nfb_flow_density_backward(nfb_flow_t* f, const float* x, const float* g_z, const float* g_ld, int64_t rows,
+                              void* ws, int64_t ws_bytes, float* g_x, float* const* grad_slots, void* stream);
 
 /* ---- host-buffer entry points (what a non-CUDA caller binds; copies are inside) ---- */
 int nfb_flow_log_prob_host(nfb_flow_t* f, const float* x_host, float* log_q_host, int64_t rows);

@@ -301,6 +301,131 @@ affine_bwd_rows_kernel(const AffineOp* __restrict__ ops, const AffBwdOp* __restr
     if (gz) for (int j = 0; j < d; ++j) gz[r * d + j] = g[j];
 }
 
+// Density-direction backward (direction = 0), the same workspace plan and reduction: recompute the stack from x taking
+// the ops last-to-first with the forward kernel's inverse expressions, then walk them first-to-last with the density
+// adjoints of nfb_affine_bwd.cuh.  Like the sampling kernel it keeps its own copy of the per-op arithmetic, so that
+// affine_stack_kernel's code stays as it is.
+__global__ void __launch_bounds__(128)
+affine_density_bwd_rows_kernel(const AffineOp* __restrict__ ops, const AffBwdOp* __restrict__ bops, int n_ops,
+                               const float* __restrict__ xin, const float* __restrict__ gzo,
+                               const float* __restrict__ gld, float* __restrict__ gx, float* __restrict__ ws,
+                               long long R, int d) {
+    const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= R) return;
+    float z[kAffMaxD];
+    for (int j = 0; j < d; ++j) z[j] = xin[r * d + j];
+    // ---- recompute (affine_stack_kernel, direction = 0) ----
+    for (int k = n_ops - 1; k >= 0; --k) {
+        const AffineOp& op = ops[k];
+        const AffBwdOp& bo = bops[k];
+        for (int j = 0; j < d; ++j) AFF_U(bo.u_z + j, r) = z[j];
+        if (op.type == kOpMasked) {
+            float zm[kAffMaxD], s[kAffMaxD], t[kAffMaxD];
+            for (int j = 0; j < d; ++j) zm[j] = __ldg(op.p0 + j) * z[j];
+            if (op.s.n_layers) mlp_eval_store(op.s, zm, s, op.slope, ws, R, r, bo.u_act[0], bo.u_del[0]);
+            else for (int j = 0; j < d; ++j) s[j] = 0.f;
+            if (op.t.n_layers) mlp_eval_store(op.t, zm, t, op.slope_t, ws, R, r, bo.u_act[1], bo.u_del[1]);
+            else for (int j = 0; j < d; ++j) t[j] = 0.f;
+            for (int j = 0; j < d; ++j) {
+                const float b = __ldg(op.p0 + j);
+                const float sj = isfinite(s[j]) ? s[j] : __int_as_float(0x7fc00000);
+                const float tj = isfinite(t[j]) ? t[j] : __int_as_float(0x7fc00000);
+                z[j] = zm[j] + (1.f - b) * (z[j] - tj) * expf(-sj);
+            }
+        } else if (op.type == kOpConst) {
+            for (int j = 0; j < d; ++j) z[j] = (z[j] - __ldg(op.p1 + j)) * expf(-__ldg(op.p0 + j));
+        } else if (op.type == kOpCoupling) {
+            const int h = (d + 1) / 2;
+            const bool inv_split = (op.flags >> 3) & 1;
+            const int o1 = inv_split ? h : 0, n1 = inv_split ? d - h : h;
+            const int o2 = inv_split ? 0 : h, n2 = d - n1;
+            float param[2 * kAffMaxD];
+            mlp_eval_store(op.s, z + o1, param, op.slope, ws, R, r, bo.u_act[0], bo.u_del[0]);
+            if (!(op.flags & 1)) {
+                for (int j = 0; j < n2; ++j) z[o2 + j] += -param[j];
+            } else {
+                const int smap = (op.flags >> 1) & 3;
+                for (int j = 0; j < n2; ++j) {
+                    const float shift = param[2 * j], sc = param[2 * j + 1];
+                    float& v = z[o2 + j];
+                    if (smap == 0) {
+                        v = (v - shift) * expf(-sc);
+                    } else {
+                        const float sg = 1.f / (1.f + expf(-(sc + 2.f)));
+                        v = smap == 1 ? (v - shift) * sg : (v - shift) / sg;
+                    }
+                }
+            }
+        } else {
+            float tmp[kAffMaxD];
+            for (int j = 0; j < d; ++j) tmp[j] = z[__ldg(op.inv_idx + j)];
+            for (int j = 0; j < d; ++j) z[j] = tmp[j];
+        }
+    }
+    // ---- adjoint, ops first-to-last ----
+    float g[kAffMaxD];
+    for (int j = 0; j < d; ++j) g[j] = gzo ? gzo[r * d + j] : 0.f;
+    const float gam = gld ? gld[r] : 0.f;
+    for (int k = 0; k < n_ops; ++k) {
+        const AffineOp& op = ops[k];
+        const AffBwdOp& bo = bops[k];
+        for (int j = 0; j < d; ++j) z[j] = AFF_U(bo.u_z + j, r);
+        if (op.type == kOpMasked) {
+            const int ls = op.s.n_layers - 1, lt = op.t.n_layers - 1;
+            float gs[kAffMaxD], gt[kAffMaxD];
+            for (int j = 0; j < d; ++j) {
+                const float s = ls >= 0 ? AFF_U(bo.u_del[0][ls] + j, r) : 0.f;
+                const float t = lt >= 0 ? AFF_U(bo.u_del[1][lt] + j, r) : 0.f;
+                float sh, th;
+                masked_affine_density_adjoint<float>(z[j], __ldg(op.p0 + j), s, t, g[j], gam, sh, th, g[j]);
+                if (ls >= 0) AFF_U(bo.u_del[0][ls] + j, r) = sh;
+                if (lt >= 0) AFF_U(bo.u_del[1][lt] + j, r) = th;
+                gs[j] = gt[j] = 0.f;
+            }
+            if (ls >= 0) mlp_backward_row(op.s, op.slope, ws, R, r, bo.u_del[0], gs);
+            if (lt >= 0) mlp_backward_row(op.t, op.slope_t, ws, R, r, bo.u_del[1], gt);
+            for (int j = 0; j < d; ++j) g[j] += __ldg(op.p0 + j) * (gs[j] + gt[j]);
+        } else if (op.type == kOpConst) {
+            for (int j = 0; j < d; ++j) {
+                float cs, ct;
+                affine_const_density_adjoint<float>(z[j], __ldg(op.p0 + j), __ldg(op.p1 + j), g[j], gam, g[j], cs, ct);
+                AFF_U(bo.u_del[0][0] + j, r) = cs;
+                AFF_U(bo.u_del[1][0] + j, r) = ct;
+            }
+        } else if (op.type == kOpCoupling) {
+            const int h = (d + 1) / 2;
+            const bool inv_split = (op.flags >> 3) & 1;
+            const int o1 = inv_split ? h : 0, n1 = inv_split ? d - h : h;
+            const int o2 = inv_split ? 0 : h, n2 = d - n1;
+            const int scale = op.flags & 1, smap = (op.flags >> 1) & 3;
+            const int lp = op.s.n_layers - 1;
+            for (int j = 0; j < n2; ++j) {
+                float gv, gsh, gsc;
+                if (scale) {
+                    float& ush = AFF_U(bo.u_del[0][lp] + 2 * j, r);
+                    float& usc = AFF_U(bo.u_del[0][lp] + 2 * j + 1, r);
+                    coupling_density_adjoint<float>(1, smap, z[o2 + j], ush, usc, g[o2 + j], gam, gv, gsh, gsc);
+                    ush = gsh;
+                    usc = gsc;
+                } else {
+                    float& up = AFF_U(bo.u_del[0][lp] + j, r);
+                    coupling_density_adjoint<float>(0, 0, z[o2 + j], up, 0.f, g[o2 + j], gam, gv, gsh, gsc);
+                    up = gsh;
+                }
+                g[o2 + j] = gv;
+            }
+            float g1[kAffMaxD];
+            mlp_backward_row(op.s, op.slope, ws, R, r, bo.u_del[0], g1);
+            for (int j = 0; j < n1; ++j) g[o1 + j] += g1[j];
+        } else {  // x[j] = z[inv[j]]  ->  g_z[i] = g_x[fwd[i]]
+            float tmp[kAffMaxD];
+            for (int j = 0; j < d; ++j) tmp[j] = g[__ldg(op.fwd_idx + j)];
+            for (int j = 0; j < d; ++j) g[j] = tmp[j];
+        }
+    }
+    if (gx) for (int j = 0; j < d; ++j) gx[r * d + j] = g[j];
+}
+
 __device__ __forceinline__ int aff_find_item(const AffRedItem* items, int n_items, long long e) {
     int lo = 0, hi = n_items - 1;   // last item with e_off <= e
     while (lo < hi) {
@@ -347,11 +472,16 @@ __global__ void affine_bwd_finish_kernel(const AffRedItem* __restrict__ items, i
 }
 #undef AFF_U
 
-int launch_affine_bwd_rows(const void* ops_dev, const void* bops_dev, int n_ops, const float* zin, const float* gx,
-                           const float* gld, float* gz, float* ws, long long R, int d, cudaStream_t st) {
+int launch_affine_bwd_rows(const void* ops_dev, const void* bops_dev, int n_ops, int direction, const float* zin,
+                           const float* gx, const float* gld, float* gz, float* ws, long long R, int d, cudaStream_t st) {
     if (R == 0) return NFB_OK;
-    affine_bwd_rows_kernel<<<(unsigned)((R + 127) / 128), 128, 0, st>>>(
-        static_cast<const AffineOp*>(ops_dev), static_cast<const AffBwdOp*>(bops_dev), n_ops, zin, gx, gld, gz, ws, R, d);
+    const AffineOp* ops = static_cast<const AffineOp*>(ops_dev);
+    const AffBwdOp* bops = static_cast<const AffBwdOp*>(bops_dev);
+    if (direction)
+        affine_bwd_rows_kernel<<<(unsigned)((R + 127) / 128), 128, 0, st>>>(ops, bops, n_ops, zin, gx, gld, gz, ws, R, d);
+    else
+        affine_density_bwd_rows_kernel<<<(unsigned)((R + 127) / 128), 128, 0, st>>>(ops, bops, n_ops, zin, gx, gld, gz,
+                                                                                     ws, R, d);
     NFB_LAUNCH_CHECK();
     return NFB_OK;
 }

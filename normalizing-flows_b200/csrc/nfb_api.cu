@@ -261,7 +261,7 @@ struct nfb_flow {
     DevBuf in_ready;                 // device int: rows of the current host batch that have landed
     // training pass workspaces (nfb_flow_backward)
     DevBuf tr_store, tr_net, tr_P, tr_gP, tr_xp, tr_gxp, tr_zp, tr_gzp, tr_in, tr_gin, tr_g0, tr_g1, tr_small, tr_glq,
-        tr_t0, tr_t1, tr_wpack;
+        tr_t0, tr_t1, tr_wpack, tr_aff;
     const int* cur_in_ready = nullptr;
     // affine sampling backward: the reduction items with this call's gradient pointers, staged through pinned memory
     AffRedItem* afb_host = nullptr;
@@ -2824,6 +2824,13 @@ int lu_layer_backward(nfb_flow* f, Layer& L, const float* zin, const float* gxp,
     return NFB_OK;
 }
 
+// the affine family's backward (defined with the sampling-direction entry points below)
+int plan_affine_bwd(nfb_flow* f, Group& g);
+long long affine_bwd_chunk_rows(const Group& g, long long rows);
+size_t affine_bwd_ws_bytes(const Group& g, long long R);
+int affine_group_backward(nfb_flow* f, Group& g, int direction, const float* in, const float* g_out, const float* g_ld,
+                          int64_t rows, float* ws, long long R, float* g_in, float* const* grad_slots, cudaStream_t st);
+
 }  // namespace
 
 extern "C" {
@@ -2854,14 +2861,18 @@ int nfb_flow_log_prob_backward(nfb_flow_t* f, const float* x, const float* g_log
                                float* gx_out, float* const* grad_slots, void* stream) {
     NFB_CHECK(f && f->finalized, NFB_ERR_STATE, "flow not finalized");
     NFB_CHECK(f->base_loc && f->base_log_scale, NFB_ERR_STATE, "no base distribution set");
-    NFB_CHECK(x && g_logq && grad_slots, NFB_ERR_ARG, "null pointer");
+    NFB_CHECK((rows == 0 || (x && g_logq)) && grad_slots, NFB_ERR_ARG, "null pointer");
     const int n_slots = nfb_flow_num_grad_slots(f);
-    NFB_CHECK(n_slots >= 0, NFB_ERR_UNSUPPORTED, "native backward covers spline blocks + LULinearPermute + DiagGaussian");
-    for (auto& grp : f->groups)   // (the affine and planar families have slots for their sampling-direction backward only)
-        NFB_CHECK(grp.kind != G_AFFINE && grp.kind != G_PLANAR, NFB_ERR_UNSUPPORTED,
-                  "native backward: affine- or planar-family group");
-    if (rows == 0) return NFB_OK;
+    NFB_CHECK(n_slots >= 0, NFB_ERR_UNSUPPORTED,
+              "native backward covers spline blocks + LULinearPermute + the affine family + DiagGaussian");
+    for (auto& grp : f->groups)   // (the planar family has slots for its sampling-direction backward only)
+        NFB_CHECK(grp.kind != G_PLANAR, NFB_ERR_UNSUPPORTED, "native backward: planar-family group");
     cudaStream_t st = S(stream);
+    if (rows == 0) {   // zero gradients
+        for (int i = 0; i < n_slots; ++i)
+            if (grad_slots[i]) NFB_CUDA(cudaMemsetAsync(grad_slots[i], 0, (size_t)nfb_flow_grad_slot_numel(f, i) * 4, st));
+        return NFB_OK;
+    }
     const int D = f->D;
     const int ng = (int)f->groups.size();
     const size_t ZS = (size_t)rows * D;
@@ -2916,7 +2927,15 @@ int nfb_flow_log_prob_backward(nfb_flow_t* f, const float* x, const float* g_log
     for (int k = ng - 1; k >= 0; --k) {
         Group& grp = f->groups[ng - 1 - k];
         const float* zin = store + (size_t)k * ZS;
-        NFB_CHECK(grp.kind != G_AFFINE, NFB_ERR_UNSUPPORTED, "native backward: affine-family group");
+        if (grp.kind == G_AFFINE) {   // recompute + adjoint walk + fixed-order reduction, chunked (internal workspace)
+            NFB_TRY(plan_affine_bwd(f, grp));
+            const long long R = affine_bwd_chunk_rows(grp, rows);
+            NFB_TRY(f->tr_aff.reserve(affine_bwd_ws_bytes(grp, R)));
+            NFB_TRY(affine_group_backward(f, grp, NFB_INVERSE, zin, g, g_logq, rows, f->tr_aff.as<float>(), R, g2,
+                                          grad_slots + off[grp.first], st));
+            std::swap(g, g2);
+            continue;
+        }
         Layer& A = *f->layers[grp.first];
         Layer* Bl = grp.last != grp.first ? f->layers[grp.last].get() : nullptr;  // pair: first = spline block, last = LU
         Layer* R = (A.kind == L_AR_RQS || A.kind == L_COUPLED_RQS) ? &A : nullptr;
@@ -3084,41 +3103,21 @@ int planar_sampling_backward(nfb_flow* f, Group& g, const float* z, const float*
     return NFB_OK;
 }
 
-int affine_only_group(nfb_flow* f, Group** out) {
+int affine_only_group(nfb_flow* f, Group** out, const char* who) {
     NFB_CHECK(f && f->finalized, NFB_ERR_STATE, "flow not finalized");
     NFB_CHECK(f->groups.size() == 1 && f->groups[0].kind == G_AFFINE, NFB_ERR_UNSUPPORTED,
-              "sampling backward: the stack must be affine-family layers only, or planar / radial layers only");
+              "%s backward: the stack must be affine-family layers only%s", who,
+              who[0] == 's' ? ", or planar / radial layers only" : "");
     *out = &f->groups[0];
     return plan_affine_bwd(f, **out);
 }
 
-}  // namespace
-
-extern "C" {
-
-int64_t nfb_flow_sampling_backward_workspace_bytes(const nfb_flow_t* fc, int64_t rows) {
-    nfb_flow* f = const_cast<nfb_flow*>(fc);
-    Group* g = planar_only_group(f);
-    if (g) return rows < 0 ? -1 : (int64_t)planar_bwd_ws_bytes(*g, planar_bwd_chunk_rows(*g, rows));
-    if (rows < 0 || affine_only_group(f, &g) != NFB_OK) return -1;
-    return (int64_t)affine_bwd_ws_bytes(*g, affine_bwd_chunk_rows(*g, rows));
-}
-
-int nfb_flow_sampling_backward(nfb_flow_t* f, const float* z, const float* g_x, const float* g_ld, int64_t rows,
-                               void* ws, int64_t ws_bytes, float* g_z, float* const* grad_slots, void* stream) {
-    if (Group* pg = planar_only_group(f))
-        return planar_sampling_backward(f, *pg, z, g_x, g_ld, rows, ws, ws_bytes, g_z, grad_slots, S(stream));
-    Group* gp = nullptr;
-    NFB_TRY(affine_only_group(f, &gp));
-    Group& g = *gp;
-    NFB_CHECK(rows >= 0, NFB_ERR_ARG, "rows < 0");
-    NFB_CHECK(rows == 0 || z, NFB_ERR_ARG, "null z");
-    const long long R = affine_bwd_chunk_rows(g, rows);
-    NFB_CHECK(ws && ws_bytes >= (int64_t)affine_bwd_ws_bytes(g, R), NFB_ERR_ARG,
-              "sampling backward: workspace of %lld bytes, %lld needed", (long long)ws_bytes,
-              (long long)affine_bwd_ws_bytes(g, R));
-    cudaStream_t st = S(stream);
-    f->launches = 0;
+// backward of one affine group in either direction (affine_bwd_rows_kernel / affine_density_bwd_rows_kernel): `in` is
+// the group's input in that direction, g_out / g_ld the cotangents of its output and log-det; writes g_in and the
+// group's slots (in grad-slot order, NULL entries skipped).  Per chunk of R rows: the row kernel, then the fixed-order
+// reduction.  ws holds affine_bwd_ws_bytes(g, R) bytes.
+int affine_group_backward(nfb_flow* f, Group& g, int direction, const float* in, const float* g_out, const float* g_ld,
+                          int64_t rows, float* ws, long long R, float* g_in, float* const* grad_slots, cudaStream_t st) {
     const int n_items = (int)g.items.size();
     if (n_items) {
         // this call's output pointers, in slot order (a Linear takes two slots, a column sum one)
@@ -3142,21 +3141,74 @@ int nfb_flow_sampling_backward(nfb_flow_t* f, const float* z, const float* g_x, 
         NFB_CUDA(cudaEventRecord(f->afb_ev, st));
     }
     const int D = f->D, n_ops = g.last - g.first + 1;
-    float* W = static_cast<float*>(ws);
-    float* partial = reinterpret_cast<float*>(static_cast<char*>(ws) + (((size_t)g.units * R * 4 + 255) & ~(size_t)255));
+    float* partial = reinterpret_cast<float*>(reinterpret_cast<char*>(ws) + (((size_t)g.units * R * 4 + 255) & ~(size_t)255));
     if (rows == 0) {   // zero parameter gradients
-        NFB_TRY(launch_affine_bwd_reduce(f->afb_items.p, n_items, g.n_elem, W, 0, partial, 0, st));
+        NFB_TRY(launch_affine_bwd_reduce(f->afb_items.p, n_items, g.n_elem, ws, 0, partial, 0, st));
         f->launches += g.n_elem ? 1 : 0;
         return NFB_OK;
     }
     for (long long r0 = 0; r0 < rows; r0 += R) {
         const long long n = std::min(R, (long long)rows - r0);
-        NFB_TRY(launch_affine_bwd_rows(g.ops.p, g.bops.p, n_ops, z + r0 * D, g_x ? g_x + r0 * D : nullptr,
-                                       g_ld ? g_ld + r0 : nullptr, g_z ? g_z + r0 * D : nullptr, W, n, D, st));
-        NFB_TRY(launch_affine_bwd_reduce(f->afb_items.p, n_items, g.n_elem, W, n, partial, r0 > 0, st));
+        NFB_TRY(launch_affine_bwd_rows(g.ops.p, g.bops.p, n_ops, direction, in + r0 * D, g_out ? g_out + r0 * D : nullptr,
+                                       g_ld ? g_ld + r0 : nullptr, g_in ? g_in + r0 * D : nullptr, ws, n, D, st));
+        NFB_TRY(launch_affine_bwd_reduce(f->afb_items.p, n_items, g.n_elem, ws, n, partial, r0 > 0, st));
         f->launches += 1 + (g.n_elem ? 2 : 0);
     }
     return NFB_OK;
+}
+
+// the entry points' common checks; R = the chunk size the workspace is planned for
+int affine_entry_checks(const char* who, Group& g, const float* in, int64_t rows, void* ws, int64_t ws_bytes,
+                        long long* R) {
+    NFB_CHECK(rows >= 0, NFB_ERR_ARG, "rows < 0");
+    NFB_CHECK(rows == 0 || in, NFB_ERR_ARG, "null input");
+    *R = affine_bwd_chunk_rows(g, rows);
+    NFB_CHECK(ws && ws_bytes >= (int64_t)affine_bwd_ws_bytes(g, *R), NFB_ERR_ARG,
+              "%s backward: workspace of %lld bytes, %lld needed", who, (long long)ws_bytes,
+              (long long)affine_bwd_ws_bytes(g, *R));
+    return NFB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int64_t nfb_flow_sampling_backward_workspace_bytes(const nfb_flow_t* fc, int64_t rows) {
+    nfb_flow* f = const_cast<nfb_flow*>(fc);
+    Group* g = planar_only_group(f);
+    if (g) return rows < 0 ? -1 : (int64_t)planar_bwd_ws_bytes(*g, planar_bwd_chunk_rows(*g, rows));
+    if (rows < 0 || affine_only_group(f, &g, "sampling") != NFB_OK) return -1;
+    return (int64_t)affine_bwd_ws_bytes(*g, affine_bwd_chunk_rows(*g, rows));
+}
+
+int nfb_flow_sampling_backward(nfb_flow_t* f, const float* z, const float* g_x, const float* g_ld, int64_t rows,
+                               void* ws, int64_t ws_bytes, float* g_z, float* const* grad_slots, void* stream) {
+    if (Group* pg = planar_only_group(f))
+        return planar_sampling_backward(f, *pg, z, g_x, g_ld, rows, ws, ws_bytes, g_z, grad_slots, S(stream));
+    Group* gp = nullptr;
+    NFB_TRY(affine_only_group(f, &gp, "sampling"));
+    long long R = 0;
+    NFB_TRY(affine_entry_checks("sampling", *gp, z, rows, ws, ws_bytes, &R));
+    f->launches = 0;
+    return affine_group_backward(f, *gp, NFB_FORWARD, z, g_x, g_ld, rows, static_cast<float*>(ws), R, g_z, grad_slots,
+                                 S(stream));
+}
+
+int64_t nfb_flow_density_backward_workspace_bytes(const nfb_flow_t* fc, int64_t rows) {
+    Group* g = nullptr;
+    if (rows < 0 || affine_only_group(const_cast<nfb_flow*>(fc), &g, "density") != NFB_OK) return -1;
+    return (int64_t)affine_bwd_ws_bytes(*g, affine_bwd_chunk_rows(*g, rows));
+}
+
+int nfb_flow_density_backward(nfb_flow_t* f, const float* x, const float* g_z, const float* g_ld, int64_t rows,
+                              void* ws, int64_t ws_bytes, float* g_x, float* const* grad_slots, void* stream) {
+    Group* gp = nullptr;
+    NFB_TRY(affine_only_group(f, &gp, "density"));
+    long long R = 0;
+    NFB_TRY(affine_entry_checks("density", *gp, x, rows, ws, ws_bytes, &R));
+    f->launches = 0;
+    return affine_group_backward(f, *gp, NFB_INVERSE, x, g_z, g_ld, rows, static_cast<float*>(ws), R, g_x, grad_slots,
+                                 S(stream));
 }
 
 }  // extern "C"

@@ -166,8 +166,10 @@ struct AffRedItem {                // one Linear's (dW, db) or, with n_in = 0, o
     float* db;
 };
 constexpr int kAffSegRows = 1024;  // rows per partial sum of the weight reduction
-int launch_affine_bwd_rows(const void* ops_dev, const void* bops_dev, int n_ops, const float* zin, const float* gx,
-                           const float* gld, float* gz, float* ws, long long R, int d, cudaStream_t st);
+// direction 1: sampling backward (zin = z, gx / gld the cotangents of x / log_det, writes g_z); direction 0: density
+// backward (zin = x, gx / gld the cotangents of z / log_det, writes g_x into gz)
+int launch_affine_bwd_rows(const void* ops_dev, const void* bops_dev, int n_ops, int direction, const float* zin,
+                           const float* gx, const float* gld, float* gz, float* ws, long long R, int d, cudaStream_t st);
 int launch_affine_bwd_reduce(const void* items_dev, int n_items, long long n_elem, const float* ws, long long R,
                              float* partial, int accumulate, cudaStream_t st);
 

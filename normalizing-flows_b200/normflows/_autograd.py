@@ -1,8 +1,10 @@
-"""Gradients for the density pass -- INTERIM (SURVEY 8f-1 "backward of the fused blocks" is the real fix).
+"""Gradients for the density pass.
 
-`forward_kld` / `log_prob` run on the hand-written CUDA path.  So that `loss.backward()` in the reference's
-examples keeps working, the autograd hook below re-materialises the same density pass in differentiable
-torch ops ON THE SAME DEVICE during backward and lets autograd produce exact gradients.  The forward
+`forward_kld` / `log_prob` run on the hand-written CUDA path.  Their backward is native for stacks of spline blocks,
+LULinearPermute and affine-family layers (`native_backward`: nfb_flow_log_prob_backward).  For other stacks -- INTERIM
+(SURVEY 8f-1 "backward of the fused blocks" is the real fix) -- and as the A/B reference of the GPU tests
+(`DensityFn.use_native_backward = False`), the autograd hook below re-materialises the same density pass in
+differentiable torch ops ON THE SAME DEVICE during backward and lets autograd produce exact gradients.  The forward
 value, the metric and every parity claim come from the CUDA kernels; this module is only reached from
 `backward()`.  It restates (mask-free) the same reference arithmetic as the kernels:
   spline utils/splines.py:16-219, MADE nets/made.py:296-304, ResidualNet nets/resnet.py:92-104,
@@ -162,11 +164,15 @@ def _net_slots(net):
 
 def grad_slot_tensors(model):
     """Parameters in the order of the C ABI's gradient slots (include/nfb200.h nfb_flow_log_prob_backward), or None
-    if a layer has no native backward."""
+    if a layer has no native backward.  An affine-family layer's slots are those of the sampling backward; a buffer
+    behind a slot (AffineConstFlow(scale=False)) gets no buffer."""
     from .flows import neural_spline as ns, mixing
+    from ._standalone import sampling_slot_tensors
     out = []
     for layer in model.flows:
-        if isinstance(layer, ns.AutoregressiveRationalQuadraticSpline):
+        if getattr(layer, "_affine_family", False):
+            out += sampling_slot_tensors([layer])
+        elif isinstance(layer, ns.AutoregressiveRationalQuadraticSpline):
             out += _net_slots(layer.mprqat.autoregressive_net)
         elif isinstance(layer, ns.CoupledRationalQuadraticSpline):
             u = layer.prqct.unconditional_transform
@@ -182,9 +188,11 @@ def grad_slot_tensors(model):
 
 def native_backward(model, x, grad_out, need_x):
     """Gradients from libnfb200.so (csrc/nfb_api.cu nfb_flow_log_prob_backward: tensor-core dgrad/wgrad + analytic
-    spline adjoint).  Returns (gx | None, {id(param): grad}) or None when the stack is not covered."""
+    spline adjoint, the affine family's per-row adjoint kernel).  Returns (gx | None, {id(param): grad}) or None when
+    the stack is not covered."""
     import ctypes as C
     from . import _lib as L
+    from ._standalone import sum_slot_grads
     slots = grad_slot_tensors(model)
     h = model._stack()
     if slots is None or h is None or h.base is None or x.dim() != 2:
@@ -209,12 +217,13 @@ def native_backward(model, x, grad_out, need_x):
     with torch.cuda.device(x.device):
         L.check(lib.nfb_flow_log_prob_backward(handle, L.ptr(xx), L.ptr(g), xx.shape[0], None, L.ptr(gx), arr,
                                                L.stream_ptr()))
-    return gx, {id(p): b for p, b in zip(slots, bufs) if b is not None}
+    return gx, sum_slot_grads(slots, bufs)
 
 
 class DensityFn(torch.autograd.Function):
     """log_prob(x) on the CUDA path.  backward: native kernels (dgrad / wgrad on the tensor core, analytic spline
-    adjoint) for spline-block + LULinearPermute stacks; other stacks re-materialise a torch graph (interim)."""
+    adjoint, the affine family's per-row adjoint kernel) for stacks of spline blocks, LULinearPermute and affine-family
+    layers; other stacks re-materialise a torch graph (interim)."""
     use_native_backward = True
 
     @staticmethod
@@ -249,8 +258,10 @@ class DensityFn(torch.autograd.Function):
 
 class LayerInverseFn(torch.autograd.Function):
     """(z', log_det) = layer.inverse(z) of ONE NativeFlow called on its own (a layer of a stack that also holds non-native
-    layers, e.g. the ActNorms between Residual blocks).  The forward is the layer's kernel (FlowHandle.layer_apply); the
-    backward re-materialises the layer with `layer_inverse` above (interim, like DensityFn's torch path)."""
+    layers, e.g. the ActNorms between Residual blocks).  The forward is the layer's kernel (FlowHandle.layer_apply).  The
+    backward of an affine-family layer is nfb_flow_density_backward on the layer's own handle; other layers
+    (LULinearPermute, leaky Planar) re-materialise the layer with `layer_inverse` above (interim, like DensityFn's torch
+    path)."""
 
     @staticmethod
     def forward(ctx, layer, z, *params):
@@ -267,6 +278,12 @@ class LayerInverseFn(torch.autograd.Function):
         if any(p._version != v for p, v in zip(ctx.params, ctx.versions)):
             raise RuntimeError(f"{type(ctx.layer).__name__} backward: a parameter was modified in place after the forward pass")
         need_z = ctx.needs_input_grad[1]
+        if getattr(ctx.layer, "_affine_family", False):
+            from . import _lib as L
+            from ._standalone import stack_backward
+            gz, gmap = stack_backward(ctx.layer._single(), [ctx.layer], L.NFB_INVERSE, z.contiguous(), g_out, g_ld,
+                                      need_z)
+            return (None, gz, *[gmap.get(id(p)) if p.requires_grad else None for p in ctx.params])
         params = [p for p in ctx.params if p.requires_grad]
         with torch.enable_grad():
             zz = z.detach().requires_grad_(need_z)

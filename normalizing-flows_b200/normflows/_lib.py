@@ -196,6 +196,8 @@ SYMBOLS = {
     "nfb_flow_log_prob_backward": (C.c_int, [_VP, _VP, _VP, _I64, _VP, _VP, C.POINTER(_VP), _VP]),
     "nfb_flow_sampling_backward_workspace_bytes": (_I64, [_VP, _I64]),
     "nfb_flow_sampling_backward": (C.c_int, [_VP, _VP, _VP, _VP, _I64, _VP, _I64, _VP, C.POINTER(_VP), _VP]),
+    "nfb_flow_density_backward_workspace_bytes": (_I64, [_VP, _I64]),
+    "nfb_flow_density_backward": (C.c_int, [_VP, _VP, _VP, _VP, _I64, _VP, _I64, _VP, C.POINTER(_VP), _VP]),
     "nfb_flow_log_prob_host": (C.c_int, [_VP, _VP, _VP, _I64]),
     "nfb_flow_forward_kld_host": (C.c_int, [_VP, _VP, _I64, _VP]),
 }

@@ -135,17 +135,53 @@ def sampling_slot_tensors(layers):
 affine_slot_tensors = sampling_slot_tensors   # (the name callers of the affine-only version use)
 
 
+def sum_slot_grads(slots, bufs):
+    """{id(parameter): gradient} from per-slot gradient buffers: a parameter behind several slots (a net or layer used
+    twice) gets the sum, as autograd would give."""
+    gmap = {}
+    for p, b in zip(slots, bufs):
+        if b is not None:
+            gmap[id(p)] = gmap[id(p)] + b if id(p) in gmap else b
+    return gmap
+
+
+def stack_backward(handle, layers, direction, z, g_out, g_ld, need_z):
+    """(g_z | None, {id(parameter): gradient}) of (out, log_det) = handle.transform(direction, z) through
+    nfb_flow_sampling_backward (NFB_FORWARD: all-affine or all-planar stacks) or nfb_flow_density_backward (NFB_INVERSE:
+    all-affine stacks); g_out / g_ld are the cotangents of out / log_det (None: zero)."""
+    slots = sampling_slot_tensors(layers)
+    bufs = [torch.empty_like(p) if isinstance(p, torch.nn.Parameter) and p.requires_grad else None for p in slots]
+    gz = torch.empty_like(z) if need_z else None
+    g_out = g_out.to(torch.float32).contiguous() if g_out is not None else None
+    g_ld = g_ld.to(torch.float32).contiguous() if g_ld is not None else None
+    lib = L.lib()
+    h = handle.ensure(z.shape[1], z.device)
+    if lib.nfb_flow_num_grad_slots(h) < len(slots):
+        raise RuntimeError("native backward: gradient slot mismatch")
+    if direction == L.NFB_FORWARD:
+        ws_bytes, call = lib.nfb_flow_sampling_backward_workspace_bytes, lib.nfb_flow_sampling_backward
+    else:
+        ws_bytes, call = lib.nfb_flow_density_backward_workspace_bytes, lib.nfb_flow_density_backward
+    ws = _workspace(ws_bytes(h, z.shape[0]), z.device)
+    arr = _vp(bufs)
+    with torch.cuda.device(z.device):
+        L.check(call(h, L.ptr(z), L.ptr(g_out), L.ptr(g_ld), z.shape[0], L.ptr(ws), ws.numel(), L.ptr(gz),
+                     C.cast(arr, C.POINTER(C.c_void_p)), L.stream_ptr()))
+    return gz, sum_slot_grads(slots, bufs)
+
+
 class StackSamplingFn(torch.autograd.Function):
-    """(x, log_det) = handle.transform(NFB_FORWARD, z) of an all-affine stack (MaskedAffineFlow, AffineConstFlow /
-    ActNorm, AffineCouplingBlock, Permute) or an all-planar one (Planar, Radial): the unchanged one-launch forward, so
-    values are bit-identical with and without grad.  The backward is one nfb_flow_sampling_backward call (recompute +
-    reverse walk, then a fixed-order reduction of the parameter terms).  Refuses to run the backward if a parameter was
-    modified in place after the forward."""
+    """(out, log_det) = handle.transform(direction, z) of an all-affine stack (MaskedAffineFlow, AffineConstFlow /
+    ActNorm, AffineCouplingBlock, Permute), or in the sampling direction of an all-planar one (Planar, Radial): the
+    unchanged one-launch forward, so values are bit-identical with and without grad.  The backward is one
+    nfb_flow_sampling_backward / nfb_flow_density_backward call (recompute + walk back through the ops, then a
+    fixed-order reduction of the parameter terms).  Refuses to run the backward if a parameter was modified in place
+    after the forward."""
 
     @staticmethod
-    def forward(ctx, handle, layers, z, *params):
-        x, ld = handle.transform(L.NFB_FORWARD, z)
-        ctx.handle, ctx.layers, ctx.params = handle, layers, params
+    def forward(ctx, handle, layers, direction, z, *params):
+        x, ld = handle.transform(direction, z)
+        ctx.handle, ctx.layers, ctx.direction, ctx.params = handle, layers, direction, params
         ctx.versions = [p._version for p in params]
         ctx.save_for_backward(require_cuda_f32(z))
         return x, ld
@@ -156,31 +192,12 @@ class StackSamplingFn(torch.autograd.Function):
         if any(p._version != v for p, v in zip(ctx.params, ctx.versions)):
             names = "+".join(sorted({type(l).__name__ for l in ctx.layers}))
             raise RuntimeError(f"{names} backward: a parameter was modified in place after the forward pass")
-        slots = sampling_slot_tensors(ctx.layers)
-        bufs = [torch.empty_like(p) if isinstance(p, torch.nn.Parameter) and p.requires_grad else None for p in slots]
-        need_z = ctx.needs_input_grad[2]
-        gz = torch.empty_like(z) if need_z else None
-        g_x = g_x.to(torch.float32).contiguous() if g_x is not None else None
-        g_ld = g_ld.to(torch.float32).contiguous() if g_ld is not None else None
-        lib = L.lib()
-        h = ctx.handle.ensure(z.shape[1], z.device)
-        if lib.nfb_flow_num_grad_slots(h) < len(slots):
-            raise RuntimeError("sampling backward: gradient slot mismatch")
-        ws = _workspace(lib.nfb_flow_sampling_backward_workspace_bytes(h, z.shape[0]), z.device)
-        arr = _vp(bufs)
-        with torch.cuda.device(z.device):
-            L.check(lib.nfb_flow_sampling_backward(h, L.ptr(z), L.ptr(g_x), L.ptr(g_ld), z.shape[0], L.ptr(ws),
-                                                   ws.numel(), L.ptr(gz), C.cast(arr, C.POINTER(C.c_void_p)),
-                                                   L.stream_ptr()))
-        gmap = {}   # a parameter behind several slots (a net or layer used twice) gets the sum, as autograd would give
-        for p, b in zip(slots, bufs):
-            if b is not None:
-                gmap[id(p)] = gmap[id(p)] + b if id(p) in gmap else b
-        return (None, None, gz, *[gmap.get(id(p)) if p.requires_grad else None for p in ctx.params])
+        gz, gmap = stack_backward(ctx.handle, ctx.layers, ctx.direction, z, g_x, g_ld, ctx.needs_input_grad[3])
+        return (None, None, None, gz, *[gmap.get(id(p)) if p.requires_grad else None for p in ctx.params])
 
 
-def stack_sampling(handle, layers, z, params):
-    return StackSamplingFn.apply(handle, list(layers), z, *params)
+def stack_sampling(handle, layers, z, params, direction=L.NFB_FORWARD):
+    return StackSamplingFn.apply(handle, list(layers), direction, z, *params)
 
 
 # ---- element adjoints ------------------------------------------------------------------------------------------

@@ -104,6 +104,9 @@ class NormalizingFlow(nn.Module):
         h = self._stack()
         self._run_pending_inits(x, inverse=True)
         if h is not None and x.dim() == 2:
+            if self._one_sampling_family() == "affine" and wants_grad(self.flows, x):   # native density backward
+                from ._standalone import stack_sampling
+                return stack_sampling(h, self.flows, x, list(self.flows.parameters()), L.NFB_INVERSE)
             return h.transform(L.NFB_INVERSE, x)
         log_det = torch.zeros(len(x), device=x.device)
         for i in range(len(self.flows) - 1, -1, -1):
@@ -142,9 +145,10 @@ class NormalizingFlow(nn.Module):
     def _one_sampling_family(self):
         """Every layer is in the affine family (MaskedAffineFlow, AffineConstFlow / ActNorm, AffineCouplingBlock,
         Permute), or every layer in the planar family (Planar, Radial): the all-native stack's sampling direction has a
-        native backward (nfb_flow_sampling_backward).  Mixes of the two families do not."""
+        native backward (nfb_flow_sampling_backward); returns that family's name ("affine" / "planar"), else None.  Mixes
+        of the two families do not."""
         fams = {f._sampling_family() if isinstance(f, NativeFlow) else None for f in self.flows}
-        return len(fams) == 1 and None not in fams
+        return fams.pop() if len(fams) == 1 else None
 
     def _no_sampling_grad(self, what, context=None):
         """Gradients through the sampling direction exist when every layer's sampling direction is differentiable (the

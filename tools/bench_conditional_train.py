@@ -20,6 +20,10 @@
          notebook's) and 4 096
     augmented examples/augmented_flow.ipynb: 32 x [MaskedAffineFlow(MLP([4, 16, 4]) s and t), ActNorm(4)] on
          DiagGaussian(4), target TwoIndependent(TwoMoons(), DiagGaussian(2)), the same step at batch 20
+    colab examples/real_nvp_colab.ipynb: 32 x [AffineCouplingBlock(MLP([1, 64, 64, 2])), Permute(2, 'swap')] on
+         DiagGaussian(2), Adam(lr 5e-4, weight decay 1e-5), batch 512 (the notebook's) and 65 536 (forward KL: gradients
+         through the density direction).  Also timed with DensityFn.use_native_backward = False (the torch restatement
+         of the backward, arm "torch_backward"), in the same run
 Prints one JSON line: ms/step (median of CUDA-event-timed steps after warm-up), samples/s, kernel launches per step
 (torch.profiler, one separate step), peak device memory, and the card's name, power limit and SM clock read in the same
 run.  When the unmodified reference is installed under oracle/_ref, the same model, seed and batch are timed through it
@@ -37,7 +41,9 @@ REF_DIR = os.path.join(ROOT, "oracle", "_ref")
 
 
 CASES = [("a", 128), ("a", 65536), ("b", 128), ("b", 65536), ("circ", 1024), ("maf", 128), ("maf", 65536),
-         ("maf16", 65536), ("paper", 16384), ("realnvp", 20), ("realnvp", 4096), ("augmented", 20)]
+         ("maf16", 65536), ("paper", 16384), ("realnvp", 20), ("realnvp", 4096), ("augmented", 20),
+         ("colab", 512), ("colab", 65536)]
+TORCH_BACKWARD_CASES = {"colab"}   # cases whose backward has a torch restatement to compare against
 NOTEBOOK_LAYERS = 4   # examples/conditional_flow.ipynb: K = 4 (spline + LU) pairs
 
 
@@ -72,6 +78,12 @@ def build(nf, kind):
         target = nf.distributions.TwoModes(2, 0.1) if d == 2 else \
             nf.distributions.TwoIndependent(nf.distributions.TwoMoons(), nf.distributions.DiagGaussian(2))
         return nf.NormalizingFlow(nf.distributions.DiagGaussian(d), flows, target), (1e-4, 1e-6), d, False
+    if kind == "colab":
+        flows = []
+        for _ in range(32):
+            flows += [nf.flows.AffineCouplingBlock(nf.nets.MLP([1, 64, 64, 2], init_zeros=True)),
+                      nf.flows.Permute(2, mode='swap')]
+        return nf.NormalizingFlow(nf.distributions.DiagGaussian(2), flows), (5e-4, 1e-5), 2, False
     if kind == "circ":
         flows = [nf.flows.CircularAutoregressiveRationalQuadraticSpline(2, 1, 128, [1], tail_bound=torch.tensor([5., math.pi]),
                                                                         permute_mask=True) for _ in range(20)]
@@ -102,6 +114,9 @@ def time_arm(arm, kind, batch, steps, warmup):
     else:
         sys.path[:0] = [ROOT, os.path.join(ROOT, "normalizing-flows_b200")]
     import normflows as nf
+    if arm == "torch_backward":
+        from normflows._autograd import DensityFn
+        DensityFn.use_native_backward = False
     dev = torch.device("cuda")
     model, (lr, wd), dim, conditional = build(nf, kind)
     model = model.to(dev)
@@ -171,16 +186,19 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--no-reference", action="store_true")
     ap.add_argument("--cases", help="comma-separated model names (default: all)")
-    ap.add_argument("--arm", choices=["native", "reference"], help=argparse.SUPPRESS)
+    ap.add_argument("--arm", choices=["native", "torch_backward", "reference"], help=argparse.SUPPRESS)
     a = ap.parse_args()
     if a.arm:   # one arm in its own process (the two packages share the name `normflows`)
         want = set(a.cases.split(",")) if a.cases else None
+        if a.arm == "torch_backward":
+            want = (want or TORCH_BACKWARD_CASES) & TORCH_BACKWARD_CASES
         print(json.dumps([time_arm(a.arm, k, b, a.steps, a.warmup) for k, b in CASES if want is None or k in want]))
         return
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("bench_conditional_train: no CUDA device")
-    arms = ["native"] + (["reference"] if not a.no_reference and os.path.isdir(os.path.join(REF_DIR, "normflows"))
+    cases = set(a.cases.split(",")) if a.cases else None
+    arms = ["native"] + (["torch_backward"] if cases is None or cases & TORCH_BACKWARD_CASES else []) + (["reference"] if not a.no_reference and os.path.isdir(os.path.join(REF_DIR, "normflows"))
                          else [])
     res = {}
     for arm in arms:
