@@ -320,6 +320,24 @@ int nfb_gaussian_table_log_prob_backward(const float* z_dev, const int64_t* y_de
                                          const float* log_scale_dev, const float* g_log_q_dev, float* g_z_dev,
                                          float* g_loc_dev, float* g_log_scale_dev, int64_t batch, int32_t dim,
                                          int32_t group, int32_t num_classes, void* stream);
+/* distributions/base.py:573-659 GaussianMixture.log_prob: log_q[r] (+)= logsumexp_k [log_softmax(weight_scores)_k
+ * - dim/2 log 2pi - sum_d log_scale[k,d] - 1/2 sum_d ((z[r,d] - loc[k,d]) / exp(log_scale[k,d]))^2], loc / log_scale
+ * [n_modes, dim], weight_scores [n_modes].  Any n_modes >= 1 and dim >= 1; one launch.  log_softmax, not log(softmax):
+ * a weight that underflows in the reference gives a finite, negligible term (and finite gradients) instead of -inf. */
+int nfb_gaussian_mixture_log_prob(const float* z_dev, const float* loc_dev, const float* log_scale_dev,
+                                  const float* weight_scores_dev, float* log_q_dev, int64_t rows, int32_t n_modes,
+                                  int32_t dim, int32_t accumulate, void* stream);
+/* Adjoint of nfb_gaussian_mixture_log_prob (accumulate = 0) with row cotangents g_log_q [rows]: g_z [rows, dim] and the
+ * parameter gradients g_loc / g_log_scale [n_modes, dim], g_weight_scores [n_modes] are overwritten (each may be NULL).
+ * Deterministic (fixed-order sums, no atomics) in two launches whatever rows and n_modes; the workspace
+ * (nfb_gaussian_mixture_log_prob_backward_workspace_bytes, -1 for a bad shape) does not grow with rows beyond 256 row
+ * blocks and stays under 64 MiB unless one copy of the parameters' gradients is larger.  rows = 0 writes zeros. */
+int64_t nfb_gaussian_mixture_log_prob_backward_workspace_bytes(int64_t rows, int32_t n_modes, int32_t dim);
+int nfb_gaussian_mixture_log_prob_backward(const float* z_dev, const float* loc_dev, const float* log_scale_dev,
+                                           const float* weight_scores_dev, const float* g_log_q_dev, int64_t rows,
+                                           int32_t n_modes, int32_t dim, void* ws, int64_t ws_bytes, float* g_z_dev,
+                                           float* g_loc_dev, float* g_log_scale_dev, float* g_weight_scores_dev,
+                                           void* stream);
 /* Adjoint of nfb_logit_transform in the density direction (NFB_INVERSE): g_in = dy/dx g_out + d log_det/dx g_log_det
  * (g_out or g_log_det may be NULL). */
 int nfb_logit_transform_backward(const float* in_dev, const float* g_out_dev, const float* g_log_det_dev, float* g_in_dev,
@@ -504,6 +522,11 @@ int nfb_flow_add_planar(nfb_flow_t* f, const nfb_planar_desc_t* d);
 int nfb_flow_add_radial(nfb_flow_t* f, const nfb_radial_desc_t* d);
 /* q0 = DiagGaussian(features): loc/log_scale [features] (distributions/base.py:71-76) */
 int nfb_flow_set_base_diag_gaussian(nfb_flow_t* f, const float* loc_dev, const float* log_scale_dev);
+/* q0 = GaussianMixture(n_modes, features): loc / log_scale [n_modes, features], weight_scores [n_modes]
+ * (distributions/base.py:573-614).  Either setter replaces any earlier base.  log_prob, forward_kld, their _host forms
+ * and nfb_flow_log_prob_backward then use the mixture (nfb_gaussian_mixture_log_prob, one launch after the stack). */
+int nfb_flow_set_base_gaussian_mixture(nfb_flow_t* f, int32_t n_modes, const float* loc_dev, const float* log_scale_dev,
+                                       const float* weight_scores_dev);
 /* pack parameters; `use_tensor_cores`=0 forces the plain-fp32 kernels for every layer (A/B parity) */
 int nfb_flow_finalize(nfb_flow_t* f, int32_t use_tensor_cores, void* stream);
 /* re-read the descriptor pointers after a parameter update (optimizer step / load_state_dict) */
@@ -533,7 +556,7 @@ int nfb_flow_forward_kld(nfb_flow_t* f, const float* x_dev, int64_t rows, float*
 /* ---- training pass (`loss.backward()` of examples/neural_spline_flow.ipynb cell 4; core.py:87-102 under autograd) ----
  * Gradients of sum_r g_logq[r] * log_prob(x_r) w.r.t. every parameter and (optionally) x, for stacks made of
  * autoregressive / coupled RQ-spline blocks (flows/neural_spline/wrapper.py), LULinearPermute (flows/mixing.py:535-563)
- * and a DiagGaussian base.  The pass re-runs the density direction keeping each layer group's input, recomputes the
+ * and a DiagGaussian or GaussianMixture base.  The pass re-runs the density direction keeping each layer group's input, recomputes the
  * conditioner activations per layer (nets/made.py:199-214, nets/resnet.py:37-50), applies the analytic adjoint of the
  * spline (utils/splines.py:100-219) and runs dgrad / wgrad of every Linear on the tensor core.
  * Gradient slots, in list order of the layers:
@@ -543,7 +566,8 @@ int nfb_flow_forward_kld(nfb_flow_t* f, const float* x_dev, int64_t rows, float*
  *   MaskedAffineFlow : net.<i>.weight, .bias of every Linear of s, then of t (an absent net has none)
  *   AffineConstFlow / ActNorm : s, t       AffineCouplingBlock : param_map's Linears       Permute : none
  *   Planar : u, w, b       Radial : beta, alpha, z_0
- *   base (last two slots) : loc, log_scale
+ *   base (last slots)     : DiagGaussian loc, log_scale [features] (two slots); GaussianMixture loc, log_scale
+ *                           [n_modes * features], weight_scores [n_modes] (three slots)
  * `grad_slots[i]` is a device buffer of nfb_flow_grad_slot_numel(f, i) floats that is OVERWRITTEN, or NULL to skip.
  * nfb_flow_num_grad_slots returns -1 when the flow holds a layer kind without a native backward.  Groups of affine-family
  * layers may sit anywhere in the stack: each runs the same recompute + adjoint walk + fixed-order reduction as
@@ -568,7 +592,7 @@ int nfb_flow_log_prob_backward(nfb_flow_t* f, const float* x_dev, const float* g
  * chunks, so the workspace (nfb_flow_sampling_backward_workspace_bytes, -1 for an unsupported stack) stays below a fixed
  * bound; the number of launches does not depend on the number of layers.
  * g_x / g_ld may be NULL (zero cotangent); g_z and individual slots may be NULL (not wanted).  grad_slots holds the
- * layers' slots in nfb_flow_grad_slot_numel order (a base's two slots, if any, are not read); rows = 0 writes zeros. */
+ * layers' slots in nfb_flow_grad_slot_numel order (a base's slots, if any, are not read); rows = 0 writes zeros. */
 int64_t nfb_flow_sampling_backward_workspace_bytes(const nfb_flow_t* f, int64_t rows);
 int nfb_flow_sampling_backward(nfb_flow_t* f, const float* z, const float* g_x, const float* g_ld, int64_t rows,
                                void* ws, int64_t ws_bytes, float* g_z, float* const* grad_slots, void* stream);
@@ -580,8 +604,8 @@ int nfb_flow_sampling_backward(nfb_flow_t* f, const float* z, const float* g_x, 
  * NFB_ERR_UNSUPPORTED).  x is the input that nfb_flow_transform was given.  One kernel recomputes the stack from x
  * taking the ops last-to-first, then walks them first-to-last; the weight reduction, the row chunking, the workspace
  * bound and the launch count are those of nfb_flow_sampling_backward.  g_z / g_ld may be NULL (zero cotangent); g_x and
- * individual slots may be NULL (not wanted); grad_slots is in nfb_flow_grad_slot_numel order (a base's two slots, if
- * any, are not read); rows = 0 writes zeros. */
+ * individual slots may be NULL (not wanted); grad_slots is in nfb_flow_grad_slot_numel order (a base's slots, if any,
+ * are not read); rows = 0 writes zeros. */
 int64_t nfb_flow_density_backward_workspace_bytes(const nfb_flow_t* f, int64_t rows);
 int nfb_flow_density_backward(nfb_flow_t* f, const float* x, const float* g_z, const float* g_ld, int64_t rows,
                               void* ws, int64_t ws_bytes, float* g_x, float* const* grad_slots, void* stream);

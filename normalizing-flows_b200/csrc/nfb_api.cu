@@ -240,6 +240,8 @@ struct nfb_flow {
     std::vector<Group> groups;
     const float* base_loc = nullptr;
     const float* base_log_scale = nullptr;
+    const float* base_weight_scores = nullptr;   // set: the base is a Gaussian mixture of base_modes modes
+    int base_modes = 0;
     // workspaces
     StagedReads reads;              // pinned staging for the packer's small device->host reads
     DevBuf wave_order;              // diagonal unit order of gated host passes (launch_fused_stack)
@@ -261,7 +263,7 @@ struct nfb_flow {
     DevBuf in_ready;                 // device int: rows of the current host batch that have landed
     // training pass workspaces (nfb_flow_backward)
     DevBuf tr_store, tr_net, tr_P, tr_gP, tr_xp, tr_gxp, tr_zp, tr_gzp, tr_in, tr_gin, tr_g0, tr_g1, tr_small, tr_glq,
-        tr_t0, tr_t1, tr_wpack, tr_aff;
+        tr_t0, tr_t1, tr_wpack, tr_aff, tr_mix;
     const int* cur_in_ready = nullptr;
     // affine sampling backward: the reduction items with this call's gradient pointers, staged through pinned memory
     AffRedItem* afb_host = nullptr;
@@ -1128,6 +1130,31 @@ int nfb_diag_gaussian_log_prob(const float* z, const float* loc, const float* lo
                                int64_t rows, int32_t dim, int32_t accumulate, void* stream) {
     NFB_CHECK(z && loc && log_scale && log_q, NFB_ERR_ARG, "nfb_diag_gaussian_log_prob: null pointer");
     return launch_diag_gauss(z, loc, log_scale, log_q, rows, dim, accumulate, S(stream));
+}
+
+int nfb_gaussian_mixture_log_prob(const float* z, const float* loc, const float* log_scale, const float* weight_scores,
+                                  float* log_q, int64_t rows, int32_t n_modes, int32_t dim, int32_t accumulate,
+                                  void* stream) {
+    NFB_CHECK(rows >= 0, NFB_ERR_ARG, "nfb_gaussian_mixture_log_prob: negative size");
+    NFB_CHECK(rows == 0 || (z && loc && log_scale && weight_scores && log_q), NFB_ERR_ARG,
+              "nfb_gaussian_mixture_log_prob: null pointer");
+    return launch_mixture_log_prob(z, loc, log_scale, weight_scores, log_q, rows, n_modes, dim, accumulate, S(stream));
+}
+
+int64_t nfb_gaussian_mixture_log_prob_backward_workspace_bytes(int64_t rows, int32_t n_modes, int32_t dim) {
+    if (rows < 0 || n_modes < 1 || dim < 1) return -1;
+    return mixture_bwd_ws_bytes(rows, n_modes, dim);
+}
+
+int nfb_gaussian_mixture_log_prob_backward(const float* z, const float* loc, const float* log_scale,
+                                           const float* weight_scores, const float* g_log_q, int64_t rows,
+                                           int32_t n_modes, int32_t dim, void* ws, int64_t ws_bytes, float* g_z,
+                                           float* g_loc, float* g_log_scale, float* g_weight_scores, void* stream) {
+    NFB_CHECK(rows >= 0, NFB_ERR_ARG, "nfb_gaussian_mixture_log_prob_backward: negative size");
+    NFB_CHECK(weight_scores && (rows == 0 || (z && loc && log_scale && g_log_q)), NFB_ERR_ARG,
+              "nfb_gaussian_mixture_log_prob_backward: null pointer");
+    return launch_mixture_bwd(z, loc, log_scale, weight_scores, g_log_q, rows, n_modes, dim, ws, ws_bytes, g_z, g_loc,
+                              g_log_scale, g_weight_scores, S(stream));
 }
 
 int nfb_conv2d(const float* x, int32_t x_channels, int32_t c0, const float* w, const float* b, float* y,
@@ -2240,6 +2267,16 @@ int nfb_flow_add_radial(nfb_flow_t* f, const nfb_radial_desc_t* d) {
 int nfb_flow_set_base_diag_gaussian(nfb_flow_t* f, const float* loc, const float* log_scale) {
     NFB_CHECK(f && loc && log_scale, NFB_ERR_ARG, "null argument");
     f->base_loc = loc; f->base_log_scale = log_scale;
+    f->base_weight_scores = nullptr; f->base_modes = 0;
+    return NFB_OK;
+}
+
+int nfb_flow_set_base_gaussian_mixture(nfb_flow_t* f, int32_t n_modes, const float* loc, const float* log_scale,
+                                       const float* weight_scores) {
+    NFB_CHECK(f && loc && log_scale && weight_scores, NFB_ERR_ARG, "null argument");
+    NFB_CHECK(n_modes >= 1, NFB_ERR_ARG, "GaussianMixture: n_modes %d < 1", n_modes);
+    f->base_loc = loc; f->base_log_scale = log_scale;
+    f->base_weight_scores = weight_scores; f->base_modes = n_modes;
     return NFB_OK;
 }
 
@@ -2565,6 +2602,16 @@ int nfb_flow_transform(nfb_flow_t* f, int32_t direction, const float* z_in, floa
     return NFB_OK;
 }
 
+namespace {
+// log_q += log q0(z): the flow's base, a DiagGaussian or a Gaussian mixture (one launch either way)
+int launch_base_log_prob(nfb_flow* f, const float* z, float* log_q, int64_t rows, cudaStream_t st) {
+    if (f->base_weight_scores)
+        return launch_mixture_log_prob(z, f->base_loc, f->base_log_scale, f->base_weight_scores, log_q, rows,
+                                       f->base_modes, f->D, 1, st);
+    return launch_diag_gauss(z, f->base_loc, f->base_log_scale, log_q, rows, f->D, 1, st);
+}
+}  // namespace
+
 int nfb_flow_log_prob(nfb_flow_t* f, const float* x, float* log_q, int64_t rows, void* stream) {
     NFB_CHECK(f && f->finalized, NFB_ERR_STATE, "flow not finalized");
     NFB_CHECK(f->base_loc && f->base_log_scale, NFB_ERR_STATE, "no base distribution set");
@@ -2574,7 +2621,7 @@ int nfb_flow_log_prob(nfb_flow_t* f, const float* x, float* log_q, int64_t rows,
     NFB_TRY(f->zfinal.reserve((size_t)rows * f->D * 4));
     float* z = f->zfinal.as<float>();
     NFB_TRY(nfb_flow_transform(f, NFB_INVERSE, x, z, log_q, rows, stream));
-    NFB_TRY(launch_diag_gauss(z, f->base_loc, f->base_log_scale, log_q, rows, f->D, 1, S(stream)));
+    NFB_TRY(launch_base_log_prob(f, z, log_q, rows, S(stream)));
     f->launches++;
     return NFB_OK;
 }
@@ -2843,7 +2890,7 @@ int nfb_flow_num_grad_slots(const nfb_flow_t* f) {
         if (k < 0) return -1;  // a layer kind without a native backward
         n += k;
     }
-    return n + (f->base_loc ? 2 : 0);
+    return n + (f->base_loc ? (f->base_weight_scores ? 3 : 2) : 0);
 }
 
 int64_t nfb_flow_grad_slot_numel(const nfb_flow_t* f, int32_t slot) {
@@ -2854,6 +2901,7 @@ int64_t nfb_flow_grad_slot_numel(const nfb_flow_t* f, int32_t slot) {
         if (slot < k) return grad_slot_numel(*L, slot);
         slot -= k;
     }
+    if (f->base_weight_scores) return slot < 2 ? (int64_t)f->base_modes * f->D : slot == 2 ? f->base_modes : -1;
     return (f->base_loc && slot < 2) ? f->D : -1;
 }
 
@@ -2864,7 +2912,7 @@ int nfb_flow_log_prob_backward(nfb_flow_t* f, const float* x, const float* g_log
     NFB_CHECK((rows == 0 || (x && g_logq)) && grad_slots, NFB_ERR_ARG, "null pointer");
     const int n_slots = nfb_flow_num_grad_slots(f);
     NFB_CHECK(n_slots >= 0, NFB_ERR_UNSUPPORTED,
-              "native backward covers spline blocks + LULinearPermute + the affine family + DiagGaussian");
+              "native backward covers spline blocks + LULinearPermute + the affine family + DiagGaussian / GaussianMixture");
     for (auto& grp : f->groups)   // (the planar family has slots for its sampling-direction backward only)
         NFB_CHECK(grp.kind != G_PLANAR, NFB_ERR_UNSUPPORTED, "native backward: planar-family group");
     cudaStream_t st = S(stream);
@@ -2900,7 +2948,7 @@ int nfb_flow_log_prob_backward(nfb_flow_t* f, const float* x, const float* g_log
                               logq, rows, st));
     }
     const float* zfin = store + (size_t)ng * ZS;
-    NFB_TRY(launch_diag_gauss(zfin, f->base_loc, f->base_log_scale, logq, rows, D, 1, st));
+    NFB_TRY(launch_base_log_prob(f, zfin, logq, rows, st));
     // ---- backward ----
     // slot offsets per layer
     std::vector<int> off(f->layers.size() + 1, 0);
@@ -2910,7 +2958,13 @@ int nfb_flow_log_prob_backward(nfb_flow_t* f, const float* x, const float* g_log
     NFB_TRY(launch_colsum(g_logq, 1, rows, 1, glq_sum, st));
     float* g = f->tr_g0.as<float>();
     float* g2 = f->tr_g1.as<float>();
-    {
+    if (f->base_weight_scores) {
+        const long long wsb = mixture_bwd_ws_bytes(rows, f->base_modes, D);
+        NFB_TRY(f->tr_mix.reserve((size_t)wsb));
+        NFB_TRY(launch_mixture_bwd(zfin, f->base_loc, f->base_log_scale, f->base_weight_scores, g_logq, rows,
+                                   f->base_modes, D, f->tr_mix.p, wsb, g, base_slots[0], base_slots[1], base_slots[2],
+                                   st));
+    } else {
         float *t0 = nullptr, *t1 = nullptr;
         if (base_slots[0] || base_slots[1]) {
             NFB_TRY(f->tr_t0.reserve(ZS * 4));

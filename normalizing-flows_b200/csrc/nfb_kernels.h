@@ -72,6 +72,14 @@ int launch_diag_gauss(const float* z, const float* loc, const float* log_scale, 
                       long long rows, int d, int accumulate, cudaStream_t st);
 int launch_sum(const float* v, long long n, double scale, double* scratch, float* out,
                double* out_sum, cudaStream_t st);
+// Gaussian-mixture base (nfb_mixture.cu): log_q (+)= log p(z); the backward writes g_z (optional) and the parameter
+// gradients (each optional) from a workspace of mixture_bwd_ws_bytes
+int launch_mixture_log_prob(const float* z, const float* loc, const float* log_scale, const float* ws, float* log_q,
+                            long long rows, int K, int D, int accumulate, cudaStream_t st);
+long long mixture_bwd_ws_bytes(long long rows, int K, int D);
+int launch_mixture_bwd(const float* z, const float* loc, const float* log_scale, const float* ws, const float* g_lq,
+                       long long rows, int K, int D, void* wsp, long long ws_bytes, float* g_z, float* g_loc,
+                       float* g_log_scale, float* g_ws, cudaStream_t st);
 
 // ---- image-shaped Glow pieces (nfb_glow.cu) ----
 // mask (optional, [B, cout, H, W]): multiply the output by LeakyReLU'(mask) = (mask > 0 ? 1 : mask_slope);

@@ -9,7 +9,7 @@ value, the metric and every parity claim come from the CUDA kernels; this module
 `backward()`.  It restates (mask-free) the same reference arithmetic as the kernels:
   spline utils/splines.py:16-219, MADE nets/made.py:296-304, ResidualNet nets/resnet.py:92-104,
   LULinearPermute flows/mixing.py:402-434,514-532, affine family flows/affine/coupling.py, DiagGaussian
-  distributions/base.py:94-103.
+  distributions/base.py:94-103, GaussianMixture distributions/base.py:645-659 (with log_softmax).
 """
 import math
 
@@ -148,7 +148,13 @@ def log_prob(model, x):
     for layer in reversed(list(model.flows)):
         z, ld = layer_inverse(layer, z)
         lq = lq + ld
+    from .distributions.base import GaussianMixture
     q0 = model.q0
+    if isinstance(q0, GaussianMixture):
+        ls, loc = q0.log_scale, q0.loc
+        e = (torch.log_softmax(q0.weight_scores, 1) - 0.5 * q0.dim * math.log(2 * math.pi)
+             - torch.sum(ls + 0.5 * ((z[:, None, :] - loc) / torch.exp(ls)) ** 2, 2))
+        return lq + torch.logsumexp(e, 1)
     ls = q0.log_scale.reshape(1, -1)
     lq = lq - 0.5 * q0.d * math.log(2 * math.pi) - torch.sum(ls + 0.5 * ((z - q0.loc.reshape(1, -1)) / torch.exp(ls)) ** 2, 1)
     return lq
@@ -183,7 +189,7 @@ def grad_slot_tensors(model):
             out += [lin.lower_entries, lin.upper_entries, lin.unconstrained_upper_diag, lin.bias]
         else:
             return None
-    return out + [model.q0.loc, model.q0.log_scale]
+    return out + model.q0._native_tensors()
 
 
 def native_backward(model, x, grad_out, need_x):

@@ -170,6 +170,9 @@ SYMBOLS = {
     "nfb_affine_coupling_image_backward": (C.c_int, [_VP] * 6 + [_I64, _I32, _I32, _I32, _I32, _I32, _VP]),
     "nfb_gaussian_table_log_prob_backward": (C.c_int, [_VP] * 8 + [_I64, _I32, _I32, _I32, _VP]),
     "nfb_logit_transform_backward": (C.c_int, [_VP, _VP, _VP, _VP, _I64, _I64, _F, _VP]),
+    "nfb_gaussian_mixture_log_prob": (C.c_int, [_VP] * 5 + [_I64, _I32, _I32, _I32, _VP]),
+    "nfb_gaussian_mixture_log_prob_backward_workspace_bytes": (_I64, [_I64, _I32, _I32]),
+    "nfb_gaussian_mixture_log_prob_backward": (C.c_int, [_VP] * 5 + [_I64, _I32, _I32, _VP, _I64] + [_VP] * 5),
     "nfb_flow_create": (C.c_int, [C.POINTER(_VP), _I32]),
     "nfb_flow_destroy": (C.c_int, [_VP]),
     "nfb_flow_add_ar_rqs": (C.c_int, [_VP, C.POINTER(ArRqsDesc)]),
@@ -182,6 +185,7 @@ SYMBOLS = {
     "nfb_flow_add_planar": (C.c_int, [_VP, C.POINTER(PlanarDesc)]),
     "nfb_flow_add_radial": (C.c_int, [_VP, C.POINTER(RadialDesc)]),
     "nfb_flow_set_base_diag_gaussian": (C.c_int, [_VP, _VP, _VP]),
+    "nfb_flow_set_base_gaussian_mixture": (C.c_int, [_VP, _I32, _VP, _VP, _VP]),
     "nfb_flow_finalize": (C.c_int, [_VP, _I32, _VP]),
     "nfb_flow_repack": (C.c_int, [_VP, _VP]),
     "nfb_flow_num_layers": (C.c_int, [_VP]),

@@ -1,7 +1,7 @@
 """Host-side glue between the nn.Module shims and the C ABI (include/nfb200.h).
 
 `FlowHandle` owns one `nfb_flow_t`: the packed device image of an ordered list of layers (plus an
-optional DiagGaussian base).  It re-reads the parameters when they change (optimizer step,
+optional DiagGaussian or GaussianMixture base).  It re-reads the parameters when they change (optimizer step,
 load_state_dict, .to()) by comparing (data_ptr, _version) signatures -- the same idea as the
 reference's cache invalidation in `_Linear.train()` (normflows/flows/mixing.py:328-332)."""
 import ctypes as C
@@ -99,7 +99,7 @@ class FlowHandle:
         for layer in self.layers:
             ts.extend(layer._native_tensors())
         if self.base is not None:
-            ts.extend([self.base.loc, self.base.log_scale])
+            ts.extend(self.base._native_tensors())
         return ts
 
     def _build_slots(self):
@@ -161,8 +161,7 @@ class FlowHandle:
                     for layer in self.layers:
                         layer._native_add(self._h, features)
                     if self.base is not None:
-                        L.check(lib.nfb_flow_set_base_diag_gaussian(
-                            self._h, L.ptr(self.base.loc), L.ptr(self.base.log_scale)))
+                        self.base._native_attach(self._h, features)
                     L.check(lib.nfb_flow_finalize(self._h, int(self.use_tc), L.stream_ptr()))
                 except Exception:
                     self.close()

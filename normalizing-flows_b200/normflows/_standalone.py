@@ -428,3 +428,35 @@ class UnitGaussianFn(torch.autograd.Function):
                                                                      L.ptr(g.contiguous()), L.ptr(gu), None, None,
                                                                      u.shape[0], u.shape[1], 1, 1, L.stream_ptr()))
         return gu
+
+
+class MixtureLogProbFn(torch.autograd.Function):
+    """GaussianMixture.log_prob(z) per row (nfb_gaussian_mixture_log_prob) and its adjoint to z, loc, log_scale and
+    weight_scores (nfb_gaussian_mixture_log_prob_backward: deterministic, two launches)."""
+
+    @staticmethod
+    def forward(ctx, z, loc, log_scale, weight_scores):
+        K, D = weight_scores.shape[-1], z.shape[1]
+        out = torch.empty(z.shape[0], dtype=torch.float32, device=z.device)
+        if z.shape[0]:
+            with torch.cuda.device(z.device):
+                L.check(L.lib().nfb_gaussian_mixture_log_prob(L.ptr(z), L.ptr(loc), L.ptr(log_scale),
+                                                              L.ptr(weight_scores), L.ptr(out), z.shape[0], K, D, 0,
+                                                              L.stream_ptr()))
+        ctx.save_for_backward(z, loc, log_scale, weight_scores)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        z, loc, log_scale, weight_scores = ctx.saved_tensors
+        K, D, rows = weight_scores.shape[-1], z.shape[1], z.shape[0]
+        lib = L.lib()
+        outs = [torch.empty_like(t) if need else None
+                for t, need in zip((z, loc, log_scale, weight_scores), ctx.needs_input_grad)]
+        ws = torch.empty(max(1, lib.nfb_gaussian_mixture_log_prob_backward_workspace_bytes(rows, K, D)),
+                         dtype=torch.uint8, device=z.device)
+        with torch.cuda.device(z.device):
+            L.check(lib.nfb_gaussian_mixture_log_prob_backward(
+                L.ptr(z), L.ptr(loc), L.ptr(log_scale), L.ptr(weight_scores), L.ptr(g.contiguous()), rows, K, D,
+                L.ptr(ws), ws.numel(), *[L.ptr(o) for o in outs], L.stream_ptr()))
+        return tuple(outs)

@@ -12,7 +12,7 @@ from torch import nn
 from . import _lib as L
 from ._image_autograd import wants_grad
 from ._native import FlowHandle
-from .distributions.base import ConditionalDiagGaussian, DiagGaussian, UniformGaussian
+from .distributions.base import ConditionalDiagGaussian, DiagGaussian, GaussianMixture, UniformGaussian
 from .flows.base import NativeFlow
 
 
@@ -28,8 +28,8 @@ class NormalizingFlow(nn.Module):
         if not all(isinstance(f, NativeFlow) for f in self.flows):
             return None
         h = self.__dict__.get("_nfb_stack")
-        base = self.q0 if isinstance(self.q0, DiagGaussian) and self.q0.temperature is None \
-            and self.q0.n_dim == 1 else None
+        base = self.q0 if (isinstance(self.q0, DiagGaussian) and self.q0.temperature is None
+                           and self.q0.n_dim == 1) or isinstance(self.q0, GaussianMixture) else None
         layers = list(self.flows)
         if (h is None or h.layers != layers or h.base is not base
                 or h.use_tc != NativeFlow.use_tensor_cores):
@@ -154,10 +154,10 @@ class NormalizingFlow(nn.Module):
         """Gradients through the sampling direction exist when every layer's sampling direction is differentiable (the
         stand-alone spline layers and the affine and planar families, `_sampling_differentiable`), the stack runs layer
         by layer or is all of one family, and the base's draw is reparameterised (UniformGaussian, DiagGaussian,
-        ConditionalDiagGaussian).  Otherwise, under grad, raise."""
+        ConditionalDiagGaussian, GaussianMixture).  Otherwise, under grad, raise."""
         if not (torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())):
             return
-        if (isinstance(self.q0, (UniformGaussian, DiagGaussian, ConditionalDiagGaussian))
+        if (isinstance(self.q0, (UniformGaussian, DiagGaussian, ConditionalDiagGaussian, GaussianMixture))
                 and (self._takes_layer_loop() or self._one_sampling_family())
                 and all(hasattr(f, "_sampling_differentiable") and f._sampling_differentiable(context)
                         for f in self.flows)):
@@ -214,14 +214,14 @@ class NormalizingFlow(nn.Module):
     def forward_kld_host(self, x_host, device=None):
         h = self._stack()
         if h is None or h.base is None:
-            raise NotImplementedError("forward_kld_host needs an all-native stack with a DiagGaussian base")
+            raise NotImplementedError("forward_kld_host needs an all-native stack with a DiagGaussian or GaussianMixture base")
         device = torch.device(device) if device is not None else next(self.parameters()).device
         return h.forward_kld_host(x_host, device)
 
     def log_prob_host(self, x_host, device=None):
         h = self._stack()
         if h is None or h.base is None:
-            raise NotImplementedError("log_prob_host needs an all-native stack with a DiagGaussian base")
+            raise NotImplementedError("log_prob_host needs an all-native stack with a DiagGaussian or GaussianMixture base")
         device = torch.device(device) if device is not None else next(self.parameters()).device
         return h.log_prob_host(x_host, device)
 

@@ -1,5 +1,5 @@
 """Base distributions: only what the density pass ends in (reference:
-normflows/distributions/base.py:8-49 BaseDistribution, :53-103 DiagGaussian)."""
+normflows/distributions/base.py:8-49 BaseDistribution, :53-103 DiagGaussian, :573-659 GaussianMixture)."""
 import numpy as np
 import torch
 from torch import nn
@@ -59,6 +59,72 @@ class DiagGaussian(BaseDistribution):
         z = require_cuda_f32(z)
         ls = _tempered(self.log_scale, self.temperature)
         return gaussian_table_log_prob(z, self.loc.reshape(self.d, 1), ls.reshape(self.d, 1), None, 1)
+
+    # the base of a flow object (_native.FlowHandle): its tensors, in the order of its gradient slots, and its setter
+    def _native_tensors(self):
+        return [self.loc, self.log_scale]
+
+    def _native_attach(self, handle, features):
+        L.check(L.lib().nfb_flow_set_base_diag_gaussian(handle, L.ptr(self.loc), L.ptr(self.log_scale)))
+
+
+class GaussianMixture(BaseDistribution):
+    """Mixture of Gaussians with diagonal covariances (reference: distributions/base.py:573-659): the same parameters
+    (or buffers, trainable=False) `loc` [1, K, D], `log_scale` [1, K, D], `weight_scores` [1, K] and the same seeded
+    construction (a `loc=None` default is drawn with np.random.randn).  The tensors are float32 (the CUDA path computes in
+    float32 only); a reference state_dict (float64) loads with strict=True, converted on load.  `log_prob` is the CUDA
+    kernel (csrc/nfb_mixture.cu) with its native backward, gradients to z and all three parameters; with log_softmax
+    in place of log(softmax), a weight that underflows gives a finite, negligible term instead of -inf.  Sampling draws
+    the modes with torch.multinomial and eps with torch.randn (plumbing RNG, like the other bases) and is
+    reparameterised: z = loc[m] + exp(log_scale[m]) eps in differentiable torch."""
+
+    def __init__(self, n_modes, dim, loc=None, scale=None, weights=None, trainable=True):
+        super().__init__()
+        self.n_modes = n_modes
+        self.dim = dim
+        if loc is None:
+            loc = np.random.randn(self.n_modes, self.dim)
+        loc = np.array(loc)[None, ...]
+        if scale is None:
+            scale = np.ones((self.n_modes, self.dim))
+        scale = np.array(scale)[None, ...]
+        if weights is None:
+            weights = np.ones(self.n_modes)
+        weights = np.array(weights)[None, ...]
+        weights = weights / weights.sum(1)
+        f32 = lambda v: torch.tensor(v, dtype=torch.float32)
+        tensors = {"loc": f32(1.0 * loc), "log_scale": f32(np.log(1.0 * scale)),
+                   "weight_scores": f32(np.log(1.0 * weights))}
+        for name, t in tensors.items():
+            if trainable:
+                setattr(self, name, nn.Parameter(t))
+            else:
+                self.register_buffer(name, t)
+
+    def forward(self, num_samples=1):
+        dev = self.loc.device
+        weights = torch.softmax(self.weight_scores.detach(), 1)
+        mode = torch.multinomial(weights[0, :], num_samples, replacement=True)
+        eps = torch.randn(num_samples, self.dim, dtype=self.loc.dtype, device=dev)
+        z = self.loc[0, mode] + torch.exp(self.log_scale[0, mode]) * eps
+        return z, self.log_prob(z)
+
+    def log_prob(self, z):
+        from .._standalone import MixtureLogProbFn
+        z = require_cuda_f32(z)
+        if z.dim() != 2 or z.shape[1] != self.dim:
+            raise ValueError(f"GaussianMixture.log_prob expects [batch, {self.dim}], got {list(z.shape)}")
+        return MixtureLogProbFn.apply(z, *(require_cuda_f32(t, "GaussianMixture parameter")
+                                           for t in self._native_tensors()))
+
+    def _native_tensors(self):
+        return [self.loc, self.log_scale, self.weight_scores]
+
+    def _native_attach(self, handle, features):
+        if features != self.dim:
+            raise ValueError(f"GaussianMixture of dim {self.dim} as the base of a {features}-feature flow")
+        L.check(L.lib().nfb_flow_set_base_gaussian_mixture(handle, self.n_modes, L.ptr(self.loc), L.ptr(self.log_scale),
+                                                           L.ptr(self.weight_scores)))
 
 
 class UniformGaussian(BaseDistribution):

@@ -48,7 +48,7 @@ def forward_kld_dp(model, x_local, group=None, async_op=False):
     rotate through a ring of 8, the oldest is waited on before reuse)."""
     h = model._stack()
     if h is None or h.base is None:
-        raise NotImplementedError("forward_kld_dp needs an all-native stack with a DiagGaussian base")
+        raise NotImplementedError("forward_kld_dp needs an all-native stack with a DiagGaussian or GaussianMixture base")
     ring = model.__dict__.get("_nfb_dp_ring")
     if ring is None or ring["bufs"][0].device != x_local.device:
         ring = {"bufs": [torch.zeros(2, dtype=torch.float64, device=x_local.device) for _ in range(8)],
