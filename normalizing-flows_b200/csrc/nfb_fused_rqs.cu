@@ -30,8 +30,9 @@
 //              second GEMM of each residual block accumulates straight onto the residual stream (h += W2 relu(...));
 //              the biases are pre-summed by the packer.
 //              In the final layer the warpgroups take different roles: warpgroup 0 multiplies both halves of every
-//              record (two features, N = 48, per half; both halves as one N = 96 product) and stores each pair of chunks to
-//              two staging tiles in shared memory; warpgroup 1 copies its (row, feature) parameters out of the tiles,
+//              record (two features, N = 48, per half; both halves as one N = 96 product) into two alternating
+//              accumulators and stores each pair of chunks, unscaled and with its biases, to two staging tiles in shared
+//              memory; warpgroup 1 copies its (row, feature) parameters out of the tiles,
 //              hands them back at once and evaluates two splines per thread.  The hand-off is a pair of named barriers
 //              ("full" / "free", one side arrives, the other waits), so the products of one pair of chunks run under the
 //              splines of the pair before.
@@ -133,17 +134,21 @@ __device__ __forceinline__ float pow2i(int e) { return __uint_as_float((uint32_t
 // one warpgroup.arrive.  Whether a record has products at all is decided by one uniform branch around the chain.
 // N = 64 (32 registers): a hidden GEMM's slice; N = 96 (48): both halves of a final-layer record at once, half 0 in
 // registers 0..23 and half 1 in 24..47 (rows [0, 48) and [48, 96) of the record's tiles).
+// FIRST: the record opens acc whatever its flags say, and its first product overwrites acc with an immediate scale-d
+// of 0, so acc needs no value before it (the final layer's pairs, whose first record always opens the accumulator).
 struct MmaOps { uint32_t a_hi, a_lo, w_hi, w_lo; bool first; uint32_t on, slabs; };
-template <int SLABS, bool QUAD, int NREG>
+template <int SLABS, bool QUAD, int NREG, bool FIRST = false>
 __device__ __forceinline__ void mma_record(float (&acc)[NREG], const MmaOps& x) {
     static_assert(NREG == 32 || NREG == 48, "N = 64 or 96");
+    static_assert(!FIRST || NREG == 48, "an opening record of its own: the final layer's N = 96 products");
     const uint64_t ah = wgmma_desc(x.a_hi), al = wgmma_desc(x.a_lo), bh = wgmma_desc(x.w_hi), bl = wgmma_desc(x.w_lo);
     auto pass = [&](uint64_t a, uint64_t b, bool opens) {
 #pragma unroll
         for (int s = 0; s < SLABS; ++s) {
             const uint32_t sd = opens && s == 0 && x.first ? 0u : 1u;
             if constexpr (NREG == 32) wgmma_f16_n64(acc, a + 2 * s, b + 2 * s, sd);
-            else wgmma_f16_n96(acc, a + 2 * s, b + 2 * s, sd);
+            else if (FIRST && opens && s == 0) wgmma_f16_n96_zero(acc, a, b);
+            else wgmma_f16_n96(acc, a + 2 * s, b + 2 * s, FIRST ? 1u : sd);
         }
     };
     pass(ah, bh, true);
@@ -163,7 +168,8 @@ enum { kClkClaim,       // unit queue, layer-to-layer flag, rows of a host batch
        kClkHidMma,      // hidden GEMMs: wgmma issue -> complete (wait_group), slot hand-back
        kClkHidEpi,      // hidden GEMMs: epilogues and the barriers around them; unconditional splines
        kClkFinRing,     // final layer: wait for the record
-       kClkFinMma,      // final layer: wgmma issue -> complete, slot hand-back
+       kClkFinMma,      // final layer: wgmma issue -> complete within a pair, slot hand-back
+       kClkFinTail,     // final layer: the wait at a pair boundary that completes the previous pair's products
        kClkFinStage,    // final layer: accumulators <-> staging tiles, hand-off waits
        kClkFinSpline,   // final layer: spline evaluation
        kClkStore,       // log-det reduction, tile store, publish
@@ -352,13 +358,17 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
         // (an empty wgmma group stands in for skipped products, so the group count stays uniform).  A slot's empty
         // barrier expects one arrival per consumer warpgroup: `arrivals` is 1 where both warpgroups walk the records
         // (LU stage, hidden GEMMs) and 2 where one walks them for both (final layer).
-        auto run_records = [&](auto issue, auto arrivals, auto clk_ring, auto clk_mma) {
-            auto hand_back = [&](int s, bool pred) {
+        auto hand_back = [&](auto arrivals, int s, bool pred) {
 #pragma unroll
-                for (int i = 0; i < decltype(arrivals)::value; ++i) mbar_arrive_if(bar(kBarWEmpty + s), pred && (et & 127) == 0);
-            };
-            int prev = -1;
-            for (;;) {
+            for (int i = 0; i < decltype(arrivals)::value; ++i) mbar_arrive_if(bar(kBarWEmpty + s), pred && (et & 127) == 0);
+        };
+        // The walker itself leaves the last record's products in flight and its slot in `prev` (-1: none), so that a run
+        // can start while the one before still multiplies.  OPEN: the first record is issued as issue(step, true_type)
+        // and completes the products in flight before it (its wait_group 1), which hands back `prev` and then runs
+        // `retire` -- the previous run's accumulator is final there.  Every other record is issue(step, false_type).
+        auto walk_records = [&](auto issue, auto arrivals, auto clk_ring, auto clk_mma, int& prev, auto open,
+                                auto retire) {
+            auto record = [&](auto first) {
                 union { uint2 raw; FusedStep s; } st;
                 st.raw = __ldg(reinterpret_cast<const uint2*>(L.steps) + sidx);
                 st.raw.x = uniform(st.raw.x);
@@ -368,16 +378,28 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
                 mbar_wait(bar(kBarWFull + slot), wpar, p.err, 220 + slot);
                 NFB_CLK(decltype(clk_ring)::value);
                 wgmma_fence();
-                const bool last = issue(st.s);
-                wgmma_commit();
+                const bool last = issue(st.s, first);   // (commits its own group)
+                if constexpr (decltype(first)::value) NFB_CLK(decltype(clk_mma)::value);
                 wgmma_wait<1>();   // the previous record's products are complete: hand its slot back
-                hand_back(prev < 0 ? 0 : prev, prev >= 0);
+                hand_back(arrivals, prev < 0 ? 0 : prev, prev >= 0);
+                if constexpr (decltype(first)::value) NFB_CLK(kClkFinTail);
                 prev = (int)slot;
                 if (++slot == kSlots) { slot = 0; wpar ^= 1; }
-                if (last) break;
+                return last;
+            };
+            bool last = false;
+            if constexpr (decltype(open)::value) {
+                last = record(std::true_type());
+                retire();
             }
+            while (!last) last = record(std::false_type());
+        };
+        // a run that ends with its products complete and every slot handed back
+        auto run_records = [&](auto issue, auto arrivals, auto clk_ring, auto clk_mma) {
+            int prev = -1;
+            walk_records(issue, arrivals, clk_ring, clk_mma, prev, std::false_type(), [] {});
             wgmma_wait<0>();
-            hand_back(prev, true);
+            hand_back(arrivals, prev, true);
             NFB_CLK(decltype(clk_mma)::value);
         };
         // operands of half h of the record in the current slot (live = 0: no products; the skip bit: the record has no
@@ -392,9 +414,10 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
         // into acc, multiplied with its K-chunk (live: the warpgroup has a slice here).  (The packer sets slab bits on
         // final-layer records only: the LU map and the hidden GEMMs always multiply all four slabs.)
         auto run_slice = [&](auto& acc, bool live, auto quad, auto clk_ring, auto clk_mma) {
-            run_records([&](const FusedStep& s) {
+            run_records([&](const FusedStep& s, auto) {
                 const MmaOps x = half_ops(s, wg, live);
                 if (x.on) mma_record<4, decltype(quad)::value>(acc, x);
+                wgmma_commit();
                 return ((wg ? s.flags1 : s.flags) & kStepLast) != 0;
             }, std::integral_constant<int, 1>(), clk_ring, clk_mma);
             wgmma_hold(acc);
@@ -674,35 +697,91 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
             //      under the splines of pair c. ----
             if (wg == 0) {
                 static_assert(kFusedFeaturesPerChunk == 2, "a final-layer record is one N = 96 product");
-                for (int ci = 0; ci < n_pairs; ++ci) {
-                    float acc[48] = {};   // (as hres: not live before) half 0 in 0..23, half 1 in 24..47
-                    run_records([&](const FusedStep& s) {
+                // The pairs alternate between two accumulators (half 0 in registers 0..23, half 1 in 24..47), so the
+                // tensor core does not drain at a pair boundary: pair c + 1's first record is issued, its wait_group 1
+                // completes pair c, and pair c goes to the staging tiles while that record multiplies.  The ring then
+                // holds two of this warpgroup's slots at most (pair c's last record, pair c + 1's first).  Neither
+                // accumulator is written by anything but wgmma while products are in flight: each pair's first product
+                // overwrites its accumulator (scale-d 0, an immediate), and each is read only after the wait that
+                // completes it -- any other definition makes ptxas serialise every wgmma of the kernel (C7515).
+                auto products = [&](float (&acc)[48]) {
+                    return [&](const FusedStep& s, auto first) {
                         // Both halves share the K-chunk and the first / last flags; one N = 96 product covers them, over
                         // the larger of their slab counts.  A half the record skips, and the slabs past a half's own
                         // count, are multiplied too: their weights are the masked-out zeros the packer wrote, which add
                         // an exact zero to every accumulator.  (A record always has a live half: the packer keeps only
-                        // K-chunk 0 and the K-chunks one of the two chunks reaches.)
+                        // K-chunk 0 and the K-chunks one of the two chunks reaches; K-chunk 0 opens the pair.)
+                        constexpr bool F = decltype(first)::value;
                         const MmaOps x = half_ops(s, 0, true), x1 = half_ops(s, 1, true);
                         const uint32_t n = max(x.on ? x.slabs : 0u, x1.on ? x1.slabs : 0u);
                         switch (n) {
-                            case 1: mma_record<1, false>(acc, x); break;
-                            case 2: mma_record<2, false>(acc, x); break;
-                            case 3: mma_record<3, false>(acc, x); break;
-                            default: mma_record<4, false>(acc, x); break;
+                            case 1: mma_record<1, false, 48, F>(acc, x); wgmma_commit(); break;
+                            case 2: mma_record<2, false, 48, F>(acc, x); wgmma_commit(); break;
+                            case 3: mma_record<3, false, 48, F>(acc, x); wgmma_commit(); break;
+                            default: mma_record<4, false, 48, F>(acc, x); wgmma_commit(); break;
                         }
                         return (s.flags & kStepLast) != 0;   // (the pair's last record is the same for both halves)
-                    }, std::integral_constant<int, 2>(), ClkPhase<kClkFinRing>(), ClkPhase<kClkFinMma>());
+                    };
+                };
+                // The tiles carry the spline parameters themselves, acc / (scale u_row) + bias -- the same fmaf the spline
+                // warpgroup applied to the raw accumulators before -- so the splines wait for no bias load.  This thread's
+                // 12 bias pairs of pair ci (columns 8 g + cq, cq + 1 of either half) are loaded one pair ahead, behind the
+                // hand-off that stages the pair before, where the products hide their latency.
+                const float fin_a = ruinv(L.a_inv[1 + n_hidden], ra), fin_b = ruinv(L.a_inv[1 + n_hidden], rb);
+                float2 fbias[2][6];
+                auto load_bias = [&](int ci) {
+                    if (ci >= n_pairs) return;
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+#pragma unroll
+                        for (int g = 0; g < 6; ++g)
+                            fbias[h][g] = __ldg(reinterpret_cast<const float2*>(L.bias_f + (2 * ci + h) * L.F * 24 + 8 * g + cq));
+                };
+                // pair ci's products are complete: to the staging tiles once the previous pair's have been taken
+                auto stage = [&](float (&acc)[48], int ci) {
                     wgmma_hold(acc);
-                    // (no slot is held here: the producer can deliver the next pair's records while this waits)
-                    if (ci > 0) stg_bar_wait<kBarStgFree>();   // the previous pair's parameters have been taken
+                    if (ci > 0) stg_bar_wait<kBarStgFree>();
 #pragma unroll
                     for (int i = 0; i < 24; i += 2) {
-                        float* dst = stg0 + ((i & 2) ? rb : ra) * kStgLd + 8 * (i >> 2) + cq;
-                        *reinterpret_cast<float2*>(dst) = make_float2(acc[i], acc[i + 1]);
-                        *reinterpret_cast<float2*>(dst + kRows * kStgLd) = make_float2(acc[24 + i], acc[25 + i]);
+                        const int g = i >> 2;
+                        const float u = (i & 2) ? fin_b : fin_a;
+                        float* dst = stg0 + ((i & 2) ? rb : ra) * kStgLd + 8 * g + cq;
+                        *reinterpret_cast<float2*>(dst) =
+                            make_float2(fmaf(acc[i], u, fbias[0][g].x), fmaf(acc[i + 1], u, fbias[0][g].y));
+                        *reinterpret_cast<float2*>(dst + kRows * kStgLd) =
+                            make_float2(fmaf(acc[24 + i], u, fbias[1][g].x), fmaf(acc[25 + i], u, fbias[1][g].y));
                     }
                     stg_bar_arrive<kBarStgFull>();
+                    load_bias(ci + 1);
                     NFB_CLK(kClkFinStage);
+                };
+                using Two = std::integral_constant<int, 2>;
+                int prev = -1;
+                // pair ci into acc; `done` holds pair ci - 1, staged under the first record of pair ci
+                auto pair = [&](float (&acc)[48], float (&done)[48], int ci) {
+                    walk_records(products(acc), Two(), ClkPhase<kClkFinRing>(), ClkPhase<kClkFinMma>(), prev,
+                                 std::true_type(), [&] { stage(done, ci - 1); });
+                };
+                // after the last pair: its products complete, its last slot back
+                auto finish = [&](float (&acc)[48], int ci) {
+                    wgmma_wait<0>();
+                    hand_back(Two(), prev, true);
+                    NFB_CLK(kClkFinTail);
+                    stage(acc, ci);
+                };
+                // (unrolled by two, so that accA and accB stay two fixed register sets; pair 0 is peeled so that every
+                // read of either comes after a pair has written it)
+                float accA[48], accB[48];
+                if (n_pairs > 0) {
+                    load_bias(0);
+                    walk_records(products(accA), Two(), ClkPhase<kClkFinRing>(), ClkPhase<kClkFinMma>(), prev,
+                                 std::true_type(), [] {});
+                    for (int ci = 1;; ci += 2) {
+                        if (ci == n_pairs) { finish(accA, ci - 1); break; }
+                        pair(accB, accA, ci);
+                        if (ci + 1 == n_pairs) { finish(accB, ci); break; }
+                        pair(accA, accB, ci + 1);
+                    }
                 }
             } else {
                 // It does not walk the final layer's records (the last of the step table): its cursors move past them
@@ -715,7 +794,6 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
                 }
                 // Row r's log-det partial sums keep their membership and order: lad_even continues the sum of the
                 // warpgroup-0 thread of (row, f) over the even chunks, ladsum this thread's own over the odd chunks.
-                const float inv_f = ruinv(L.a_inv[1 + n_hidden], r);
                 const int f = (et >> 6) & 1;   // feature of each chunk this thread evaluates (for row r)
                 lad_even = ldsum[f * kRows + r];
                 for (int ci = 0; ci < n_pairs; ++ci) {
@@ -726,17 +804,17 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
 #pragma unroll 1
                     for (int h = 0; h < 2; ++h) {
                         const int t = (2 * ci + h) * L.F + f;
-                        // the packer folded log2(e) (and the layer's 1/sqrt(H)) into the w/h columns and biases
+                        // (the packer folded log2(e) and the layer's 1/sqrt(H) into the w/h columns and biases; the product
+                        // warpgroup has unscaled the products and added the biases)
                         const float4* sp = reinterpret_cast<const float4*>(stg0 + (h * kRows + r) * kStgLd + 24 * f);
-                        const float4* bp = reinterpret_cast<const float4*>(L.bias_f + t * 24);
                         float pv[24];
 #pragma unroll
                         for (int q = 0; q < 6; ++q) {
-                            const float4 s4 = sp[q], b4 = __ldg(bp + q);
-                            pv[4 * q] = fmaf(s4.x, inv_f, b4.x);
-                            pv[4 * q + 1] = fmaf(s4.y, inv_f, b4.y);
-                            pv[4 * q + 2] = fmaf(s4.z, inv_f, b4.z);
-                            pv[4 * q + 3] = fmaf(s4.w, inv_f, b4.w);
+                            const float4 s4 = sp[q];
+                            pv[4 * q] = s4.x;
+                            pv[4 * q + 1] = s4.y;
+                            pv[4 * q + 2] = s4.z;
+                            pv[4 * q + 3] = s4.w;
                         }
                         if (h == 1 && ci + 1 < n_pairs) stg_bar_arrive<kBarStgFree>();   // (the last pair's tiles have no next writer)
                         NFB_CLK(kClkFinStage);
@@ -822,6 +900,8 @@ extern "C" __attribute__((visibility("default"))) int nfb_phase_clocks_read(unsi
     }
     return NFB_OK;
 }
+// the phases per role in nfb_phase_clocks_read's rows, the unit count (the last entry) included
+extern "C" __attribute__((visibility("default"))) int nfb_phase_clocks_count() { return kClkCount; }
 #endif
 
 // -----------------------------------------------------------------------------------------

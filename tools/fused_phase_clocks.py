@@ -21,8 +21,9 @@ sys.path[:0] = [ROOT, os.path.join(ROOT, "normalizing-flows_b200")]
 
 PHASES = ["claim / dependency wait", "tile load, row units, first A operand", "LU stage", "hidden: ring wait",
           "hidden: wgmma issue -> complete", "hidden: epilogues + barriers", "final: ring wait",
-          "final: wgmma issue -> complete", "final: staging + barriers", "final: spline", "log-det, store, publish",
-          "producer: empty-slot wait", "producer: other"]
+          "final: wgmma issue -> complete", "final: pair tail (wait for a pair's last products)",
+          "final: staging + barriers", "final: spline", "log-det, store, publish", "producer: empty-slot wait",
+          "producer: other"]
 ROLES = ["warpgroup 0", "warpgroup 1", "producer"]
 
 
@@ -50,7 +51,13 @@ def main():
         raise SystemExit(f"fused_phase_clocks: {_lib.LIB_PATH} has no phase clocks; build it with `make CLOCKS=1 "
                          "OUT=../libnfb200_clocks.so` and select it with NFB200_LIB")
     read.argtypes, read.restype = [C.c_void_p, C.c_int], C.c_int
-    n = len(PHASES) + 1
+    phases = PHASES
+    try:
+        n = lib.nfb_phase_clocks_count()
+    except AttributeError:   # a build from before the pair-tail phase: its pair tails are inside issue -> complete
+        phases = [p for p in PHASES if not p.startswith("final: pair tail")]
+        n = len(phases) + 1
+    assert n == len(phases) + 1, f"{_lib.LIB_PATH}: {n - 1} phases, this tool knows {len(phases)}"
     torch.set_grad_enabled(False)
     model = bench.build_model(args.kind).cuda()
     x = (torch.randn(bench.BATCH, bench.D, generator=torch.Generator().manual_seed(1)) * 1.5).cuda()
@@ -67,11 +74,11 @@ def main():
     print("gpu:", during)
     print(f"{args.kind} stack, batch {bench.BATCH}, {args.passes} passes; SM cycles per unit")
     units = [buf[r][n - 1] for r in range(3)]
-    print(f"{'phase':42s}" + "".join(f"{r:>14s}" for r in ROLES))
-    for ph, name in enumerate(PHASES):
-        print(f"{name:42s}" + "".join(f"{buf[r][ph] / max(1, units[r]):14.0f}" for r in range(3)))
-    print(f"{'sum':42s}" + "".join(f"{sum(buf[r][:n - 1]) / max(1, units[r]):14.0f}" for r in range(3)))
-    print(f"{'units':42s}" + "".join(f"{units[r]:14d}" for r in range(3)))
+    print(f"{'phase':50s}" + "".join(f"{r:>14s}" for r in ROLES))
+    for ph, name in enumerate(phases):
+        print(f"{name:50s}" + "".join(f"{buf[r][ph] / max(1, units[r]):14.0f}" for r in range(3)))
+    print(f"{'sum':50s}" + "".join(f"{sum(buf[r][:n - 1]) / max(1, units[r]):14.0f}" for r in range(3)))
+    print(f"{'units':50s}" + "".join(f"{units[r]:14d}" for r in range(3)))
 
 
 if __name__ == "__main__":
