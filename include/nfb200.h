@@ -338,6 +338,48 @@ int nfb_gaussian_mixture_log_prob_backward(const float* z_dev, const float* loc_
                                            int32_t n_modes, int32_t dim, void* ws, int64_t ws_bytes, float* g_z_dev,
                                            float* g_loc_dev, float* g_log_scale_dev, float* g_weight_scores_dev,
                                            void* stream);
+/* ---- flow-VAE encoders and decoders (distributions/encoder.py, distributions/decoder.py) ----
+ * Row r = b samples + s of a flattened [batch, samples] grid belongs to data row b.  A parameter row (mean and scale
+ * column, each dim floats) sits at row * param_stride floats; param_stride = 0 is one row shared by every row.  The
+ * scale column holds the log variance (NFB_VAE_LOGVAR: sd = exp(p / 2)) or the standard deviation (NFB_VAE_SCALE).
+ * Every backward is deterministic (fixed-order sums, no atomics), one launch, and overwrites its outputs; rows = 0
+ * writes zeros into the gradients of a shared (param_stride = 0) row. */
+#define NFB_VAE_LOGVAR 0
+#define NFB_VAE_SCALE 1
+/* z [rows, dim] = mean[b] + sd[b] eps[r] and log_q [rows] = -dim/2 log 2pi - sum (log sd + eps^2 / 2), one launch. */
+int nfb_vae_reparam_sample(const float* mean_dev, const float* scale_dev, int64_t param_stride, int32_t scale_kind,
+                           const float* eps_dev, int64_t batch, int32_t samples, int32_t dim, float* z_dev,
+                           float* log_q_dev, void* stream);
+/* Adjoint of nfb_vae_reparam_sample with cotangents g_z [rows, dim] and g_log_q [rows] (either may be NULL): g_mean and
+ * g_scale (the scale column's gradient) in the parameter layout, summed over each row's samples (over all rows for
+ * param_stride = 0). */
+int nfb_vae_reparam_sample_backward(const float* mean_dev, const float* scale_dev, int64_t param_stride,
+                                    int32_t scale_kind, const float* eps_dev, const float* g_z_dev,
+                                    const float* g_log_q_dev, int64_t batch, int32_t samples, int32_t dim,
+                                    float* g_mean_dev, float* g_scale_dev, void* stream);
+/* out[r] = -norm_dim/2 log 2pi - sum_j (log sd + (v - mean)^2 / (2 sd^2)) with value row r / v_div of v [., dim]
+ * and parameter row r / p_div. */
+int nfb_vae_gaussian_log_prob(const float* v_dev, const float* mean_dev, const float* scale_dev, int64_t param_stride,
+                              int32_t scale_kind, int64_t rows, int32_t dim, int64_t v_div, int64_t p_div,
+                              float norm_dim, float* out_dev, void* stream);
+/* Adjoint of nfb_vae_gaussian_log_prob with cotangent g_out [rows]: g_v (summed over the rows that share a value row),
+ * g_mean / g_scale (summed over the rows that share a parameter row); each may be NULL.  Value rows and parameter rows
+ * may not both repeat (NFB_ERR_UNSUPPORTED). */
+int nfb_vae_gaussian_log_prob_backward(const float* v_dev, const float* mean_dev, const float* scale_dev,
+                                       int64_t param_stride, int32_t scale_kind, const float* g_out_dev, int64_t rows,
+                                       int32_t dim, int64_t v_div, int64_t p_div, float* g_v_dev, float* g_mean_dev,
+                                       float* g_scale_dev, void* stream);
+/* Bernoulli log-likelihood of x row r / x_div under logits score [rows, dim]: out[r] = sum_j x log_sig(s) +
+ * (1 - x) log_sig(-s) (NNBernoulliDecoder.log_prob). */
+int nfb_bernoulli_log_prob(const float* score_dev, const float* x_dev, int64_t rows, int32_t dim, int64_t x_div,
+                           float* out_dev, void* stream);
+/* Adjoint with cotangent g_out [rows]: g_score = g (x - sigmoid(s)), 0 where s == 0 exactly (as the reference's
+ * relu / abs derivatives give); g_x [rows / x_div, dim] = sum over the rows sharing x of g s.  Either may be NULL. */
+int nfb_bernoulli_log_prob_backward(const float* score_dev, const float* x_dev, const float* g_out_dev, int64_t rows,
+                                    int32_t dim, int64_t x_div, float* g_score_dev, float* g_x_dev, void* stream);
+/* out = sigmoid(in) elementwise (NNBernoulliDecoder.forward), and its adjoint g_in = g_out out (1 - out). */
+int nfb_sigmoid(const float* in_dev, float* out_dev, int64_t n, void* stream);
+int nfb_sigmoid_backward(const float* out_dev, const float* g_out_dev, float* g_in_dev, int64_t n, void* stream);
 /* Adjoint of nfb_logit_transform in the density direction (NFB_INVERSE): g_in = dy/dx g_out + d log_det/dx g_log_det
  * (g_out or g_log_det may be NULL). */
 int nfb_logit_transform_backward(const float* in_dev, const float* g_out_dev, const float* g_log_det_dev, float* g_in_dev,

@@ -8,7 +8,7 @@ behind the reference's `nf.NormalizingFlow` / `nf.flows.*` nn.Module API.
 Scope: SURVEY.md section 8 / DESIGN.md.  Compute happens in libnfb200.so (C ABI: include/nfb200.h);
 there is no CPU/eager fallback."""
 from . import distributions, flows, nets, transforms, utils
-from .core import NormalizingFlow, ConditionalNormalizingFlow, ClassCondFlow, MultiscaleFlow
+from .core import NormalizingFlow, ConditionalNormalizingFlow, ClassCondFlow, MultiscaleFlow, NormalizingFlowVAE
 from . import parallel
 from ._native import invalidate_packed_weights
 

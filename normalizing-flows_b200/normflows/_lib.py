@@ -11,6 +11,7 @@ LIB_PATH = os.environ.get("NFB200_LIB") or os.path.join(os.path.dirname(_HERE), 
 
 NFB_INVERSE, NFB_FORWARD = 0, 1
 NFB_PLANAR_TANH, NFB_PLANAR_LEAKY_RELU = 0, 1   # nfb_planar_desc_t.act
+NFB_VAE_LOGVAR, NFB_VAE_SCALE = 0, 1   # scale_kind of the nfb_vae_* calls
 _FP = C.POINTER(C.c_float)
 _I64P = C.POINTER(C.c_int64)
 _I32P = C.POINTER(C.c_int32)
@@ -173,6 +174,15 @@ SYMBOLS = {
     "nfb_gaussian_mixture_log_prob": (C.c_int, [_VP] * 5 + [_I64, _I32, _I32, _I32, _VP]),
     "nfb_gaussian_mixture_log_prob_backward_workspace_bytes": (_I64, [_I64, _I32, _I32]),
     "nfb_gaussian_mixture_log_prob_backward": (C.c_int, [_VP] * 5 + [_I64, _I32, _I32, _VP, _I64] + [_VP] * 5),
+    "nfb_vae_reparam_sample": (C.c_int, [_VP, _VP, _I64, _I32, _VP, _I64, _I32, _I32, _VP, _VP, _VP]),
+    "nfb_vae_reparam_sample_backward": (C.c_int, [_VP, _VP, _I64, _I32, _VP, _VP, _VP, _I64, _I32, _I32, _VP, _VP, _VP]),
+    "nfb_vae_gaussian_log_prob": (C.c_int, [_VP, _VP, _VP, _I64, _I32, _I64, _I32, _I64, _I64, _F, _VP, _VP]),
+    "nfb_vae_gaussian_log_prob_backward": (C.c_int, [_VP, _VP, _VP, _I64, _I32, _VP, _I64, _I32, _I64, _I64, _VP, _VP,
+                                                     _VP, _VP]),
+    "nfb_bernoulli_log_prob": (C.c_int, [_VP, _VP, _I64, _I32, _I64, _VP, _VP]),
+    "nfb_bernoulli_log_prob_backward": (C.c_int, [_VP, _VP, _VP, _I64, _I32, _I64, _VP, _VP, _VP]),
+    "nfb_sigmoid": (C.c_int, [_VP, _VP, _I64, _VP]),
+    "nfb_sigmoid_backward": (C.c_int, [_VP, _VP, _VP, _I64, _VP]),
     "nfb_flow_create": (C.c_int, [C.POINTER(_VP), _I32]),
     "nfb_flow_destroy": (C.c_int, [_VP]),
     "nfb_flow_add_ar_rqs": (C.c_int, [_VP, C.POINTER(ArRqsDesc)]),

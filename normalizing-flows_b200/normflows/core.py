@@ -13,6 +13,7 @@ from . import _lib as L
 from ._image_autograd import wants_grad
 from ._native import FlowHandle
 from .distributions.base import ConditionalDiagGaussian, DiagGaussian, GaussianMixture, UniformGaussian
+from .distributions.encoder import Dirac
 from .flows.base import NativeFlow
 
 
@@ -150,21 +151,23 @@ class NormalizingFlow(nn.Module):
         fams = {f._sampling_family() if isinstance(f, NativeFlow) else None for f in self.flows}
         return fams.pop() if len(fams) == 1 else None
 
+    def _flows_sampling_differentiable(self, context=None):
+        """Every layer's sampling direction is differentiable (the stand-alone spline layers and the affine and planar
+        families, `_sampling_differentiable`), and the stack runs layer by layer or is all of one family."""
+        return ((self._takes_layer_loop() or self._one_sampling_family())
+                and all(hasattr(f, "_sampling_differentiable") and f._sampling_differentiable(context)
+                        for f in self.flows))
+
     def _no_sampling_grad(self, what, context=None):
-        """Gradients through the sampling direction exist when every layer's sampling direction is differentiable (the
-        stand-alone spline layers and the affine and planar families, `_sampling_differentiable`), the stack runs layer
-        by layer or is all of one family, and the base's draw is reparameterised (UniformGaussian, DiagGaussian,
-        ConditionalDiagGaussian, GaussianMixture).  Otherwise, under grad, raise."""
+        """Gradients through the sampling direction exist when the layers' are (_flows_sampling_differentiable) and the
+        base's draw is reparameterised (UniformGaussian, DiagGaussian, ConditionalDiagGaussian, GaussianMixture).
+        Otherwise, under grad, raise."""
         if not (torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())):
             return
         if (isinstance(self.q0, (UniformGaussian, DiagGaussian, ConditionalDiagGaussian, GaussianMixture))
-                and (self._takes_layer_loop() or self._one_sampling_family())
-                and all(hasattr(f, "_sampling_differentiable") and f._sampling_differentiable(context)
-                        for f in self.flows)):
+                and self._flows_sampling_differentiable(context)):
             return
-        raise NotImplementedError(
-            f"{what}: gradients through the sampling direction are not on the CUDA path yet "
-            "(evaluate under torch.no_grad(); forward_kld / log_prob are differentiable)")
+        raise NotImplementedError(_no_sampling_grad_message(what) + "; forward_kld / log_prob are differentiable)")
 
     def _log_q_no_param_grad(self, z, **context):
         """log q(z) by the density pass with the parameters' requires_grad switched off and back on, as the reference
@@ -224,6 +227,22 @@ class NormalizingFlow(nn.Module):
             raise NotImplementedError("log_prob_host needs an all-native stack with a DiagGaussian or GaussianMixture base")
         device = torch.device(device) if device is not None else next(self.parameters()).device
         return h.log_prob_host(x_host, device)
+
+
+def _no_sampling_grad_message(what):
+    return (f"{what}: gradients through the sampling direction are not on the CUDA path yet "
+            "(evaluate under torch.no_grad()")
+
+
+def _inner_flow(owner):
+    """A NormalizingFlow without a base that shares `owner.flows`' layer modules, for drivers that push samples through
+    the layers (ClassCondFlow, NormalizingFlowVAE): its stack handle, data-dependent initialisation and sampling-direction
+    backward are NormalizingFlow's own."""
+    inner = owner.__dict__.get("_nfb_inner")
+    if inner is None or list(inner.flows) != list(owner.flows):
+        inner = NormalizingFlow(None, list(owner.flows))
+        owner.__dict__["_nfb_inner"] = inner
+    return inner
 
 
 class ConditionalNormalizingFlow(NormalizingFlow):
@@ -293,12 +312,7 @@ class ClassCondFlow(nn.Module):
         self._inner = None
 
     def _flow(self):
-        # an inner NormalizingFlow that shares the layer modules (no base: only its transform paths are used)
-        inner = self.__dict__.get("_nfb_inner")
-        if inner is None or list(inner.flows) != list(self.flows):
-            inner = NormalizingFlow(None, list(self.flows))
-            self.__dict__["_nfb_inner"] = inner
-        return inner
+        return _inner_flow(self)
 
     def log_prob(self, x, y):
         z, log_q = self._flow().inverse_and_log_det(x)
@@ -431,3 +445,44 @@ class MultiscaleFlow(nn.Module):
 
     def load(self, path):
         self.load_state_dict(torch.load(path))
+
+
+class NormalizingFlowVAE(nn.Module):
+    """VAE whose approximate posterior is an encoder q0(z | x) followed by flows (reference: core.py:656-700).
+
+    `forward(x, num_samples)` returns z [B, S, d], log_q [B, S] and log_p [B, S]; row b S + s of the flattened samples
+    belongs to x[b].  The encoder's draw, its log-density and the decoder's likelihood are kernels with a native
+    backward (distributions/encoder.py, distributions/decoder.py); the flows go through one stack, as in
+    NormalizingFlow.forward_and_log_det: one launch and one native backward for an all-planar or all-affine list, the
+    layer loop otherwise.  Under grad, flows without a differentiable sampling direction (spline, LU, MAF in a stack)
+    raise instead of being silently detached.  `prior` is used as given (a torch distribution stays torch)."""
+
+    def __init__(self, prior, q0=Dirac(), flows=None, decoder=None):
+        super().__init__()
+        self.prior = prior
+        self.decoder = decoder
+        self.flows = nn.ModuleList(flows)
+        self.q0 = q0
+
+    def _flows_forward(self, z):
+        if len(self.flows) == 0:
+            return z, torch.zeros(len(z), device=z.device)
+        inner = _inner_flow(self)
+        if wants_grad(self.flows, z) and not inner._flows_sampling_differentiable():
+            names = "+".join(sorted({type(f).__name__ for f in self.flows}))
+            raise NotImplementedError(_no_sampling_grad_message(f"NormalizingFlowVAE with {names} flows") + ")")
+        return inner.forward_and_log_det(z)
+
+    def forward(self, x, num_samples=1):
+        z, log_q = self.q0(x, num_samples=num_samples)
+        z = z.reshape(-1, *z.size()[2:])
+        log_q = log_q.reshape(-1, *log_q.size()[2:])
+        z, log_det = self._flows_forward(z)
+        log_q = log_q - log_det
+        log_p = self.prior.log_prob(z)
+        if self.decoder is not None:
+            log_p = log_p + self.decoder.log_prob(x, z)
+        z = z.view(-1, num_samples, *z.size()[1:])
+        log_q = log_q.view(-1, num_samples, *log_q.size()[1:])
+        log_p = log_p.view(-1, num_samples, *log_p.size()[1:])
+        return z, log_q, log_p

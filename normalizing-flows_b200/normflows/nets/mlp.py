@@ -13,6 +13,7 @@ class MLP(nn.Module):
             raise NotImplementedError("MLP output_fn / scaling is not on the CUDA path")
         if dropout is not None:
             raise NotImplementedError("MLP dropout is not on the CUDA path")
+        layers = [int(n) for n in layers]   # (the VAE notebook passes numpy arrays)
         mods = []
         for k in range(len(layers) - 2):
             mods += [nn.Linear(layers[k], layers[k + 1]), nn.LeakyReLU(leaky)]
