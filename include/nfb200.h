@@ -556,6 +556,11 @@ int nfb_flow_destroy(nfb_flow_t* f);
 int nfb_flow_add_ar_rqs(nfb_flow_t* f, const nfb_ar_rqs_desc_t* d);
 int nfb_flow_add_coupled_rqs(nfb_flow_t* f, const nfb_coupled_rqs_desc_t* d);
 int nfb_flow_add_lu_linear_permute(nfb_flow_t* f, const nfb_lu_desc_t* d);
+/* Affine family (MaskedAffineFlow, AffineCouplingBlock, AffineConstFlow / ActNorm, Permute): any number of features and
+ * any net width, nets of at most 6 Linear layers.  A run of consecutive affine layers with at most 16 features and nets at
+ * most 128 wide executes as one launch of the one-thread-per-row stack kernel; a run with any layer over either limit
+ * executes layer by layer on the wide path (nets on the tensor-core GEMM, element kernels for the coupling).  The choice
+ * is made from the shapes at finalize. */
 int nfb_flow_add_masked_affine(nfb_flow_t* f, const nfb_masked_affine_desc_t* d);
 int nfb_flow_add_affine_coupling(nfb_flow_t* f, const nfb_affine_coupling_desc_t* d);
 int nfb_flow_add_affine_const(nfb_flow_t* f, const nfb_affine_const_desc_t* d);
@@ -632,7 +637,10 @@ int nfb_flow_log_prob_backward(nfb_flow_t* f, const float* x_dev, const float* g
  * recomputes the stack from z (the forward kernel's own arithmetic), walks the ops in reverse in one kernel, then reduces
  * every Linear's weight and bias gradient in a fixed order (no atomics: two calls give identical bits).  Rows run in
  * chunks, so the workspace (nfb_flow_sampling_backward_workspace_bytes, -1 for an unsupported stack) stays below a fixed
- * bound; the number of launches does not depend on the number of layers.
+ * bound; the number of launches does not depend on the number of layers.  A stack on the wide path (over 16 features or a
+ * net wider than 128, see nfb_flow_add_masked_affine) recomputes each chunk layer by layer and back-propagates each layer
+ * with GEMMs: its launches grow linearly with depth, and weight gradients summed by split-K GEMMs are not bitwise
+ * reproducible from call to call.
  * g_x / g_ld may be NULL (zero cotangent); g_z and individual slots may be NULL (not wanted).  grad_slots holds the
  * layers' slots in nfb_flow_grad_slot_numel order (a base's slots, if any, are not read); rows = 0 writes zeros. */
 int64_t nfb_flow_sampling_backward_workspace_bytes(const nfb_flow_t* f, int64_t rows);
@@ -645,7 +653,7 @@ int nfb_flow_sampling_backward(nfb_flow_t* f, const float* z, const float* g_x, 
  * AffineConstFlow / ActNorm, AffineCouplingBlock and Permute only (any other stack, Planar / Radial included:
  * NFB_ERR_UNSUPPORTED).  x is the input that nfb_flow_transform was given.  One kernel recomputes the stack from x
  * taking the ops last-to-first, then walks them first-to-last; the weight reduction, the row chunking, the workspace
- * bound and the launch count are those of nfb_flow_sampling_backward.  g_z / g_ld may be NULL (zero cotangent); g_x and
+ * bound and the launch count (and the wide path) are those of nfb_flow_sampling_backward.  g_z / g_ld may be NULL (zero cotangent); g_x and
  * individual slots may be NULL (not wanted); grad_slots is in nfb_flow_grad_slot_numel order (a base's slots, if any,
  * are not read); rows = 0 writes zeros. */
 int64_t nfb_flow_density_backward_workspace_bytes(const nfb_flow_t* f, int64_t rows);

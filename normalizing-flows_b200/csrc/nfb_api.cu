@@ -20,6 +20,7 @@
 
 #include "../../include/nfb200.h"
 #include "nfb_kernels.h"
+#include "nfb_affine_wide.cuh"
 #include "nfb_planar_bwd.cuh"
 
 static thread_local std::string g_err;
@@ -227,6 +228,11 @@ struct Group {
     // sums, rebased per call), workspace units per row, and whether every layer has a density direction
     std::vector<PlanarOp> pops;
     bool invertible = true;
+    // affine group over affine_stack_kernel's limits (kAffMaxD features, kAffMaxW net width): runs layer by layer on the
+    // wide path, with scratch widths per row: wo the nets' outputs (at least D), hs / ht the hidden activations of the s
+    // (param_map) / t nets, wy the widest Linear
+    bool wide = false;
+    int wo = 0, hs = 0, ht = 0, wy = 1;
 };
 
 }  // namespace
@@ -263,7 +269,7 @@ struct nfb_flow {
     DevBuf in_ready;                 // device int: rows of the current host batch that have landed
     // training pass workspaces (nfb_flow_backward)
     DevBuf tr_store, tr_net, tr_P, tr_gP, tr_xp, tr_gxp, tr_zp, tr_gzp, tr_in, tr_gin, tr_g0, tr_g1, tr_small, tr_glq,
-        tr_t0, tr_t1, tr_wpack, tr_aff, tr_mix;
+        tr_t0, tr_t1, tr_wpack, tr_aff, tr_mix, aw_fwd;
     const int* cur_in_ready = nullptr;
     // affine sampling backward: the reduction items with this call's gradient pointers, staged through pinned memory
     AffRedItem* afb_host = nullptr;
@@ -1019,7 +1025,7 @@ int copy_mlp(const nfb_mlp_desc_t& d, AffMlp& m, float* slope) {
     m.n_layers = d.num_layers;
     if (d.num_layers == 0) return NFB_OK;   // absent net (MaskedAffineFlow with s or t = None)
     for (int i = 0; i <= d.num_layers; ++i) {
-        NFB_CHECK(d.sizes[i] >= 1 && d.sizes[i] <= kAffMaxW, NFB_ERR_UNSUPPORTED, "MLP: layer width %d > %d", d.sizes[i], kAffMaxW);
+        NFB_CHECK(d.sizes[i] >= 1, NFB_ERR_ARG, "MLP: layer width %d < 1", d.sizes[i]);
         m.sizes[i] = d.sizes[i];
     }
     for (int i = 0; i < d.num_layers; ++i) {
@@ -1031,6 +1037,9 @@ int copy_mlp(const nfb_mlp_desc_t& d, AffMlp& m, float* slope) {
 }
 
 cudaStream_t S(void* s) { return static_cast<cudaStream_t>(s); }
+
+int affine_wide_apply(nfb_flow* f, const Group& g, int first, int last, int dir, const float* zin, float* zout,
+                      float* logdet, long long rows, cudaStream_t st);
 
 int ensure_ws(nfb_flow* f, long long rows) {
     NFB_TRY(f->zA.reserve((size_t)rows * f->D * 4));
@@ -1054,6 +1063,7 @@ int run_group(nfb_flow* f, Group& g, int direction, const float* zin, float* zou
             return launch_fused_layer(f, *f->layers[g.first], nullptr, zin, zout, logdet, rows, 1, st);
         break;
     case G_AFFINE:
+        if (g.wide) return affine_wide_apply(f, g, g.first, g.last, direction, zin, zout, logdet, rows, st);
         NFB_TRY(launch_affine_stack(g.ops.p, g.last - g.first + 1, zin, zout, logdet, rows, f->D, 1, direction, st));
         f->launches++;
         return NFB_OK;
@@ -1668,19 +1678,20 @@ GemmTcArgs dgrad_args(const float* gY, const float* W, float* gX, long long M, i
     a.A = gY; a.lda = n_out; a.B = W; a.ldb = n_in; a.b_mn = 1; a.C = gX; a.ldc = n_in; a.M = M; a.N = n_in; a.K = n_out;
     return a;
 }
-// dW = gY^T act(X) (* mask), db = colsum(gY)
+// dW = gY^T act(X) (* mask), db = colsum(gY); accumulate: added to dW and db
 int wgrad(const GemmRun& g, const float* gY, int n_out, const float* X, long long ldx, int n_in, int relu_x,
-          const float* mask, long long rows, float* dW, float* db) {
+          const float* mask, long long rows, float* dW, float* db, int accumulate = 0) {
     if (dW) {
         GemmTcArgs a{};
         a.A = gY; a.lda = n_out; a.a_mn = 1; a.B = X; a.ldb = ldx; a.b_mn = 1; a.b_relu = relu_x;
         a.C = dW; a.ldc = n_in; a.M = n_out; a.N = n_in; a.K = rows; a.mulm = mask; a.ldmask = n_in;
+        a.accumulate = accumulate;
         NFB_TRY(g(a));
     }
     if (db) {
-        NFB_CUDA(cudaMemsetAsync(db, 0, (size_t)n_out * 4, g.st));
+        if (!accumulate) { NFB_CUDA(cudaMemsetAsync(db, 0, (size_t)n_out * 4, g.st)); g.count(1); }
         NFB_TRY(launch_colsum(gY, n_out, rows, n_out, db, g.st));
-        g.count(2);
+        g.count(1);
     }
     return NFB_OK;
 }
@@ -2058,6 +2069,61 @@ int64_t mlp_layout(const nfb_mlp_desc_t* d, long long rows, char* base, float** 
     for (int i = 0; i < 2; ++i) { float* p = c.take<float>((size_t)rows * wmax); if (Y) Y[i] = p; }
     return (int64_t)c.off;
 }
+
+// nets.MLP on the tensor core: L Linear layers, LeakyReLU(slope) after every one but the last
+struct MlpNet { int L; const int* sizes; const float* const* w; const float* const* b; float slope; };
+
+// A[l] = act(A[l - 1] W_l^T + b_l), l < L - 1 (A[-1] = x, row stride ldx; ReLU fused into the GEMM for slope 0); with
+// `out`, the last Linear into out [rows, sizes[L]]
+int mlp_forward(const GemmRun& g, const MlpNet& m, const float* x, long long ldx, long long rows, float* const* A,
+                float* out) {
+    const int* w = m.sizes;
+    for (int l = 0; l < m.L; ++l) {
+        const bool last = l + 1 == m.L;
+        if (last && !out) break;
+        GemmTcArgs a = fwd_args(l ? A[l - 1] : x, l ? w[l] : ldx, 0, m.w[l], m.b[l], last ? out : A[l], rows, w[l + 1], w[l]);
+        a.relu_out = !last && m.slope == 0.f;
+        NFB_TRY(g.w(a));
+        if (!last && m.slope != 0.f) {
+            NFB_TRY(launch_leaky_gate(A[l], A[l], m.slope, rows * w[l + 1], A[l], g.st));
+            g.count(1);
+        }
+    }
+    return NFB_OK;
+}
+
+// back-propagates gY [rows, sizes[L]] through the net whose hidden activations mlp_forward left in A (Y: two cotangent
+// buffers [rows, widest hidden layer]): weight / bias gradients (each optional; accumulate: added to), and the input
+// gradient g_x (optional, row stride ldgx), written or, with gx_add, added after a product with the row vector gx_mul
+// (optional)
+int mlp_adjoint(const GemmRun& g, const MlpNet& m, const float* x, long long ldx, const float* gY, long long rows,
+                float* const* A, float* const* Y, float* g_x, long long ldgx, int gx_add, const float* gx_mul,
+                float* const* g_w, float* const* g_b, int accumulate) {
+    const int* w = m.sizes;
+    for (int l = m.L - 1; l >= 0; --l) {
+        const float* X = l ? A[l - 1] : x;
+        NFB_TRY(wgrad(g, gY, w[l + 1], X, l ? w[l] : ldx, w[l], 0, nullptr, rows, g_w ? g_w[l] : nullptr,
+                      g_b ? g_b[l] : nullptr, accumulate));
+        if (l == 0) {
+            if (g_x) {
+                GemmTcArgs a = dgrad_args(gY, m.w[0], g_x, rows, w[0], w[1]);
+                a.ldc = ldgx; a.accumulate = gx_add; a.mulm = gx_mul;
+                NFB_TRY(g.w(a));
+            }
+            break;
+        }
+        float* gA = Y[l & 1];
+        GemmTcArgs a = dgrad_args(gY, m.w[l], gA, rows, w[l], w[l + 1]);
+        if (m.slope == 0.f) { a.mask = A[l - 1]; a.ldmask = w[l]; }
+        NFB_TRY(g.w(a));
+        if (m.slope != 0.f) {
+            NFB_TRY(launch_leaky_gate(gA, A[l - 1], m.slope, rows * w[l], gA, g.st));
+            g.count(1);
+        }
+        gY = gA;
+    }
+    return NFB_OK;
+}
 }  // namespace
 
 int64_t nfb_mlp_backward_workspace_bytes(const nfb_mlp_desc_t* d, int64_t rows) {
@@ -2087,30 +2153,9 @@ int nfb_mlp_backward(const nfb_mlp_desc_t* d, const float* x, const float* g_out
     int* err_dev = nullptr;
     NFB_TRY(glow_err_buf(&err_dev));
     const GemmRun g{err_dev, st};
-    const float slope = d->leaky;
-    // recompute: A[l] = leaky(A[l-1] W_l^T + b_l)  (ReLU fused into the GEMM for slope 0)
-    for (int l = 0; l + 1 < L; ++l) {
-        GemmTcArgs a = fwd_args(l ? A[l - 1] : x, w[l], 0, d->w[l], d->b[l], A[l], rows, w[l + 1], w[l]);
-        a.relu_out = slope == 0.f;
-        NFB_TRY(g(a));
-        if (slope != 0.f) NFB_TRY(launch_leaky_gate(A[l], A[l], slope, (long long)rows * w[l + 1], A[l], st));
-    }
-    const float* gY = g_out;
-    for (int l = L - 1; l >= 0; --l) {
-        const float* X = l ? A[l - 1] : x;
-        NFB_TRY(wgrad(g, gY, w[l + 1], X, w[l], w[l], 0, nullptr, rows, g_w ? g_w[l] : nullptr, g_b ? g_b[l] : nullptr));
-        if (l == 0) {
-            if (g_x) NFB_TRY(g(dgrad_args(gY, d->w[0], g_x, rows, w[0], w[1])));
-            break;
-        }
-        float* gA = Y[l & 1];
-        GemmTcArgs a = dgrad_args(gY, d->w[l], gA, rows, w[l], w[l + 1]);
-        if (slope == 0.f) { a.mask = A[l - 1]; a.ldmask = w[l]; }
-        NFB_TRY(g(a));
-        if (slope != 0.f) NFB_TRY(launch_leaky_gate(gA, A[l - 1], slope, (long long)rows * w[l], gA, st));
-        gY = gA;
-    }
-    return NFB_OK;
+    const MlpNet m{L, w, d->w, d->b, d->leaky};
+    NFB_TRY(mlp_forward(g, m, x, w[0], rows, A, nullptr));
+    return mlp_adjoint(g, m, x, w[0], g_out, rows, A, Y, g_x, w[0], 0, nullptr, g_w, g_b, 0);
 }
 
 int nfb_flow_create(nfb_flow_t** out, int32_t features) {
@@ -2187,7 +2232,6 @@ int nfb_flow_add_lu_linear_permute(nfb_flow_t* f, const nfb_lu_desc_t* d) {
 
 int nfb_flow_add_masked_affine(nfb_flow_t* f, const nfb_masked_affine_desc_t* d) {
     NFB_NEW_LAYER(L_MASKED_AFFINE);
-    NFB_CHECK(f->D <= kAffMaxD, NFB_ERR_UNSUPPORTED, "MaskedAffineFlow: features %d > %d", f->D, kAffMaxD);
     NFB_CHECK(d->b, NFB_ERR_ARG, "MaskedAffineFlow: null mask");
     L->op.type = kOpMasked; L->op.p0 = d->b; L->op.slope = 0.f;
     NFB_TRY(copy_mlp(d->s, L->op.s, &L->op.slope));
@@ -2201,14 +2245,13 @@ int nfb_flow_add_masked_affine(nfb_flow_t* f, const nfb_masked_affine_desc_t* d)
 
 int nfb_flow_add_affine_coupling(nfb_flow_t* f, const nfb_affine_coupling_desc_t* d) {
     NFB_NEW_LAYER(L_AFFINE_COUPLING);
-    NFB_CHECK(f->D <= kAffMaxD, NFB_ERR_UNSUPPORTED, "AffineCouplingBlock: features %d > %d", f->D, kAffMaxD);
     NFB_CHECK(d->scale_map >= 0 && d->scale_map <= 2, NFB_ERR_UNSUPPORTED, "This scale map is not implemented.");
     NFB_CHECK(d->split_mode == 0 || d->split_mode == 1, NFB_ERR_UNSUPPORTED, "split mode is not implemented.");
     L->op.type = kOpCoupling;
     L->op.flags = (d->scale ? 1 : 0) | (d->scale_map << 1) | (d->split_mode << 3);
     NFB_TRY(copy_mlp(d->param_map, L->op.s, &L->op.slope));
-    const int h = (f->D + 1) / 2;
-    const int n1 = d->split_mode ? f->D - h : h, n2 = f->D - n1;
+    const CouplingSplit c(f->D, d->split_mode != 0);
+    const int n1 = c.n1, n2 = c.n2;
     NFB_CHECK(d->param_map.num_layers >= 1 && d->param_map.sizes[0] == n1 &&
               d->param_map.sizes[d->param_map.num_layers] == (d->scale ? 2 : 1) * n2,
               NFB_ERR_ARG, "param_map must map %d -> %d", n1, (d->scale ? 2 : 1) * n2);
@@ -2218,7 +2261,6 @@ int nfb_flow_add_affine_coupling(nfb_flow_t* f, const nfb_affine_coupling_desc_t
 
 int nfb_flow_add_affine_const(nfb_flow_t* f, const nfb_affine_const_desc_t* d) {
     NFB_NEW_LAYER(L_AFFINE_CONST);
-    NFB_CHECK(f->D <= kAffMaxD, NFB_ERR_UNSUPPORTED, "AffineConstFlow: features %d > %d", f->D, kAffMaxD);
     NFB_CHECK(d->s && d->t, NFB_ERR_ARG, "AffineConstFlow: null s/t");
     L->op.type = kOpConst; L->op.p0 = d->s; L->op.p1 = d->t;
     f->layers.push_back(std::move(L));
@@ -2227,7 +2269,6 @@ int nfb_flow_add_affine_const(nfb_flow_t* f, const nfb_affine_const_desc_t* d) {
 
 int nfb_flow_add_permute(nfb_flow_t* f, const nfb_permute_desc_t* d) {
     NFB_NEW_LAYER(L_PERMUTE);
-    NFB_CHECK(f->D <= kAffMaxD, NFB_ERR_UNSUPPORTED, "Permute: features %d > %d", f->D, kAffMaxD);
     NFB_CHECK(d->perm && d->inv_perm, NFB_ERR_ARG, "Permute: null index list");
     L->perm_fwd.assign(d->perm, d->perm + f->D);
     L->perm_inv.assign(d->inv_perm, d->inv_perm + f->D);
@@ -2440,6 +2481,22 @@ int nfb_flow_finalize(nfb_flow_t* f, int32_t use_tensor_cores, void* stream) {
             Group g; g.kind = G_AFFINE; g.first = i; g.last = j;
             std::vector<AffineOp> ops;
             for (int k = i; k <= j; ++k) ops.push_back(f->layers[k]->op);
+            // the narrow kernel holds a row, and every net's activations, in one thread: over its limits the group
+            // takes the wide path
+            g.wide = f->D > kAffMaxD;
+            g.wo = f->D;
+            for (const AffineOp& op : ops)
+                for (int n = 0; n < 2; ++n) {
+                    const AffMlp& m = n ? op.t : op.s;
+                    int hidden = 0;
+                    for (int l = 0; l <= m.n_layers && m.n_layers; ++l) {
+                        g.wide = g.wide || m.sizes[l] > kAffMaxW;
+                        g.wy = std::max(g.wy, m.sizes[l]);
+                        if (l > 0 && l < m.n_layers) hidden += m.sizes[l];
+                    }
+                    if (m.n_layers) g.wo = std::max(g.wo, m.sizes[m.n_layers]);
+                    (n ? g.ht : g.hs) = std::max(n ? g.ht : g.hs, hidden);
+                }
             NFB_TRY(g.ops.upload(ops));
             f->groups.push_back(std::move(g));
             i = j + 1;
@@ -2507,6 +2564,17 @@ int nfb_flow_finalize(nfb_flow_t* f, int32_t use_tensor_cores, void* stream) {
 }
 
 int nfb_flow_num_layers(const nfb_flow_t* f) { return f ? (int)f->layers.size() : 0; }
+}  // extern "C"
+
+namespace {
+const Group* affine_group_of(const nfb_flow* f, int index) {
+    for (auto& g : f->groups)
+        if (g.kind == G_AFFINE && index >= g.first && index <= g.last) return &g;
+    return nullptr;
+}
+}  // namespace
+
+extern "C" {
 int64_t nfb_flow_last_launch_count(const nfb_flow_t* f) { return f ? f->launches : 0; }
 int nfb_flow_layer_is_fused(const nfb_flow_t* f, int32_t index) {
     if (!f || index < 0 || index >= (int)f->layers.size()) return 0;
@@ -2541,6 +2609,8 @@ int nfb_flow_layer_apply(nfb_flow_t* f, int32_t index, int32_t direction, const 
                   "This flow has no algebraic inverse.");
         rc = launch_planar_stack(static_cast<const PlanarOp*>(gp->ops.p) + (index - gp->first), 1, z_in, out, log_det,
                                  rows, f->D, 1, direction, st);
+    } else if (is_affine_kind(L) && affine_group_of(f, index)->wide) {
+        rc = affine_wide_apply(f, *affine_group_of(f, index), index, index, direction, z_in, out, log_det, rows, st);
     } else if (is_affine_kind(L)) {
         DevBuf ops;
         std::vector<AffineOp> v{L.op};
@@ -2873,8 +2943,8 @@ int lu_layer_backward(nfb_flow* f, Layer& L, const float* zin, const float* gxp,
 
 // the affine family's backward (defined with the sampling-direction entry points below)
 int plan_affine_bwd(nfb_flow* f, Group& g);
-long long affine_bwd_chunk_rows(const Group& g, long long rows);
-size_t affine_bwd_ws_bytes(const Group& g, long long R);
+long long affine_bwd_chunk_rows(const nfb_flow* f, const Group& g, long long rows);
+size_t affine_bwd_ws_bytes(const nfb_flow* f, const Group& g, long long R);
 int affine_group_backward(nfb_flow* f, Group& g, int direction, const float* in, const float* g_out, const float* g_ld,
                           int64_t rows, float* ws, long long R, float* g_in, float* const* grad_slots, cudaStream_t st);
 
@@ -2983,8 +3053,8 @@ int nfb_flow_log_prob_backward(nfb_flow_t* f, const float* x, const float* g_log
         const float* zin = store + (size_t)k * ZS;
         if (grp.kind == G_AFFINE) {   // recompute + adjoint walk + fixed-order reduction, chunked (internal workspace)
             NFB_TRY(plan_affine_bwd(f, grp));
-            const long long R = affine_bwd_chunk_rows(grp, rows);
-            NFB_TRY(f->tr_aff.reserve(affine_bwd_ws_bytes(grp, R)));
+            const long long R = affine_bwd_chunk_rows(f, grp, rows);
+            NFB_TRY(f->tr_aff.reserve(affine_bwd_ws_bytes(f, grp, R)));
             NFB_TRY(affine_group_backward(f, grp, NFB_INVERSE, zin, g, g_logq, rows, f->tr_aff.as<float>(), R, g2,
                                           grad_slots + off[grp.first], st));
             std::swap(g, g2);
@@ -3027,9 +3097,222 @@ namespace {
 
 constexpr long long kAffBwdWsCap = 256ll << 20;   // workspace bound: rows are processed in chunks below it
 
+// ---- wide path: an affine group over affine_stack_kernel's limits, layer by layer ----------------------------------------
+// Per layer: the nets on gemm_tc (mlp_forward / mlp_adjoint, weights split once per GEMM into f->tr_wpack), the coupling
+// arithmetic in nfb_affine_wide.cu.  Rows go in chunks whose scratch stays under kAffBwdWsCap.
+struct WideWs {
+    std::vector<float*> zs;   // backward: the input of op k (application order), k >= 1; forward: two ping-pong rows
+    float* g[2];              // backward: the running input cotangent and a spare (Permute)
+    float *zm, *S, *T, *As, *At;
+    float* Y[2];              // backward: mlp_adjoint's cotangent buffers
+};
+
+size_t wide_layout(const Group& g, int D, long long R, bool bwd, char* base, WideWs* ws) {
+    Carver c{base};
+    WideWs w{};
+    const int nz = bwd ? g.last - g.first : 2;
+    for (int k = 0; k < nz; ++k) w.zs.push_back(c.take<float>((size_t)R * D));
+    if (bwd) for (auto& p : w.g) p = c.take<float>((size_t)R * D);
+    w.zm = c.take<float>((size_t)R * D);
+    w.S = c.take<float>((size_t)R * g.wo);
+    w.T = c.take<float>((size_t)R * g.wo);
+    w.As = c.take<float>((size_t)R * g.hs);
+    w.At = c.take<float>((size_t)R * g.ht);
+    if (bwd) for (auto& p : w.Y) p = c.take<float>((size_t)R * g.wy);
+    if (ws) *ws = std::move(w);
+    return c.off;
+}
+
+long long wide_chunk_rows(const Group& g, int D, long long rows, bool bwd) {
+    const size_t fixed = wide_layout(g, D, 0, bwd, nullptr, nullptr) + 256 * 32;   // alignment slack of the pieces
+    const size_t per_row = (wide_layout(g, D, 1024, bwd, nullptr, nullptr) + 1023) / 1024;
+    long long R = std::max(1ll, (long long)((kAffBwdWsCap - (long long)fixed) / (long long)per_row));
+    if (R > kAffSegRows) R -= R % kAffSegRows;
+    return std::max(1ll, std::min(R, rows));
+}
+
+MlpNet mlp_net(const AffMlp& m, float slope) { return MlpNet{m.n_layers, m.sizes, m.w, m.b, slope}; }
+
+// the hidden activation buffers of net m inside the region `base` of R rows
+void hidden_ptrs(const AffMlp& m, float* base, long long R, float** A) {
+    long long off = 0;
+    for (int l = 0; l + 1 < m.n_layers; ++l) { A[l] = base + off * R; off += m.sizes[l + 1]; }
+}
+
+// one layer in direction dir: zi -> zo (m rows), log-det added into ld (optional); leaves the nets' activations and
+// outputs in ws (R-row buffers) for the adjoint.  zo = null: the nets only (the backward's recompute of a layer)
+int wide_layer_fwd(nfb_flow* f, const GemmRun& gr, const Layer& L, int dir, const float* zi, float* zo, float* ld,
+                   long long m, long long R, const WideWs& ws, cudaStream_t st) {
+    const int D = f->D;
+    const AffineOp& op = L.op;
+    float* A[kAffMaxLayers];
+    if (!zo && (L.kind == L_PERMUTE || L.kind == L_AFFINE_CONST)) return NFB_OK;
+    switch (L.kind) {
+    case L_PERMUTE:
+        NFB_TRY(launch_gather_cols(zi, zo, dir ? op.fwd_idx : op.inv_idx, m, D, 1, st));
+        break;
+    case L_AFFINE_CONST:
+        NFB_TRY(launch_affine_wide_elem(op, D, dir, zi, nullptr, nullptr, zo, ld, m, st));
+        break;
+    case L_MASKED_AFFINE:
+        NFB_TRY(launch_affine_wide_mask(zi, op.p0, ws.zm, m, D, st));
+        f->launches++;
+        if (op.s.n_layers) {
+            hidden_ptrs(op.s, ws.As, R, A);
+            NFB_TRY(mlp_forward(gr, mlp_net(op.s, op.slope), ws.zm, D, m, A, ws.S));
+        }
+        if (op.t.n_layers) {
+            hidden_ptrs(op.t, ws.At, R, A);
+            NFB_TRY(mlp_forward(gr, mlp_net(op.t, op.slope_t), ws.zm, D, m, A, ws.T));
+        }
+        if (!zo) return NFB_OK;
+        NFB_TRY(launch_affine_wide_elem(op, D, dir, zi, op.s.n_layers ? ws.S : nullptr, op.t.n_layers ? ws.T : nullptr,
+                                        zo, ld, m, st));
+        break;
+    case L_AFFINE_COUPLING: {
+        const CouplingSplit c(D, (op.flags >> 3) & 1);
+        hidden_ptrs(op.s, ws.As, R, A);
+        NFB_TRY(mlp_forward(gr, mlp_net(op.s, op.slope), zi + c.o1, D, m, A, ws.S));
+        if (!zo) return NFB_OK;
+        NFB_TRY(launch_affine_wide_elem(op, D, dir, zi, ws.S, nullptr, zo, ld, m, st));
+        break;
+    }
+    default:
+        nfb_set_error("wide affine path: layer kind %d", (int)L.kind);
+        return NFB_ERR_STATE;
+    }
+    f->launches++;
+    return NFB_OK;
+}
+
+// layers first..last of wide group g in direction dir (density: last to first), zin -> zout (distinct), log-det added into
+// logdet (optional)
+int affine_wide_apply(nfb_flow* f, const Group& g, int first, int last, int dir, const float* zin, float* zout,
+                      float* logdet, long long rows, cudaStream_t st) {
+    if (rows == 0) return NFB_OK;
+    const int D = f->D, n = last - first + 1;
+    const long long R = wide_chunk_rows(g, D, rows, false);
+    NFB_TRY(f->aw_fwd.reserve(wide_layout(g, D, R, false, nullptr, nullptr)));
+    WideWs ws;
+    wide_layout(g, D, R, false, f->aw_fwd.as<char>(), &ws);
+    const GemmRun gr{f->err.as<int>(), st, &f->tr_wpack, &f->launches};
+    for (long long r0 = 0; r0 < rows; r0 += R) {
+        const long long m = std::min(R, rows - r0);
+        const float* cur = zin + r0 * D;
+        for (int k = 0; k < n; ++k) {
+            float* out = k == n - 1 ? zout + r0 * D : ws.zs[k & 1];
+            NFB_TRY(wide_layer_fwd(f, gr, *f->layers[dir ? first + k : last - k], dir, cur, out,
+                                   logdet ? logdet + r0 : nullptr, m, R, ws, st));
+            cur = out;
+        }
+    }
+    return NFB_OK;
+}
+
+// backward of wide group g in direction dir (the arguments of affine_group_backward).  Per chunk: recompute every op's
+// input, then take the ops in reverse: recompute the layer's nets, the adjoint element kernel, the nets' dgrad / wgrad
+// (bias gradients by launch_colsum), their input gradient added into g (masked by b, or into the identity half).
+int affine_wide_backward(nfb_flow* f, Group& g, int dir, const float* in, const float* g_out, const float* g_ld,
+                         int64_t rows, float* wsp, long long R, float* g_in, float* const* grad_slots, cudaStream_t st) {
+    const int D = f->D, n_ops = g.last - g.first + 1;
+    std::vector<int> off(n_ops + 1, 0);
+    for (int k = 0; k < n_ops; ++k) off[k + 1] = off[k] + grad_slots_of(*f->layers[g.first + k]);
+    if (rows == 0) {   // zero parameter gradients
+        for (int k = 0; k < n_ops; ++k)
+            for (int s = off[k]; s < off[k + 1]; ++s)
+                if (grad_slots && grad_slots[s]) {
+                    NFB_CUDA(cudaMemsetAsync(grad_slots[s], 0, (size_t)grad_slot_numel(*f->layers[g.first + k], s - off[k]) * 4, st));
+                    f->launches++;
+                }
+        return NFB_OK;
+    }
+    WideWs ws;
+    wide_layout(g, D, R, true, reinterpret_cast<char*>(wsp), &ws);
+    const GemmRun gr{f->err.as<int>(), st, &f->tr_wpack, &f->launches};
+    // application order: sampling first..last, density last..first
+    auto layer_at = [&](int k) -> int { return dir ? g.first + k : g.last - k; };
+    for (long long r0 = 0; r0 < rows; r0 += R) {
+        const long long m = std::min(R, (long long)rows - r0);
+        const int acc = r0 > 0;
+        std::vector<const float*> zs(n_ops);
+        zs[0] = in + r0 * D;
+        for (int k = 0; k + 1 < n_ops; ++k) {
+            NFB_TRY(wide_layer_fwd(f, gr, *f->layers[layer_at(k)], dir, zs[k], ws.zs[k], nullptr, m, R, ws, st));
+            zs[k + 1] = ws.zs[k];
+        }
+        float* G = ws.g[0];
+        float* G2 = ws.g[1];
+        if (g_out) NFB_CUDA(cudaMemcpyAsync(G, g_out + r0 * D, (size_t)m * D * 4, cudaMemcpyDeviceToDevice, st));
+        else NFB_CUDA(cudaMemsetAsync(G, 0, (size_t)m * D * 4, st));
+        f->launches++;
+        const float* gl = g_ld ? g_ld + r0 : nullptr;
+        for (int k = n_ops - 1; k >= 0; --k) {
+            const int li = layer_at(k);
+            const Layer& L = *f->layers[li];
+            const AffineOp& op = L.op;
+            float* const* slots = grad_slots ? grad_slots + off[li - g.first] : nullptr;
+            auto slot = [&](int s) -> float* { return slots ? slots[s] : nullptr; };
+            float* A[kAffMaxLayers];
+            float *gw[kAffMaxLayers], *gb[kAffMaxLayers];
+            auto net_slots = [&](int s0, int n_lin) {
+                for (int l = 0; l < n_lin; ++l) { gw[l] = slot(s0 + 2 * l); gb[l] = slot(s0 + 2 * l + 1); }
+            };
+            if (L.kind == L_PERMUTE) {   // sampling x[j] = z[fwd[j]]: g_z[i] = g_x[inv[i]]; density the other way
+                NFB_TRY(launch_gather_cols(G, G2, dir ? op.inv_idx : op.fwd_idx, m, D, 1, st));
+                f->launches++;
+                std::swap(G, G2);
+                continue;
+            }
+            if (L.kind == L_AFFINE_CONST) {
+                NFB_TRY(launch_affine_wide_adjoint(op, D, dir, zs[k], ws.S, ws.T, G, gl, m, st));
+                f->launches++;
+                for (int j = 0; j < 2; ++j)
+                    if (slot(j)) {
+                        if (!acc) { NFB_CUDA(cudaMemsetAsync(slot(j), 0, (size_t)D * 4, st)); f->launches++; }
+                        NFB_TRY(launch_colsum(j ? ws.T : ws.S, D, m, D, slot(j), st));
+                        f->launches++;
+                    }
+                continue;
+            }
+            // recompute the layer's nets (and the masked input) on its input
+            NFB_TRY(wide_layer_fwd(f, gr, L, dir, zs[k], nullptr, nullptr, m, R, ws, st));
+            if (L.kind == L_MASKED_AFFINE) {
+                NFB_TRY(launch_affine_wide_adjoint(op, D, dir, zs[k], op.s.n_layers ? ws.S : nullptr,
+                                                   op.t.n_layers ? ws.T : nullptr, G, gl, m, st));
+                f->launches++;
+                if (op.s.n_layers) {
+                    hidden_ptrs(op.s, ws.As, R, A);
+                    net_slots(0, op.s.n_layers);
+                    NFB_TRY(mlp_adjoint(gr, mlp_net(op.s, op.slope), ws.zm, D, ws.S, m, A, ws.Y, G, D, 1, op.p0, gw, gb,
+                                        acc));
+                }
+                if (op.t.n_layers) {
+                    hidden_ptrs(op.t, ws.At, R, A);
+                    net_slots(2 * op.s.n_layers, op.t.n_layers);
+                    NFB_TRY(mlp_adjoint(gr, mlp_net(op.t, op.slope_t), ws.zm, D, ws.T, m, A, ws.Y, G, D, 1, op.p0, gw,
+                                        gb, acc));
+                }
+            } else {
+                const CouplingSplit c(D, (op.flags >> 3) & 1);
+                NFB_TRY(launch_affine_wide_adjoint(op, D, dir, zs[k], ws.S, nullptr, G, gl, m, st));
+                f->launches++;
+                hidden_ptrs(op.s, ws.As, R, A);
+                net_slots(0, op.s.n_layers);
+                NFB_TRY(mlp_adjoint(gr, mlp_net(op.s, op.slope), zs[k] + c.o1, D, ws.S, m, A, ws.Y, G + c.o1, D, 1,
+                                    nullptr, gw, gb, acc));
+            }
+        }
+        if (g_in) {
+            NFB_CUDA(cudaMemcpyAsync(g_in + r0 * D, G, (size_t)m * D * 4, cudaMemcpyDeviceToDevice, st));
+            f->launches++;
+        }
+    }
+    return NFB_OK;
+}
+
 // units per row of the workspace, each op's unit table and the weight reduction's items, in grad-slot order
 int plan_affine_bwd(nfb_flow* f, Group& g) {
-    if (g.bwd_planned) return NFB_OK;
+    if (g.bwd_planned || g.wide) return NFB_OK;
     std::vector<AffBwdOp> bops;
     g.items.clear();
     int u = 0;
@@ -3067,14 +3350,16 @@ int plan_affine_bwd(nfb_flow* f, Group& g) {
     return NFB_OK;
 }
 
-long long affine_bwd_chunk_rows(const Group& g, long long rows) {
+long long affine_bwd_chunk_rows(const nfb_flow* f, const Group& g, long long rows) {
+    if (g.wide) return wide_chunk_rows(g, f->D, rows, true);
     const long long per_row = 4ll * g.units + (4 * g.n_elem + kAffSegRows - 1) / kAffSegRows + 1;
     long long R = std::max(1ll, kAffBwdWsCap / per_row);
     if (R > kAffSegRows) R -= R % kAffSegRows;
     return std::max(1ll, std::min(R, rows));
 }
 
-size_t affine_bwd_ws_bytes(const Group& g, long long R) {
+size_t affine_bwd_ws_bytes(const nfb_flow* f, const Group& g, long long R) {
+    if (g.wide) return wide_layout(g, f->D, R, true, nullptr, nullptr);
     const size_t data = ((size_t)g.units * R * 4 + 255) & ~(size_t)255;
     return data + (size_t)((R + kAffSegRows - 1) / kAffSegRows) * g.n_elem * 4;
 }
@@ -3172,6 +3457,7 @@ int affine_only_group(nfb_flow* f, Group** out, const char* who) {
 // reduction.  ws holds affine_bwd_ws_bytes(g, R) bytes.
 int affine_group_backward(nfb_flow* f, Group& g, int direction, const float* in, const float* g_out, const float* g_ld,
                           int64_t rows, float* ws, long long R, float* g_in, float* const* grad_slots, cudaStream_t st) {
+    if (g.wide) return affine_wide_backward(f, g, direction, in, g_out, g_ld, rows, ws, R, g_in, grad_slots, st);
     const int n_items = (int)g.items.size();
     if (n_items) {
         // this call's output pointers, in slot order (a Linear takes two slots, a column sum one)
@@ -3212,14 +3498,14 @@ int affine_group_backward(nfb_flow* f, Group& g, int direction, const float* in,
 }
 
 // the entry points' common checks; R = the chunk size the workspace is planned for
-int affine_entry_checks(const char* who, Group& g, const float* in, int64_t rows, void* ws, int64_t ws_bytes,
-                        long long* R) {
+int affine_entry_checks(const char* who, nfb_flow* f, Group& g, const float* in, int64_t rows, void* ws,
+                        int64_t ws_bytes, long long* R) {
     NFB_CHECK(rows >= 0, NFB_ERR_ARG, "rows < 0");
     NFB_CHECK(rows == 0 || in, NFB_ERR_ARG, "null input");
-    *R = affine_bwd_chunk_rows(g, rows);
-    NFB_CHECK(ws && ws_bytes >= (int64_t)affine_bwd_ws_bytes(g, *R), NFB_ERR_ARG,
+    *R = affine_bwd_chunk_rows(f, g, rows);
+    NFB_CHECK(ws && ws_bytes >= (int64_t)affine_bwd_ws_bytes(f, g, *R), NFB_ERR_ARG,
               "%s backward: workspace of %lld bytes, %lld needed", who, (long long)ws_bytes,
-              (long long)affine_bwd_ws_bytes(g, *R));
+              (long long)affine_bwd_ws_bytes(f, g, *R));
     return NFB_OK;
 }
 
@@ -3232,7 +3518,7 @@ int64_t nfb_flow_sampling_backward_workspace_bytes(const nfb_flow_t* fc, int64_t
     Group* g = planar_only_group(f);
     if (g) return rows < 0 ? -1 : (int64_t)planar_bwd_ws_bytes(*g, planar_bwd_chunk_rows(*g, rows));
     if (rows < 0 || affine_only_group(f, &g, "sampling") != NFB_OK) return -1;
-    return (int64_t)affine_bwd_ws_bytes(*g, affine_bwd_chunk_rows(*g, rows));
+    return (int64_t)affine_bwd_ws_bytes(f, *g, affine_bwd_chunk_rows(f, *g, rows));
 }
 
 int nfb_flow_sampling_backward(nfb_flow_t* f, const float* z, const float* g_x, const float* g_ld, int64_t rows,
@@ -3242,7 +3528,7 @@ int nfb_flow_sampling_backward(nfb_flow_t* f, const float* z, const float* g_x, 
     Group* gp = nullptr;
     NFB_TRY(affine_only_group(f, &gp, "sampling"));
     long long R = 0;
-    NFB_TRY(affine_entry_checks("sampling", *gp, z, rows, ws, ws_bytes, &R));
+    NFB_TRY(affine_entry_checks("sampling", f, *gp, z, rows, ws, ws_bytes, &R));
     f->launches = 0;
     return affine_group_backward(f, *gp, NFB_FORWARD, z, g_x, g_ld, rows, static_cast<float*>(ws), R, g_z, grad_slots,
                                  S(stream));
@@ -3250,8 +3536,9 @@ int nfb_flow_sampling_backward(nfb_flow_t* f, const float* z, const float* g_x, 
 
 int64_t nfb_flow_density_backward_workspace_bytes(const nfb_flow_t* fc, int64_t rows) {
     Group* g = nullptr;
-    if (rows < 0 || affine_only_group(const_cast<nfb_flow*>(fc), &g, "density") != NFB_OK) return -1;
-    return (int64_t)affine_bwd_ws_bytes(*g, affine_bwd_chunk_rows(*g, rows));
+    nfb_flow* f = const_cast<nfb_flow*>(fc);
+    if (rows < 0 || affine_only_group(f, &g, "density") != NFB_OK) return -1;
+    return (int64_t)affine_bwd_ws_bytes(f, *g, affine_bwd_chunk_rows(f, *g, rows));
 }
 
 int nfb_flow_density_backward(nfb_flow_t* f, const float* x, const float* g_z, const float* g_ld, int64_t rows,
@@ -3259,7 +3546,7 @@ int nfb_flow_density_backward(nfb_flow_t* f, const float* x, const float* g_z, c
     Group* gp = nullptr;
     NFB_TRY(affine_only_group(f, &gp, "density"));
     long long R = 0;
-    NFB_TRY(affine_entry_checks("density", *gp, x, rows, ws, ws_bytes, &R));
+    NFB_TRY(affine_entry_checks("density", f, *gp, x, rows, ws, ws_bytes, &R));
     f->launches = 0;
     return affine_group_backward(f, *gp, NFB_INVERSE, x, g_z, g_ld, rows, static_cast<float*>(ws), R, g_x, grad_slots,
                                  S(stream));

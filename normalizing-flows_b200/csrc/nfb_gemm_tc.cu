@@ -388,10 +388,12 @@ int launch_gemm_tc(const GemmTcArgs& a, int* err, cudaStream_t st) {
     const int nt = gemm_tc_n_tile(a.N, a.b_mn);
     const long long m_tiles = (a.M + 127) / 128;
     const int n_tiles = (int)((a.N + nt - 1) / nt);
-    // split K only when there are too few output tiles to fill the machine (weight gradients: K = batch)
+    // split K only when there are too few output tiles to fill the machine (weight gradients: K = batch), and only
+    // for a linear epilogue (the partial products are added with red.global.add)
     int ks = 1;
     const long long tiles = m_tiles * n_tiles;
-    if (tiles < sm_count && a.K >= 2048) {
+    const bool linear_epilogue = !a.bias && !a.mask && !a.resid && !a.relu_out;
+    if (tiles < sm_count && a.K >= 2048 && linear_epilogue) {
         ks = (int)((2LL * sm_count) / tiles);  // <= 2 units per CTA: no third, mostly empty wave
         const long long max_ks = (a.K + 511) / 512;  // at least 8 chunks per split
         if (ks > max_ks) ks = (int)max_ks;

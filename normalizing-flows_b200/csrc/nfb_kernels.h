@@ -132,8 +132,9 @@ int launch_logit_bwd(const float* in, const float* g_out, const float* g_ld, flo
                      float alpha, cudaStream_t st);
 
 // ---- small-dimension affine stack (nfb_affine.cu) ----
+// A group of affine layers within both limits runs on affine_stack_kernel; any layer over one selects the wide path.
 constexpr int kAffMaxD = 16;
-constexpr int kAffMaxW = 128;  // widest MLP layer supported
+constexpr int kAffMaxW = 128;  // widest MLP layer of the one-thread-per-row kernel
 constexpr int kAffMaxLayers = 6;
 
 struct AffMlp {
@@ -180,6 +181,14 @@ int launch_affine_bwd_rows(const void* ops_dev, const void* bops_dev, int n_ops,
                            const float* gx, const float* gld, float* gz, float* ws, long long R, int d, cudaStream_t st);
 int launch_affine_bwd_reduce(const void* items_dev, int n_items, long long n_elem, const float* ws, long long R,
                              float* partial, int accumulate, cudaStream_t st);
+
+// ---- wide affine path (nfb_affine_wide.cu): groups over kAffMaxD features or with a net wider than kAffMaxW, run layer
+// by layer with the nets on gemm_tc (nfb_api.cu).  dir: 1 sampling, 0 density.
+int launch_affine_wide_mask(const float* z, const float* b, float* zm, long long rows, int d, cudaStream_t st);
+int launch_affine_wide_elem(const AffineOp& op, int d, int dir, const float* zin, const float* S, const float* T,
+                            float* zout, float* ld, long long rows, cudaStream_t st);
+int launch_affine_wide_adjoint(const AffineOp& op, int d, int dir, const float* zin, float* S, float* T, float* G,
+                               const float* gld, long long rows, cudaStream_t st);
 
 // ---- planar / radial stack (nfb_planar.cu) ----
 constexpr int kPlanarMaxD = 64;
