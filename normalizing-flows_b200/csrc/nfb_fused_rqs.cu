@@ -32,8 +32,9 @@
 //              In the final layer the warpgroups take different roles: warpgroup 0 multiplies both halves of every
 //              record (two features, N = 48, per half; both halves as one N = 96 product) into two alternating
 //              accumulators and stores each pair of chunks, unscaled and with its biases, to two staging tiles in shared
-//              memory; warpgroup 1 copies its (row, feature) parameters out of the tiles,
-//              hands them back at once and evaluates two splines per thread.  The hand-off is a pair of named barriers
+//              memory; warpgroup 1 copies its (row, feature) parameters of both chunks out of the tiles, hands them
+//              back before any spline runs and evaluates the two splines per thread as one two-lane chain
+//              (rqs_core_lanes, nfb_spline.cuh).  The hand-off is a pair of named barriers
 //              ("full" / "free", one side arrives, the other waits), so the products of one pair of chunks run under the
 //              splines of the pair before.
 // Shared memory: A operand 64 KB (hi|lo x K=256), weight ring 96 KB, x/y tile 16 KB (XOR-swizzled, conflict-free
@@ -796,43 +797,53 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
                 // warpgroup-0 thread of (row, f) over the even chunks, ladsum this thread's own over the odd chunks.
                 const int f = (et >> 6) & 1;   // feature of each chunk this thread evaluates (for row r)
                 lad_even = ldsum[f * kRows + r];
+                const int F = L.F, T = L.T;
                 for (int ci = 0; ci < n_pairs; ++ci) {
                     stg_bar_wait<kBarStgFull>();
-                    // One spline after the other, as a loop: two evaluations in one block need more registers than
-                    // a thread has, and spills go through the little L1 the shared memory leaves.  The tiles are
-                    // handed back when the second spline's parameters are in registers.
-#pragma unroll 1
+                    // Both splines' parameters to registers (chunk 2 ci's tile, then 2 ci + 1's), and the tiles go back
+                    // before any spline runs, so that the next pair can be staged under both.  (The packer folded log2(e)
+                    // and the layer's 1/sqrt(H) into the w/h columns and biases; the product warpgroup has unscaled the
+                    // products and added the biases.)
+                    float pv[2][24];
+#pragma unroll
                     for (int h = 0; h < 2; ++h) {
-                        const int t = (2 * ci + h) * L.F + f;
-                        // (the packer folded log2(e) and the layer's 1/sqrt(H) into the w/h columns and biases; the product
-                        // warpgroup has unscaled the products and added the biases)
                         const float4* sp = reinterpret_cast<const float4*>(stg0 + (h * kRows + r) * kStgLd + 24 * f);
-                        float pv[24];
 #pragma unroll
                         for (int q = 0; q < 6; ++q) {
                             const float4 s4 = sp[q];
-                            pv[4 * q] = s4.x;
-                            pv[4 * q + 1] = s4.y;
-                            pv[4 * q + 2] = s4.z;
-                            pv[4 * q + 3] = s4.w;
+                            pv[h][4 * q] = s4.x;
+                            pv[h][4 * q + 1] = s4.y;
+                            pv[h][4 * q + 2] = s4.z;
+                            pv[h][4 * q + 3] = s4.w;
                         }
-                        if (h == 1 && ci + 1 < n_pairs) stg_bar_arrive<kBarStgFree>();   // (the last pair's tiles have no next writer)
-                        NFB_CLK(kClkFinStage);
-                        if (t < L.T) {
-                            float lw[8], lh[8], dd[8];
-#pragma unroll
-                            for (int q = 0; q < 8; ++q) { lw[q] = pv[q]; lh[q] = pv[8 + q]; dd[q] = pv[16 + q]; }
-                            const int col = L.tr_idx[t];
-                            float y, l;
-                            float xin = get_x(col);
-                            if (arsamp) xin = row_live ? __ldcg(zdst + grow * D + col) : 0.f;
-                            rqs_core<8, SAMPLE>(xin, lw, lh, [&dd](int k) { return dd[k]; }, L.tail, y, l);
-                            put_y(col, y);
-                            if (h) ladsum += l;
-                            else lad_even += l;
-                        }
-                        NFB_CLK(kClkFinSpline);
                     }
+                    if (ci + 1 < n_pairs) stg_bar_arrive<kBarStgFree>();   // (the last pair's tiles have no next writer)
+                    NFB_CLK(kClkFinStage);
+                    // The features t0 (even chunk) and t0 + F (odd chunk): both as one two-lane evaluation, whose
+                    // chains interleave, when both are transformed, else the even one alone.  (Warp-uniform: t0
+                    // depends on ci and f only.)
+                    const int t0 = 2 * ci * F + f;
+                    auto splines = [&](auto lanes) {
+                        constexpr int N = decltype(lanes)::value;
+                        int col[N];
+                        float xin[N], y[N], l[N];
+#pragma unroll
+                        for (int h = 0; h < N; ++h) {
+                            col[h] = L.tr_idx[t0 + h * F];
+                            xin[h] = get_x(col[h]);
+                            if (arsamp) xin[h] = row_live ? __ldcg(zdst + grow * D + col[h]) : 0.f;
+                        }
+                        rqs_core_lanes<N, 8, SAMPLE>(xin, [&pv](int h, int i) { return pv[h][i]; },
+                                                     [&pv](int h, int i) { return pv[h][8 + i]; },
+                                                     [&pv](int h, int i) { return pv[h][16 + i]; }, L.tail, y, l);
+#pragma unroll
+                        for (int h = 0; h < N; ++h) put_y(col[h], y[h]);
+                        lad_even += l[0];
+                        if constexpr (N == 2) ladsum += l[1];
+                    };
+                    if (t0 + F < T) splines(std::integral_constant<int, 2>());
+                    else if (t0 < T) splines(std::integral_constant<int, 1>());
+                    NFB_CLK(kClkFinSpline);
                 }
             }
             cons_bar_sync();   // (AR sampling: every output of this pass is in xs before the next pass reads it)

@@ -1,4 +1,4 @@
-// nfb_spline.cuh -- monotone rational-quadratic spline, one element per call.
+// nfb_spline.cuh -- monotone rational-quadratic spline, one element per call (rqs_core_lanes: N independent ones).
 //
 // Mask-free restatement of normflows/utils/splines.py:16-219 (`unconstrained_rational_
 // quadratic_spline` with tails="linear" -> `rational_quadratic_spline`):
@@ -100,100 +100,134 @@ __host__ __device__ __forceinline__ float rqs_inverse_root(float a, float b, flo
 // carrying {left, right} of both axes and the two derivative logits, instead of a 7-step scan.
 // ud_first / ud_last: raw derivative parameters of the two boundary knots.  Linear tails pin both to the constant that
 // makes the derivative exactly 1 (:35-38); circular tails (:42-45, :48-57) pass learned values (last = first).
+//
+// N independent evaluations in one call (lane n: input x[n], parameters w(n, i), h(n, i), d(n, i)), one stage after the
+// other for all lanes: each stage is a dependent chain of MUFU ops and FMAs, and the lanes' chains interleave where one
+// thread has nothing else to issue.  A lane's arithmetic is that of a single evaluation, expression for expression, so
+// its results do not depend on N.  Branch-free up to the inverse root's division, so the lanes stay in one basic block.
+template <int N, int K, bool INVERSE, typename PW, typename PH, typename PD>
+__host__ __device__ __forceinline__ void rqs_core_lanes(const float (&x)[N], PW pw, PH ph, PD pd, float tail,
+                                                        float (&y)[N], float (&lad)[N],
+                                                        float ud_first = NFB_BOUNDARY_UD,
+                                                        float ud_last = NFB_BOUNDARY_UD) {
+    // softmax of the width and height logits -> knots on the unit interval, with the raw derivative parameters
+    float kw[N][K + 1], kh[N][K + 1], ud[N][K + 1];
+#pragma unroll
+    for (int n = 0; n < N; ++n) {
+        float mw = pw(n, 0), mh = ph(n, 0);
+#pragma unroll
+        for (int i = 1; i < K; ++i) {
+            mw = fmaxf(mw, pw(n, i));
+            mh = fmaxf(mh, ph(n, i));
+        }
+        float cw[K], ch[K];
+        float sw = 0.f, sh = 0.f;
+#pragma unroll
+        for (int i = 0; i < K; ++i) {
+            sw += fast_ex2(pw(n, i) - mw);
+            sh += fast_ex2(ph(n, i) - mh);
+            cw[i] = sw;
+            ch[i] = sh;
+        }
+        const float aw = (1.f - kMinBinWidth * K) * rcp_nr(sw);
+        const float ah = (1.f - kMinBinHeight * K) * rcp_nr(sh);
+        kw[n][0] = 0.f; kh[n][0] = 0.f; kw[n][K] = 1.f; kh[n][K] = 1.f;
+        ud[n][0] = ud_first; ud[n][K] = ud_last;
+#pragma unroll
+        for (int i = 0; i < K - 1; ++i) {
+            kw[n][i + 1] = fmaf(aw, cw[i], kMinBinWidth * (float)(i + 1));
+            kh[n][i + 1] = fmaf(ah, ch[i], kMinBinHeight * (float)(i + 1));
+            ud[n][i + 1] = pd(n, i);
+        }
+    }
+    // the bin of x, its derivatives and slope
+    const float two_b = 2.f * tail;
+    float xu[N], l_w[N], l_h[N], in_w[N], in_h[N], d0[N], d1[N], rw[N], delta[N], s[N];
+#pragma unroll
+    for (int n = 0; n < N; ++n) {
+        xu[n] = fmaf(x[n], rcp_nr(two_b), 0.5f);
+        float r_w, r_h, ud0, ud1;
+        if (K == 8) {
+            const float* ks = INVERSE ? kh[n] : kw[n];
+            const bool c1 = xu[n] >= ks[4];
+            float a_w[5], a_h[5], a_d[5];
+#pragma unroll
+            for (int j = 0; j < 5; ++j) {
+                a_w[j] = c1 ? kw[n][4 + j] : kw[n][j];
+                a_h[j] = c1 ? kh[n][4 + j] : kh[n][j];
+                a_d[j] = c1 ? ud[n][4 + j] : ud[n][j];
+            }
+            const bool c2 = xu[n] >= (INVERSE ? a_h[2] : a_w[2]);
+            float b_w[3], b_h[3], b_d[3];
+#pragma unroll
+            for (int j = 0; j < 3; ++j) {
+                b_w[j] = c2 ? a_w[2 + j] : a_w[j];
+                b_h[j] = c2 ? a_h[2 + j] : a_h[j];
+                b_d[j] = c2 ? a_d[2 + j] : a_d[j];
+            }
+            const bool c3 = xu[n] >= (INVERSE ? b_h[1] : b_w[1]);
+            l_w[n] = c3 ? b_w[1] : b_w[0]; r_w = c3 ? b_w[2] : b_w[1];
+            l_h[n] = c3 ? b_h[1] : b_h[0]; r_h = c3 ? b_h[2] : b_h[1];
+            ud0 = c3 ? b_d[1] : b_d[0]; ud1 = c3 ? b_d[2] : b_d[1];
+        } else {
+            l_w[n] = kw[n][0]; r_w = kw[n][1]; l_h[n] = kh[n][0]; r_h = kh[n][1]; ud0 = ud[n][0]; ud1 = ud[n][1];
+#pragma unroll
+            for (int i = 1; i < K; ++i) {
+                if (xu[n] >= (INVERSE ? kh[n][i] : kw[n][i])) {  // knot i <= x
+                    l_w[n] = kw[n][i]; r_w = kw[n][i + 1]; l_h[n] = kh[n][i]; r_h = kh[n][i + 1];
+                    ud0 = ud[n][i]; ud1 = ud[n][i + 1];
+                }
+            }
+        }
+        in_w[n] = r_w - l_w[n];
+        in_h[n] = r_h - l_h[n];
+        d0[n] = kMinDerivative + softplus_f(ud0);
+        d1[n] = kMinDerivative + softplus_f(ud1);
+        rw[n] = rcp_nr(in_w[n]);
+        delta[n] = in_h[n] * rw[n];
+        s[n] = d0[n] + d1[n] - 2.f * delta[n];
+    }
+    // the rational function and its log-derivative
+#pragma unroll
+    for (int n = 0; n < N; ++n) {
+        const bool inside = (x[n] >= -tail) && (x[n] <= tail);
+        float outu, theta, tomt, den;
+        if (INVERSE) {
+            const float t = xu[n] - l_h[n];
+            const float a = t * s[n] + in_h[n] * (delta[n] - d0[n]);
+            const float b = in_h[n] * d0[n] - t * s[n];
+            const float c = -delta[n] * t;
+            theta = rqs_inverse_root(a, b, c);
+            outu = theta * in_w[n] + l_w[n];
+            tomt = theta * (1.f - theta);
+            den = delta[n] + s[n] * tomt;
+        } else {
+            theta = (xu[n] - l_w[n]) * rw[n];
+            tomt = theta * (1.f - theta);
+            den = delta[n] + s[n] * tomt;
+            const float num = in_h[n] * (delta[n] * theta * theta + d0[n] * tomt);
+            outu = l_h[n] + num * rcp_nr(den);
+        }
+        const float omt = 1.f - theta;
+        const float dnum = delta[n] * delta[n] * (d1[n] * theta * theta + 2.f * delta[n] * tomt + d0[n] * omt * omt);
+        float l = kLn2 * (fast_lg2(dnum) - 2.f * fast_lg2(den));
+        if (INVERSE) l = -l;
+        y[n] = inside ? fmaf(outu, two_b, -tail) : x[n];
+        lad[n] = inside ? l : 0.f;
+    }
+}
+
+// one evaluation: lw / lh the logits, pd(i) the interior derivative parameters
 template <int K, bool INVERSE, typename PD>
 __host__ __device__ __forceinline__ void rqs_core(float x, const float (&lw)[K], const float (&lh)[K], PD pd,
                                                   float tail, float& y, float& lad,
                                                   float ud_first = NFB_BOUNDARY_UD, float ud_last = NFB_BOUNDARY_UD) {
-    const bool inside = (x >= -tail) && (x <= tail);
-    float mw = lw[0], mh = lh[0];
-#pragma unroll
-    for (int i = 1; i < K; ++i) {
-        mw = fmaxf(mw, lw[i]);
-        mh = fmaxf(mh, lh[i]);
-    }
-    float cw[K], ch[K];
-    float sw = 0.f, sh = 0.f;
-#pragma unroll
-    for (int i = 0; i < K; ++i) {
-        sw += fast_ex2(lw[i] - mw);
-        sh += fast_ex2(lh[i] - mh);
-        cw[i] = sw;
-        ch[i] = sh;
-    }
-    const float aw = (1.f - kMinBinWidth * K) * rcp_nr(sw);
-    const float ah = (1.f - kMinBinHeight * K) * rcp_nr(sh);
-    float kw[K + 1], kh[K + 1], ud[K + 1];
-    kw[0] = 0.f; kh[0] = 0.f; kw[K] = 1.f; kh[K] = 1.f;
-    ud[0] = ud_first; ud[K] = ud_last;
-#pragma unroll
-    for (int i = 0; i < K - 1; ++i) {
-        kw[i + 1] = fmaf(aw, cw[i], kMinBinWidth * (float)(i + 1));
-        kh[i + 1] = fmaf(ah, ch[i], kMinBinHeight * (float)(i + 1));
-        ud[i + 1] = pd(i);
-    }
-    const float two_b = 2.f * tail;
-    const float xu = fmaf(x, rcp_nr(two_b), 0.5f);
-    float l_w, r_w, l_h, r_h, ud0, ud1;
-    if (K == 8) {
-        const float* ks = INVERSE ? kh : kw;
-        const bool c1 = xu >= ks[4];
-        float a_w[5], a_h[5], a_d[5];
-#pragma unroll
-        for (int j = 0; j < 5; ++j) {
-            a_w[j] = c1 ? kw[4 + j] : kw[j];
-            a_h[j] = c1 ? kh[4 + j] : kh[j];
-            a_d[j] = c1 ? ud[4 + j] : ud[j];
-        }
-        const bool c2 = xu >= (INVERSE ? a_h[2] : a_w[2]);
-        float b_w[3], b_h[3], b_d[3];
-#pragma unroll
-        for (int j = 0; j < 3; ++j) {
-            b_w[j] = c2 ? a_w[2 + j] : a_w[j];
-            b_h[j] = c2 ? a_h[2 + j] : a_h[j];
-            b_d[j] = c2 ? a_d[2 + j] : a_d[j];
-        }
-        const bool c3 = xu >= (INVERSE ? b_h[1] : b_w[1]);
-        l_w = c3 ? b_w[1] : b_w[0]; r_w = c3 ? b_w[2] : b_w[1];
-        l_h = c3 ? b_h[1] : b_h[0]; r_h = c3 ? b_h[2] : b_h[1];
-        ud0 = c3 ? b_d[1] : b_d[0]; ud1 = c3 ? b_d[2] : b_d[1];
-    } else {
-        l_w = kw[0]; r_w = kw[1]; l_h = kh[0]; r_h = kh[1]; ud0 = ud[0]; ud1 = ud[1];
-#pragma unroll
-        for (int i = 1; i < K; ++i) {
-            if (xu >= (INVERSE ? kh[i] : kw[i])) {  // knot i <= x
-                l_w = kw[i]; r_w = kw[i + 1]; l_h = kh[i]; r_h = kh[i + 1]; ud0 = ud[i]; ud1 = ud[i + 1];
-            }
-        }
-    }
-    const float in_w = r_w - l_w, in_h = r_h - l_h;
-    const float d0 = kMinDerivative + softplus_f(ud0);
-    const float d1 = kMinDerivative + softplus_f(ud1);
-    const float rw = rcp_nr(in_w);
-    const float delta = in_h * rw;
-    const float s = d0 + d1 - 2.f * delta;
-    float outu, theta, tomt, den;
-    if (INVERSE) {
-        const float t = xu - l_h;
-        const float a = t * s + in_h * (delta - d0);
-        const float b = in_h * d0 - t * s;
-        const float c = -delta * t;
-        theta = rqs_inverse_root(a, b, c);
-        outu = theta * in_w + l_w;
-        tomt = theta * (1.f - theta);
-        den = delta + s * tomt;
-    } else {
-        theta = (xu - l_w) * rw;
-        tomt = theta * (1.f - theta);
-        den = delta + s * tomt;
-        const float num = in_h * (delta * theta * theta + d0 * tomt);
-        outu = l_h + num * rcp_nr(den);
-    }
-    const float omt = 1.f - theta;
-    const float dnum = delta * delta * (d1 * theta * theta + 2.f * delta * tomt + d0 * omt * omt);
-    float l = kLn2 * (fast_lg2(dnum) - 2.f * fast_lg2(den));
-    if (INVERSE) l = -l;
-    y = inside ? fmaf(outu, two_b, -tail) : x;
-    lad = inside ? l : 0.f;
+    const float xs[1] = {x};
+    float ys[1], ls[1];
+    rqs_core_lanes<1, K, INVERSE>(xs, [&lw](int, int i) { return lw[i]; }, [&lh](int, int i) { return lh[i]; },
+                                  [&pd](int, int i) { return pd(i); }, tail, ys, ls, ud_first, ud_last);
+    y = ys[0];
+    lad = ls[0];
 }
 
 // Param accessor: P(i) returns the i-th of the 3K-1 raw parameters [w(K) | h(K) | d(K-1)] of this
