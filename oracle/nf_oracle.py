@@ -490,16 +490,24 @@ def _chunk2(z):
 def affine_coupling_block(z, sd, p, L, direction):
     """flows/affine/coupling.py:253-267 (Split/AffineCoupling/Merge) ->
     AffineCoupling.forward :113-147 / .inverse :149-171; reshape.py:27-31,61-65."""
-    mode = L.get("split_mode", "channel")
-    smap = L.get("scale_map", "exp")
-    scale = L.get("scale", True)
     a, b = _chunk2(z)
-    z1, z2 = (a, b) if mode == "channel" else (b, a)
+    z1 = a if L.get("split_mode", "channel") == "channel" else b
     pm = p + "flows.1.param_map."
     if L.get("net", "mlp") == "mlp":
         param = mlp(z1, sd, pm, L.get("leaky", 0.0))
     else:
         param = convnet2d(z1, sd, pm, L.get("leaky", 0.0))
+    return affine_coupling_apply(z, param, L, direction)
+
+
+def affine_coupling_apply(z, param, L, direction):
+    """The coupling of affine_coupling_block given its conditioner's output `param` (AffineCoupling.forward /
+    .inverse after param_map)."""
+    mode = L.get("split_mode", "channel")
+    smap = L.get("scale_map", "exp")
+    scale = L.get("scale", True)
+    a, b = _chunk2(z)
+    z1, z2 = (a, b) if mode == "channel" else (b, a)
     red = tuple(range(1, z.ndim))
     if not scale:
         z2 = z2 + param if direction == "forward" else z2 - param
