@@ -627,20 +627,28 @@ int nfb_flow_log_prob_backward(nfb_flow_t* f, const float* x_dev, const float* g
                                float* log_q_dev /* optional out */, float* gx_dev /* optional out */,
                                float* const* grad_slots, void* stream);
 
-/* ---- sampling-direction backward of an all-affine or all-planar/radial stack (reverse_kld / reverse_alpha_div of
- * examples/real_nvp.ipynb, planar.ipynb) -- gradients of sum_r <g_x[r], x_r> + g_ld[r] log_det_r, with (x, log_det) =
- * nfb_flow_transform(f, NFB_FORWARD, z), w.r.t. z and every parameter, for stacks of MaskedAffineFlow, AffineConstFlow /
- * ActNorm, AffineCouplingBlock and Permute only, or of Planar and Radial only (any other stack, mixes of the two
- * families included: NFB_ERR_UNSUPPORTED).  z is the input that nfb_flow_transform was given.  A planar / radial stack
- * reduces each layer's row terms the same way, then takes the sums through u_hat(u, w), softplus(beta) and |alpha| in
- * one more launch (3 launches per chunk of rows + 1).  The affine call
- * recomputes the stack from z (the forward kernel's own arithmetic), walks the ops in reverse in one kernel, then reduces
+/* ---- sampling-direction backward of an all-affine, all-planar/radial or coupled-spline / LU stack (reverse_kld /
+ * reverse_alpha_div of examples/real_nvp.ipynb, planar.ipynb, a coupling NSF) -- gradients of
+ * sum_r <g_x[r], x_r> + g_ld[r] log_det_r, with (x, log_det) = nfb_flow_transform(f, NFB_FORWARD, z), w.r.t. z and every
+ * parameter, for stacks of MaskedAffineFlow, AffineConstFlow / ActNorm, AffineCouplingBlock and Permute only, of Planar
+ * and Radial only, or of CoupledRationalQuadraticSpline (num_bins 8) and LULinearPermute only (any other stack, mixes of
+ * these families and autoregressive blocks included: NFB_ERR_UNSUPPORTED).  z is the input that nfb_flow_transform was
+ * given.  A planar / radial stack reduces each layer's row terms the same way, then takes the sums through u_hat(u, w),
+ * softplus(beta) and |alpha| in one more launch (3 launches per chunk of rows + 1).  The affine call recomputes the
+ * stack from z (the forward kernel's own arithmetic), walks the ops in reverse in one kernel, then reduces
  * every Linear's weight and bias gradient in a fixed order (no atomics: two calls give identical bits).  Rows run in
  * chunks, so the workspace (nfb_flow_sampling_backward_workspace_bytes, -1 for an unsupported stack) stays below a fixed
  * bound; the number of launches does not depend on the number of layers.  A stack on the wide path (over 16 features or a
  * net wider than 128, see nfb_flow_add_masked_affine) recomputes each chunk layer by layer and back-propagates each layer
  * with GEMMs: its launches grow linearly with depth, and weight gradients summed by split-K GEMMs are not bitwise
  * reproducible from call to call.
+ * A coupled-spline / LU stack recomputes the sampling pass from z keeping every layer's input (the whole-stack
+ * persistent launch when the stack takes it, each unit writing its own slice, else layer by layer), then walks the
+ * layers last-to-first: an LU layer by two GEMMs (g_y = W^-T g_t; W's gradient -sum_rows g_y t^T) and the LU factor
+ * gradient, a coupled block by the inverse-spline adjoint of its transform columns, its conditioner's recompute and
+ * adjoint at the identity columns' output, and the inverse adjoint of the unconditional CDF.  It runs in the flow's
+ * own training buffers (those of nfb_flow_log_prob_backward): its workspace size is 0; its launches grow linearly with
+ * depth, and weight gradients summed by split-K GEMMs or atomics are not bitwise reproducible from call to call.
  * g_x / g_ld may be NULL (zero cotangent); g_z and individual slots may be NULL (not wanted).  grad_slots holds the
  * layers' slots in nfb_flow_grad_slot_numel order (a base's slots, if any, are not read); rows = 0 writes zeros. */
 int64_t nfb_flow_sampling_backward_workspace_bytes(const nfb_flow_t* f, int64_t rows);

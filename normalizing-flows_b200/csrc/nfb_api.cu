@@ -2847,19 +2847,16 @@ long long grad_slot_numel(const Layer& L, int s) {
     return (long long)L.n_id * (u == 2 ? L.K - 1 : L.K);
 }
 
-// backward of one spline layer: xp = the layer's input [rows x D], gy = gradient w.r.t. its output; writes the
-// gradient w.r.t. its input into gxp ([rows x D]) and the parameter gradients into `slots`.
-int rqs_layer_backward(nfb_flow* f, Layer& L, const float* xp, const float* gy, const float* glq, long long rows,
-                       float* gxp, float* const* slots, cudaStream_t st) {
+// The conditioner of a spline block (no context), recomputed on the forward's effective weights (L.pack), each weight
+// operand split to bf16 records before its GEMM.  x: [rows x D]; the conditioner reads all its columns (autoregressive)
+// or the identity columns x[:, id], gathered into f->tr_in (coupling).  Sets up d / r for the adjoint and leaves the
+// conditioner's output in f->tr_P.
+int conditioner_recompute(nfb_flow* f, Layer& L, const float* x, long long rows, nfb_resnet_ctx_desc_t& d,
+                          ResnetPass& r, cudaStream_t st) {
     const NetDesc& n = L.net;
-    const int D = L.D, H = n.H, T = L.n_tr, P = 3 * L.K - 1;
-    const bool coupled = L.kind == L_COUPLED_RQS;
-    NFB_CHECK(L.K == 8, NFB_ERR_UNSUPPORTED, "native backward: num_bins %d != 8", L.K);
-    // the conditioner's backward (no context) on the forward's effective weights (L.pack), each weight operand split
-    // to bf16 records before its GEMM
-    nfb_resnet_ctx_desc_t d{};
+    d = nfb_resnet_ctx_desc_t{};
     d.net = {n.in, n.H, n.out, n.nb, n.w0, n.b0, n.m0, n.wb.data(), n.bb.data(), n.mb.data(), n.wf, n.bf, n.mf};
-    ResnetPass r{&d, rows, {f->err.as<int>(), st, &f->tr_wpack, &f->launches}};
+    r = ResnetPass{&d, rows, {f->err.as<int>(), st, &f->tr_wpack, &f->launches}};
     r.w0 = L.pack.w0; r.wf = L.pack.wf; r.wb = L.pack.wb;
     Carver c;
     resnet_layout(&d, rows, c, r.ws, false);
@@ -2868,18 +2865,43 @@ int rqs_layer_backward(nfb_flow* f, Layer& L, const float* xp, const float* gy, 
     resnet_layout(&d, rows, c, r.ws, false);
     NFB_TRY(f->tr_P.reserve((size_t)rows * n.out * 4));
     NFB_TRY(f->tr_gP.reserve((size_t)rows * n.out * 4));
-    float* Pm = f->tr_P.as<float>();
-    float* gP = f->tr_gP.as<float>();
-    // conditioner input: all columns (autoregressive) or the gathered identity columns (coupling)
-    const float* in = xp;
-    if (coupled) {
+    const float* in = x;
+    if (L.kind == L_COUPLED_RQS) {
         NFB_TRY(f->tr_in.reserve((size_t)rows * L.n_id * 4));
         NFB_TRY(f->tr_gin.reserve((size_t)rows * L.n_id * 4));
-        NFB_TRY(launch_gather_cols_ld(xp, D, f->tr_in.as<float>(), L.n_id, L.id_idx.as<int>(), rows, st));
+        NFB_TRY(launch_gather_cols_ld(x, L.D, f->tr_in.as<float>(), L.n_id, L.id_idx.as<int>(), rows, st));
         in = f->tr_in.as<float>();
     }
     NFB_TRY(resnet_recompute(r, in, nullptr));
-    NFB_TRY(r.g.w(fwd_args(r.ws.h[n.nb], H, 0, r.wf, n.bf, Pm, rows, n.out, H)));
+    return r.g.w(fwd_args(r.ws.h[n.nb], n.H, 0, r.wf, n.bf, f->tr_P.as<float>(), rows, n.out, n.H));
+}
+
+// The coupling block's conditioner adjoint from the gradient on its output (f->tr_gP): weight gradients into `slots`
+// (each Linear's weight and bias interleaved: w0, b0, w_blocks..., wf, bf), and the data gradient of the identity
+// columns (W0 read unpacked) scatter-added into g[:, id].
+int coupled_conditioner_adjoint(nfb_flow* f, Layer& L, const ResnetPass& r, long long rows, float* const* slots,
+                                float* g, cudaStream_t st) {
+    const Slots g_w(slots, 2), g_b(slots + 1, 2);
+    NFB_TRY(resnet_adjoint(r, nullptr, f->tr_gP.as<float>(), false, nullptr, nullptr, g_w, g_b, {}, {}));
+    NFB_TRY(r.g(dgrad_args(r.ws.ga, r.w0, f->tr_gin.as<float>(), rows, L.n_id, L.net.H)));
+    NFB_TRY(launch_scatter_cols(f->tr_gin.as<float>(), g, L.id_idx.as<int>(), rows, L.n_id, L.D, 1, st));
+    f->launches++;
+    return NFB_OK;
+}
+
+// backward of one spline layer: xp = the layer's input [rows x D], gy = gradient w.r.t. its output; writes the
+// gradient w.r.t. its input into gxp ([rows x D]) and the parameter gradients into `slots`.
+int rqs_layer_backward(nfb_flow* f, Layer& L, const float* xp, const float* gy, const float* glq, long long rows,
+                       float* gxp, float* const* slots, cudaStream_t st) {
+    const NetDesc& n = L.net;
+    const int D = L.D, T = L.n_tr, P = 3 * L.K - 1;
+    const bool coupled = L.kind == L_COUPLED_RQS;
+    NFB_CHECK(L.K == 8, NFB_ERR_UNSUPPORTED, "native backward: num_bins %d != 8", L.K);
+    nfb_resnet_ctx_desc_t d;
+    ResnetPass r;
+    NFB_TRY(conditioner_recompute(f, L, xp, rows, d, r, st));
+    float* Pm = f->tr_P.as<float>();
+    float* gP = f->tr_gP.as<float>();
     // spline element backward -> gP, gxp (transformed columns)
     NFB_TRY(launch_spline_bwd_rows(xp, D, Pm, gy, glq, coupled ? L.tr_idx.as<int>() : nullptr, rows, T, L.K, L.tail,
                                    L.wh_scale, gP, gxp, st));
@@ -2894,16 +2916,11 @@ int rqs_layer_backward(nfb_flow* f, Layer& L, const float* xp, const float* gy, 
         NFB_TRY(launch_split_table(gtab, L.n_id, slots[2 * nlin], slots[2 * nlin + 1], slots[2 * nlin + 2], st));
         f->launches += 3;
     }
-    // the slots interleave each Linear's weight and bias gradients: w0, b0, w_blocks..., wf, bf
-    const Slots g_w(slots, 2), g_b(slots + 1, 2);
-    if (!coupled)   // gxp += the conditioner's data gradient (in place)
+    if (!coupled) {  // gxp += the conditioner's data gradient (in place)
+        const Slots g_w(slots, 2), g_b(slots + 1, 2);
         return resnet_adjoint(r, nullptr, gP, false, gxp, nullptr, g_w, g_b, {}, {}, true);
-    NFB_TRY(resnet_adjoint(r, nullptr, gP, false, nullptr, nullptr, g_w, g_b, {}, {}));
-    // the identity columns' data gradient (W0 read unpacked), scatter-added into gxp
-    NFB_TRY(r.g(dgrad_args(r.ws.ga, r.w0, f->tr_gin.as<float>(), rows, L.n_id, H)));
-    NFB_TRY(launch_scatter_cols(f->tr_gin.as<float>(), gxp, L.id_idx.as<int>(), rows, L.n_id, D, 1, st));
-    f->launches++;
-    return NFB_OK;
+    }
+    return coupled_conditioner_adjoint(f, L, r, rows, slots, gxp, st);
 }
 
 // backward of LULinearPermute (density direction x' = W z[:, perm] + b): gxp = gradient w.r.t. x'; writes gradient
@@ -3446,7 +3463,7 @@ int affine_only_group(nfb_flow* f, Group** out, const char* who) {
     NFB_CHECK(f && f->finalized, NFB_ERR_STATE, "flow not finalized");
     NFB_CHECK(f->groups.size() == 1 && f->groups[0].kind == G_AFFINE, NFB_ERR_UNSUPPORTED,
               "%s backward: the stack must be affine-family layers only%s", who,
-              who[0] == 's' ? ", or planar / radial layers only" : "");
+              who[0] == 's' ? ", planar / radial layers only, or coupled splines / LULinearPermute only" : "");
     *out = &f->groups[0];
     return plan_affine_bwd(f, **out);
 }
@@ -3509,6 +3526,175 @@ int affine_entry_checks(const char* who, nfb_flow* f, Group& g, const float* in,
     return NFB_OK;
 }
 
+// ---- sampling-direction backward of a coupled-spline / LULinearPermute stack ----------------------------------------
+// Every layer a CoupledRationalQuadraticSpline (no context; num_bins 8, the limit of the spline adjoint kernels) or an
+// LULinearPermute (D <= 64): the coupled blocks fused or not, the LU maps paired with the block before them or alone.
+bool coupled_lu_stack(const nfb_flow* f) {
+    if (!f || !f->finalized || f->layers.empty()) return false;
+    for (auto& Lp : f->layers)
+        if (!(Lp->kind == L_LU || (Lp->kind == L_COUPLED_RQS && Lp->K == 8))) return false;
+    return true;
+}
+
+// LULinearPermute, sampling direction: t = W^-1 (y - b) = y Ws^T + bs, x = t[:, inv_perm], log_det = -sum log diag.
+// Given g (the cotangent of x) and xin (= y): g_t = g[:, perm], g_y = g_t Ws -> gin; W's gradient is
+// -W^-T g_t t^T = -sum_rows g_y t^T, b's is -colsum(g_y), and -sum(g_ld) is the cotangent of log|det W|: the sums enter
+// lu_param_bwd_kernel negated.  gld_sum: device scalar sum of g_ld; scratch: 64 + 64 x 64 floats (b's sums, dW).
+int lu_sampling_backward(nfb_flow* f, Layer& L, const float* xin, const float* g, const float* gld_sum, long long rows,
+                         float* gin, float* const* slots, float* scratch, cudaStream_t st) {
+    const int D = L.D;
+    NFB_TRY(f->tr_zp.reserve((size_t)rows * D * 4));
+    NFB_TRY(f->tr_gzp.reserve((size_t)rows * D * 4));
+    float* t = f->tr_zp.as<float>();
+    float* gt = f->tr_gzp.as<float>();
+    const GemmRun gr{f->err.as<int>(), st, nullptr, &f->launches};
+    NFB_TRY(launch_gather_cols(g, gt, L.lu_perm.as<int>(), rows, D, 1, st));
+    f->launches++;
+    GemmTcArgs a{};
+    a.A = gt; a.lda = D; a.B = L.lu_Ws.as<float>(); a.ldb = D; a.b_mn = 1; a.C = gin; a.ldc = D; a.M = rows; a.N = D; a.K = D;
+    NFB_TRY(gr(a));
+    if (slots[0] || slots[1] || slots[2]) {
+        NFB_TRY(launch_linear(xin, D, nullptr, L.lu_Ws.as<float>(), L.lu_bs.as<float>(), nullptr, 0, t, D, rows, D, D, 0, 0,
+                              0.f, st));
+        f->launches++;
+        float* dW = scratch + 64;
+        GemmTcArgs w{};
+        w.A = gin; w.lda = D; w.a_mn = 1; w.B = t; w.ldb = D; w.b_mn = 1; w.C = dW; w.ldc = D; w.M = D; w.N = D; w.K = rows;
+        NFB_TRY(gr(w));
+        NFB_TRY(launch_lu_param_bwd(dW, L.lu.lower_entries, L.lu.upper_entries, L.lu.unconstrained_upper_diag, L.lu.eps, D,
+                                    gld_sum, slots[0], slots[1], slots[2], st, 1));
+        f->launches++;
+    }
+    if (slots[3]) {
+        NFB_CUDA(cudaMemsetAsync(scratch, 0, (size_t)D * 4, st));
+        NFB_TRY(launch_colsum(gin, D, rows, D, scratch, st));
+        NFB_TRY(launch_axpy(scratch, -1.f, slots[3], D, 0, st));
+        f->launches += 3;
+    }
+    return NFB_OK;
+}
+
+// Coupling block, sampling direction (Coupling.inverse): x_id = the unconditional CDF's inverse at z_id, the conditioner
+// reads x_id, x_tr = the inverse spline at z_tr with its per-row parameters.  zin: the block's input z, xout: its output x,
+// g: the cotangent of x (its identity columns are updated in place), gld: of the log-det; writes g_z into gin.
+int coupled_sampling_backward(nfb_flow* f, Layer& L, const float* zin, const float* xout, float* g, const float* gld,
+                              long long rows, float* gin, float* const* slots, float* gtab, cudaStream_t st) {
+    const int D = L.D, P = 3 * L.K - 1, nlin = 2 + 2 * L.net.nb;
+    nfb_resnet_ctx_desc_t d;
+    ResnetPass r;
+    NFB_TRY(conditioner_recompute(f, L, xout, rows, d, r, st));
+    // transform columns: inverse-spline adjoint -> gP, gin[:, tr]
+    NFB_TRY(launch_spline_bwd_rows(zin, D, f->tr_P.as<float>(), g, gld, L.tr_idx.as<int>(), rows, L.n_tr, L.K, L.tail,
+                                   L.wh_scale, f->tr_gP.as<float>(), gin, st, 1));
+    f->launches++;
+    // the conditioner's weights, and g[:, id] += its data gradient
+    NFB_TRY(coupled_conditioner_adjoint(f, L, r, rows, slots, g, st));
+    // identity columns: the unconditional CDF's inverse adjoint on the whole cotangent of x_id -> gin[:, id], table
+    NFB_CUDA(cudaMemsetAsync(gtab, 0, (size_t)L.n_id * P * 4, st));
+    NFB_TRY(launch_spline_bwd_shared(zin, D, L.uncond.as<float>(), g, gld, L.id_idx.as<int>(), rows, L.n_id, L.K, L.tail,
+                                     gtab, gin, st, 1));
+    NFB_TRY(launch_split_table(gtab, L.n_id, slots[2 * nlin], slots[2 * nlin + 1], slots[2 * nlin + 2], st));
+    f->launches += 3;
+    return NFB_OK;
+}
+
+// Recompute, then walk the layers last-to-first.  The recompute keeps each layer's input and, for a coupled block, its
+// output (the conditioner reads x_id).  Whole-stack plan (f->fwd_n > 0): one launch of the persistent kernel, unit u
+// ([LU map of layer fwd_units[u].first, if any] + block fwd_units[u].second) reading store[u] and writing store[u + 1];
+// a block behind an LU map gets its input by that map again (launch_linear on lu_Ws / lu_bs), a trailing LU reads
+// store[fwd_n].  Otherwise layer i runs on its own from store[i] into store[i + 1], as nfb_flow_transform runs it.
+// Workspace: the flow's training buffers (tr_*).
+int coupled_lu_sampling_backward(nfb_flow* f, const float* z, const float* g_x, const float* g_ld, int64_t rows,
+                                 float* g_z, float* const* grad_slots, cudaStream_t st) {
+    NFB_CHECK(rows >= 0, NFB_ERR_ARG, "rows < 0");
+    NFB_CHECK(rows == 0 || z, NFB_ERR_ARG, "null z");
+    const int n = (int)f->layers.size(), D = f->D;
+    std::vector<int> off(n + 1, 0);
+    for (int i = 0; i < n; ++i) off[i + 1] = off[i] + grad_slots_of(*f->layers[i]);
+    std::vector<float*> slots(off[n], nullptr);
+    if (grad_slots) std::copy(grad_slots, grad_slots + off[n], slots.begin());
+    f->launches = 0;
+    if (rows == 0) {   // zero gradients
+        for (int i = 0; i < off[n]; ++i)
+            if (slots[i]) NFB_CUDA(cudaMemsetAsync(slots[i], 0, (size_t)nfb_flow_grad_slot_numel(f, i) * 4, st));
+        return NFB_OK;
+    }
+    const size_t ZS = (size_t)rows * D;
+    const bool whole = f->fwd_n > 0;
+    const int n_store = whole ? f->fwd_n + 1 : n + 1;
+    int max_id = 0;
+    for (auto& Lp : f->layers) max_id = std::max(max_id, Lp->n_id);
+    NFB_TRY(ensure_ws(f, rows));
+    NFB_TRY(f->tr_store.reserve((size_t)n_store * ZS * 4));
+    NFB_TRY(f->tr_glq.reserve((size_t)rows * 4 + 64));
+    NFB_TRY(f->tr_g0.reserve(ZS * 4));
+    NFB_TRY(f->tr_g1.reserve(ZS * 4));
+    NFB_TRY(f->tr_xp.reserve(ZS * 4));
+    NFB_TRY(f->tr_small.reserve((size_t)(64 + 64 * 64 + 64 + (size_t)max_id * 23) * 4));
+    float* store = f->tr_store.as<float>();
+    float* lu_scratch = f->tr_small.as<float>();              // [64] LU bias sums, then [64 x 64] dW
+    float* gld_sum = lu_scratch + 64 + 64 * 64;
+    float* gtab = gld_sum + 64;
+    // ---- recompute ----
+    NFB_CUDA(cudaMemcpyAsync(store, z, ZS * 4, cudaMemcpyDeviceToDevice, st));
+    float* ld = f->logq.as<float>();   // (the recompute's log-det is not used)
+    NFB_TRY(launch_fill(ld, rows, 0.f, st));
+    f->launches++;
+    std::vector<const float*> src(n), out(n, nullptr);
+    std::vector<int> lu_before(n, -1);
+    if (whole) {
+        NFB_TRY(launch_fused_stack(f, store, store + ZS, ld, rows, st, 1, (long long)ZS));
+        for (int u = 0; u < f->fwd_n; ++u) {
+            const int lu = f->fwd_units[u].first, b = f->fwd_units[u].second;
+            if (lu >= 0) src[lu] = store + u * ZS;
+            src[b] = store + u * ZS;
+            lu_before[b] = lu;
+            out[b] = store + (u + 1) * ZS;
+        }
+        if (f->fwd_trailing_lu >= 0) src[f->fwd_trailing_lu] = store + (size_t)f->fwd_n * ZS;
+    } else {
+        for (int i = 0; i < n; ++i) {
+            Layer& L = *f->layers[i];
+            src[i] = store + i * ZS;
+            out[i] = store + (i + 1) * ZS;
+            float* o = store + (i + 1) * ZS;
+            if (L.kind == L_COUPLED_RQS && L.fused.ok)
+                NFB_TRY(launch_fused_layer(f, L, nullptr, src[i], o, ld, rows, 1, st, 1));
+            else
+                NFB_TRY(apply_layer_generic(f, L, NFB_FORWARD, src[i], o, ld, rows, 1, st));
+        }
+    }
+    // ---- backward ----
+    float* g = f->tr_g0.as<float>();
+    float* g2 = f->tr_g1.as<float>();
+    if (g_x) NFB_CUDA(cudaMemcpyAsync(g, g_x, ZS * 4, cudaMemcpyDeviceToDevice, st));
+    else NFB_CUDA(cudaMemsetAsync(g, 0, ZS * 4, st));
+    const float* gld = g_ld;
+    if (!gld) {
+        NFB_TRY(launch_fill(f->tr_glq.as<float>(), rows, 0.f, st));
+        gld = f->tr_glq.as<float>();
+    }
+    NFB_CUDA(cudaMemsetAsync(gld_sum, 0, 4, st));
+    NFB_TRY(launch_colsum(gld, 1, rows, 1, gld_sum, st));
+    f->launches += 3;
+    for (int i = n - 1; i >= 0; --i) {
+        Layer& L = *f->layers[i];
+        const float* xin = src[i];
+        if (lu_before[i] >= 0) {   // the block's input: the LU map in front of it, again
+            NFB_TRY(apply_layer_generic(f, *f->layers[lu_before[i]], NFB_FORWARD, src[i], f->tr_xp.as<float>(), nullptr,
+                                        rows, 1, st));
+            xin = f->tr_xp.as<float>();
+        }
+        if (L.kind == L_LU)
+            NFB_TRY(lu_sampling_backward(f, L, xin, g, gld_sum, rows, g2, slots.data() + off[i], lu_scratch, st));
+        else
+            NFB_TRY(coupled_sampling_backward(f, L, xin, out[i], g, gld, rows, g2, slots.data() + off[i], gtab, st));
+        std::swap(g, g2);
+    }
+    if (g_z) NFB_CUDA(cudaMemcpyAsync(g_z, g, ZS * 4, cudaMemcpyDeviceToDevice, st));
+    return NFB_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -3517,6 +3703,7 @@ int64_t nfb_flow_sampling_backward_workspace_bytes(const nfb_flow_t* fc, int64_t
     nfb_flow* f = const_cast<nfb_flow*>(fc);
     Group* g = planar_only_group(f);
     if (g) return rows < 0 ? -1 : (int64_t)planar_bwd_ws_bytes(*g, planar_bwd_chunk_rows(*g, rows));
+    if (coupled_lu_stack(f)) return rows < 0 ? -1 : 0;   // (the flow's own training buffers serve)
     if (rows < 0 || affine_only_group(f, &g, "sampling") != NFB_OK) return -1;
     return (int64_t)affine_bwd_ws_bytes(f, *g, affine_bwd_chunk_rows(f, *g, rows));
 }
@@ -3525,6 +3712,7 @@ int nfb_flow_sampling_backward(nfb_flow_t* f, const float* z, const float* g_x, 
                                void* ws, int64_t ws_bytes, float* g_z, float* const* grad_slots, void* stream) {
     if (Group* pg = planar_only_group(f))
         return planar_sampling_backward(f, *pg, z, g_x, g_ld, rows, ws, ws_bytes, g_z, grad_slots, S(stream));
+    if (coupled_lu_stack(f)) return coupled_lu_sampling_backward(f, z, g_x, g_ld, rows, g_z, grad_slots, S(stream));
     Group* gp = nullptr;
     NFB_TRY(affine_only_group(f, &gp, "sampling"));
     long long R = 0;

@@ -21,7 +21,17 @@ constexpr int kP = 23;  // 3K - 1 for K = 8
 
 // One thread per (row, feature) element, 256 consecutive elements per block; the block's 256 x 23 parameter slab is
 // contiguous in memory: staged through shared memory with coalesced loads, read at the conflict-free odd stride 23,
-// gradients written back the same way.
+// gradients written back the same way.  INV: the inverse spline of the sampling direction (rqs_inv_fwd_bwd): xin is its
+// input z, g_out the cotangent of its output x, gx receives g_z.
+template <int K, typename T>
+__device__ __forceinline__ void rqs_dir_fwd_bwd(bool inv, T x, const T (&lw)[K], const T (&lh)[K], const T (&ud)[K - 1],
+                                                T tail, T gy, T glad, T& y, T& lad, T& gx, T (&glw)[K], T (&glh)[K],
+                                                T (&gud)[K - 1]) {
+    if (inv) rqs_inv_fwd_bwd<K, T>(x, lw, lh, ud, tail, gy, glad, y, lad, gx, glw, glh, gud);
+    else rqs_fwd_bwd<K, T>(x, lw, lh, ud, tail, gy, glad, y, lad, gx, glw, glh, gud);
+}
+
+template <bool INV>
 __global__ void __launch_bounds__(256) spline_bwd_rows_kernel(
     const float* __restrict__ xin, int ldx, const float* __restrict__ params, const float* __restrict__ g_out,
     const float* __restrict__ g_lq, const int* __restrict__ fidx, long long rows, int T, float tail, float wh_scale,
@@ -47,8 +57,8 @@ __global__ void __launch_bounds__(256) spline_bwd_rows_kernel(
 #pragma unroll
         for (int k = 0; k < 7; ++k) ud[k] = p[16 + k];
         float y, lad, g;
-        rqs_fwd_bwd<8, float>(xin[row * ldx + col], lw, lh, ud, tail, g_out[row * ldx + col], g_lq[row], y, lad, g, glw,
-                              glh, gud);
+        rqs_dir_fwd_bwd<8, float>(INV, xin[row * ldx + col], lw, lh, ud, tail, g_out[row * ldx + col], g_lq[row], y, lad,
+                                  g, glw, glh, gud);
         gx[row * ldx + col] = g;
 #pragma unroll
         for (int k = 0; k < 8; ++k) { glw[k] *= s2; glh[k] *= s2; }
@@ -67,18 +77,20 @@ __global__ void __launch_bounds__(256) spline_bwd_rows_kernel(
 }
 int launch_spline_bwd_rows(const float* xin, int ldx, const float* params, const float* g_out, const float* g_lq,
                            const int* fidx, long long rows, int T, int K, float tail, float wh_scale, float* g_params,
-                           float* gx, cudaStream_t st) {
+                           float* gx, cudaStream_t st, int inverse) {
     NFB_CHECK(K == 8, NFB_ERR_UNSUPPORTED, "spline backward: num_bins %d != 8", K);
     const long long n = rows * T;
     if (n == 0) return NFB_OK;
-    spline_bwd_rows_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(xin, ldx, params, g_out, g_lq, fidx, rows, T,
-                                                                        tail, wh_scale, g_params, gx);
+    (inverse ? spline_bwd_rows_kernel<true> : spline_bwd_rows_kernel<false>)<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
+        xin, ldx, params, g_out, g_lq, fidx, rows, T, tail, wh_scale, g_params, gx);
     NFB_LAUNCH_CHECK();
     return NFB_OK;
 }
 
 // Unconditional CDF of the identity features: table [n_id][23] shared by every row.  grid = (row chunks, n_id);
 // each thread walks rows of its chunk for ONE feature and keeps 23 partial sums; block reduce, 23 atomics per block.
+// INV: the inverse CDF of the sampling direction (see spline_bwd_rows_kernel).
+template <bool INV>
 __global__ void __launch_bounds__(256) spline_bwd_shared_kernel(
     const float* __restrict__ xin, int ldx, const float* __restrict__ table, const float* __restrict__ g_out,
     const float* __restrict__ g_lq, const int* __restrict__ fidx, long long rows, long long rows_per_block, float tail,
@@ -98,8 +110,8 @@ __global__ void __launch_bounds__(256) spline_bwd_shared_kernel(
     const long long r1 = r0 + rows_per_block < rows ? r0 + rows_per_block : rows;
     for (long long row = r0 + threadIdx.x; row < r1; row += 256) {
         float glw[8], glh[8], gud[7], y, lad, g;
-        rqs_fwd_bwd<8, float>(xin[row * ldx + col], lw, lh, ud, tail, g_out[row * ldx + col], g_lq[row], y, lad, g, glw,
-                              glh, gud);
+        rqs_dir_fwd_bwd<8, float>(INV, xin[row * ldx + col], lw, lh, ud, tail, g_out[row * ldx + col], g_lq[row], y, lad,
+                                  g, glw, glh, gud);
         gx[row * ldx + col] = g;
 #pragma unroll
         for (int k = 0; k < 8; ++k) { acc[k] += glw[k]; acc[8 + k] += glh[k]; }
@@ -122,12 +134,13 @@ __global__ void __launch_bounds__(256) spline_bwd_shared_kernel(
 }
 int launch_spline_bwd_shared(const float* xin, int ldx, const float* table, const float* g_out, const float* g_lq,
                              const int* fidx, long long rows, int n_id, int K, float tail, float* g_table, float* gx,
-                             cudaStream_t st) {
+                             cudaStream_t st, int inverse) {
     NFB_CHECK(K == 8, NFB_ERR_UNSUPPORTED, "spline backward: num_bins %d != 8", K);
     if (rows == 0 || n_id == 0) return NFB_OK;
     const long long rpb = 2048;
     dim3 grid((unsigned)((rows + rpb - 1) / rpb), (unsigned)n_id);
-    spline_bwd_shared_kernel<<<grid, 256, 0, st>>>(xin, ldx, table, g_out, g_lq, fidx, rows, rpb, tail, g_table, gx);
+    (inverse ? spline_bwd_shared_kernel<true> : spline_bwd_shared_kernel<false>)<<<grid, 256, 0, st>>>(
+        xin, ldx, table, g_out, g_lq, fidx, rows, rpb, tail, g_table, gx);
     NFB_LAUNCH_CHECK();
     return NFB_OK;
 }
@@ -441,6 +454,8 @@ int launch_diag_gauss_bwd(const float* z, const float* loc, const float* ls, con
 // LULinearPermute parameters from dW (gradient of W = L U), flows/mixing.py:402-412 (L unit-lower from
 // lower_entries, U = upper_entries + diag(softplus(unconstrained_upper_diag) + eps)) and :514-532
 // (logabsdet = sum log diag; `g_logdet` = sum over rows of the upstream gradient on it).  One block, n <= 64.
+// NEG: dW and g_logdet enter negated (the sampling direction's map W^-1 (y - b) and its log-det -logabsdet).
+template <bool NEG>
 __global__ void lu_param_bwd_kernel(const float* __restrict__ dW, const float* __restrict__ lower_e,
                                     const float* __restrict__ upper_e, const float* __restrict__ udiag, float eps, int n,
                                     const float* __restrict__ g_logdet, float* __restrict__ g_lower,
@@ -459,7 +474,7 @@ __global__ void lu_param_bwd_kernel(const float* __restrict__ dW, const float* _
             u = (d > 20.f ? d : log1pf(expf(d))) + eps;
         }
         if (c > r) u = upper_e[r * n - r * (r + 1) / 2 + (c - r - 1)];
-        L[i] = l; U[i] = u; G[i] = dW[i];
+        L[i] = l; U[i] = u; G[i] = NEG ? -dW[i] : dW[i];
     }
     __syncthreads();
     for (int i = threadIdx.x; i < n * n; i += blockDim.x) {
@@ -476,16 +491,18 @@ __global__ void lu_param_bwd_kernel(const float* __restrict__ dW, const float* _
             } else if (g_udiag) {
                 const float d = udiag[r];
                 const float sg = d > 20.f ? 1.f : 1.f / (1.f + expf(-d));
-                g_udiag[r] = (acc + (g_logdet ? *g_logdet : 0.f) / U[r * n + r]) * sg;
+                const float gld = g_logdet ? (NEG ? -*g_logdet : *g_logdet) : 0.f;
+                g_udiag[r] = (acc + gld / U[r * n + r]) * sg;
             }
         }
     }
 }
 int launch_lu_param_bwd(const float* dW, const float* lower_e, const float* upper_e, const float* udiag, float eps,
-                        int n, const float* g_logdet, float* g_lower, float* g_upper, float* g_udiag, cudaStream_t st) {
+                        int n, const float* g_logdet, float* g_lower, float* g_upper, float* g_udiag, cudaStream_t st,
+                        int negate) {
     NFB_CHECK(n >= 1 && n <= 64, NFB_ERR_UNSUPPORTED, "LULinearPermute backward: features %d > 64", n);
-    lu_param_bwd_kernel<<<1, 256, (size_t)3 * n * n * sizeof(float), st>>>(dW, lower_e, upper_e, udiag, eps, n, g_logdet,
-                                                                           g_lower, g_upper, g_udiag);
+    (negate ? lu_param_bwd_kernel<true> : lu_param_bwd_kernel<false>)<<<1, 256, (size_t)3 * n * n * sizeof(float), st>>>(
+        dW, lower_e, upper_e, udiag, eps, n, g_logdet, g_lower, g_upper, g_udiag);
     NFB_LAUNCH_CHECK();
     return NFB_OK;
 }

@@ -278,15 +278,16 @@ int launch_gemm_pack_b(const float* B, long long ldb, int b_mn, long long N, lon
 // ---- training pass: element-wise / reduction kernels (nfb_backward.cu) ----
 int launch_spline_bwd_rows(const float* xin, int ldx, const float* params, const float* g_out, const float* g_lq,
                            const int* fidx, long long rows, int T, int K, float tail, float wh_scale, float* g_params,
-                           float* gx, cudaStream_t st);
+                           float* gx, cudaStream_t st, int inverse = 0);
 int launch_spline_bwd_shared(const float* xin, int ldx, const float* table, const float* g_out, const float* g_lq,
                              const int* fidx, long long rows, int n_id, int K, float tail, float* g_table, float* gx,
-                             cudaStream_t st);
+                             cudaStream_t st, int inverse = 0);
 int launch_colsum(const float* G, long long ld, long long M, int N, float* out, cudaStream_t st);
 int launch_diag_gauss_bwd(const float* z, const float* loc, const float* ls, const float* g_lq, long long rows, int d,
                           float* gz, float* t_loc, float* t_ls, cudaStream_t st);
 int launch_lu_param_bwd(const float* dW, const float* lower_e, const float* upper_e, const float* udiag, float eps,
-                        int n, const float* g_logdet, float* g_lower, float* g_upper, float* g_udiag, cudaStream_t st);
+                        int n, const float* g_logdet, float* g_lower, float* g_upper, float* g_udiag, cudaStream_t st,
+                        int negate = 0);
 int launch_scatter_cols(const float* in, float* out, const int* idx, long long rows, int n_in, int ld_out, int accumulate,
                         cudaStream_t st);
 int launch_gather_cols_ld(const float* in, int ld_in, float* out, int n_out, const int* idx, long long rows,

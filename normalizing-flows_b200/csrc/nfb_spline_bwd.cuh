@@ -208,6 +208,20 @@ __host__ __device__ inline void rqs_fwd_bwd(T x, const T (&lw)[K], const T (&lh)
     for (int i = 0; i < K - 1; ++i) gud[i] = gudk[i + 1];
 }
 
+// The same layout, inverse element: z in, (x, ld) out, gz = g_z given the cotangents (gx_out, gld) of (x, ld).
+template <int K, typename T>
+__host__ __device__ inline void rqs_inv_fwd_bwd(T z, const T (&lw)[K], const T (&lh)[K], const T (&ud)[K - 1], T tail,
+                                                T gx_out, T gld, T& x, T& ld, T& gz, T (&glw)[K], T (&glh)[K],
+                                                T (&gud)[K - 1]) {
+    T udk[K + 1], gudk[K + 1];
+    udk[0] = (T)NFB_BOUNDARY_UD; udk[K] = (T)NFB_BOUNDARY_UD;
+#pragma unroll
+    for (int i = 0; i < K - 1; ++i) udk[i + 1] = ud[i];
+    rqs_inverse_adjoint<K, T>(K, z, lw, lh, udk, tail, gx_out, gld, false, x, ld, gz, glw, glh, gudk);
+#pragma unroll
+    for (int i = 0; i < K - 1; ++i) gud[i] = gudk[i + 1];
+}
+
 // One element of the stand-alone splines (nfb_rqs_spline / nfb_rqs_spline_tails), on its raw parameter record
 // p[2K + nd] = [widths(K) | heights(K) | derivatives(nd)], with the knot layout of rqs_eval_dyn (nfb_spline.cuh):
 //   nd = K - 1: linear tails, boundary knots pinned to the constant of utils/splines.py:35-38;

@@ -176,17 +176,11 @@ def grad_slot_tensors(model):
     from ._standalone import sampling_slot_tensors
     out = []
     for layer in model.flows:
-        if getattr(layer, "_affine_family", False):
+        if getattr(layer, "_affine_family", False) or isinstance(layer, (ns.CoupledRationalQuadraticSpline,
+                                                                          mixing.LULinearPermute)):
             out += sampling_slot_tensors([layer])
         elif isinstance(layer, ns.AutoregressiveRationalQuadraticSpline):
             out += _net_slots(layer.mprqat.autoregressive_net)
-        elif isinstance(layer, ns.CoupledRationalQuadraticSpline):
-            u = layer.prqct.unconditional_transform
-            out += _net_slots(layer.prqct.transform_net)
-            out += [u.unnormalized_widths, u.unnormalized_heights, u.unnormalized_derivatives]
-        elif isinstance(layer, mixing.LULinearPermute):
-            lin = layer.linear
-            out += [lin.lower_entries, lin.upper_entries, lin.unconstrained_upper_diag, lin.bias]
         else:
             return None
     return out + model.q0._native_tensors()

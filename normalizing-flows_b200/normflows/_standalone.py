@@ -109,13 +109,22 @@ def apply_sampling(module, z, context=None):
 
 
 def sampling_slot_tensors(layers):
-    """The tensors behind the gradient slots of an affine-family or planar-family stack (include/nfb200.h
-    nfb_flow_grad_slot_numel): each layer's parameters in registration order; an AffineConstFlow s / t registered as a
-    buffer keeps its slot."""
-    from .flows import affine, mixing, planar, radial
+    """The tensors behind the gradient slots of an affine-family, planar-family or coupled-spline / LU stack
+    (include/nfb200.h nfb_flow_grad_slot_numel): an affine or planar layer's parameters in registration order (an
+    AffineConstFlow s / t registered as a buffer keeps its slot); a coupled spline's conditioner Linears (weight, bias)
+    then its unconditional widths, heights, derivatives; an LULinearPermute's lower, upper, diagonal, bias."""
+    from ._autograd import _net_slots
+    from .flows import affine, mixing, neural_spline, planar, radial
     out = []
     for layer in layers:
-        if isinstance(layer, planar.Planar):
+        if isinstance(layer, neural_spline.CoupledRationalQuadraticSpline):
+            u = layer.prqct.unconditional_transform
+            out += _net_slots(layer.prqct.transform_net)
+            out += [u.unnormalized_widths, u.unnormalized_heights, u.unnormalized_derivatives]
+        elif isinstance(layer, mixing.LULinearPermute):
+            lin = layer.linear
+            out += [lin.lower_entries, lin.upper_entries, lin.unconstrained_upper_diag, lin.bias]
+        elif isinstance(layer, planar.Planar):
             out += [layer.u, layer.w, layer.b]
         elif isinstance(layer, radial.Radial):
             out += [layer.beta, layer.alpha, layer.z_0]
@@ -128,7 +137,7 @@ def sampling_slot_tensors(layers):
         elif isinstance(layer, affine.AffineCouplingBlock):
             out += [p for lin in layer.flows[1].param_map.linear_layers() for p in (lin.weight, lin.bias)]
         elif not isinstance(layer, mixing.Permute):
-            raise NotImplementedError(f"{type(layer).__name__} is in neither the affine nor the planar family")
+            raise NotImplementedError(f"{type(layer).__name__} has no native sampling-direction backward")
     return out
 
 
@@ -147,7 +156,8 @@ def sum_slot_grads(slots, bufs):
 
 def stack_backward(handle, layers, direction, z, g_out, g_ld, need_z):
     """(g_z | None, {id(parameter): gradient}) of (out, log_det) = handle.transform(direction, z) through
-    nfb_flow_sampling_backward (NFB_FORWARD: all-affine or all-planar stacks) or nfb_flow_density_backward (NFB_INVERSE:
+    nfb_flow_sampling_backward (NFB_FORWARD: all-affine, all-planar or coupled-spline / LU stacks) or
+    nfb_flow_density_backward (NFB_INVERSE:
     all-affine stacks); g_out / g_ld are the cotangents of out / log_det (None: zero)."""
     slots = sampling_slot_tensors(layers)
     bufs = [torch.empty_like(p) if isinstance(p, torch.nn.Parameter) and p.requires_grad else None for p in slots]
@@ -172,10 +182,10 @@ def stack_backward(handle, layers, direction, z, g_out, g_ld, need_z):
 
 class StackSamplingFn(torch.autograd.Function):
     """(out, log_det) = handle.transform(direction, z) of an all-affine stack (MaskedAffineFlow, AffineConstFlow /
-    ActNorm, AffineCouplingBlock, Permute), or in the sampling direction of an all-planar one (Planar, Radial): the
-    unchanged one-launch forward, so values are bit-identical with and without grad.  The backward is one
-    nfb_flow_sampling_backward / nfb_flow_density_backward call (recompute + walk back through the ops, then a
-    fixed-order reduction of the parameter terms).  Refuses to run the backward if a parameter was modified in place
+    ActNorm, AffineCouplingBlock, Permute), or in the sampling direction of an all-planar one (Planar, Radial) or of a
+    coupled-spline / LU one (CoupledRationalQuadraticSpline, LULinearPermute): the unchanged forward, so values are
+    bit-identical with and without grad.  The backward is one nfb_flow_sampling_backward / nfb_flow_density_backward
+    call (recompute + walk back through the layers).  Refuses to run the backward if a parameter was modified in place
     after the forward."""
 
     @staticmethod

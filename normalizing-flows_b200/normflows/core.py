@@ -80,7 +80,7 @@ class NormalizingFlow(nn.Module):
         h = self._stack()
         self._run_pending_inits(z, inverse=False)
         if h is not None and z.dim() == 2:
-            if self._one_sampling_family() and wants_grad(self.flows, z):   # one launch forward, one native backward
+            if self._stack_sampling_backward() and wants_grad(self.flows, z):   # one native backward
                 from ._standalone import stack_sampling
                 return stack_sampling(h, self.flows, z, list(self.flows.parameters()))
             return h.transform(L.NFB_FORWARD, z)
@@ -151,10 +151,30 @@ class NormalizingFlow(nn.Module):
         fams = {f._sampling_family() if isinstance(f, NativeFlow) else None for f in self.flows}
         return fams.pop() if len(fams) == 1 else None
 
-    def _flows_sampling_differentiable(self, context=None):
-        """Every layer's sampling direction is differentiable (the stand-alone spline layers and the affine and planar
-        families, `_sampling_differentiable`), and the stack runs layer by layer or is all of one family."""
-        return ((self._takes_layer_loop() or self._one_sampling_family())
+    def _coupled_spline_stack(self):
+        """Every layer a CoupledRationalQuadraticSpline without a context and with 8 bins, or an LULinearPermute: the
+        all-native stack's sampling direction has a native backward (nfb_flow_sampling_backward).  A stack-level rule:
+        LULinearPermute on its own, or between layers outside the native stack, stays without one."""
+        from .flows.mixing import LULinearPermute
+        from .flows.neural_spline import CoupledRationalQuadraticSpline
+        return len(self.flows) > 0 and all(
+            type(f) is LULinearPermute or (type(f) is CoupledRationalQuadraticSpline and f.num_context_channels is None
+                                            and f.num_bins == 8) for f in self.flows)
+
+    def _stack_sampling_backward(self):
+        """The all-native stack's sampling direction has a native backward: all-affine, all-planar, or coupled splines
+        with LU layers."""
+        return self._one_sampling_family() is not None or self._coupled_spline_stack()
+
+    def _flows_sampling_differentiable(self, context=None, rows=True):
+        """The sampling direction is differentiable where it runs.  On the all-native stack (rows: z is [rows, features],
+        so forward_and_log_det takes the stack) when the stack has a native backward (_stack_sampling_backward).  In the
+        layer loop (a stack with a layer that is not native, a conditional flow, or an all-one-family stack fed z of
+        another shape) when every layer's is (`_sampling_differentiable`: the stand-alone spline layers, the coupled
+        spline layer, the affine and planar families; not LULinearPermute)."""
+        if rows and not self._takes_layer_loop():
+            return self._stack_sampling_backward()
+        return ((self._takes_layer_loop() or self._one_sampling_family() is not None)
                 and all(hasattr(f, "_sampling_differentiable") and f._sampling_differentiable(context)
                         for f in self.flows))
 
@@ -165,7 +185,7 @@ class NormalizingFlow(nn.Module):
         if not (torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())):
             return
         if (isinstance(self.q0, (UniformGaussian, DiagGaussian, ConditionalDiagGaussian, GaussianMixture))
-                and self._flows_sampling_differentiable(context)):
+                and self._flows_sampling_differentiable(context, rows=getattr(self.q0, "n_dim", 1) == 1)):
             return
         raise NotImplementedError(_no_sampling_grad_message(what) + "; forward_kld / log_prob are differentiable)")
 
@@ -182,8 +202,8 @@ class NormalizingFlow(nn.Module):
         """core.py:104-131.  z ~ q0 pushed through every layer's `.forward` (one persistent launch for coupling
         stacks), log_q = log q0(z0) - sum log_det; `score_fn=False` re-evaluates log_q by the density pass of the
         drawn samples with parameter gradients switched off, like the reference.  Differentiable for the stacks
-        _no_sampling_grad admits (the stand-alone spline layers, the affine or the planar family on a reparameterised
-        base)."""
+        _no_sampling_grad admits (the stand-alone spline layers, the affine or the planar family, coupled spline + LU
+        stacks, on a reparameterised base)."""
         self._no_sampling_grad("reverse_kld")
         z, log_q = self.sample(num_samples)
         if not score_fn:
@@ -453,9 +473,9 @@ class NormalizingFlowVAE(nn.Module):
     `forward(x, num_samples)` returns z [B, S, d], log_q [B, S] and log_p [B, S]; row b S + s of the flattened samples
     belongs to x[b].  The encoder's draw, its log-density and the decoder's likelihood are kernels with a native
     backward (distributions/encoder.py, distributions/decoder.py); the flows go through one stack, as in
-    NormalizingFlow.forward_and_log_det: one launch and one native backward for an all-planar or all-affine list, the
-    layer loop otherwise.  Under grad, flows without a differentiable sampling direction (spline, LU, MAF in a stack)
-    raise instead of being silently detached.  `prior` is used as given (a torch distribution stays torch)."""
+    NormalizingFlow.forward_and_log_det: one native backward for an all-planar, all-affine or coupled-spline / LU list,
+    the layer loop otherwise.  Under grad, flows without a differentiable sampling direction (autoregressive splines,
+    MAF, mixed families in a stack; LU in a layer loop) raise instead of being silently detached.  `prior` is used as given (a torch distribution stays torch)."""
 
     def __init__(self, prior, q0=Dirac(), flows=None, decoder=None):
         super().__init__()
@@ -468,7 +488,7 @@ class NormalizingFlowVAE(nn.Module):
         if len(self.flows) == 0:
             return z, torch.zeros(len(z), device=z.device)
         inner = _inner_flow(self)
-        if wants_grad(self.flows, z) and not inner._flows_sampling_differentiable():
+        if wants_grad(self.flows, z) and not inner._flows_sampling_differentiable(rows=z.dim() == 2):
             names = "+".join(sorted({type(f).__name__ for f in self.flows}))
             raise NotImplementedError(_no_sampling_grad_message(f"NormalizingFlowVAE with {names} flows") + ")")
         return inner.forward_and_log_det(z)

@@ -15,6 +15,7 @@ import torch
 from torch import nn
 
 from .. import _lib as L
+from .._image_autograd import wants_grad
 from .._native import resnet_desc
 from ..nets.made import MADE
 from ..nets.resnet import ResidualNet
@@ -202,7 +203,9 @@ class CoupledRationalQuadraticSpline(NativeFlow):
         return _coupling_sampling_adjoint(self.prqct, z, context, keep, g_x, g_ld, spline, need_z, need_ctx)
 
     def _sampling_differentiable(self, context=None):
-        return self.num_context_channels is not None or context is not None
+        """The stand-alone (context) path, and the native one with 8 bins (nfb_flow_sampling_backward on the layer's own
+        handle)."""
+        return self.num_context_channels is not None or context is not None or self.num_bins == 8
 
     def _value(self, z, context, keep):
         from .._native import rqs_spline
@@ -225,6 +228,9 @@ class CoupledRationalQuadraticSpline(NativeFlow):
     def forward(self, z, context=None):
         if self.num_context_channels is not None or context is not None:
             return self._conditional(z, context, True)
+        if self.num_bins == 8 and wants_grad(self, z):   # the one-layer stack's native sampling backward
+            from .._standalone import stack_sampling
+            return stack_sampling(self._single(), [self], z, list(self.parameters()))
         return super().forward(z)
 
     def inverse(self, z, context=None):
