@@ -192,6 +192,19 @@ __device__ __forceinline__ void wgmma_f16_n96(float (&d)[48], uint64_t a, uint64
 }
 // D = A * B^T with scale-d an immediate 0: D is written, not read, so it needs no value before (a zero-initialised
 // accumulator would be instructions defining it, which ptxas does not allow while another wgmma of the stage is in flight)
+__device__ __forceinline__ void wgmma_f16_n64_zero(float (&d)[32], uint64_t a, uint64_t b) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{"
+        "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31"
+        "}, %32, %33, 0, 1, 1, 0, 0;"
+        : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3]), "=f"(d[4]), "=f"(d[5]), "=f"(d[6]), "=f"(d[7]), "=f"(d[8]),
+          "=f"(d[9]), "=f"(d[10]), "=f"(d[11]), "=f"(d[12]), "=f"(d[13]), "=f"(d[14]), "=f"(d[15]), "=f"(d[16]),
+          "=f"(d[17]), "=f"(d[18]), "=f"(d[19]), "=f"(d[20]), "=f"(d[21]), "=f"(d[22]), "=f"(d[23]), "=f"(d[24]),
+          "=f"(d[25]), "=f"(d[26]), "=f"(d[27]), "=f"(d[28]), "=f"(d[29]), "=f"(d[30]), "=f"(d[31])
+        : "l"(a), "l"(b));
+}
 __device__ __forceinline__ void wgmma_f16_n96_zero(float (&d)[48], uint64_t a, uint64_t b) {
     asm volatile(
         "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 "
@@ -269,6 +282,12 @@ __device__ __forceinline__ uint32_t pack_f16x2(float lo_elem, float hi_elem) {
 }
 __device__ __forceinline__ float2 unpack_f16x2(uint32_t h) {  // .x = lower half, .y = upper half
     return __half22float2(*reinterpret_cast<const __half2*>(&h));
+}
+// four 8 x 8 b16 matrices to shared memory (whole warp): lanes 8 i .. 8 i + 7 give the row addresses of matrix i, and
+// r[i] of lane l holds its row l / 4, columns 2 (l % 4), + 1 -- the layout of a wgmma accumulator's packed halves
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1),
+                 "r"(r2), "r"(r3) : "memory");
 }
 
 __device__ __forceinline__ float warp_sum(float v) {

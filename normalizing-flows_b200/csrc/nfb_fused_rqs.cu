@@ -83,9 +83,6 @@ __device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t
     asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d)
                  : "memory");
 }
-__device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) {
-    asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
-}
 __device__ __forceinline__ void cons_bar_sync() {  // both consumer warpgroups
     asm volatile("bar.sync 1, %0;" ::"n"(kCons) : "memory");
 }
@@ -130,26 +127,29 @@ template <typename T> __device__ __forceinline__ T uniform(T v) {
 __device__ __forceinline__ float pow2i(int e) { return __uint_as_float((uint32_t)(127 + e) << 23); }
 
 // the products of one record: acc (+)= A[K-chunk] W^T as W_hi A_hi + W_hi A_lo + W_lo A_hi (+ W_lo A_lo), the first
-// SLABS K = 16 slabs each, in that order (first: the first product overwrites the accumulator; the slabs after SLABS are
-// all zero).  One straight chain: no wgmma of it has a predicate of its own, so ptxas issues them back to back behind
-// one warpgroup.arrive.  Whether a record has products at all is decided by one uniform branch around the chain.
-// N = 64 (32 registers): a hidden GEMM's slice; N = 96 (48): both halves of a final-layer record at once, half 0 in
-// registers 0..23 and half 1 in 24..47 (rows [0, 48) and [48, 96) of the record's tiles).
-// FIRST: the record opens acc whatever its flags say, and its first product overwrites acc with an immediate scale-d
-// of 0, so acc needs no value before it (the final layer's pairs, whose first record always opens the accumulator).
-struct MmaOps { uint32_t a_hi, a_lo, w_hi, w_lo; bool first; uint32_t on, slabs; };
+// SLABS K = 16 slabs each, in that order (the slabs after SLABS are all zero).  One straight chain: no wgmma of it has a
+// predicate of its own, so ptxas issues them back to back behind one warpgroup.arrive.  Whether a record has products at
+// all is decided by one uniform branch around the chain.
+// N = 64 (32 registers): a hidden GEMM's slice or the LU map; N = 96 (48): both halves of a final-layer record at once,
+// half 0 in registers 0..23 and half 1 in 24..47 (rows [0, 48) and [48, 96) of the record's tiles).
+// FIRST: the record opens acc (the packer's kStepFirst), and its first product overwrites acc with an immediate scale-d
+// of 0, so acc needs no value before it; every other product accumulates.  Callers issue an opening record as FIRST
+// unconditionally, so that to the compiler acc is written before it is read.
+struct MmaOps { uint32_t a_hi, a_lo, w_hi, w_lo, on, slabs; };
 template <int SLABS, bool QUAD, int NREG, bool FIRST = false>
 __device__ __forceinline__ void mma_record(float (&acc)[NREG], const MmaOps& x) {
     static_assert(NREG == 32 || NREG == 48, "N = 64 or 96");
-    static_assert(!FIRST || NREG == 48, "an opening record of its own: the final layer's N = 96 products");
     const uint64_t ah = wgmma_desc(x.a_hi), al = wgmma_desc(x.a_lo), bh = wgmma_desc(x.w_hi), bl = wgmma_desc(x.w_lo);
     auto pass = [&](uint64_t a, uint64_t b, bool opens) {
 #pragma unroll
         for (int s = 0; s < SLABS; ++s) {
-            const uint32_t sd = opens && s == 0 && x.first ? 0u : 1u;
-            if constexpr (NREG == 32) wgmma_f16_n64(acc, a + 2 * s, b + 2 * s, sd);
-            else if (FIRST && opens && s == 0) wgmma_f16_n96_zero(acc, a, b);
-            else wgmma_f16_n96(acc, a + 2 * s, b + 2 * s, FIRST ? 1u : sd);
+            if constexpr (NREG == 32) {
+                if (FIRST && opens && s == 0) wgmma_f16_n64_zero(acc, a, b);
+                else wgmma_f16_n64(acc, a + 2 * s, b + 2 * s, 1u);
+            } else {
+                if (FIRST && opens && s == 0) wgmma_f16_n96_zero(acc, a, b);
+                else wgmma_f16_n96(acc, a + 2 * s, b + 2 * s, 1u);
+            }
         }
     };
     pass(ah, bh, true);
@@ -178,7 +178,11 @@ enum { kClkClaim,       // unit queue, layer-to-layer flag, rows of a host batch
        kClkProdOther,   // producer: everything else (claim, step table, issue)
        kClkUnits,       // (a count, not cycles) units this role worked on
        kClkCount };
-template <int P> using ClkPhase = std::integral_constant<int, P>;
+// the phases a run of records charges its ring waits, its products and its first record's wait to
+template <int RING, int MMA, int TAIL> struct WalkClk { static constexpr int ring = RING, mma = MMA, tail = TAIL; };
+using LuClk = WalkClk<kClkLu, kClkLu, kClkLu>;
+using HidClk = WalkClk<kClkHidRing, kClkHidMma, kClkHidMma>;
+using FinClk = WalkClk<kClkFinRing, kClkFinMma, kClkFinTail>;
 #ifdef NFB_PHASE_CLOCKS
 __device__ unsigned long long g_phase_clocks[3][kClkCount];   // [consumer warpgroup 0, 1, producer][phase]
 struct PhaseClock {   // 32-bit sums: one launch is far below 2^32 cycles
@@ -367,23 +371,24 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
         // can start while the one before still multiplies.  OPEN: the first record is issued as issue(step, true_type)
         // and completes the products in flight before it (its wait_group 1), which hands back `prev` and then runs
         // `retire` -- the previous run's accumulator is final there.  Every other record is issue(step, false_type).
-        auto walk_records = [&](auto issue, auto arrivals, auto clk_ring, auto clk_mma, int& prev, auto open,
-                                auto retire) {
+        // phases: the clock phases its ring waits, its products and its first record's wait are charged to.
+        auto walk_records = [&](auto issue, auto arrivals, auto phases, int& prev, auto open, auto retire) {
+            using Clk = decltype(phases);
             auto record = [&](auto first) {
                 union { uint2 raw; FusedStep s; } st;
                 st.raw = __ldg(reinterpret_cast<const uint2*>(L.steps) + sidx);
                 st.raw.x = uniform(st.raw.x);
                 st.raw.y = uniform(st.raw.y);
                 sidx = sidx + 1 == n_steps ? lu_steps : sidx + 1;
-                NFB_CLK(decltype(clk_mma)::value);
+                NFB_CLK(Clk::mma);
                 mbar_wait(bar(kBarWFull + slot), wpar, p.err, 220 + slot);
-                NFB_CLK(decltype(clk_ring)::value);
+                NFB_CLK(Clk::ring);
                 wgmma_fence();
                 const bool last = issue(st.s, first);   // (commits its own group)
-                if constexpr (decltype(first)::value) NFB_CLK(decltype(clk_mma)::value);
+                if constexpr (decltype(first)::value) NFB_CLK(Clk::mma);
                 wgmma_wait<1>();   // the previous record's products are complete: hand its slot back
                 hand_back(arrivals, prev < 0 ? 0 : prev, prev >= 0);
-                if constexpr (decltype(first)::value) NFB_CLK(kClkFinTail);
+                if constexpr (decltype(first)::value) NFB_CLK(Clk::tail);
                 prev = (int)slot;
                 if (++slot == kSlots) { slot = 0; wpar ^= 1; }
                 return last;
@@ -395,34 +400,41 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
             }
             while (!last) last = record(std::false_type());
         };
-        // a run that ends with its products complete and every slot handed back
-        auto run_records = [&](auto issue, auto arrivals, auto clk_ring, auto clk_mma) {
-            int prev = -1;
-            walk_records(issue, arrivals, clk_ring, clk_mma, prev, std::false_type(), [] {});
-            wgmma_wait<0>();
-            hand_back(arrivals, prev, true);
-            NFB_CLK(decltype(clk_mma)::value);
-        };
-        // operands of half h of the record in the current slot (live = 0: no products; the skip bit: the record has no
-        // half h, or an all-zero one)
-        auto half_ops = [&](const FusedStep& s, int h, bool live) {
+        // operands of half h of the record in the current slot (the skip bit: the record has no half h, or an all-zero one)
+        auto half_ops = [&](const FusedStep& s, int h) {
             const uint32_t kc = h ? s.kc1 : s.kc, fl = h ? s.flags1 : s.flags;
             const uint32_t w = sbase + kOffW + slot * kSlotBytes + ((fl & kStepHalf) ? 0u : (uint32_t)h * s.n8 * 1024u);
-            return MmaOps{aA + kc * kTileA, aA + (4 + kc) * kTileA, w, w + ((uint32_t)s.bytes16 << 3), (fl & kStepFirst) != 0,
-                          (uint32_t)(live && !(fl & kStepSkip)), 4u - ((fl >> kStepSlabShift) & 3u)};
+            return MmaOps{aA + kc * kTileA, aA + (4 + kc) * kTileA, w, w + ((uint32_t)s.bytes16 << 3),
+                          (uint32_t)!(fl & kStepSkip), 4u - ((fl >> kStepSlabShift) & 3u)};
         };
         // The records of one output slice of this warpgroup (until the one its flags mark last): its half of each goes
-        // into acc, multiplied with its K-chunk (live: the warpgroup has a slice here).  (The packer sets slab bits on
-        // final-layer records only: the LU map and the hidden GEMMs always multiply all four slabs.)
-        auto run_slice = [&](auto& acc, bool live, auto quad, auto clk_ring, auto clk_mma) {
-            run_records([&](const FusedStep& s, auto) {
-                const MmaOps x = half_ops(s, wg, live);
-                if (x.on) mma_record<4, decltype(quad)::value>(acc, x);
-                wgmma_commit();
+        // into acc, multiplied with its K-chunk.  OPENS: the slice's first record opens acc (FIRST; the packer keeps
+        // K-chunk 0 of every slice, so that record always has products); otherwise every product accumulates onto acc.
+        // Each record commits inside its own branch: a commit after the join would close the chain's group at the end
+        // of its block and add a second, empty one, and wait_group 1 would then wait for the record's own products.
+        // (The packer sets slab bits on final-layer records only: the LU map and the hidden GEMMs multiply all four.)
+        auto slice_products = [&](float (&acc)[32], auto opens, auto quad) {
+            return [&](const FusedStep& s, auto first) {
+                constexpr bool Q = decltype(quad)::value;
+                const MmaOps x = half_ops(s, wg);
+                if constexpr (decltype(first)::value && decltype(opens)::value) {
+                    mma_record<4, Q, 32, true>(acc, x);
+                    wgmma_commit();
+                } else if (x.on) {
+                    mma_record<4, Q, 32>(acc, x);
+                    wgmma_commit();
+                } else {
+                    wgmma_commit();
+                }
                 return ((wg ? s.flags1 : s.flags) & kStepLast) != 0;
-            }, std::integral_constant<int, 1>(), clk_ring, clk_mma);
-            wgmma_hold(acc);
+            };
         };
+        // a warpgroup without a slice passes the GEMM's records as one slice with no products
+        auto no_products = [&](const FusedStep& s, auto) {
+            wgmma_commit();
+            return ((wg ? s.flags1 : s.flags) & kStepLast) != 0;
+        };
+        using One = std::integral_constant<int, 1>;
         using NoQuad = std::integral_constant<bool, false>;
 
         // layers >= 1 update z in place (z_stride = 0) or, for the training pass, every layer writes its own
@@ -553,10 +565,15 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
         const bool folded = uniform(!SAMPLE && L.has_lu && L.fold_lu);
         if (lu_steps) {
             store_a([&](int k) { return k < D ? xs[xs_index(ar, k)] : 0.f; }, L.a_sc[0]);
-            float acc[32];
             NFB_CLK(kClkLoad);
-            run_slice(acc, wg == 0, std::integral_constant<bool, true>(), ClkPhase<kClkLu>(), ClkPhase<kClkLu>());   // (no half for warpgroup 1)
+            int prev = -1;
             if (wg == 0) {
+                float acc[32];
+                walk_records(slice_products(acc, std::true_type(), std::true_type()), One(), LuClk(), prev,
+                             std::true_type(), [] {});
+                wgmma_wait<0>();
+                hand_back(One(), prev, true);
+                wgmma_hold(acc);
                 // x' = acc + b (this thread: rows ra / rb, two columns of every 8-column group)
                 const float ia = ruinv(L.a_inv[0], ra), ib = ruinv(L.a_inv[0], rb);
 #pragma unroll
@@ -565,6 +582,10 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
                     const int rr = (i & 2) ? rb : ra;
                     if (c < D) xs[xs_index(rr, c)] = fmaf(acc[i], (i & 2) ? ib : ia, __ldg(L.bias_lu + c));
                 }
+            } else {   // (the LU record has no half for warpgroup 1)
+                walk_records(no_products, One(), LuClk(), prev, std::false_type(), [] {});
+                wgmma_wait<0>();
+                hand_back(One(), prev, true);
             }
             cons_bar_sync();   // x' of the whole tile is visible to both warpgroups
             NFB_CLK(kClkLu);
@@ -636,60 +657,96 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
             // the final layer's splines all run on warpgroup 1: warpgroup 0's sums so far go with them
             if (wg == 0) ldsum[rq * kRows + r] = ladsum;
             // ---- hidden layers: warpgroup wg owns the 64-column slices own(0), own(1) of every output (the packer's
-            //      choice, nfb_fused_plan.h); a warpgroup without a slice passes the GEMM's records as one dead slice ----
-            // (Both are written first by a wgmma whose scale-d operand is a run-time flag, so to the compiler they would be
-            // read before they are written and stay live across the whole pass, final layer included: 128 registers
-            // the splines and the final layer's accumulators need.  The zeros end that; no product reads them.)
-            float hres[2][32] = {};   // its part of the residual stream h
-            for (int ph = 0; ph < n_hidden; ++ph) {
-                const bool t_phase = (ph & 1) != 0;   // first GEMM of a residual block: its own accumulator
-                const bool relu = ph + 1 < n_hidden;
-                float tacc[2][32] = {};
+            //      choice, nfb_fused_plan.h); a warpgroup without a slice passes the GEMM's records as one slice with
+            //      no products ----
+            // One walk per GEMM and warpgroup: slice own(1)'s first record is issued while own(0)'s last one multiplies,
+            // its wait_group 1 completes own(0), and own(0)'s epilogue arithmetic (unscale + pre-summed bias, ReLU, scale
+            // to the next GEMM's units, fp16 hi/lo) runs under own(1)'s products.  The tensor core drains once per GEMM;
+            // only the stores wait for the barrier after that: the products of both warpgroups read the one A operand
+            // that the output overwrites.
+            // The slice count NS (0, 1, 2) is a template argument, and the residual stream and each t-phase temporary
+            // are opened by a FIRST record on every path that reads them, so to the compiler they are written before
+            // they are read: they are not live outside the hidden layers (the splines and the final layer's
+            // accumulators need those registers), and nothing but a wgmma defines them while products are in flight
+            // (anything else makes ptxas serialise every wgmma of the kernel, C7515).
+            auto hidden = [&](auto ns) {
+                constexpr int NA = decltype(ns)::value > 0 ? decltype(ns)::value : 1;
+                // GEMM ph into acc (OPENS: its first record of each slice opens it), then its output -> A K-chunks own(q)
+                auto gemm = [&](auto& acc, auto opens, int ph) {
+                    constexpr int NS = decltype(ns)::value, NA = NS > 0 ? NS : 1;
+                    const bool relu = ph + 1 < n_hidden;
+                    const float inv_a = ruinv(L.a_inv[1 + ph], ra), inv_b = ruinv(L.a_inv[1 + ph], rb);
+                    const float sc_a = ru(L.a_sc[2 + ph], ra), sc_b = ru(L.a_sc[2 + ph], rb);
+                    // this thread's bias pairs (columns 8 g + cq, + 1 of each of its slices), loaded before the first
+                    // record: the layer flag's acquire emptied L1, and the L2 round trip hides under the products
+                    float2 bias[NA][8];
 #pragma unroll
-                for (int q = 0; q < 2; ++q) {
-                    const int j = own(q);
-                    if (q == 0 || j >= 0) {
-                        if (t_phase) run_slice(tacc[q], j >= 0, NoQuad(), ClkPhase<kClkHidRing>(), ClkPhase<kClkHidMma>());
-                        else run_slice(hres[q], j >= 0, NoQuad(), ClkPhase<kClkHidRing>(), ClkPhase<kClkHidMma>());
-                    }
-                }
-                cons_bar_sync();   // every product of this GEMM has read the A operand: overwrite it with the output
-                const float inv_a = ruinv(L.a_inv[1 + ph], ra), inv_b = ruinv(L.a_inv[1 + ph], rb);
-                const float sc_a = ru(L.a_sc[2 + ph], ra), sc_b = ru(L.a_sc[2 + ph], rb);
-                // output slice j: bias, ReLU, scale to the next GEMM's units, fp16 hi/lo -> A K-chunk j
-                auto epilogue = [&](const float (&acc)[32], int j) {
-                    const float* bias = L.bias_h + ph * 256 + 64 * j;
+                    for (int q = 0; q < NS; ++q)
 #pragma unroll
-                    for (int g = 0; g < 8; ++g) {
-                        const float2 b2 = __ldg(reinterpret_cast<const float2*>(bias + 8 * g + cq));
+                        for (int g = 0; g < 8; ++g)
+                            bias[q][g] = __ldg(reinterpret_cast<const float2*>(L.bias_h + ph * 256 + 64 * own(q) + 8 * g + cq));
+                    // slice q's output as packed fp16 pairs, hi (pk[q][0]) and lo (pk[q][1]); pair p = 2 g + hb holds
+                    // row (hb ? rb : ra), columns 8 g + cq, + 1 -- accumulator registers 2 p, 2 p + 1
+                    uint32_t pk[NA][2][16];
+                    auto pack = [&](int q, float (&a)[32]) {
+                        wgmma_hold(a);
 #pragma unroll
-                        for (int hb = 0; hb < 2; ++hb) {
-                            const int rr = hb ? rb : ra;
-                            float v0 = fmaf(acc[4 * g + 2 * hb], hb ? inv_b : inv_a, b2.x);
-                            float v1 = fmaf(acc[4 * g + 2 * hb + 1], hb ? inv_b : inv_a, b2.y);
+                        for (int p = 0; p < 16; ++p) {
+                            const int g = p >> 1, hb = p & 1;
+                            float v0 = fmaf(a[2 * p], hb ? inv_b : inv_a, bias[q][g].x);
+                            float v1 = fmaf(a[2 * p + 1], hb ? inv_b : inv_a, bias[q][g].y);
                             if (relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
                             v0 *= hb ? sc_b : sc_a;
                             v1 *= hb ? sc_b : sc_a;
                             const uint32_t hi = pack_f16x2(v0, v1);
                             const float2 hf = unpack_f16x2(hi);
-                            const uint32_t off = (rr >> 3) * 1024 + (rr & 7) * 128 + ((g ^ (rr & 7)) << 4) + cq * 2;
-                            st_shared_b32(aA + j * kTileA + off, hi);
-                            st_shared_b32(aA + (4 + j) * kTileA + off, pack_f16x2(v0 - hf.x, v1 - hf.y));
+                            pk[q][0][p] = hi;
+                            pk[q][1][p] = pack_f16x2(v0 - hf.x, v1 - hf.y);
                         }
+                    };
+                    int prev = -1;
+                    if constexpr (NS == 0) {
+                        walk_records(no_products, One(), HidClk(), prev, std::false_type(), [] {});
+                    } else {
+                        walk_records(slice_products(acc[0], opens, NoQuad()), One(), HidClk(), prev, std::true_type(),
+                                     [] {});
+                        if constexpr (NS == 2)
+                            walk_records(slice_products(acc[1], opens, NoQuad()), One(), HidClk(), prev, std::true_type(),
+                                         [&] { pack(0, acc[0]); NFB_CLK(kClkHidEpi); });
                     }
-                };
+                    wgmma_wait<0>();
+                    hand_back(One(), prev, true);
+                    NFB_CLK(kClkHidMma);
+                    if constexpr (NS > 0) pack(NS - 1, acc[NS - 1]);
+                    cons_bar_sync();   // every product of this GEMM has read the A operand: overwrite it with the output
+                    // Each 8 x 8 block of a warp's accumulator rows and columns is one stmatrix matrix: stmatrix k writes
+                    // column groups 2 k, 2 k + 1 of rows 16 wl .. 16 wl + 15, lane l giving row 16 wl + l % 16 of group
+                    // 2 k + l / 16 (its SW128 chunk address).
 #pragma unroll
-                for (int q = 0; q < 2; ++q) {
-                    const int j = own(q);   // output slice = A K-chunk j of the next GEMM
-                    if (j >= 0) {
-                        if (t_phase) epilogue(tacc[q], j);
-                        else epilogue(hres[q], j);
-                    }
+                    for (int q = 0; q < NS; ++q)
+#pragma unroll
+                        for (int h = 0; h < 2; ++h)
+#pragma unroll
+                            for (int k = 0; k < 4; ++k)
+                                stmatrix_x4(aA + (4 * h + own(q)) * kTileA + a_chunk_off(16 * wl + (lane & 15), 2 * k + (lane >> 4)),
+                                            pk[q][h][4 * k], pk[q][h][4 * k + 1], pk[q][h][4 * k + 2], pk[q][h][4 * k + 3]);
+                    fence_proxy_async_smem();
+                    cons_bar_sync();   // the next GEMM's A operand is complete
+                    NFB_CLK(kClkHidEpi);
+                };
+                float hres[NA][32];   // its part of the residual stream h
+                gemm(hres, std::true_type(), 0);
+                // residual blocks (n_hidden = 1 + 2 x blocks): the first GEMM into a temporary of its own, the second
+                // onto the residual stream (h += W2 relu(...))
+                for (int ph = 1; ph + 1 < n_hidden; ph += 2) {
+                    float tacc[NA][32];
+                    gemm(tacc, std::true_type(), ph);
+                    gemm(hres, std::false_type(), ph + 1);
                 }
-                fence_proxy_async_smem();
-                cons_bar_sync();   // the next GEMM's A operand is complete
-                NFB_CLK(kClkHidEpi);
-            }
+            };
+            if (own(0) < 0) hidden(std::integral_constant<int, 0>());
+            else if (own(1) < 0) hidden(std::integral_constant<int, 1>());
+            else hidden(std::integral_constant<int, 2>());
 
             // ---- final layer: record c = chunks 2c and 2c + 1, kFusedFeaturesPerChunk features (x 24 columns) each.
             //      Warpgroup 0 multiplies both halves of every record and stores the two accumulators to the staging
@@ -713,7 +770,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
                         // an exact zero to every accumulator.  (A record always has a live half: the packer keeps only
                         // K-chunk 0 and the K-chunks one of the two chunks reaches; K-chunk 0 opens the pair.)
                         constexpr bool F = decltype(first)::value;
-                        const MmaOps x = half_ops(s, 0, true), x1 = half_ops(s, 1, true);
+                        const MmaOps x = half_ops(s, 0), x1 = half_ops(s, 1);
                         const uint32_t n = max(x.on ? x.slabs : 0u, x1.on ? x1.slabs : 0u);
                         switch (n) {
                             case 1: mma_record<1, false, 48, F>(acc, x); wgmma_commit(); break;
@@ -759,9 +816,8 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
                 using Two = std::integral_constant<int, 2>;
                 int prev = -1;
                 // pair ci into acc; `done` holds pair ci - 1, staged under the first record of pair ci
-                auto pair = [&](float (&acc)[48], float (&done)[48], int ci) {
-                    walk_records(products(acc), Two(), ClkPhase<kClkFinRing>(), ClkPhase<kClkFinMma>(), prev,
-                                 std::true_type(), [&] { stage(done, ci - 1); });
+                auto pair = [&](float (&acc)[48], float (&done)[48], int ci) __attribute__((always_inline)) {
+                    walk_records(products(acc), Two(), FinClk(), prev, std::true_type(), [&] { stage(done, ci - 1); });
                 };
                 // after the last pair: its products complete, its last slot back
                 auto finish = [&](float (&acc)[48], int ci) {
@@ -775,8 +831,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
                 float accA[48], accB[48];
                 if (n_pairs > 0) {
                     load_bias(0);
-                    walk_records(products(accA), Two(), ClkPhase<kClkFinRing>(), ClkPhase<kClkFinMma>(), prev,
-                                 std::true_type(), [] {});
+                    walk_records(products(accA), Two(), FinClk(), prev, std::true_type(), [] {});
                     for (int ci = 1;; ci += 2) {
                         if (ci == n_pairs) { finish(accA, ci - 1); break; }
                         pair(accB, accA, ci);
@@ -786,7 +841,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) fused_rqs_kernel(const Fused
                 }
             } else {
                 // It does not walk the final layer's records (the last of the step table): its cursors move past them
-                // as run_records moves warpgroup 0's.
+                // as walk_records moves warpgroup 0's.
                 if (n_pairs > 0) {
                     const uint32_t adv = slot + (uint32_t)(n_steps - sidx);
                     slot = adv % kSlots;
