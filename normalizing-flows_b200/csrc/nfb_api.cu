@@ -2806,8 +2806,9 @@ namespace {
 
 int grad_slots_of(const Layer& L) {
     switch (L.kind) {
-    case L_AR_RQS: return 4 + 4 * L.net.nb;
-    case L_COUPLED_RQS: return 4 + 4 * L.net.nb + 3;
+    // the spline adjoint kernels take 8 bins only: other counts have no native backward (the caller falls back)
+    case L_AR_RQS: return L.K == 8 ? 4 + 4 * L.net.nb : -1;
+    case L_COUPLED_RQS: return L.K == 8 ? 4 + 4 * L.net.nb + 3 : -1;
     case L_LU: return 4;
     // affine family, in each layer's parameter registration order: MaskedAffineFlow s then t (weight, bias per Linear),
     // AffineConstFlow s, t, AffineCouplingBlock param_map, Permute none
@@ -2908,7 +2909,8 @@ int rqs_layer_backward(nfb_flow* f, Layer& L, const float* xp, const float* gy, 
     f->launches++;
     const int nlin = 2 + 2 * n.nb;
     if (coupled) {
-        NFB_TRY(f->tr_small.reserve((size_t)(64 * 64 + 64 * 23 + 64) * 4));
+        // the table gradient [n_id x P] at the front; at least the LU scratch behind it (lu_layer_backward's layout)
+        NFB_TRY(f->tr_small.reserve((size_t)(64 * 64 + std::max(64, L.n_id) * P + 64) * 4));
         float* gtab = f->tr_small.as<float>();
         NFB_CUDA(cudaMemsetAsync(gtab, 0, (size_t)L.n_id * P * 4, st));
         NFB_TRY(launch_spline_bwd_shared(xp, D, L.uncond.as<float>(), gy, glq, L.id_idx.as<int>(), rows, L.n_id, L.K, L.tail,

@@ -1,5 +1,5 @@
-"""Gradient oracle: hand-written reverse mode of `NormalizingFlow.forward_kld` (core.py:87-102) for
-neural-spline stacks, in numpy.  TEST INFRASTRUCTURE ONLY (same rules as nf_oracle.py): it is the checker the
+"""Gradient oracle: hand-written reverse mode of `NormalizingFlow.log_prob` (any per-row weighting; `forward_kld`,
+core.py:87-102, is the uniform one) for neural-spline stacks, in numpy.  TEST INFRASTRUCTURE ONLY (same rules as nf_oracle.py): it is the checker the
 native backward kernels (SURVEY 8f-1) will be compared with at shapes for which no golden fixture exists.
 
 Pinned: tests/test_oracle_golden.py checks every parameter gradient and the input gradient against
@@ -8,7 +8,7 @@ fp64 (tests/golden/make_golden.py grads).
 
 Covers the density pass of: AutoregressiveRationalQuadraticSpline (MADE, nets/made.py),
 CoupledRationalQuadraticSpline (ResidualNet, nets/resnet.py, + unconditional CDF), LULinearPermute
-(flows/mixing.py:368-563) and a non-trainable DiagGaussian base.  Each `*_bwd` takes the upstream gradients
+(flows/mixing.py:368-563), Permute and a DiagGaussian base (trainable or not).  Each `*_bwd` takes the upstream gradients
 (g_out w.r.t. the layer output, g_ld w.r.t. its per-sample log-det) and returns the gradient w.r.t. the layer
 input, adding parameter gradients into `grads` under their state_dict names."""
 import numpy as np
@@ -210,12 +210,25 @@ def lu_bwd(z, sd, p, L, g_out, g_ld, grads):
     return gz
 
 
+def permute_bwd(z, sd, p, L, g_out, g_ld, grads):
+    """Adjoint of nf_oracle.permute (density direction): the inverse gather."""
+    c = z.shape[1]
+    gz = np.zeros_like(g_out)
+    if L.get("mode", "shuffle") == "shuffle":
+        gz[:, sd[p + "inv_perm"].astype(np.int64)] = g_out
+    else:
+        h = (c + 1) // 2
+        gz[:, h:], gz[:, :h] = g_out[:, :c - h], g_out[:, c - h:]
+    return gz
+
+
 _BWD = {"AutoregressiveRationalQuadraticSpline": ar_rqs_bwd, "CoupledRationalQuadraticSpline": coupled_rqs_bwd,
-        "LULinearPermute": lu_bwd}
+        "LULinearPermute": lu_bwd, "Permute": permute_bwd}
 
 
-def forward_kld_grads(spec, sd, x):
-    """loss = -mean(log q(x)); returns (loss, {state_dict name: gradient}, d loss / d x) in x's dtype."""
+def log_prob_grads(spec, sd, x, w, trainable_base=False):
+    """Gradients of sum(w * log q(x)) for per-row weights w[B]: (log q(x), {state_dict name: gradient}, d / d x) in x's
+    dtype.  trainable_base: also the DiagGaussian base's q0.loc and q0.log_scale."""
     sd = O._cast(sd, x.dtype)
     flows = spec["flows"]
     zs = [x]
@@ -226,14 +239,23 @@ def forward_kld_grads(spec, sd, x):
         tot = tot + ld
         zs.append(z)
     lp = tot + O.diag_gaussian_log_prob(z, sd, "q0.")
-    loss = -np.mean(lp)
-    bsz = x.shape[0]
-    g_lp = np.full(bsz, -1.0 / bsz, dtype=x.dtype)
+    g_lp = np.asarray(w, dtype=x.dtype)
     loc = sd["q0.loc"].reshape(-1)
     ls = sd["q0.log_scale"].reshape(-1)
-    g_z = g_lp[:, None] * (-(z - loc) / np.exp(2 * ls))  # d log N / d z
+    u = (z - loc) / np.exp(2 * ls)
+    g_z = g_lp[:, None] * (-u)  # d log N / d z
     grads = {}
-    for j, i in enumerate(range(len(flows))):  # backward: layers in list order, inputs from the cache
+    if trainable_base:
+        grads["q0.loc"] = (g_lp[:, None] * u).sum(0).reshape(sd["q0.loc"].shape)
+        grads["q0.log_scale"] = (g_lp[:, None] * ((z - loc) * u - 1)).sum(0).reshape(sd["q0.log_scale"].shape)
+    for i in range(len(flows)):  # backward: layers in list order, inputs from the cache
         z_in = zs[len(flows) - 1 - i]
         g_z = _BWD[flows[i]["type"]](z_in, sd, f"flows.{i}.", flows[i], g_z, g_lp, grads)
-    return loss, grads, g_z
+    return lp, grads, g_z
+
+
+def forward_kld_grads(spec, sd, x):
+    """loss = -mean(log q(x)); returns (loss, {state_dict name: gradient}, d loss / d x) in x's dtype."""
+    bsz = x.shape[0]
+    lp, grads, g_z = log_prob_grads(spec, sd, x, np.full(bsz, -1.0 / bsz, dtype=x.dtype))
+    return -np.mean(lp), grads, g_z
