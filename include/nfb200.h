@@ -668,6 +668,57 @@ int64_t nfb_flow_density_backward_workspace_bytes(const nfb_flow_t* f, int64_t r
 int nfb_flow_density_backward(nfb_flow_t* f, const float* x, const float* g_z, const float* g_ld, int64_t rows,
                               void* ws, int64_t ws_bytes, float* g_x, float* const* grad_slots, void* stream);
 
+/* ---- stochastic layers and HAIS (flows/stochastic.py HamiltonianMonteCarlo / MetropolisHastings, sampling/hais.py) ----
+ * A native density is log p(z) = sum_i coef_i log p_i(z) over n_terms Gaussian mixtures p_i (loc / log_scale
+ * [n_modes, dim], weight_scores [n_modes]); a DiagGaussian is the one-mode mixture with weight score 0, a
+ * LinearInterpolation(d1, d2, alpha) the two terms (alpha, 1 - alpha).  The coefficients are per transition (coef
+ * [transitions, n_terms]) so that one call runs a whole annealing chain.  One thread per row; dim <= NFB_STOCHASTIC_MAX_DIM
+ * (a larger dim: NFB_ERR_UNSUPPORTED).  Every random number is an input, drawn by the caller:
+ * noise [transitions, rows, dim] standard normals, uniforms [transitions, rows] on [0, 1). */
+#define NFB_DENSITY_MAX_TERMS 4
+#define NFB_STOCHASTIC_MAX_DIM 64
+typedef struct {
+    int32_t n_modes;
+    const float* loc;
+    const float* log_scale;
+    const float* weight_scores;
+} nfb_density_term_t;
+typedef struct {
+    int32_t n_terms;
+    int32_t dim;
+    nfb_density_term_t term[NFB_DENSITY_MAX_TERMS];
+} nfb_density_t;
+
+/* `transitions` HMC transitions of HamiltonianMonteCarlo.forward (flows/stochastic.py:54-96), transition t with its own
+ * log_step_size / log_mass [transitions, dim] and coefficients: momentum p = noise exp(log_mass / 2), `leapfrog` leapfrog
+ * steps with grad log p clamped to +-max_abs_grad unless max_abs_grad is 0, accept when uniform < exp(log p(z') -
+ * log p(z) - K(p') + K(p)) (a NaN exponent rejects, an overflowing one accepts).  z_out [rows, dim] is the last state;
+ * log_w [rows] (may be NULL) is incremented by log p_t(z_t) - log p_t(z_{t+1}) for every t (0 on a rejected row);
+ * accept [transitions, rows] (may be NULL) receives each decision.  z_out may alias z.  One launch. */
+int nfb_hmc_chain(const nfb_density_t* density, int64_t rows, int32_t transitions, int32_t leapfrog, float max_abs_grad,
+                  const float* coef, const float* log_step_size, const float* log_mass, const float* noise,
+                  const float* uniforms, const float* z, float* z_out, float* log_w, uint8_t* accept, void* stream);
+/* Gradients of one HMC transition (transitions = 1) with respect to log_step_size and log_mass [dim] (overwritten), given
+ * the cotangent g_z_out [rows, dim] of z_out and the accept decisions of nfb_hmc_chain: grad log p is a constant and the
+ * accept mask has none, so only accepted rows contribute, through the leapfrog arithmetic and the momentum draw.  One
+ * kernel recomputes the leapfrog per row into the workspace ([dim, rows] floats,
+ * nfb_hmc_backward_workspace_bytes), a second sums each feature in a fixed order: no atomics, identical bits on every
+ * call.  g_log_mass is exactly -g_log_step_size / 2 (dz_out/dlog_mass = -dz_out/dlog_step_size / 2).  rows = 0 writes
+ * zeros. */
+int64_t nfb_hmc_backward_workspace_bytes(int64_t rows, int32_t dim);
+int nfb_hmc_backward(const nfb_density_t* density, int64_t rows, int32_t leapfrog, float max_abs_grad, const float* coef,
+                     const float* log_step_size, const float* log_mass, const float* noise, const float* z,
+                     const uint8_t* accept, const float* g_z_out, void* ws, int64_t ws_bytes, float* g_log_step_size,
+                     float* g_log_mass, void* stream);
+/* `steps` steps of MetropolisHastings.forward (flows/stochastic.py:23-45) with DiagGaussianProposal(scale [dim]) on the
+ * density with coefficients coef [n_terms]:
+ * z' = noise scale + z, accept when uniform <= min(exp(log p(z') - log p(z)), 1).  z_out [rows, dim]; log_det [rows]
+ * (overwritten) accumulates log p(z) - log p(z') over the accepted steps; moved [rows] (may be NULL) is 1 where any step
+ * was accepted.  z_out may alias z.  One launch. */
+int nfb_mh_chain(const nfb_density_t* density, int64_t rows, int32_t steps, const float* coef, const float* scale,
+                 const float* noise,
+                 const float* uniforms, const float* z, float* z_out, float* log_det, uint8_t* moved, void* stream);
+
 /* ---- host-buffer entry points (what a non-CUDA caller binds; copies are inside) ---- */
 int nfb_flow_log_prob_host(nfb_flow_t* f, const float* x_host, float* log_q_host, int64_t rows);
 int nfb_flow_forward_kld_host(nfb_flow_t* f, const float* x_host, int64_t rows, float* loss_host);

@@ -1167,6 +1167,35 @@ int nfb_gaussian_mixture_log_prob_backward(const float* z, const float* loc, con
                               g_log_scale, g_weight_scores, S(stream));
 }
 
+int nfb_hmc_chain(const nfb_density_t* density, int64_t rows, int32_t transitions, int32_t leapfrog, float max_abs_grad,
+                  const float* coef, const float* log_step_size, const float* log_mass, const float* noise,
+                  const float* uniforms, const float* z, float* z_out, float* log_w, uint8_t* accept, void* stream) {
+    NFB_CHECK(density, NFB_ERR_ARG, "nfb_hmc_chain: null density");
+    return launch_hmc_chain(*density, rows, transitions, leapfrog, max_abs_grad, coef, log_step_size, log_mass, noise,
+                            uniforms, z, z_out, log_w, accept, S(stream));
+}
+
+int64_t nfb_hmc_backward_workspace_bytes(int64_t rows, int32_t dim) {
+    if (rows < 0 || dim < 1) return -1;
+    return hmc_bwd_ws_bytes(rows, dim);
+}
+
+int nfb_hmc_backward(const nfb_density_t* density, int64_t rows, int32_t leapfrog, float max_abs_grad, const float* coef,
+                     const float* log_step_size, const float* log_mass, const float* noise, const float* z,
+                     const uint8_t* accept, const float* g_z_out, void* ws, int64_t ws_bytes, float* g_log_step_size,
+                     float* g_log_mass, void* stream) {
+    NFB_CHECK(density, NFB_ERR_ARG, "nfb_hmc_backward: null density");
+    return launch_hmc_bwd(*density, rows, leapfrog, max_abs_grad, coef, log_step_size, log_mass, noise, z, accept,
+                          g_z_out, ws, ws_bytes, g_log_step_size, g_log_mass, S(stream));
+}
+
+int nfb_mh_chain(const nfb_density_t* density, int64_t rows, int32_t steps, const float* coef, const float* scale,
+                 const float* noise, const float* uniforms, const float* z, float* z_out, float* log_det, uint8_t* moved,
+                 void* stream) {
+    NFB_CHECK(density, NFB_ERR_ARG, "nfb_mh_chain: null density");
+    return launch_mh_chain(*density, rows, steps, coef, scale, noise, uniforms, z, z_out, log_det, moved, S(stream));
+}
+
 int nfb_conv2d(const float* x, int32_t x_channels, int32_t c0, const float* w, const float* b, float* y,
                int64_t batch, int32_t cin, int32_t height, int32_t width, int32_t cout, int32_t ksize,
                float leaky, void* stream) {

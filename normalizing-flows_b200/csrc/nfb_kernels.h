@@ -1,6 +1,7 @@
 // nfb_kernels.h -- internal launch interface between the C-ABI layer (nfb_api.cu) and the kernels.
 #pragma once
 #include "nfb_common.cuh"
+#include "../../include/nfb200.h"
 #include "nfb_fused_plan.h"
 
 #include <mutex>
@@ -77,6 +78,19 @@ int launch_sum(const float* v, long long n, double scale, double* scratch, float
 int launch_mixture_log_prob(const float* z, const float* loc, const float* log_scale, const float* ws, float* log_q,
                             long long rows, int K, int D, int accumulate, cudaStream_t st);
 long long mixture_bwd_ws_bytes(long long rows, int K, int D);
+// HMC / MH transitions on a native density (nfb_stochastic.cu; arguments as nfb_hmc_chain, nfb_hmc_backward,
+// nfb_mh_chain of include/nfb200.h)
+int launch_hmc_chain(const nfb_density_t& P, long long rows, int L, int leapfrog, float max_abs_grad,
+                     const float* coef, const float* log_step, const float* log_mass, const float* noise,
+                     const float* unif, const float* z, float* z_out, float* log_w, uint8_t* accept, cudaStream_t st);
+long long hmc_bwd_ws_bytes(long long rows, int D);
+int launch_hmc_bwd(const nfb_density_t& P, long long rows, int leapfrog, float max_abs_grad, const float* coef,
+                   const float* log_step, const float* log_mass, const float* noise, const float* z,
+                   const uint8_t* accept, const float* g_out, void* wsp, long long ws_bytes, float* g_log_step,
+                   float* g_log_mass, cudaStream_t st);
+int launch_mh_chain(const nfb_density_t& P, long long rows, int steps, const float* coef, const float* scale,
+                    const float* noise, const float* unif, const float* z, float* z_out, float* log_det,
+                    uint8_t* moved, cudaStream_t st);
 int launch_mixture_bwd(const float* z, const float* loc, const float* log_scale, const float* ws, const float* g_lq,
                        long long rows, int K, int D, void* wsp, long long ws_bytes, float* g_z, float* g_loc,
                        float* g_log_scale, float* g_ws, cudaStream_t st);

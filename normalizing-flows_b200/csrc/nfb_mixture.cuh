@@ -96,4 +96,42 @@ __host__ __device__ inline void mixture_row_adjoint(const T* z, const T* mu, con
     }
 }
 
+// log p of one row of at most DMAX features and, when grad is not null, c * grad_z log p added to grad [D]:
+// grad_d -= c resp_k t_kd exp(-ls_kd), the g_z of mixture_row_adjoint with cotangent c.  The feature loops unroll
+// over DMAX, so a caller's z / grad arrays stay in registers (the HMC / MH kernels of nfb_stochastic.cu, one row per
+// thread); the mode loop streams, so K is unbounded.  Two passes over the modes: the log-sum-exp, then the
+// responsibilities.
+template <int DMAX, typename T>
+__host__ __device__ __forceinline__ T mixture_row_log_prob_grad(const T* z, int D, const T* mu, const T* ls,
+                                                                const T* ws, int K, T c, T* grad) {
+    const T wl = mix_weight_lse(ws, K);
+    T m = -(T)INFINITY, s = (T)0;
+    for (int k = 0; k < K; ++k) {
+        T q = (T)0;
+#pragma unroll
+        for (int d = 0; d < DMAX; ++d)
+            if (d < D) q += mix_quad_term(z[d], mu[k * D + d], mx_exp(-ls[k * D + d]), ls[k * D + d]);
+        mix_lse_push(m, s, mix_mode_exponent(ws[k], wl, D, q));
+    }
+    const T lp = mix_lse_value(m, s);
+    if (grad) {
+        for (int k = 0; k < K; ++k) {
+            T q = (T)0;
+#pragma unroll
+            for (int d = 0; d < DMAX; ++d)
+                if (d < D) q += mix_quad_term(z[d], mu[k * D + d], mx_exp(-ls[k * D + d]), ls[k * D + d]);
+            const T a = c * mx_exp(mix_mode_exponent(ws[k], wl, D, q) - lp);
+#pragma unroll
+            for (int d = 0; d < DMAX; ++d) {
+                if (d < D) {
+                    const T inv = mx_exp(-ls[k * D + d]);
+                    const T t = (z[d] - mu[k * D + d]) * inv;
+                    grad[d] -= a * t * inv;
+                }
+            }
+        }
+    }
+    return lp;
+}
+
 }  // namespace nfb

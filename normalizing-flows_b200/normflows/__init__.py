@@ -10,6 +10,8 @@ there is no CPU/eager fallback."""
 from . import distributions, flows, nets, transforms, utils
 from .core import NormalizingFlow, ConditionalNormalizingFlow, ClassCondFlow, MultiscaleFlow, NormalizingFlowVAE
 from . import parallel
+from . import sampling
+from .sampling import HAIS
 from ._native import invalidate_packed_weights
 
 __version__ = "0.1.0+b200"

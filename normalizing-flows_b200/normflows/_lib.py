@@ -103,6 +103,18 @@ class LipschitzMlpDesc(C.Structure):
                 ("b", C.c_float * LIPSCHITZ_MLP_MAX_LAYERS)]
 
 
+DENSITY_MAX_TERMS = 4
+STOCHASTIC_MAX_DIM = 64
+
+
+class DensityTerm(C.Structure):
+    _fields_ = [("n_modes", C.c_int32), ("loc", C.c_void_p), ("log_scale", C.c_void_p), ("weight_scores", C.c_void_p)]
+
+
+class DensityDesc(C.Structure):
+    _fields_ = [("n_terms", C.c_int32), ("dim", C.c_int32), ("term", DensityTerm * DENSITY_MAX_TERMS)]
+
+
 # every symbol include/nfb200.h declares: (restype, argtypes)
 _VP, _I32, _I64, _F = C.c_void_p, C.c_int32, C.c_int64, C.c_float
 SYMBOLS = {
@@ -183,6 +195,10 @@ SYMBOLS = {
     "nfb_bernoulli_log_prob_backward": (C.c_int, [_VP, _VP, _VP, _I64, _I32, _I64, _VP, _VP, _VP]),
     "nfb_sigmoid": (C.c_int, [_VP, _VP, _I64, _VP]),
     "nfb_sigmoid_backward": (C.c_int, [_VP, _VP, _VP, _I64, _VP]),
+    "nfb_hmc_chain": (C.c_int, [C.POINTER(DensityDesc), _I64, _I32, _I32, _F] + [_VP] * 10),
+    "nfb_hmc_backward_workspace_bytes": (_I64, [_I64, _I32]),
+    "nfb_hmc_backward": (C.c_int, [C.POINTER(DensityDesc), _I64, _I32, _F] + [_VP] * 7 + [_VP, _I64, _VP, _VP, _VP]),
+    "nfb_mh_chain": (C.c_int, [C.POINTER(DensityDesc), _I64, _I32] + [_VP] * 9),
     "nfb_flow_create": (C.c_int, [C.POINTER(_VP), _I32]),
     "nfb_flow_destroy": (C.c_int, [_VP]),
     "nfb_flow_add_ar_rqs": (C.c_int, [_VP, C.POINTER(ArRqsDesc)]),

@@ -9,3 +9,4 @@ from .glow import GlowBlock, Invertible1x1Conv, Squeeze, ImageMerge
 from .residual import Residual, iResBlock
 from .planar import Planar
 from .radial import Radial
+from .stochastic import MetropolisHastings, HamiltonianMonteCarlo
