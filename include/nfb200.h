@@ -583,6 +583,9 @@ int nfb_flow_num_layers(const nfb_flow_t* f);
 int64_t nfb_flow_last_launch_count(const nfb_flow_t* f);
 /* 1 if layer `index` runs on the fused tensor-core kernel in the density direction */
 int nfb_flow_layer_is_fused(const nfb_flow_t* f, int32_t index);
+/* units of the whole-stack sampling plan (one persistent launch for the sampling direction and for its backward's
+   recompute); 0: the sampling direction runs layer by layer */
+int nfb_flow_sampling_units(const nfb_flow_t* f);
 
 /* flows/base.py:13-24: apply ONE layer.  log_det_dev [rows]: overwritten (accumulate=0) or += . */
 int nfb_flow_layer_apply(nfb_flow_t* f, int32_t index, int32_t direction, const float* z_in_dev,

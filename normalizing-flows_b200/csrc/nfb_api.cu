@@ -2611,6 +2611,7 @@ int nfb_flow_layer_is_fused(const nfb_flow_t* f, int32_t index) {
         if ((g.kind == G_FUSED || g.kind == G_FUSED_PAIR) && index >= g.first && index <= g.last) return 1;
     return 0;
 }
+int nfb_flow_sampling_units(const nfb_flow_t* f) { return f ? f->fwd_n : 0; }
 
 int nfb_flow_layer_apply(nfb_flow_t* f, int32_t index, int32_t direction, const float* z_in, float* z_out,
                          float* log_det, int64_t rows, int32_t accumulate, void* stream) {

@@ -217,6 +217,7 @@ SYMBOLS = {
     "nfb_flow_num_layers": (C.c_int, [_VP]),
     "nfb_flow_last_launch_count": (_I64, [_VP]),
     "nfb_flow_layer_is_fused": (C.c_int, [_VP, _I32]),
+    "nfb_flow_sampling_units": (C.c_int, [_VP]),
     "nfb_flow_layer_apply": (C.c_int, [_VP, _I32, _I32, _VP, _VP, _VP, _I64, _I32, _VP]),
     "nfb_flow_transform": (C.c_int, [_VP, _I32, _VP, _VP, _VP, _I64, _VP]),
     "nfb_flow_log_prob": (C.c_int, [_VP, _VP, _VP, _I64, _VP]),

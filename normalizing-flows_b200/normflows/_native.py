@@ -252,6 +252,10 @@ class FlowHandle:
     def launch_count(self):
         return int(L.lib().nfb_flow_last_launch_count(self._h)) if self._h is not None else 0
 
+    def sampling_units(self):
+        """Units of the whole-stack sampling plan (0: the sampling direction runs layer by layer)."""
+        return int(L.lib().nfb_flow_sampling_units(self._h)) if self._h is not None else 0
+
     def fused_layers(self):
         if self._h is None:
             return []

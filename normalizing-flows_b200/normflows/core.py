@@ -80,8 +80,10 @@ class NormalizingFlow(nn.Module):
         h = self._stack()
         self._run_pending_inits(z, inverse=False)
         if h is not None and z.dim() == 2:
-            if self._stack_sampling_backward() and wants_grad(self.flows, z):   # one native backward
-                from ._standalone import stack_sampling
+            if wants_grad(self.flows, z):
+                if not self._stack_sampling_backward():   # h.transform would return a result detached from the graph
+                    raise NotImplementedError(_no_sampling_grad_message("forward_and_log_det") + ")")
+                from ._standalone import stack_sampling   # one native backward
                 return stack_sampling(h, self.flows, z, list(self.flows.parameters()))
             return h.transform(L.NFB_FORWARD, z)
         log_det = torch.zeros(len(z), device=z.device)

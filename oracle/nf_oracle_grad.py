@@ -10,7 +10,10 @@ Covers the density pass of: AutoregressiveRationalQuadraticSpline (MADE, nets/ma
 CoupledRationalQuadraticSpline (ResidualNet, nets/resnet.py, + unconditional CDF), LULinearPermute
 (flows/mixing.py:368-563), Permute and a DiagGaussian base (trainable or not).  Each `*_bwd` takes the upstream gradients
 (g_out w.r.t. the layer output, g_ld w.r.t. its per-sample log-det) and returns the gradient w.r.t. the layer
-input, adding parameter gradients into `grads` under their state_dict names."""
+input, adding parameter gradients into `grads` under their state_dict names.
+
+`sampling_grads` covers the sampling direction (forward_and_log_det) of CoupledRationalQuadraticSpline /
+LULinearPermute stacks, with the reparameterised DiagGaussian draw; its inverse-spline adjoint is built on rqs_bwd."""
 import numpy as np
 
 from . import nf_oracle as O
@@ -252,6 +255,108 @@ def log_prob_grads(spec, sd, x, w, trainable_base=False):
         z_in = zs[len(flows) - 1 - i]
         g_z = _BWD[flows[i]["type"]](z_in, sd, f"flows.{i}.", flows[i], g_z, g_lp, grads)
     return lp, grads, g_z
+
+
+# --------------------------------------------------------------------------
+# sampling direction (forward_and_log_det): coupled spline blocks and LU maps
+# --------------------------------------------------------------------------
+def rqs_inv_bwd(x, uw, uh, ud, gx, g_ld, tail_bound):
+    """Adjoint of nf_oracle.unconstrained_rqs(inverse=True) at its OUTPUT x = f^-1(y) (the inverse's log-det is
+    -log f'(x)), through the implicit-function relation on the forward adjoint rqs_bwd: with
+    lam = gx - g_ld d/dx log f'(x), g_y = lam / f'(x) and the parameters' gradient is rqs_bwd's for
+    (gy = -g_y, glad = -g_ld).  Outside the tails f is the identity: g_y = gx.  Returns (gy, guw, guh, gud)."""
+    zero, one = np.zeros_like(x), np.ones_like(x)
+    fp = rqs_bwd(x, uw, uh, ud, one, zero, tail_bound)[0]        # f'(x) (1 outside)
+    dlog = rqs_bwd(x, uw, uh, ud, zero, one, tail_bound)[0]      # d/dx log f'(x) (0 outside)
+    gy = (gx - g_ld * dlog) / fp
+    _, guw, guh, gud = rqs_bwd(x, uw, uh, ud, -gy, -g_ld, tail_bound)
+    return gy, guw, guh, gud
+
+
+def coupled_rqs_sampling_bwd(z, x, sd, p, L, g_out, g_ld, grads):
+    """Coupling.inverse: x_id = the unconditional CDF's inverse at z_id, the conditioner reads x_id, x_tr = the inverse
+    spline at z_tr.  The conditioner's data gradient joins g_out[id] before the identity columns' inverse adjoint."""
+    k, tb = L.get("num_bins", 8), float(L.get("tail_bound", 3.0))
+    q = p + "prqct."
+    idf = sd[q + "identity_features"].astype(np.int64)
+    trf = sd[q + "transform_features"].astype(np.int64)
+    sc = np.sqrt(sd[q + "transform_net.initial_layer.weight"].shape[0])
+    bsz = z.shape[0]
+    xi, xt = x[:, idf], x[:, trf]
+    params, acts, n, W = _net_fwd(xi, sd, q + "transform_net.", masked=False)
+    pr = params.reshape(bsz, len(trf), 3 * k - 1)
+    uw, uh, ud = pr[..., :k] / sc, pr[..., k:2 * k] / sc, pr[..., 2 * k:]
+    gzt, guw, guh, gud = rqs_inv_bwd(xt, uw, uh, ud, g_out[:, trf], np.broadcast_to(g_ld[:, None], xt.shape), tb)
+    g_params = np.concatenate([guw / sc, guh / sc, gud], axis=-1).reshape(bsz, -1)
+    g_xi = g_out[:, idf] + _net_bwd(g_params, acts, n, W, sd, q + "transform_net.", False, grads)
+    u = q + "unconditional_transform."
+    bc = lambda a: np.broadcast_to(a[None], (bsz,) + a.shape)
+    gzi, g1, g2, g3 = rqs_inv_bwd(xi, bc(sd[u + "unnormalized_widths"]), bc(sd[u + "unnormalized_heights"]),
+                                  bc(sd[u + "unnormalized_derivatives"]), g_xi,
+                                  np.broadcast_to(g_ld[:, None], xi.shape), tb)
+    for name, gg in (("unnormalized_widths", g1), ("unnormalized_heights", g2), ("unnormalized_derivatives", g3)):
+        grads[u + name] = grads.get(u + name, 0) + gg.sum(0)
+    gz = np.zeros_like(z)
+    gz[:, idf] = gzi
+    gz[:, trf] = gzt
+    return gz
+
+
+def lu_sampling_bwd(z, x, sd, p, L, g_out, g_ld, grads):
+    """t = W^-1 (y - b) per row (W = L U), x = t[:, inv_perm], log_det = -sum log diag U:  g_t = g_x[:, perm],
+    g_y = W^-T g_t, dW = -sum_rows g_y t^T, g_b = -colsum(g_y); -sum(g_ld) is the cotangent of log|det W|."""
+    perm = sd[p + "permutation._permutation"].astype(np.int64)
+    lower, upper, diag = O.lu_matrices(sd, p, z.dtype)
+    n = len(perm)
+    t = x[:, perm]                        # x = t[:, inv_perm]
+    g_t = g_out[:, perm]
+    w = lower @ upper
+    g_y = np.linalg.solve(w.T, g_t.T).T   # row form of W^-T g_t
+    d_w = -(g_y.T @ t)
+    grads[p + "linear.bias"] = grads.get(p + "linear.bias", 0) - g_y.sum(0)
+    g_lower = d_w @ upper.T
+    g_upper = lower.T @ d_w
+    grads[p + "linear.lower_entries"] = grads.get(p + "linear.lower_entries", 0) + g_lower[np.tril_indices(n, -1)]
+    grads[p + "linear.upper_entries"] = grads.get(p + "linear.upper_entries", 0) + g_upper[np.triu_indices(n, 1)]
+    ud = sd[p + "linear.unconstrained_upper_diag"].astype(z.dtype)
+    g_diag = np.diag(g_upper) - g_ld.sum() / diag
+    grads[p + "linear.unconstrained_upper_diag"] = grads.get(p + "linear.unconstrained_upper_diag", 0) + \
+        g_diag * O.sigmoid(ud)
+    return g_y
+
+
+_SAMPLING_BWD = {"CoupledRationalQuadraticSpline": coupled_rqs_sampling_bwd, "LULinearPermute": lu_sampling_bwd}
+
+
+def sampling_grads(spec, sd, z, g_x, g_ld, trainable_base=False, g_lq0=None):
+    """Gradients of sum(g_x * x) + sum(g_ld * log_det) of (x, log_det) = nf_oracle.forward_and_log_det(spec, sd, z) for
+    stacks of CoupledRationalQuadraticSpline and LULinearPermute: (x, log_det, {state_dict name: gradient}, d / d z) in
+    z's dtype.  trainable_base: z is the DiagGaussian base's standardised draw eps, the stack's input is
+    loc + exp(log_scale) eps (the reparameterised draw), and g_lq0 [rows] (default 0) is the cotangent of the base's
+    log-density of that draw; q0.loc and q0.log_scale get their gradients and d / d eps is returned."""
+    sd = O._cast(sd, z.dtype)
+    flows = spec["flows"]
+    g_x, g_ld = np.asarray(g_x, z.dtype), np.asarray(g_ld, z.dtype)
+    eps = z
+    if trainable_base:
+        loc, ls = sd["q0.loc"].reshape(-1), sd["q0.log_scale"].reshape(-1)
+        z = loc + np.exp(ls) * eps
+    zs = [z]
+    tot = np.zeros(z.shape[0], dtype=z.dtype)
+    for i, L in enumerate(flows):   # sampling pass, keeping every layer's input and output
+        z, ld = O.LAYERS[L["type"]](z, sd, f"flows.{i}.", L, "forward")
+        tot = tot + ld
+        zs.append(z)
+    grads = {}
+    g = g_x
+    for i in range(len(flows) - 1, -1, -1):
+        g = _SAMPLING_BWD[flows[i]["type"]](zs[i], zs[i + 1], sd, f"flows.{i}.", flows[i], g, g_ld, grads)
+    if trainable_base:
+        glq = np.zeros(eps.shape[0], z.dtype) if g_lq0 is None else np.asarray(g_lq0, z.dtype)
+        grads["q0.loc"] = g.sum(0).reshape(sd["q0.loc"].shape)
+        grads["q0.log_scale"] = ((g * eps * np.exp(ls)).sum(0) - glq.sum()).reshape(sd["q0.log_scale"].shape)
+        g = g * np.exp(ls) - glq[:, None] * eps   # log q0 = -D/2 log 2 pi - sum(log_scale + eps^2 / 2)
+    return z, tot, grads, g
 
 
 def forward_kld_grads(spec, sd, x):

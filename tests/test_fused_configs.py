@@ -87,7 +87,7 @@ def _blocks(cfg):
     if lay == "mixed":
         return cfg["blocks"], "SL" * len(cfg["blocks"])
     pattern = {"SL": "SL", "SLx2": "SLSL", "LS": "LS", "SSL": "SSL", "SPSL": "SPSL", "SPS": "SPS", "S": "S",
-               "SS": "SS"}[lay]
+               "SS": "SS", "SLLS": "SLLS", "LLS": "LLS", "L": "L", "LL": "LL"}[lay]
     n = pattern.count("S")
     kinds = [cfg["kind"]] * n
     if cfg["kind"] in (CPL, CPL_R):   # consecutive coupling blocks alternate their masks, the first one as configured

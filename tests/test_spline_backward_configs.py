@@ -161,7 +161,7 @@ def perturbed_spread(spec, sd, x, w, base):
     return {k: a[k] - b[k] for k in b}
 
 
-def check_grads(got, ref, interim, what, spread=None):
+def check_grads(got, ref, interim, what, spread=None, bars=None):
     """Per tensor (every parameter gradient and "x"), scale = max|ref|: the bulk of the entries within BULK_TOL * scale
     (tensors of BULK_MIN entries or more), the relative Frobenius error within FRO_MULT x the interim path's (never
     below FRO_FLOOR nor above FRO_CAP), the worst entry within ENTRY_TOL * scale.  A reference that is exactly zero
@@ -169,7 +169,9 @@ def check_grads(got, ref, interim, what, spread=None):
     (`spread`: perturbed_spread): there each entry may also miss by 10 x the larger of the interim path's and that
     spread's error on it, and the Frobenius and entry bars are at least 10 x theirs, as test_fused_configs.check_layer
     does for the forward.  Returns the worst native / interim Frobenius ratio, relative
-    Frobenius error, entry / scale and bulk fraction over the tensors."""
+    Frobenius error, entry / scale and bulk fraction over the tensors.  bars: (BULK_TOL, FRO_MULT, FRO_FLOOR, FRO_CAP,
+    ENTRY_TOL) of another backward (default: this file's)."""
+    bulk_tol, fro_mult, fro_floor, fro_cap, entry_tol = bars or (BULK_TOL, FRO_MULT, FRO_FLOOR, FRO_CAP, ENTRY_TOL)
     assert set(got) == set(ref), f"{what}: gradients for {sorted(set(got) ^ set(ref))}"
     worst = [0.0, 0.0, 0.0, 1.0]
     for k, r in ref.items():
@@ -184,15 +186,15 @@ def check_grads(got, ref, interim, what, spread=None):
         nr = np.linalg.norm(r)
         fro, fro_i = np.linalg.norm(d) / nr, np.linalg.norm(di) / nr
         e, e_i = np.abs(d).max() / scale, np.abs(di).max() / scale
-        tol = BULK_TOL * scale
-        fro_bar, e_bar = min(FRO_CAP, max(FRO_FLOOR, FRO_MULT * fro_i)), ENTRY_TOL
+        tol = bulk_tol * scale
+        fro_bar, e_bar = min(fro_cap, max(fro_floor, fro_mult * fro_i)), entry_tol
         if spread is not None:
             ds = np.maximum(np.abs(di), np.abs(spread[k]))
             tol = np.maximum(tol, 10 * ds)
             fro_bar, e_bar = max(fro_bar, 10 * np.linalg.norm(ds) / nr), max(e_bar, 10 * ds.max() / scale)
         frac = float(np.mean(np.abs(d) <= tol))
         assert (frac >= BULK_FRAC or r.size < BULK_MIN) and fro <= fro_bar and e <= e_bar, \
-            f"{what} {k}: {frac:.4f} within {BULK_TOL:g} x scale, rel. Frobenius {fro:.3e} (bar {fro_bar:.3e}, " \
+            f"{what} {k}: {frac:.4f} within {bulk_tol:g} x scale, rel. Frobenius {fro:.3e} (bar {fro_bar:.3e}, " \
             f"interim {fro_i:.3e}), worst entry {e:.3e} x scale (bar {e_bar:.3e}), scale {scale:.3e}"
         worst = [max(worst[0], fro / max(fro_i, 1e-300)), max(worst[1], fro), max(worst[2], e), min(worst[3], frac)]
     return worst
